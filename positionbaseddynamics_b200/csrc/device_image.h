@@ -16,7 +16,7 @@ constexpr int kMaxMat = 5;   // material parameters per type (stiffness, Young's
 constexpr int kMaxGeoV = 6;  // float4 geometry arrays per type
 constexpr int kMaxGeoS = 2;  // scalar geometry arrays per type
 
-// Particle placement in the device arrays.  Layout 1 ("de-interleaved") puts the even-numbered particles first and the
+// Particle placement in the device arrays: the de-interleaved layout puts the even-numbered particles first and the
 // odd-numbered ones behind them.  Reason: the graph-mode step is bound by L2 *sector* throughput, and
 // constraints of one colour never share a particle, so consecutive constraints of a bucket touch particles 2 apart --
 // with the identity layout a warp's gather then uses only one 16-byte half of every 32-byte sector.  After de-interleaving
@@ -25,8 +25,8 @@ constexpr int kMaxGeoS = 2;  // scalar geometry arrays per type
 #if defined(__CUDACC__)
 __host__ __device__
 #endif
-inline unsigned particle_slot(unsigned i, unsigned n, int layout) {
-    return layout == 1 ? (i >> 1) + (i & 1u) * ((n + 1u) >> 1) : i;
+inline unsigned particle_slot(unsigned i, unsigned n) {
+    return (i >> 1) + (i & 1u) * ((n + 1u) >> 1);
 }
 
 struct TypeArrays {
@@ -76,8 +76,6 @@ inline TypeShape type_shape(int t) {
     default:                  return {0, 0, 0, 0, 0, false};
     }
 }
-
-#define type_shape_dev type_shape
 
 // Algorithmic bytes per projection (SURVEY.md section 8d): indices + particle float4 read + per-constraint constants
 // + particle float4 write (+ lambda read/write for XPBD).  Isometric bending uses the rank-1 figure (4 floats Kp).

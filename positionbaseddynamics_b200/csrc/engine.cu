@@ -25,17 +25,17 @@
 #include "host/pbd_model.h"
 
 using namespace pbdk;
+using pbd_b200::host_threads;
+
+// PBD_B200_VERBOSE: flatten and the resident planner report their stages and timings on stderr
+static bool verbose() {
+    static const bool v = getenv("PBD_B200_VERBOSE") != nullptr;
+    return v;
+}
 
 // ------------------------------------------------------------------------------------------------------------
 // error plumbing
 // ------------------------------------------------------------------------------------------------------------
-// OpenMP team of the host-side flatten.  GPU hosts expose far more hardware threads (128 here) than a process may actually use
-// (measured: a 128-thread team made flatten 9x slower than the serial code, 8-16 threads 3x faster), so the team is capped.
-static int host_threads() {
-    static const int n = [] { const char *g = getenv("PBD_B200_HOST_THREADS"); const int want = g ? atoi(g) : 8; return std::max(1, std::min(want, omp_get_max_threads())); }();
-    return n;
-}
-
 static thread_local std::string g_err;
 static int fail(const char *fmt, ...) {
     char buf[1024];
@@ -132,8 +132,7 @@ struct pbd_engine {
     unsigned contactTotal = 0, contactCap = 0;
     float contactTolerance = 0.01f, contactStiffness = 100.0f; unsigned maxIterV = 5;  // CollisionDetection.cpp:25, SimulationModel.cpp:34, TimeStepController.cpp:23
     bool timingPending = false;
-    bool mergeColours = true;             // one launch per colour when it holds several types (PBD_B200_MERGE=0 disables)
-    std::vector<unsigned> slot;           // host particle index -> device slot (formula layouts or the tile-major permutation)
+    std::vector<unsigned> slot;          // host particle index -> device slot (formula layouts or the tile-major permutation)
     DevBuf dSlot, dSlotOld, relayoutTmp;
     bool slotIsTiled = false;
     // resident mode (resident.cuh): G clusters x C CTAs = nTiles tiles, block size and type mask of the instantiation
@@ -141,9 +140,6 @@ struct pbd_engine {
     bool resChecked = false;              // co-residency of the clusters verified for the current image
     DevBuf dColourStart, dTileOff, dTileStart, dTileSmem, dXArrive, dXCounter;
     unsigned long long xBase = 0, xPerStep = 0;  // arrival counter of the X items: value at the next launch, arrivals per substep-sweep unit
-    int layout = 1;                       // particle placement (device_image.h particle_slot); PBD_B200_LAYOUT=linear selects 0
-    bool usePDL = true;                   // programmatic dependent launch between the kernels of a step (PBD_B200_PDL=0 disables)
-    bool gatherCA = true;                 // particle gathers through L1 (tuning knob: PBD_B200_GATHER=cg selects L2-only loads)
     std::vector<unsigned long long> xArriveInt, xArriveCol;  // per-launch bookkeeping of the X counter (host copy of dXArrive)
 };
 
@@ -180,10 +176,6 @@ extern "C" int pbd_create(int device, void *stream, pbd_engine **out) {
         e->ownsStream = true;
     }
     cudaEventCreate(&e->evStart); cudaEventCreate(&e->evStop);
-    if (const char *g = getenv("PBD_B200_GATHER")) e->gatherCA = (strcmp(g, "cg") != 0);
-    if (const char *g = getenv("PBD_B200_PDL")) e->usePDL = (strcmp(g, "0") != 0);
-    if (const char *g = getenv("PBD_B200_MERGE")) e->mergeColours = (strcmp(g, "0") != 0);
-    if (const char *g = getenv("PBD_B200_LAYOUT")) e->layout = (strcmp(g, "linear") == 0) ? 0 : 1;
     *out = e;
     return 0;
 }
@@ -247,7 +239,7 @@ static int upload_slot_map(pbd_engine *e) {
 }
 static void formula_slot_map(pbd_engine *e, std::vector<unsigned> &m) {
     m.resize(e->n);
-    for (unsigned i = 0; i < e->n; i++) m[i] = particle_slot(i, e->n, e->layout);
+    for (unsigned i = 0; i < e->n; i++) m[i] = particle_slot(i, e->n);
 }
 // move every particle array from the current slot map to `newSlot`
 static int relayout(pbd_engine *e, const std::vector<unsigned> &newSlot) {
@@ -408,24 +400,32 @@ extern "C" int pbd_clear_constraints(pbd_engine *e) {
     return 0;
 }
 
+// body k of a constraint of this type is a rigid body (else a particle)
+static bool is_rb_body(int type, int k) { return type == PBD_BALLJOINT || (type == PBD_RB_PARTICLE_BALLJOINT && k == 0); }
+
+// Body indices of `count` constraints of one type against the engine's particle and rigid-body counts, all threads (millions of
+// indices for a big cloth).  Returns the position in `bodies` of the last index out of range, or -1.
+static long long bad_body_index(const pbd_engine *e, int type, const unsigned *bodies, size_t count) {
+    const int nb = type_shape(type).nBodies;
+    long long badAt = -1;
+    #pragma omp parallel for schedule(static) num_threads(host_threads()) reduction(max : badAt) if (count * nb > 100000)
+    for (long long c = 0; c < (long long)count; c++)
+        for (int k = 0; k < nb; k++) {
+            const long long i = c * nb + k;
+            if (bodies[i] >= (is_rb_body(type, k) ? e->nRb : e->n)) badAt = std::max(badAt, i);
+        }
+    return badAt;
+}
+
 extern "C" int pbd_add_constraints(pbd_engine *e, int type, unsigned count, const unsigned *bodies, const float *params, const unsigned *ids) {
     if (!e) return fail("null engine");
     if (type < 0 || type >= PBD_NUM_TYPES) return fail("pbd_add_constraints: unknown constraint type %d", type);
     if (count && (!bodies || !params)) return fail("pbd_add_constraints: null arrays");
     const TypeShape s = type_shape(type);
-    {   // index validation, all threads (millions of indices for a big cloth)
-        const size_t nIdx = (size_t)count * s.nBodies;
-        long long badAt = -1;
-        #pragma omp parallel for schedule(static) num_threads(host_threads()) reduction(max : badAt) if (nIdx > 100000)
-        for (long long i = 0; i < (long long)nIdx; i++) {
-            const bool isRb = (type == PBD_BALLJOINT) || (type == PBD_RB_PARTICLE_BALLJOINT && (i % 2) == 0);
-            if (bodies[i] >= (isRb ? e->nRb : e->n)) badAt = std::max(badAt, i);
-        }
-        if (badAt >= 0) {
-            const bool isRb = (type == PBD_BALLJOINT) || (type == PBD_RB_PARTICLE_BALLJOINT && (badAt % 2) == 0);
-            if (isRb) return fail("pbd_add_constraints: rigid-body index %u out of range (%u bodies; call pbd_set_rigid_bodies first)", bodies[badAt], e->nRb);
-            return fail("pbd_add_constraints: particle index %u out of range (n=%u)", bodies[badAt], e->n);
-        }
+    const long long badAt = bad_body_index(e, type, bodies, count);
+    if (badAt >= 0) {
+        if (is_rb_body(type, (int)(badAt % s.nBodies))) return fail("pbd_add_constraints: rigid-body index %u out of range (%u bodies; call pbd_set_rigid_bodies first)", bodies[badAt], e->nRb);
+        return fail("pbd_add_constraints: particle index %u out of range (n=%u)", bodies[badAt], e->n);
     }
     HostType &h = e->host[type];
     {
@@ -739,8 +739,6 @@ struct ResidentPlan {
     std::vector<unsigned char> homedGlobal;   // host particle lives in global memory (touched by a constraint that spans clusters)
 };
 
-static bool is_rb_body(int type, int k) { return type == PBD_BALLJOINT || (type == PBD_RB_PARTICLE_BALLJOINT && k == 0); }
-
 // Executing tile of a constraint: the tile that holds most of its shared-memory particles (ties: the lowest tile); none -> the tile of
 // its first particle (0 for a joint between rigid bodies).  *touchesGlobal: one of its particles is global-homed.
 static inline unsigned exec_tile(int t, const unsigned *b, int nb, const std::vector<unsigned> &tileOf, const std::vector<unsigned char> &homedGlobal, bool *touchesGlobal) {
@@ -758,27 +756,23 @@ static inline unsigned exec_tile(int t, const unsigned *b, int nb, const std::ve
     return (best != 0xffffffffu) ? best : (first != 0xffffffffu ? first : 0u);
 }
 
-// the compiled instantiations of k_step_resident: F(kernel pointer) for the engine's (mask, block size, one CTA per cluster?)
+// Block size of the resident instantiation of a type mask: the largest it compiles for without spilling (cloth 96 registers,
+// light 128, everything 236).
+constexpr unsigned resident_threads(unsigned mask) { return mask == kMaskClothXPBD ? 640u : (mask == kMaskAll ? 256u : 512u); }
+template <unsigned M, class F> static int resident_kernel(bool single, F &&f) {
+    return single ? f(k_step_resident<M, resident_threads(M), true>) : f(k_step_resident<M, resident_threads(M), false>);
+}
+// the compiled instantiations of k_step_resident: F(kernel pointer) for the engine's type mask, one CTA per cluster or not
 template <class F> static int with_resident_kernel(const pbd_engine *e, unsigned C, F &&f) {
-    const unsigned th = e->resThreads;
     const bool single = (C == 1);
-    if (e->resMask == kMaskClothXPBD) {
-        if (th == 512) return single ? f(k_step_resident<kMaskClothXPBD, 512, true>) : f(k_step_resident<kMaskClothXPBD, 512, false>);
-        if (th == 768) return single ? f(k_step_resident<kMaskClothXPBD, 768, true>) : f(k_step_resident<kMaskClothXPBD, 768, false>);
-        return single ? f(k_step_resident<kMaskClothXPBD, 640, true>) : f(k_step_resident<kMaskClothXPBD, 640, false>);
+    switch (e->resMask) {
+    case kMaskClothXPBD: return resident_kernel<kMaskClothXPBD>(single, f);
+    case kMaskCloth: return resident_kernel<kMaskCloth>(single, f);
+    case kMaskLight: return resident_kernel<kMaskLight>(single, f);
+    case kMaskFem: return resident_kernel<kMaskFem>(single, f);
+    case kMaskSolid: return resident_kernel<kMaskSolid>(single, f);
+    default: return resident_kernel<kMaskAll>(single, f);
     }
-    if (e->resMask == kMaskCloth) return single ? f(k_step_resident<kMaskCloth, 512, true>) : f(k_step_resident<kMaskCloth, 512, false>);
-    if (e->resMask == kMaskLight) return single ? f(k_step_resident<kMaskLight, 512, true>) : f(k_step_resident<kMaskLight, 512, false>);
-    if (e->resMask == kMaskFem) {
-        if (th == 256) return single ? f(k_step_resident<kMaskFem, 256, true>) : f(k_step_resident<kMaskFem, 256, false>);
-        return single ? f(k_step_resident<kMaskFem, 512, true>) : f(k_step_resident<kMaskFem, 512, false>);
-    }
-    if (e->resMask == kMaskSolid) {
-        if (th == 256) return single ? f(k_step_resident<kMaskSolid, 256, true>) : f(k_step_resident<kMaskSolid, 256, false>);
-        return single ? f(k_step_resident<kMaskSolid, 512, true>) : f(k_step_resident<kMaskSolid, 512, false>);
-    }
-    if (th == 512) return single ? f(k_step_resident<kMaskAll, 512, true>) : f(k_step_resident<kMaskAll, 512, false>);
-    return single ? f(k_step_resident<kMaskAll, 256, true>) : f(k_step_resident<kMaskAll, 256, false>);
 }
 
 static void resident_launch_config(const pbd_engine *e, unsigned C, unsigned grid, size_t smem, cudaStream_t s, cudaLaunchConfig_t &cfg, cudaLaunchAttribute *attr) {
@@ -809,12 +803,7 @@ static int choose_resident_shape(pbd_engine *e) {
     e->resMask = kMaskAll;
     for (unsigned m : {kMaskClothXPBD, kMaskCloth, kMaskFem, kMaskLight, kMaskSolid})  // the leanest instantiation that covers the model
         if ((present & ~m) == 0) { e->resMask = m; break; }
-    // the block sizes the instantiations compile for without spilling (cloth 96 registers, light 128, everything 236)
-    e->resThreads = (e->resMask == kMaskClothXPBD) ? 640u : ((e->resMask == kMaskAll) ? 256u : 512u);
-    if (const char *g = getenv("PBD_B200_RTHREADS")) { const int k = atoi(g); if (k == 256 || k == 512 || k == 640 || k == 768) e->resThreads = (unsigned)k; }
-    if (e->resMask == kMaskAll && e->resThreads > 512u) e->resThreads = 512u;
-    if (e->resMask == kMaskLight || e->resMask == kMaskCloth) e->resThreads = 512u;
-    if (e->resMask == kMaskClothXPBD && e->resThreads == 256u) e->resThreads = 512u;
+    e->resThreads = resident_threads(e->resMask);
     const unsigned nGroups = (unsigned)std::max<size_t>(e->groupOff.size(), 2) - 1;
     const unsigned perPhase = e->numConstraints / std::max(1u, nGroups);
     // particles a tile can hold: what is left of the CTA's shared memory after the phase tables (bound: one bucket per colour and type)
@@ -891,7 +880,7 @@ static int prepare_resident(pbd_engine *e, ResidentPlan &pl) {
             }
         // threads of a CTA dedicated to the X items: in proportion to their share, times 3.1 because an X item waits for L2 where
         // the others read shared memory.  The factor is carried over from an earlier GPU; on an H100 80GB HBM3 (400 W) cfg2 is flat in
-        // it: 160 / 192 / 224 / 256 X threads (PBD_B200_XTHREADS) -> 2.07 / 2.05 / 2.09 / 2.11 ms, within the run-to-run spread.
+        // it: 160 / 192 / 224 / 256 X threads -> 2.07 / 2.05 / 2.09 / 2.11 ms, within the run-to-run spread.
         if (G > 1) {
             unsigned long long xItems = 0;
             for (int t = 0; t < PBD_NUM_TYPES; t++) {
@@ -906,9 +895,7 @@ static int prepare_resident(pbd_engine *e, ResidentPlan &pl) {
             }
             const double share = (double)xItems / std::max(1u, e->numConstraints);
             unsigned xt = ((unsigned)(e->resThreads * share * 3.1) + 31u) & ~31u;
-            xt = std::max(64u, std::min(xt, (e->resThreads / 2u) & ~31u));
-            if (const char *g = getenv("PBD_B200_XTHREADS")) { const int k = atoi(g); if (k >= 32 && k % 32 == 0 && (unsigned)k < e->resThreads) xt = (unsigned)k; }
-            e->resXThreads = xt;
+            e->resXThreads = std::max(64u, std::min(xt, (e->resThreads / 2u) & ~31u));
         }
         // tile-major slots: shared-memory particles first (host order), global-homed behind them
         std::vector<unsigned> cntS(T, 0), cntG(T, 0);
@@ -921,7 +908,7 @@ static int prepare_resident(pbd_engine *e, ResidentPlan &pl) {
         for (unsigned t = 0; t < T; t++) { curS[t] = pl.tileStart[t]; curG[t] = pl.tileStart[t] + cntS[t]; }
         for (unsigned i = 0; i < n; i++) newSlot[i] = pl.homedGlobal[i] ? curG[pl.tileOf[i]]++ : curS[pl.tileOf[i]]++;
         CKE(relayout(e, newSlot));
-        if (getenv("PBD_B200_VERBOSE")) {
+        if (verbose()) {
             unsigned long long nGl = 0;
             for (unsigned i = 0; i < n; i++) nGl += pl.homedGlobal[i];
             fprintf(stderr, "[pbd_b200] resident: %u clusters x %u CTAs, %u threads (%u for X items), %u particles, %.2f %% global-homed, max tile %u\n", G, C, e->resThreads, e->resXThreads, n,
@@ -956,445 +943,431 @@ static int flatten(pbd_engine *e) {
     e->active = auto_prefers_resident(e) ? PBD_MODE_RESIDENT : PBD_MODE_GRAPH;
     int rc = flatten_image(e);
     if (rc && e->active == PBD_MODE_RESIDENT) {  // refused (does not fit, user-modified bending Q, ...): the graph mode takes every model
-        if (getenv("PBD_B200_VERBOSE")) fprintf(stderr, "[pbd_b200] auto mode: resident refused (%s), using the graph mode\n", g_err.c_str());
+        if (verbose()) fprintf(stderr, "[pbd_b200] auto mode: resident refused (%s), using the graph mode\n", g_err.c_str());
         e->autoNoResident = true; e->active = PBD_MODE_GRAPH; e->imageDirty = true;
         rc = flatten_image(e);
     }
     return rc;
 }
-static int flatten_image(pbd_engine *e) {
-    if (!e->imageDirty) return 0;
-    CKE(use(e));
-    static const bool verbose = getenv("PBD_B200_VERBOSE") != nullptr;
-    double tPrev = omp_get_wtime();
-    auto lap = [&](const char *what) { if (verbose) { const double t = omp_get_wtime(); fprintf(stderr, "[pbd_b200] flatten: %-34s %.3f s\n", what, t - tPrev); tPrev = t; } };
-    if (!e->groupsSet) {
-        if (e->numConstraints == 0) { e->groupOff.assign(1, 0u); e->groupIds.clear(); e->groupsSet = true; }
-        else {
-            // the reference-order-preserving first fit on the GPU (colouring.cuh); the host version is the fallback and the
-            // PBD_B200_HOST_COLOURING=1 choice
-            static const bool hostColouring = [] { const char *g = getenv("PBD_B200_HOST_COLOURING"); return g && atoi(g) != 0; }();
-            if (hostColouring || pbd_color_first_fit_device(e, nullptr, nullptr)) CKE(pbd_color_first_fit(e));
-        }
+// ---- the stages of flatten_image -----------------------------------------------------------------------------------------------
+// stage timings on stderr (PBD_B200_VERBOSE)
+struct Lap {
+    double prev = omp_get_wtime();
+    void operator()(const char *what) {
+        if (!verbose()) return;
+        const double t = omp_get_wtime();
+        fprintf(stderr, "[pbd_b200] flatten: %-34s %.3f s\n", what, t - prev);
+        prev = t;
     }
-    drop_graph(e);
-    // the particle / rigid-body counts may have shrunk since the constraints were added (pbd_set_particles, pbd_set_rigid_bodies)
+};
+
+// colour groups when none were given: the reference-order-preserving first fit on the GPU (colouring.cuh), the host version as the fallback
+static int colour_if_needed(pbd_engine *e) {
+    if (e->groupsSet) return 0;
+    if (e->numConstraints == 0) { e->groupOff.assign(1, 0u); e->groupIds.clear(); e->groupsSet = true; return 0; }
+    if (pbd_color_first_fit_device(e, nullptr, nullptr)) CKE(pbd_color_first_fit(e));
+    return 0;
+}
+
+// the particle / rigid-body counts may have shrunk since the constraints were added (pbd_set_particles, pbd_set_rigid_bodies)
+static int validate_bodies(const pbd_engine *e) {
     for (int t = 0; t < PBD_NUM_TYPES; t++) {
         const HostType &h = e->host[t];
-        const int nb = type_shape(t).nBodies;
-        long long badAt = -1;
-        #pragma omp parallel for schedule(static) num_threads(host_threads()) reduction(max : badAt) if (h.bodies.size() > 100000)
-        for (long long i = 0; i < (long long)h.bodies.size(); i++) {
-            const bool isRb = (t == PBD_BALLJOINT) || (t == PBD_RB_PARTICLE_BALLJOINT && (i % nb) == 0);
-            if (h.bodies[i] >= (isRb ? e->nRb : e->n)) badAt = std::max(badAt, i);
-        }
-        if (badAt >= 0) {
-            const bool isRb = (t == PBD_BALLJOINT) || (t == PBD_RB_PARTICLE_BALLJOINT && (badAt % nb) == 0);
-            return fail("constraint of type %d refers to %s %u, but the engine holds %u: re-add the constraints after shrinking the model", t,
-                        isRb ? "rigid body" : "particle", h.bodies[badAt], isRb ? e->nRb : e->n);
-        }
+        const long long badAt = bad_body_index(e, t, h.bodies.data(), h.ids.size());
+        if (badAt < 0) continue;
+        const bool isRb = is_rb_body(t, (int)(badAt % type_shape(t).nBodies));
+        return fail("constraint of type %d refers to %s %u, but the engine holds %u: re-add the constraints after shrinking the model", t,
+                    isRb ? "rigid body" : "particle", h.bodies[badAt], isRb ? e->nRb : e->n);
     }
-    std::vector<std::pair<int, unsigned>> map;
-    CKE(build_id_map(e, map));
-    const unsigned nGroups = (unsigned)e->groupOff.size() - 1;
+    return 0;
+}
 
-    // 0. particle placement: tile-major for the resident mode, the formula layout otherwise
-    const bool tiled = (e->active == PBD_MODE_RESIDENT);
-    ResidentPlan pl;
-    std::vector<unsigned> tileOff;
-    std::vector<unsigned> &tileOf = pl.tileOf;
-    if (tiled) CKE(prepare_resident(e, pl));
-    else if (e->slotIsTiled) {
+// particle placement: tile-major for the resident mode, the formula layout otherwise
+static int place_particles(pbd_engine *e, bool tiled, ResidentPlan &pl) {
+    if (tiled) return prepare_resident(e, pl);
+    if (e->slotIsTiled) {
         std::vector<unsigned> m;
         formula_slot_map(e, m);
         CKE(relayout(e, m));
         e->slotIsTiled = false;
     }
+    return 0;
+}
 
-    lap("colouring + validation + placement");
-    // 1. order every type's constraints bucket by bucket
-    // order of the items inside a run by kind of element (see the sort key below): it slows the cloth scenes (H100 80GB HBM3, 400 W:
-    // cfg2 2.07 -> 2.13 ms), so it is on for the solid instantiations only, where the H100 shows no difference either way (cfg3 7.68 /
-    // 7.69 ms); PBD_B200_SIGSORT=0/1 forces it
-    static const int sigSortEnv = [] { const char *g = getenv("PBD_B200_SIGSORT"); return g ? (atoi(g) != 0 ? 1 : 0) : -1; }();
-    const bool sigSort = tiled && (sigSortEnv >= 0 ? sigSortEnv != 0 : (e->resMask == kMaskFem || e->resMask == kMaskSolid));
-    // bank-group fill of the shared-memory runs (below), H100: cfg2 2.14 -> 2.08 ms, cfg5 1.221 -> 1.216 ms; PBD_B200_BANKSORT=0 switches it off
-    static const bool bankSortEnv = [] { const char *g = getenv("PBD_B200_BANKSORT"); return !g || atoi(g) != 0; }();
-    const bool bankSort = tiled && bankSortEnv;
-    static const bool bankSortClusters = [] { const char *g = getenv("PBD_B200_BANKSORT_CLUSTERS"); return !g || atoi(g) != 0; }();  // H100: cfg3 7.81 -> 7.69 ms (bank group taken inside the CTA that holds the particle)
-    std::vector<unsigned> order[PBD_NUM_TYPES];  // device position -> local host index
+typedef std::pair<unsigned long long, unsigned> KeyedItem;  // (sort key, local host index of the constraint)
+struct Wavefronts { double before = 0, after = 0, requests = 0; };
+
+// Shared-memory bank groups of one run of a resident tile.  The eight lanes of a quarter-warp (eight consecutive items of the run) read
+// operand k of their items with one LDS.128; it takes as many wavefronts as the fullest 16-byte bank group (slot & 7 after the swizzle).
+// Greedy re-ordering: each group of eight is filled with the items, out of the next `kWindow` unused ones, that add the fewest
+// collisions over all operands.  The order inside a colour is free; results are bit-identical.  H100 80GB HBM3 (400 W), without / with
+// the fill: cfg2 2.14 / 2.08 ms, cfg5 1.221 / 1.216 ms, cfg3 7.81 / 7.69 ms (bank group taken inside the CTA that holds the particle).
+// With `wf`: the wavefronts of the run's quarter-warp gathers before and after, and their number.
+static void bank_group_fill(KeyedItem *run, size_t cnt, int t, const pbd_engine *e, const ResidentPlan &pl, Wavefronts *wf) {
+    constexpr int kWindow = 64;
+    const int nb = type_shape(t).nBodies, nk = std::min(nb, 4);
+    const unsigned *bod = e->host[t].bodies.data();
+    std::vector<unsigned char> bg(cnt * 4, 0);
+    for (size_t i = 0; i < cnt; i++) {
+        const unsigned *b = bod + (size_t)run[i].second * nb;
+        for (int k = 0; k < nk; k++) bg[i * 4 + k] = (unsigned char)(tile_swizzle(e->slot[b[k]] - pl.tileStart[pl.tileOf[b[k]]]) & 7u);  // bank group inside the CTA that holds the particle
+    }
+    // greedy fill from a sliding pool of the next kWindow unused items (kept in run order)
+    std::vector<unsigned> out; out.reserve(cnt);
+    unsigned pool[kWindow]; int nPool = 0; size_t head = 0;
+    while (out.size() < cnt) {
+        unsigned char load[4][8] = {};
+        for (int j = 0; j < 8 && out.size() < cnt; j++) {
+            while (nPool < kWindow && head < cnt) pool[nPool++] = (unsigned)head++;
+            int best = 0, bestCost = 1 << 30;
+            for (int c = 0; c < nPool; c++) {
+                const unsigned char *g4 = &bg[(size_t)pool[c] * 4];
+                int cost = 0;
+                for (int k = 0; k < nk; k++) cost += load[k][g4[k]];
+                if (cost < bestCost) { bestCost = cost; best = c; if (!cost) break; }
+            }
+            const unsigned pick = pool[best];
+            for (int c = best; c + 1 < nPool; c++) pool[c] = pool[c + 1];
+            nPool--;
+            out.push_back(pick);
+            for (int k = 0; k < nk; k++) load[k][bg[(size_t)pick * 4 + k]]++;
+        }
+    }
+    if (wf) {
+        auto wavefronts = [&](const std::vector<unsigned> &ord) {
+            double w = 0;
+            for (size_t g8 = 0; g8 + 8 <= cnt; g8 += 8)
+                for (int k = 0; k < nk; k++) {
+                    unsigned char c8[8] = {0, 0, 0, 0, 0, 0, 0, 0}; unsigned mx = 0;
+                    for (int j = 0; j < 8; j++) mx = std::max<unsigned>(mx, ++c8[bg[ord[g8 + j] * 4 + k]]);
+                    w += mx;
+                }
+            return w;
+        };
+        std::vector<unsigned> asSorted(cnt);
+        std::iota(asSorted.begin(), asSorted.end(), 0u);
+        wf->before += wavefronts(asSorted); wf->after += wavefronts(out); wf->requests += (double)(cnt / 8) * nk;
+    }
+    const std::vector<KeyedItem> sorted(run, run + cnt);
+    for (size_t i = 0; i < cnt; i++) run[i] = sorted[out[i]];
+}
+
+// The items (local host indices) of the bucket (colour g, type t), re-ordered.  The order inside a colour is free: sorted by lowest
+// particle slot for gather locality (joints keep their order); resident: major key = executing tile, then the X items (touching a
+// global-homed particle) before the others, the shared-memory runs bank-group filled, and the runs of every tile appended to tileOff:
+// [2 tile] X items, [2 tile + 1] the others.
+static void sort_bucket(const pbd_engine *e, unsigned g, int t, std::vector<unsigned> &items, bool tiled, const ResidentPlan &pl, std::vector<unsigned> &tileOff) {
+    const bool joint = (t == PBD_BALLJOINT || t == PBD_RB_PARTICLE_BALLJOINT);
+    const int nb = type_shape(t).nBodies;
+    const unsigned *bod = e->host[t].bodies.data();
+    std::vector<KeyedItem> keyed(items.size());
+    #pragma omp parallel for schedule(static) num_threads(host_threads())
+    for (long long i = 0; i < (long long)items.size(); i++) {
+        const unsigned *b = bod + (size_t)items[i] * nb;
+        unsigned mn = 0xffffffffu;
+        for (int k = 0; k < nb; k++) if (!is_rb_body(t, k)) mn = std::min(mn, e->slot[b[k]]);
+        if (joint) mn = (unsigned)i;
+        // resident: run = executing tile and kind (X items first) in key bits 51 and up.  Ordering a run by kind of element as well
+        // (constraints with the same slot offsets between their particles first) made no difference on an H100 80GB HBM3 (700 W):
+        // cfg3 7.66 / 7.62 ms, cfg4 0.625 / 0.625 ms with / without.
+        unsigned long long run = 0;
+        if (tiled) {
+            bool x = false;
+            const unsigned exec = exec_tile(t, b, nb, pl.tileOf, pl.homedGlobal, &x);
+            run = 2ull * exec + (x ? 0u : 1u);
+        }
+        keyed[i] = std::make_pair((run << 51) | mn, items[i]);
+    }
+    __gnu_parallel::stable_sort(keyed.begin(), keyed.end(), [](const KeyedItem &a, const KeyedItem &b) { return a.first < b.first; },
+                                __gnu_parallel::default_parallel_tag(host_threads()));
+    if (tiled && !joint) {
+        std::vector<size_t> runStart;
+        for (size_t i = 0; i < keyed.size(); i++) if (i == 0 || (keyed[i].first >> 51) != (keyed[i - 1].first >> 51)) runStart.push_back(i);
+        runStart.push_back(keyed.size());
+        double before = 0, after = 0, requests = 0;
+        const long long nRuns = (long long)runStart.size() - 1;
+        #pragma omp parallel for schedule(dynamic, 1) num_threads(host_threads()) reduction(+ : before, after, requests)
+        for (long long r = 0; r < nRuns; r++) {
+            const size_t lo = runStart[r], cnt = runStart[r + 1] - lo;
+            if (!((keyed[lo].first >> 51) & 1ull) || cnt < 16) continue;  // X runs gather from global memory: left alone
+            Wavefronts w;
+            bank_group_fill(&keyed[lo], cnt, t, e, pl, verbose() ? &w : nullptr);
+            before += w.before; after += w.after; requests += w.requests;
+        }
+        if (verbose() && requests > 0) fprintf(stderr, "[pbd_b200] flatten:   colour %u type %d: %.2f wavefronts per quarter-warp gather as sorted, %.2f after the bank-group fill\n", g, t,
+                                               before / requests, after / requests);
+    }
+    #pragma omp parallel for schedule(static) num_threads(host_threads())
+    for (long long i = 0; i < (long long)keyed.size(); i++) items[i] = keyed[i].second;
+    if (tiled) {
+        const size_t base = tileOff.size();
+        tileOff.resize(base + 2 * e->nTiles + 1, 0u);
+        for (size_t i = 0; i < keyed.size(); i++) tileOff[base + (keyed[i].first >> 51) + 1]++;
+        for (unsigned k = 0; k < 2 * e->nTiles; k++) tileOff[base + k + 1] += tileOff[base + k];
+    }
+}
+
+// every colour group split by type into (colour, type) buckets; order[t]: device position -> local host index
+static void order_buckets(pbd_engine *e, const std::vector<std::pair<int, unsigned>> &map, bool tiled, const ResidentPlan &pl,
+                          std::vector<unsigned> (&order)[PBD_NUM_TYPES], std::vector<unsigned> &tileOff) {
+    const unsigned nGroups = (unsigned)e->groupOff.size() - 1;
     e->buckets.clear();
-    std::vector<unsigned> tmp[PBD_NUM_TYPES];
+    std::vector<unsigned> items[PBD_NUM_TYPES];
     for (unsigned g = 0; g < nGroups; g++) {
-        for (auto &v : tmp) v.clear();
+        for (auto &v : items) v.clear();
         for (unsigned i = e->groupOff[g]; i < e->groupOff[g + 1]; i++) {
             const auto &m = map[e->groupIds[i]];
-            tmp[m.first].push_back(m.second);
+            items[m.first].push_back(m.second);
         }
         for (int t = 0; t < PBD_NUM_TYPES; t++) {
-            if (tmp[t].empty()) continue;
+            if (items[t].empty()) continue;
             const bool joint = (t == PBD_BALLJOINT || t == PBD_RB_PARTICLE_BALLJOINT);
-            if ((e->sortBuckets && !joint) || tiled) {  // order inside a colour is free: sort by lowest particle slot for gather locality
-                const int nb = type_shape(t).nBodies;
-                const unsigned *bod = e->host[t].bodies.data();
-                std::vector<std::pair<unsigned long long, unsigned>> keyed(tmp[t].size());
-                #pragma omp parallel for schedule(static) num_threads(host_threads())
-                for (long long i = 0; i < (long long)tmp[t].size(); i++) {
-                    const unsigned *b = bod + (size_t)tmp[t][i] * nb;
-                    unsigned mn = 0xffffffffu;
-                    for (int k = 0; k < nb; k++) if (!is_rb_body(t, k)) mn = std::min(mn, e->slot[b[k]]);
-                    if (joint) mn = (unsigned)i;  // joints keep their order
-                    // resident: major key = executing tile, then X items (touching a global-homed particle) before the others
-                    unsigned long long major = 0;
-                    if (tiled) {
-                        bool x = false;
-                        const unsigned exec = exec_tile(t, b, nb, tileOf, pl.homedGlobal, &x);
-                        major = 2ull * exec + (x ? 0u : 1u);
-                        // Inside a run, constraints that are translates of each other (same slot offsets between their particles: the same
-                        // kind of element of a regular mesh) come first by kind, then by position: consecutive lanes then read addresses that
-                        // advance by one constant stride in every operand, which the tile's XOR swizzle spreads over the bank groups -- a mixed
-                        // order makes the eight lanes of a quarter-warp hit random bank groups (2 wavefronts per 128 bytes on cfg2).
-                        if (sigSort && !joint) {
-                            unsigned long long hsh = 1469598103934665603ull;
-                            for (int k = 1; k < nb; k++) { hsh ^= (unsigned long long)(e->slot[b[k]] - e->slot[b[0]]); hsh *= 1099511628211ull; }
-                            major = (major << 19) | ((hsh ^ (hsh >> 23) ^ (hsh >> 41)) & 0x7ffffull);
-                        } else major <<= 19;
-                    }
-                    keyed[i] = std::make_pair((major << 32) | mn, tmp[t][i]);
-                }
-                __gnu_parallel::stable_sort(keyed.begin(), keyed.end(), [](const std::pair<unsigned long long, unsigned> &a, const std::pair<unsigned long long, unsigned> &b) { return a.first < b.first; },
-                                            __gnu_parallel::default_parallel_tag(host_threads()));
-                if (tiled && (e->resC == 1 || bankSortClusters) && !joint && bankSort) {
-                    // Shared-memory bank groups.  The eight lanes of a quarter-warp (eight consecutive items of a tile's run) read operand k of
-                    // their items with one LDS.128; it takes as many wavefronts as the fullest 16-byte bank group (slot & 7 after the swizzle).
-                    // Greedy re-ordering inside every run: each group of eight is filled with the items, out of the next `kWindow` unused
-                    // ones, that add the fewest collisions over all operands.  The order inside a colour is free; results are bit-identical.
-                    constexpr int kWindow = 64;
-                    std::vector<size_t> runStart;
-                    for (size_t i = 0; i < keyed.size(); i++) if (i == 0 || (keyed[i].first >> 51) != (keyed[i - 1].first >> 51)) runStart.push_back(i);
-                    runStart.push_back(keyed.size());
-                    double wfBefore = 0, wfAfter = 0, requests = 0;
-                    const long long nRuns = (long long)runStart.size() - 1;
-                    #pragma omp parallel for schedule(dynamic, 1) num_threads(host_threads()) reduction(+ : wfBefore, wfAfter, requests)
-                    for (long long r = 0; r < nRuns; r++) {
-                        const size_t lo = runStart[r], hi = runStart[r + 1], cnt = hi - lo;
-                        if (!((keyed[lo].first >> 51) & 1ull) || cnt < 16) continue;  // X runs gather from global memory: left alone
-                        std::vector<unsigned char> bg(cnt * 4, 0);
-                        for (size_t i = 0; i < cnt; i++) {
-                            const unsigned *b = bod + (size_t)keyed[lo + i].second * nb;
-                            for (int k = 0; k < nb && k < 4; k++) bg[i * 4 + k] = (unsigned char)(tile_swizzle(e->slot[b[k]] - pl.tileStart[tileOf[b[k]]]) & 7u);  // bank group inside the CTA that holds the particle
-                        }
-                        auto wavefronts = [&](const std::vector<unsigned> &ord) {
-                            double w = 0;
-                            for (size_t g8 = 0; g8 + 8 <= cnt; g8 += 8)
-                                for (int k = 0; k < nb && k < 4; k++) {
-                                    unsigned char c8[8] = {0, 0, 0, 0, 0, 0, 0, 0}; unsigned mx = 0;
-                                    for (int j = 0; j < 8; j++) mx = std::max<unsigned>(mx, ++c8[bg[ord[g8 + j] * 4 + k]]);
-                                    w += mx;
-                                }
-                            return w;
-                        };
-                        std::vector<unsigned> ord(cnt);
-                        for (size_t i = 0; i < cnt; i++) ord[i] = (unsigned)i;
-                        wfBefore += wavefronts(ord); requests += (double)(cnt / 8) * std::min(nb, 4);
-                        // greedy fill from a sliding pool of the next kWindow unused items (kept in run order)
-                        std::vector<unsigned> out; out.reserve(cnt);
-                        unsigned pool[kWindow]; int nPool = 0; size_t head = 0;
-                        while (out.size() < cnt) {
-                            unsigned char load[4][8] = {};
-                            for (int j = 0; j < 8 && out.size() < cnt; j++) {
-                                while (nPool < kWindow && head < cnt) pool[nPool++] = (unsigned)head++;
-                                int best = 0, bestCost = 1 << 30;
-                                for (int c = 0; c < nPool; c++) {
-                                    const unsigned char *g4 = &bg[(size_t)pool[c] * 4];
-                                    int cost = 0;
-                                    for (int k = 0; k < nb && k < 4; k++) cost += load[k][g4[k]];
-                                    if (cost < bestCost) { bestCost = cost; best = c; if (!cost) break; }
-                                }
-                                const unsigned pick = pool[best];
-                                for (int c = best; c + 1 < nPool; c++) pool[c] = pool[c + 1];
-                                nPool--;
-                                out.push_back(pick);
-                                for (int k = 0; k < nb && k < 4; k++) load[k][bg[(size_t)pick * 4 + k]]++;
-                            }
-                        }
-                        wfAfter += wavefronts(out);
-                        if (bankSort) {
-                            std::vector<std::pair<unsigned long long, unsigned>> tmpRun(cnt);
-                            for (size_t i = 0; i < cnt; i++) tmpRun[i] = keyed[lo + out[i]];
-                            for (size_t i = 0; i < cnt; i++) keyed[lo + i] = tmpRun[i];
-                        }
-                    }
-                    if (verbose && requests > 0) fprintf(stderr, "[pbd_b200] flatten:   colour %u type %d: %.2f wavefronts per quarter-warp gather as sorted, %.2f after the bank-group fill%s\n", g, t,
-                                                         wfBefore / requests, wfAfter / requests, bankSort ? " (applied)" : "");
-                }
-                #pragma omp parallel for schedule(static) num_threads(host_threads())
-                for (long long i = 0; i < (long long)keyed.size(); i++) tmp[t][i] = keyed[i].second;
-                if (tiled) {  // runs of every tile inside this bucket: [2 tile] X items, [2 tile + 1] the others
-                    const size_t base = tileOff.size();
-                    tileOff.resize(base + 2 * e->nTiles + 1, 0u);
-                    for (size_t i = 0; i < keyed.size(); i++) tileOff[base + (keyed[i].first >> 51) + 1]++;
-                    for (unsigned k = 0; k < 2 * e->nTiles; k++) tileOff[base + k + 1] += tileOff[base + k];
-                }
-            }
-            Bucket b; b.type = t; b.first = (unsigned)order[t].size(); b.count = (unsigned)tmp[t].size(); b.colour = g;
+            if ((e->sortBuckets && !joint) || tiled) sort_bucket(e, g, t, items[t], tiled, pl, tileOff);
+            Bucket b; b.type = t; b.first = (unsigned)order[t].size(); b.count = (unsigned)items[t].size(); b.colour = g;
             e->buckets.push_back(b);
-            order[t].insert(order[t].end(), tmp[t].begin(), tmp[t].end());
+            order[t].insert(order[t].end(), items[t].begin(), items[t].end());
         }
     }
+}
 
-    lap("bucket ordering");
-    // debug-grade safety: inside a colour no particle may be used twice (race freedom by construction, SURVEY.md section 5)
-    {
-        // particles and rigid bodies are stamped in separate index spaces (the reference's colouring shares one, which only
-        // ever over-separates; a body really used twice in a colour would be a race here)
-        std::vector<unsigned> stamp((size_t)e->n + e->nRb, 0xffffffffu);
-        size_t bi = 0;
-        for (unsigned g = 0; g < nGroups; g++) {
-            for (; bi < e->buckets.size() && e->buckets[bi].colour == g; bi++) {
-                const Bucket &b = e->buckets[bi];
-                const int nb = type_shape(b.type).nBodies;
-                long long bad = -1;  // items of a bucket in parallel: the stamp of a slot is exchanged atomically
-                #pragma omp parallel for schedule(static) num_threads(host_threads()) reduction(max : bad) if (b.count > 20000)
-                for (long long i = 0; i < (long long)b.count; i++) {
-                    const unsigned *bd = &e->host[b.type].bodies[(size_t)order[b.type][b.first + i] * nb];
-                    for (int k = 0; k < nb; k++) {
-                        const bool isRb = (b.type == PBD_BALLJOINT) || (b.type == PBD_RB_PARTICLE_BALLJOINT && k == 0);
-                        const size_t slot = isRb ? (size_t)e->n + bd[k] : bd[k];
-                        if (__atomic_exchange_n(&stamp[slot], g, __ATOMIC_RELAXED) == g) bad = std::max(bad, (long long)slot);
-                    }
-                }
-                if (bad >= 0) {
-                    const bool isRb = (size_t)bad >= e->n;
-                    return fail("colour group %u uses %s %u twice: the groups are not a valid colouring", g, isRb ? "rigid body" : "particle", (unsigned)(isRb ? bad - e->n : bad));
-                }
+// Debug-grade safety: inside a colour no particle may be used twice (race freedom by construction, SURVEY.md section 5).  Particles
+// and rigid bodies are stamped in separate index spaces (the reference's colouring shares one, which only ever over-separates; a body
+// really used twice in a colour would be a race here).
+static int check_colouring(const pbd_engine *e, const std::vector<unsigned> (&order)[PBD_NUM_TYPES]) {
+    std::vector<unsigned> stamp((size_t)e->n + e->nRb, 0xffffffffu);
+    for (const Bucket &b : e->buckets) {  // colour after colour
+        const unsigned g = b.colour;
+        const int nb = type_shape(b.type).nBodies;
+        long long bad = -1;  // items of a bucket in parallel: the stamp of a slot is exchanged atomically
+        #pragma omp parallel for schedule(static) num_threads(host_threads()) reduction(max : bad) if (b.count > 20000)
+        for (long long i = 0; i < (long long)b.count; i++) {
+            const unsigned *bd = &e->host[b.type].bodies[(size_t)order[b.type][b.first + i] * nb];
+            for (int k = 0; k < nb; k++) {
+                const size_t slot = is_rb_body(b.type, k) ? (size_t)e->n + bd[k] : bd[k];
+                if (__atomic_exchange_n(&stamp[slot], g, __ATOMIC_RELAXED) == g) bad = std::max(bad, (long long)slot);
             }
         }
+        if (bad >= 0) {
+            const bool isRb = (size_t)bad >= e->n;
+            return fail("colour group %u uses %s %u twice: the groups are not a valid colouring", g, isRb ? "rigid body" : "particle", (unsigned)(isRb ? bad - e->n : bad));
+        }
     }
+    return 0;
+}
 
-    lap("colouring validity check");
-    // 2. build and upload the SoA arrays of every type
-    double bytesPerSweep = 0.0;
-    for (int t = 0; t < PBD_NUM_TYPES; t++) {
-        DevType &d = e->dev[t];
-        const HostType &h = e->host[t];
-        const TypeShape s = type_shape(t);
-        const unsigned cnt = (unsigned)order[t].size();
-        d.count = cnt;
-        e->stats.constraints_per_type[t] = cnt;
-        d.arrays = TypeArrays{};
-        d.order.resize(cnt);
-        if (cnt == 0) continue;
+// Parameter columns (include/pbd_b200.h) of a type's SoA arrays: float4 geometry array k = columns gv[k][0..3], scalar geometry
+// array k = column gs[k], material slot k = column mat[k]; -1 = zero-filled component, or no such array / slot.
+struct PackColumns { signed char gv[kMaxGeoV][4], gs[kMaxGeoS], mat[kMaxMat]; };
+static PackColumns pack_columns(int t) {
+    PackColumns p;
+    memset(&p, -1, sizeof(p));
+    auto gv = [&](int k, int c0, int c1, int c2, int c3) { p.gv[k][0] = c0; p.gv[k][1] = c1; p.gv[k][2] = c2; p.gv[k][3] = c3; };
+    auto mat = [&](int first, int count) { for (int k = 0; k < count; k++) p.mat[k] = first + k; };
+    switch (t) {
+    case PBD_DISTANCE: case PBD_DISTANCE_XPBD: case PBD_DIHEDRAL: case PBD_VOLUME: case PBD_VOLUME_XPBD: p.gs[0] = 0; mat(1, 1); break;
+    case PBD_ISOBENDING: case PBD_ISOBENDING_XPBD: for (int r = 0; r < 4; r++) gv(r, 1 + 4 * r, 2 + 4 * r, 3 + 4 * r, 4 + 4 * r); mat(0, 1); break;  // full Q (see pack_type)
+    case PBD_FEMTRIANGLE: p.gs[0] = 0; gv(0, 1, 2, 3, 4); mat(5, 5); break;
+    case PBD_STRAINTRIANGLE: gv(0, 0, 1, 2, 3); mat(4, 5); break;
+    case PBD_FEMTET: case PBD_FEMTET_XPBD: gv(0, 1, 2, 3, 4); gv(1, 5, 6, 7, 8); p.gs[0] = 9; p.gs[1] = 0; mat(10, 2); break;
+    case PBD_STRAINTET: gv(0, 0, 1, 2, 3); gv(1, 4, 5, 6, 7); p.gs[0] = 8; mat(9, 4); break;
+    // local connectors (jointInfo columns 0 [and 1]); the global columns are recomputed per solve
+    case PBD_BALLJOINT: gv(0, 0, 1, 2, -1); gv(1, 3, 4, 5, -1); break;
+    case PBD_RB_PARTICLE_BALLJOINT: gv(0, 0, 1, 2, -1); break;
+    // restCm | x0[0..3] packed in 3 float4 | w | numClusters ; stiffness is the material slot
+    case PBD_SHAPEMATCHING: gv(0, 1, 2, 3, -1); for (int k = 1; k < 6; k++) gv(k, 4 * k, 4 * k + 1, 4 * k + 2, 4 * k + 3); mat(0, 1); break;
+    }
+    return p;
+}
+
+// build and upload the SoA arrays of type t in device order (order: device position -> local host index)
+static int pack_type(pbd_engine *e, int t, const std::vector<unsigned> &order, bool tiled, const ResidentPlan &pl, Lap &lap) {
+    DevType &d = e->dev[t];
+    const HostType &h = e->host[t];
+    const TypeShape s = type_shape(t);
+    const unsigned cnt = (unsigned)order.size();
+    d.count = cnt;
+    e->stats.constraints_per_type[t] = cnt;
+    d.arrays = TypeArrays{};
+    d.order.resize(cnt);
+    if (cnt == 0) return 0;
+    #pragma omp parallel for schedule(static) num_threads(host_threads())
+    for (long long i = 0; i < (long long)cnt; i++) d.order[i] = h.ids[order[i]];
+    auto P = [&](unsigned i, int k) { return h.params[(size_t)order[i] * s.nParams + k]; };
+    auto B = [&](unsigned i, int k) {
+        const unsigned raw = h.bodies[(size_t)order[i] * s.nBodies + k];
+        if (is_rb_body(t, k)) return raw;
+        if (tiled && !pl.homedGlobal[raw]) {  // lives in the shared memory of CTA (tile % C) of the executing cluster
+            const unsigned tl = pl.tileOf[raw];
+            return kSmemFlag | ((tl % e->resC) << kRankShift) | tile_swizzle(e->slot[raw] - pl.tileStart[tl]);
+        }
+        return e->slot[raw];
+    };
+
+    if (verbose()) fprintf(stderr, "[pbd_b200] flatten:   type %d (%u constraints)\n", t, cnt);
+    lap("  order ids");
+    // indices
+    if (s.nBodies == 2) {
+        PodVector<uint2> v(cnt);
         #pragma omp parallel for schedule(static) num_threads(host_threads())
-        for (long long i = 0; i < (long long)cnt; i++) d.order[i] = h.ids[order[t][i]];
-        auto P = [&](unsigned i, int k) { return h.params[(size_t)order[t][i] * s.nParams + k]; };
-        auto B = [&](unsigned i, int k) {
-            const unsigned raw = h.bodies[(size_t)order[t][i] * s.nBodies + k];
-            if (is_rb_body(t, k)) return raw;
-            if (tiled && !pl.homedGlobal[raw]) {  // lives in the shared memory of CTA (tile % C) of the executing cluster
-                const unsigned tl = tileOf[raw];
-                return kSmemFlag | ((tl % e->resC) << kRankShift) | tile_swizzle(e->slot[raw] - pl.tileStart[tl]);
-            }
-            return e->slot[raw];
-        };
-
-        if (verbose) fprintf(stderr, "[pbd_b200] flatten:   type %d (%u constraints)\n", t, cnt);
-        lap("  order ids");
-        // indices
-        if (s.nBodies == 2) {
-            PodVector<uint2> v(cnt);
+        for (long long i = 0; i < (long long)cnt; i++) v[i] = make_uint2(B(i, 0), B(i, 1));
+        CKE(upload_vec(d.idx[0], v, e->stream)); d.arrays.idx2 = (const uint2 *)d.idx[0].p;
+    } else if (s.nBodies == 4) {
+        PodVector<uint4> v(cnt);
+        #pragma omp parallel for schedule(static) num_threads(host_threads())
+        for (long long i = 0; i < (long long)cnt; i++) v[i] = make_uint4(B(i, 0), B(i, 1), B(i, 2), B(i, 3));
+        CKE(upload_vec(d.idx[0], v, e->stream)); d.arrays.idx4 = (const uint4 *)d.idx[0].p;
+    } else {
+        for (int k = 0; k < 3; k++) {
+            PodVector<unsigned> v(cnt);
             #pragma omp parallel for schedule(static) num_threads(host_threads())
-            for (long long i = 0; i < (long long)cnt; i++) v[i] = make_uint2(B(i, 0), B(i, 1));
-            CKE(upload_vec(d.idx[0], v, e->stream)); d.arrays.idx2 = (const uint2 *)d.idx[0].p;
-        } else if (s.nBodies == 4) {
-            PodVector<uint4> v(cnt);
-            #pragma omp parallel for schedule(static) num_threads(host_threads())
-            for (long long i = 0; i < (long long)cnt; i++) v[i] = make_uint4(B(i, 0), B(i, 1), B(i, 2), B(i, 3));
-            CKE(upload_vec(d.idx[0], v, e->stream)); d.arrays.idx4 = (const uint4 *)d.idx[0].p;
-        } else {
-            for (int k = 0; k < 3; k++) {
-                PodVector<unsigned> v(cnt);
-                #pragma omp parallel for schedule(static) num_threads(host_threads())
-                for (long long i = 0; i < (long long)cnt; i++) v[i] = B(i, k);
-                CKE(upload_vec(d.idx[k], v, e->stream)); d.arrays.idx3[k] = (const unsigned *)d.idx[k].p;
-            }
+            for (long long i = 0; i < (long long)cnt; i++) v[i] = B(i, k);
+            CKE(upload_vec(d.idx[k], v, e->stream)); d.arrays.idx3[k] = (const unsigned *)d.idx[k].p;
         }
-
-        lap("  indices (remap + upload)");
-        // geometry + material slots: (param index of each material slot)
-        int matSlot[kMaxMat] = {-1, -1, -1, -1, -1};
-        PodVector<float4> gv[kMaxGeoV]; PodVector<float> gs[kMaxGeoS];
-        int variant = 0;
-        switch (t) {
-        case PBD_DISTANCE: case PBD_DISTANCE_XPBD: case PBD_DIHEDRAL: case PBD_VOLUME: case PBD_VOLUME_XPBD:
-            gs[0].resize(cnt);
-            #pragma omp parallel for schedule(static) num_threads(host_threads())
-            for (long long i = 0; i < (long long)cnt; i++) gs[0][i] = P(i, 0);
-            matSlot[0] = 1;
-            break;
-        case PBD_ISOBENDING: case PBD_ISOBENDING_XPBD: {
-            matSlot[0] = 0;
-            gv[0].resize(cnt);
-            int notRank1 = 0;
-            #pragma omp parallel for schedule(static) num_threads(host_threads()) reduction(| : notRank1)
-            for (long long i = 0; i < (long long)cnt; i++) {
-                float Q[16], Kp[4] = {0.f, 0.f, 0.f, 0.f};
-                for (int k = 0; k < 16; k++) Q[k] = P((unsigned)i, 1 + k);
-                if (!factor_rank1(Q, Kp)) notRank1 |= 1;
-                gv[0][i] = make_float4(Kp[0], Kp[1], Kp[2], Kp[3]);
-            }
-            const bool rank1 = !notRank1;
-            if (!rank1 && tiled) return fail("resident mode: IsometricBending with a user-modified Q matrix (not of the rank-one form) is evaluated by the per-bucket kernels only (use PBD_MODE_GRAPH)");
-            if (!rank1) {  // user-modified Q somewhere in this type: literal 4x4 evaluation for the whole type
-                variant = 1;
-                for (int r = 0; r < 4; r++) {
-                    gv[r].resize(cnt);
-                    #pragma omp parallel for schedule(static) num_threads(host_threads())
-                    for (long long i = 0; i < (long long)cnt; i++) gv[r][i] = make_float4(P(i, 1 + 4 * r), P(i, 2 + 4 * r), P(i, 3 + 4 * r), P(i, 4 + 4 * r));
-                }
-            }
-            break; }
-        case PBD_FEMTRIANGLE:
-            gv[0].resize(cnt); gs[0].resize(cnt);
-            #pragma omp parallel for schedule(static) num_threads(host_threads())
-            for (long long i = 0; i < (long long)cnt; i++) { gs[0][i] = P(i, 0); gv[0][i] = make_float4(P(i, 1), P(i, 2), P(i, 3), P(i, 4)); }
-            for (int k = 0; k < 5; k++) matSlot[k] = 5 + k;
-            break;
-        case PBD_STRAINTRIANGLE:
-            gv[0].resize(cnt);
-            #pragma omp parallel for schedule(static) num_threads(host_threads())
-            for (long long i = 0; i < (long long)cnt; i++) gv[0][i] = make_float4(P(i, 0), P(i, 1), P(i, 2), P(i, 3));
-            for (int k = 0; k < 5; k++) matSlot[k] = 4 + k;
-            break;
-        case PBD_FEMTET: case PBD_FEMTET_XPBD:
-            gv[0].resize(cnt); gv[1].resize(cnt); gs[0].resize(cnt); gs[1].resize(cnt);
-            #pragma omp parallel for schedule(static) num_threads(host_threads())
-            for (long long i = 0; i < (long long)cnt; i++) {
-                gv[0][i] = make_float4(P(i, 1), P(i, 2), P(i, 3), P(i, 4));
-                gv[1][i] = make_float4(P(i, 5), P(i, 6), P(i, 7), P(i, 8));
-                gs[0][i] = P(i, 9); gs[1][i] = P(i, 0);
-            }
-            matSlot[0] = 10; matSlot[1] = 11;
-            break;
-        case PBD_STRAINTET:
-            gv[0].resize(cnt); gv[1].resize(cnt); gs[0].resize(cnt);
-            #pragma omp parallel for schedule(static) num_threads(host_threads())
-            for (long long i = 0; i < (long long)cnt; i++) {
-                gv[0][i] = make_float4(P(i, 0), P(i, 1), P(i, 2), P(i, 3));
-                gv[1][i] = make_float4(P(i, 4), P(i, 5), P(i, 6), P(i, 7));
-                gs[0][i] = P(i, 8);
-            }
-            for (int k = 0; k < 4; k++) matSlot[k] = 9 + k;
-            break;
-        case PBD_BALLJOINT: case PBD_RB_PARTICLE_BALLJOINT:  // local connectors (jointInfo columns 0 [and 1]); global columns are recomputed per solve
-            gv[0].resize(cnt);
-            #pragma omp parallel for schedule(static) num_threads(host_threads())
-            for (long long i = 0; i < (long long)cnt; i++) gv[0][i] = make_float4(P(i, 0), P(i, 1), P(i, 2), 0.0f);
-            if (t == PBD_BALLJOINT) { gv[1].resize(cnt); for (unsigned i = 0; i < cnt; i++) gv[1][i] = make_float4(P(i, 3), P(i, 4), P(i, 5), 0.0f); }
-            break;
-        case PBD_SHAPEMATCHING:  // restCm | x0[0..3] packed in 3 float4 | w | numClusters ; stiffness is the material slot
-            for (int k = 0; k < 6; k++) gv[k].resize(cnt);
-            for (unsigned i = 0; i < cnt; i++) {
-                gv[0][i] = make_float4(P(i, 1), P(i, 2), P(i, 3), 0.0f);
-                gv[1][i] = make_float4(P(i, 4), P(i, 5), P(i, 6), P(i, 7));
-                gv[2][i] = make_float4(P(i, 8), P(i, 9), P(i, 10), P(i, 11));
-                gv[3][i] = make_float4(P(i, 12), P(i, 13), P(i, 14), P(i, 15));
-                gv[4][i] = make_float4(P(i, 16), P(i, 17), P(i, 18), P(i, 19));
-                gv[5][i] = make_float4(P(i, 20), P(i, 21), P(i, 22), P(i, 23));
-                for (int k = 20; k < 24; k++) if (!(P(i, k) >= 1.0f)) return fail("ShapeMatching constraint: numClusters must be >= 1");
-            }
-            matSlot[0] = 0;
-            break;
-        default: return fail("flatten: constraint type %d has no kernel", t);
-        }
-        d.arrays.variant = variant;
-        if (t == PBD_BALLJOINT || t == PBD_RB_PARTICLE_BALLJOINT) {
-            d.arrays.rbX = (float4 *)e->rbX.p; d.arrays.rbQ = (float4 *)e->rbQ.p; d.arrays.rbIinv = (const float4 *)e->rbIinv.p;
-        }
-        lap("  geometry (host fill)");
-        for (int k = 0; k < kMaxGeoV; k++) if (!gv[k].empty()) { CKE(upload_vec(d.gv[k], gv[k], e->stream)); d.arrays.gv[k] = (const float4 *)d.gv[k].p; }
-        for (int k = 0; k < kMaxGeoS; k++) if (!gs[k].empty()) { CKE(upload_vec(d.gs[k], gs[k], e->stream)); d.arrays.gs[k] = (const float *)d.gs[k].p; }
-        lap("  geometry (upload)");
-        // material parameters: one uniform per type when every constraint agrees, else a per-constraint array
-        for (int k = 0; k < kMaxMat; k++) {
-            if (matSlot[k] < 0) continue;
-            const float first = P(0, matSlot[k]);
-            int differs = 0;
-            #pragma omp parallel for schedule(static) num_threads(host_threads()) reduction(| : differs) if (cnt > 100000)
-            for (long long i = 1; i < (long long)cnt; i++) differs |= (P((unsigned)i, matSlot[k]) != first) ? 1 : 0;
-            const bool uniform = !differs;
-            d.arrays.matU[k] = first;
-            if (!uniform) {
-                PodVector<float> v(cnt);
-                #pragma omp parallel for schedule(static) num_threads(host_threads())
-                for (long long i = 0; i < (long long)cnt; i++) v[i] = P(i, matSlot[k]);
-                CKE(upload_vec(d.mat[k], v, e->stream)); d.arrays.mat[k] = (const float *)d.mat[k].p;
-            }
-        }
-        if (s.xpbd) {
-            CKE(d.lambda.alloc((size_t)cnt * sizeof(float) + 16));  // + 16 like the other streamed arrays: the L2 prefetch of a run rounds its end up to 16 bytes
-            CK(cudaMemsetAsync(d.lambda.p, 0, (size_t)cnt * sizeof(float), e->stream));
-            d.arrays.lambda = (float *)d.lambda.p;
-        }
-        lap("  material + multipliers");
-        bytesPerSweep += (double)cnt * algorithmic_bytes(t, variant);
     }
 
-    lap("SoA arrays + upload");
-    // 3. bucket table; resident mode: colour ranges, per-tile runs and the arrival counts of the X items
-    CKE(upload_vec(e->dBuckets, e->buckets, e->stream));
-    if (tiled) {
-        const unsigned T = e->nTiles, warps = e->resXThreads / 32u;  // the dedicated X warps of a CTA
-        std::vector<unsigned> colourStart;
-        for (size_t i = 0; i < e->buckets.size(); i++)
-            if (i == 0 || e->buckets[i].colour != e->buckets[i - 1].colour) colourStart.push_back((unsigned)i);
-        e->resColours = (unsigned)colourStart.size();
-        colourStart.push_back((unsigned)e->buckets.size());
-        if (tileOff.size() != e->buckets.size() * (2 * (size_t)T + 1)) return fail("flatten: internal error (tile runs)");
-        // arrivals on the X counter: one per CTA that owns X work in the phase -- integration phase (global-homed particles), then every colour
-        std::vector<unsigned> xArrive(1 + e->resColours, 0u);
-        (void)warps;
-        for (unsigned t = 0; t < T; t++) xArrive[0] += (pl.tileStart[t + 1] - pl.tileStart[t] - pl.tileSmem[t]) ? 1u : 0u;
-        for (unsigned c = 0; c < e->resColours; c++)
+    lap("  indices (remap + upload)");
+    // geometry: the parameter columns of the table, with two exceptions
+    const PackColumns pc = pack_columns(t);
+    PodVector<float4> gv[kMaxGeoV]; PodVector<float> gs[kMaxGeoS];
+    bool fromColumns = true;
+    if (t == PBD_ISOBENDING || t == PBD_ISOBENDING_XPBD) {
+        // the rank-one form Q = -Kp Kp^T of init_IsometricBendingConstraint: gv[0] = Kp; a user-modified Q anywhere in this type:
+        // the literal 4x4 evaluation (variant 1) for the whole type, Q row by row from the columns of the table
+        gv[0].resize(cnt);
+        int notRank1 = 0;
+        #pragma omp parallel for schedule(static) num_threads(host_threads()) reduction(| : notRank1)
+        for (long long i = 0; i < (long long)cnt; i++) {
+            float Q[16], Kp[4] = {0.f, 0.f, 0.f, 0.f};
+            for (int k = 0; k < 16; k++) Q[k] = P((unsigned)i, 1 + k);
+            if (!factor_rank1(Q, Kp)) notRank1 |= 1;
+            gv[0][i] = make_float4(Kp[0], Kp[1], Kp[2], Kp[3]);
+        }
+        if (notRank1 && tiled) return fail("resident mode: IsometricBending with a user-modified Q matrix (not of the rank-one form) is evaluated by the per-bucket kernels only (use PBD_MODE_GRAPH)");
+        d.arrays.variant = notRank1 ? 1 : 0;
+        fromColumns = notRank1 != 0;
+    }
+    if (t == PBD_SHAPEMATCHING)
+        for (unsigned i = 0; i < cnt; i++)
+            for (int k = 20; k < 24; k++) if (!(P(i, k) >= 1.0f)) return fail("ShapeMatching constraint: numClusters must be >= 1");
+    auto col = [&](unsigned i, int c) { return c < 0 ? 0.0f : P(i, c); };
+    for (int k = 0; k < kMaxGeoV && fromColumns; k++) {
+        const signed char *c = pc.gv[k];
+        if (c[0] < 0 && c[1] < 0 && c[2] < 0 && c[3] < 0) continue;
+        gv[k].resize(cnt);
+        #pragma omp parallel for schedule(static) num_threads(host_threads())
+        for (long long i = 0; i < (long long)cnt; i++) gv[k][i] = make_float4(col(i, c[0]), col(i, c[1]), col(i, c[2]), col(i, c[3]));
+    }
+    for (int k = 0; k < kMaxGeoS; k++) {
+        if (pc.gs[k] < 0) continue;
+        gs[k].resize(cnt);
+        #pragma omp parallel for schedule(static) num_threads(host_threads())
+        for (long long i = 0; i < (long long)cnt; i++) gs[k][i] = P(i, pc.gs[k]);
+    }
+    if (t == PBD_BALLJOINT || t == PBD_RB_PARTICLE_BALLJOINT) {
+        d.arrays.rbX = (float4 *)e->rbX.p; d.arrays.rbQ = (float4 *)e->rbQ.p; d.arrays.rbIinv = (const float4 *)e->rbIinv.p;
+    }
+    lap("  geometry (host fill)");
+    for (int k = 0; k < kMaxGeoV; k++) if (!gv[k].empty()) { CKE(upload_vec(d.gv[k], gv[k], e->stream)); d.arrays.gv[k] = (const float4 *)d.gv[k].p; }
+    for (int k = 0; k < kMaxGeoS; k++) if (!gs[k].empty()) { CKE(upload_vec(d.gs[k], gs[k], e->stream)); d.arrays.gs[k] = (const float *)d.gs[k].p; }
+    lap("  geometry (upload)");
+    // material parameters: one uniform per type when every constraint agrees, else a per-constraint array
+    for (int k = 0; k < kMaxMat; k++) {
+        const int c = pc.mat[k];
+        if (c < 0) continue;
+        const float first = P(0, c);
+        int differs = 0;
+        #pragma omp parallel for schedule(static) num_threads(host_threads()) reduction(| : differs) if (cnt > 100000)
+        for (long long i = 1; i < (long long)cnt; i++) differs |= (P((unsigned)i, c) != first) ? 1 : 0;
+        d.arrays.matU[k] = first;
+        if (differs) {
+            PodVector<float> v(cnt);
+            #pragma omp parallel for schedule(static) num_threads(host_threads())
+            for (long long i = 0; i < (long long)cnt; i++) v[i] = P(i, c);
+            CKE(upload_vec(d.mat[k], v, e->stream)); d.arrays.mat[k] = (const float *)d.mat[k].p;
+        }
+    }
+    if (s.xpbd) {
+        CKE(d.lambda.alloc((size_t)cnt * sizeof(float) + 16));  // + 16 like the other streamed arrays: the L2 prefetch of a run rounds its end up to 16 bytes
+        CK(cudaMemsetAsync(d.lambda.p, 0, (size_t)cnt * sizeof(float), e->stream));
+        d.arrays.lambda = (float *)d.lambda.p;
+    }
+    lap("  material + multipliers");
+    return 0;
+}
+
+// resident mode: colour ranges of the bucket table, the per-tile runs and the arrival counts of the X items
+static int build_phase_tables(pbd_engine *e, const ResidentPlan &pl, const std::vector<unsigned> &tileOff) {
+    const unsigned T = e->nTiles;
+    std::vector<unsigned> colourStart;
+    for (size_t i = 0; i < e->buckets.size(); i++)
+        if (i == 0 || e->buckets[i].colour != e->buckets[i - 1].colour) colourStart.push_back((unsigned)i);
+    e->resColours = (unsigned)colourStart.size();
+    colourStart.push_back((unsigned)e->buckets.size());
+    if (tileOff.size() != e->buckets.size() * (2 * (size_t)T + 1)) return fail("flatten: internal error (tile runs)");
+    // arrivals on the X counter: one per CTA that owns X work in the phase -- integration phase (global-homed particles), then every colour
+    std::vector<unsigned> xArrive(1 + e->resColours, 0u);
+    for (unsigned t = 0; t < T; t++) xArrive[0] += (pl.tileStart[t + 1] - pl.tileStart[t] - pl.tileSmem[t]) ? 1u : 0u;
+    for (unsigned c = 0; c < e->resColours; c++)
+        for (unsigned t = 0; t < T; t++) {
+            unsigned any = 0;
+            for (unsigned bi = colourStart[c]; bi < colourStart[c + 1]; bi++) {
+                const unsigned *off = &tileOff[(size_t)bi * (2 * T + 1) + 2 * t];
+                any |= (off[1] - off[0]);
+            }
+            xArrive[1 + c] += any ? 1u : 0u;
+        }
+    unsigned long long perSweep = 0;
+    for (unsigned c = 0; c < e->resColours; c++) perSweep += xArrive[1 + c];
+    e->xArriveInt.assign(1, xArrive[0]); e->xArriveCol.assign(1, perSweep);
+    CKE(upload_vec(e->dColourStart, colourStart, e->stream));
+    CKE(upload_vec(e->dTileOff, tileOff, e->stream));
+    CKE(upload_vec(e->dXArrive, xArrive, e->stream));
+    CKE(e->dXCounter.alloc(256));
+    CK(cudaMemsetAsync(e->dXCounter.p, 0, 256, e->stream));
+    e->xBase = 0;
+    if (verbose()) {
+        unsigned long long xItems = 0, mxRun = 0;
+        for (size_t bi = 0; bi < e->buckets.size(); bi++)
             for (unsigned t = 0; t < T; t++) {
-                unsigned any = 0;
-                for (unsigned bi = colourStart[c]; bi < colourStart[c + 1]; bi++) {
-                    const unsigned *off = &tileOff[(size_t)bi * (2 * T + 1) + 2 * t];
-                    any |= (off[1] - off[0]);
-                }
-                xArrive[1 + c] += any ? 1u : 0u;
+                const unsigned *off = &tileOff[bi * (2 * (size_t)T + 1) + 2 * t];
+                xItems += off[1] - off[0];
+                mxRun = std::max<unsigned long long>(mxRun, off[2] - off[0]);
             }
-        unsigned long long perSweep = 0;
-        for (unsigned c = 0; c < e->resColours; c++) perSweep += xArrive[1 + c];
-        e->xArriveInt.assign(1, xArrive[0]); e->xArriveCol.assign(1, perSweep);
-        CKE(upload_vec(e->dColourStart, colourStart, e->stream));
-        CKE(upload_vec(e->dTileOff, tileOff, e->stream));
-        CKE(upload_vec(e->dXArrive, xArrive, e->stream));
-        CKE(e->dXCounter.alloc(256));
-        CK(cudaMemsetAsync(e->dXCounter.p, 0, 256, e->stream));
-        e->xBase = 0;
-        if (getenv("PBD_B200_VERBOSE")) {
-            unsigned long long xItems = 0, mxRun = 0;
-            for (size_t bi = 0; bi < e->buckets.size(); bi++)
-                for (unsigned t = 0; t < T; t++) {
-                    const unsigned *off = &tileOff[bi * (2 * (size_t)T + 1) + 2 * t];
-                    xItems += off[1] - off[0];
-                    mxRun = std::max<unsigned long long>(mxRun, off[2] - off[0]);
-                }
-            fprintf(stderr, "[pbd_b200] resident: %u colours, %zu buckets, %.2f %% X items, largest run of a tile in a bucket %llu (mean %.0f), X arrivals per sweep %llu\n",
-                    e->resColours, e->buckets.size(), 100.0 * xItems / std::max(1u, e->numConstraints), mxRun,
-                    (double)e->numConstraints / std::max<size_t>(1, e->buckets.size()) / T, perSweep);
-        }
+        fprintf(stderr, "[pbd_b200] resident: %u colours, %zu buckets, %.2f %% X items, largest run of a tile in a bucket %llu (mean %.0f), X arrivals per sweep %llu\n",
+                e->resColours, e->buckets.size(), 100.0 * xItems / std::max(1u, e->numConstraints), mxRun,
+                (double)e->numConstraints / std::max<size_t>(1, e->buckets.size()) / T, perSweep);
     }
-    CK(cudaStreamSynchronize(e->stream));
+    return 0;
+}
 
+// constraints + colour groups -> the device image of the active mode
+static int flatten_image(pbd_engine *e) {
+    if (!e->imageDirty) return 0;
+    CKE(use(e));
+    Lap lap;
+    CKE(colour_if_needed(e));
+    drop_graph(e);
+    CKE(validate_bodies(e));
+    std::vector<std::pair<int, unsigned>> map;
+    CKE(build_id_map(e, map));
+    const bool tiled = (e->active == PBD_MODE_RESIDENT);
+    ResidentPlan pl;
+    CKE(place_particles(e, tiled, pl));
+    lap("colouring + validation + placement");
+    std::vector<unsigned> order[PBD_NUM_TYPES], tileOff;
+    order_buckets(e, map, tiled, pl, order, tileOff);
+    lap("bucket ordering");
+    CKE(check_colouring(e, order));
+    lap("colouring validity check");
+    for (int t = 0; t < PBD_NUM_TYPES; t++) CKE(pack_type(e, t, order[t], tiled, pl, lap));
+    lap("SoA arrays + upload");
+    CKE(upload_vec(e->dBuckets, e->buckets, e->stream));
+    if (tiled) CKE(build_phase_tables(e, pl, tileOff));
+    CK(cudaStreamSynchronize(e->stream));
     lap("phase tables");
     e->stats.num_constraints = e->numConstraints;
-    e->stats.num_groups = nGroups;
+    e->stats.num_groups = (unsigned)e->groupOff.size() - 1;
     e->stats.num_buckets = (unsigned)e->buckets.size();
-    // algorithmic bytes of one step: sweeps + prologue/epilogue per particle per substep (integrate 48 read + 64 write
-    // when lastX is tracked, velocity update 32 (+16 second order) read + 16 write)  -- SURVEY.md section 8d
-    e->stats.bytes_per_step = bytesPerSweep;  // finalised in pbd_get_stats with the current parameters
     e->imageDirty = false;
     return 0;
 }
@@ -1405,52 +1378,78 @@ static int flatten_image(pbd_engine *e) {
 // Block size of a projection launch (kProjectThreads is only the compiled upper bound).  128 threads rather than 256: more,
 // smaller CTAs ramp up and drain faster in each dependent launch (H100 80GB HBM3, 400 W, graph mode: cfg3 8.48 ms against 11.14 ms
 // with 256; cfg2 5.60 / 5.57 ms); a launch that would not even give every SM one CTA is spread
-// further, down to one warp per CTA, because such phases are pure latency chains (cfg1, cfg3).  PBD_B200_BLOCK=<n> pins the size (development knob).
+// further, down to one warp per CTA, because such phases are pure latency chains (cfg1, cfg3).
 static unsigned project_block(const pbd_engine *e, unsigned count) {
-    static const int pinned = [] { const char *g = getenv("PBD_B200_BLOCK"); return g ? atoi(g) : 0; }();
-    if (pinned >= 32 && pinned <= kProjectThreads) return (unsigned)pinned & ~31u;
     const unsigned perSM = (count + (unsigned)e->smCount - 1) / (unsigned)e->smCount;
     return std::max(32u, std::min(128u, (perSM + 31u) & ~31u));
 }
 
-static int launch_bucket(pbd_engine *e, const Bucket &b, float h, int iterZero, cudaStream_t s) {
-    float4 *pos = (float4 *)e->pos.p;
-    const TypeArrays &a = e->dev[b.type].arrays;
-    const unsigned block = project_block(e, b.count);
-    const unsigned grid = nblk(b.count, block);
+// One kernel of a step.  With `pdl` the launch carries the programmatic-stream-serialization attribute, so that the whole step is one
+// programmatic dependency chain (kernels.cuh); pbd_profile_step launches without it, so that each kernel's duration is its own.
+template <typename... KArgs, typename... Args>
+static cudaError_t launch_step_kernel(void (*kernel)(KArgs...), unsigned grid, unsigned block, cudaStream_t s, bool pdl, Args... args) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(grid); cfg.blockDim = dim3(block); cfg.stream = s;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = e->usePDL ? 1 : 0;
-    cudaError_t le = cudaSuccess;
-#define LBV(T, V) (e->gatherCA ? cudaLaunchKernelEx(&cfg, k_project<T, true, V>, pos, a, b.first, b.count, h, iterZero) \
-                                : cudaLaunchKernelEx(&cfg, k_project<T, false, V>, pos, a, b.first, b.count, h, iterZero))
-#define LB(T) case T: le = LBV(T, 0); break;
-    switch (b.type) {
-    case PBD_ISOBENDING: le = a.variant ? LBV(PBD_ISOBENDING, 1) : LBV(PBD_ISOBENDING, 0); break;
-    case PBD_ISOBENDING_XPBD: le = a.variant ? LBV(PBD_ISOBENDING_XPBD, 1) : LBV(PBD_ISOBENDING_XPBD, 0); break;
-        LB(PBD_DISTANCE) LB(PBD_DISTANCE_XPBD) LB(PBD_DIHEDRAL)
-        LB(PBD_FEMTRIANGLE) LB(PBD_STRAINTRIANGLE) LB(PBD_VOLUME) LB(PBD_VOLUME_XPBD) LB(PBD_FEMTET)
-        LB(PBD_FEMTET_XPBD) LB(PBD_STRAINTET) LB(PBD_SHAPEMATCHING) LB(PBD_BALLJOINT) LB(PBD_RB_PARTICLE_BALLJOINT)
-    default: return fail("no kernel for constraint type %d", b.type);
-    }
-#undef LB
-#undef LBV
-    CK(le);
-    return 0;
+    cfg.attrs = attr; cfg.numAttrs = pdl ? 1 : 0;
+    return cudaLaunchKernelEx(&cfg, kernel, args...);
 }
 
-// all buckets [b0, b1) belong to one colour: one launch for up to kMultiSegments of them
-static int launch_colour(pbd_engine *e, size_t b0, size_t b1, float h, int iterZero, cudaStream_t s, unsigned long long *launches) {
+// (constraint type, layout variant) -> f(T, VAR): the compile-time arguments of the k_project / k_project_jacobi instantiation
+template <int V> using IntC = std::integral_constant<int, V>;
+template <class F> static int with_project_type(int type, int variant, F &&f) {
+    switch (type) {
+    case PBD_ISOBENDING: return variant ? f(IntC<PBD_ISOBENDING>{}, IntC<1>{}) : f(IntC<PBD_ISOBENDING>{}, IntC<0>{});
+    case PBD_ISOBENDING_XPBD: return variant ? f(IntC<PBD_ISOBENDING_XPBD>{}, IntC<1>{}) : f(IntC<PBD_ISOBENDING_XPBD>{}, IntC<0>{});
+#define PT(T) case T: return f(IntC<T>{}, IntC<0>{});
+    PT(PBD_DISTANCE) PT(PBD_DISTANCE_XPBD) PT(PBD_DIHEDRAL) PT(PBD_FEMTRIANGLE) PT(PBD_STRAINTRIANGLE) PT(PBD_VOLUME) PT(PBD_VOLUME_XPBD)
+    PT(PBD_FEMTET) PT(PBD_FEMTET_XPBD) PT(PBD_STRAINTET) PT(PBD_SHAPEMATCHING) PT(PBD_BALLJOINT) PT(PBD_RB_PARTICLE_BALLJOINT)
+#undef PT
+    default: return fail("no kernel for constraint type %d", type);
+    }
+}
+
+static int launch_bucket(pbd_engine *e, const Bucket &b, float h, int iterZero, cudaStream_t s, bool pdl) {
+    const TypeArrays &a = e->dev[b.type].arrays;
+    const unsigned block = project_block(e, b.count);
+    return with_project_type(b.type, a.variant, [&](auto T, auto V) -> int {
+        constexpr int TT = decltype(T)::value, VAR = decltype(V)::value;
+        CK(launch_step_kernel(k_project<TT, VAR>, nblk(b.count, block), block, s, pdl, (float4 *)e->pos.p, a, b.first, b.count, h, iterZero));
+        return 0;
+    });
+}
+
+// Per-kernel timing (pbd_profile_step): an event recorded after every launch and what the launch was -- a constraint type,
+// kLaunchIntegrate or kLaunchVelocity; ev[0] marks the start.
+enum { kLaunchStart = -3, kLaunchVelocity = -2, kLaunchIntegrate = -1 };
+struct LaunchLog {
+    std::vector<cudaEvent_t> ev;
+    std::vector<int> what;
+    ~LaunchLog() { for (cudaEvent_t x : ev) cudaEventDestroy(x); }
+    int mark(cudaStream_t s, int kind) {
+        cudaEvent_t x;
+        CK(cudaEventCreate(&x));
+        ev.push_back(x); what.push_back(kind);
+        CK(cudaEventRecord(x, s));
+        return 0;
+    }
+};
+
+// all buckets [b0, b1) belong to one colour: one launch for up to kMultiSegments of them; with `log` one launch per bucket
+static int launch_colour(pbd_engine *e, size_t b0, size_t b1, float h, int iterZero, cudaStream_t s, LaunchLog *log, unsigned long long *launches) {
     // One launch per colour pays off when the colour is small (latency-bound phases; H100 80GB HBM3, 400 W, graph mode: cfg3 11.0 ->
     // 7.95 ms); a large colour keeps the specialised single-type kernels (cfg2, 250k-constraint colours: 5.59 ms either way).
     constexpr unsigned kMergeMaxConstraints = 65536;
     unsigned colourTotal = 0;
     for (size_t i = b0; i < b1; i++) colourTotal += e->buckets[i].count;
-    if (b1 - b0 == 1 || !e->mergeColours || colourTotal > kMergeMaxConstraints) {
-        for (size_t i = b0; i < b1; i++) { CKE(launch_bucket(e, e->buckets[i], h, iterZero, s)); (*launches)++; }
+    if (b1 - b0 == 1 || log || colourTotal > kMergeMaxConstraints) {
+        for (size_t i = b0; i < b1; i++) {
+            CKE(launch_bucket(e, e->buckets[i], h, iterZero, s, !log));
+            (*launches)++;
+            if (log) CKE(log->mark(s, e->buckets[i].type));
+        }
         return 0;
     }
     for (size_t c0 = b0; c0 < b1; c0 += kMultiSegments) {
@@ -1468,60 +1467,45 @@ static int launch_colour(pbd_engine *e, size_t b0, size_t b1, float h, int iterZ
             blocks += nblk(b.count, block);
         }
         for (int k = m.nSeg; k <= kMultiSegments; k++) m.blockStart[k] = blocks;
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(blocks); cfg.blockDim = dim3(block); cfg.stream = s;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[0].val.programmaticStreamSerializationAllowed = 1;
-        cfg.attrs = attr; cfg.numAttrs = e->usePDL ? 1 : 0;
-        float4 *pos = (float4 *)e->pos.p;
-        CK(e->gatherCA ? cudaLaunchKernelEx(&cfg, k_project_multi<true>, pos, m, h, iterZero)
-                       : cudaLaunchKernelEx(&cfg, k_project_multi<false>, pos, m, h, iterZero));
+        CK(launch_step_kernel(k_project_multi, blocks, block, s, true, (float4 *)e->pos.p, m, h, iterZero));
         (*launches)++;
     }
     return 0;
 }
 
-// prologue / epilogue launches share the PDL attribute so that the whole step is one programmatic dependency chain
-template <typename... KArgs, typename... Args>
-static cudaError_t launch_particles(pbd_engine *e, cudaStream_t s, void (*kernel)(KArgs...), unsigned n, Args... args) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((n + 255) / 256); cfg.blockDim = dim3(256); cfg.stream = s;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = e->usePDL ? 1 : 0;
-    return cudaLaunchKernelEx(&cfg, kernel, args...);
+static RbState rb_state(const pbd_engine *e) {
+    return RbState{(float4 *)e->rbX.p, (float4 *)e->rbQ.p, (float4 *)e->rbV.p, (float4 *)e->rbW.p, (float4 *)e->rbOldX.p, (float4 *)e->rbLastX.p,
+                   (float4 *)e->rbOldQ.p, (float4 *)e->rbLastQ.p, (const float4 *)e->rbI.p, (const float4 *)e->rbIinv.p, e->nRb};
 }
 
-static inline int track_last(const pbd_engine *e) { return 1; }  // lastX is part of the reference's particle state
-
-// one TimeStepController::step as individual launches on stream s; returns the number of kernels launched
-static int enqueue_step_launches(pbd_engine *e, cudaStream_t s, unsigned long long *launches) {
+// One TimeStepController::step as individual launches on stream s; returns the number of kernels launched.  With `log`
+// (pbd_profile_step): one launch per bucket, no PDL, and an event after every launch.
+static int enqueue_step_launches(pbd_engine *e, cudaStream_t s, unsigned long long *launches, LaunchLog *log = nullptr) {
     const float h = e->dt / (float)e->subSteps;  // TimeStepController.cpp:91
     const float invH = (float)(1.0 / (double)h);
     const unsigned n = e->n;
+    const bool pdl = !log;
+    const RbState rb = rb_state(e);
     unsigned long long L = 0;
-    RbState rb{(float4 *)e->rbX.p, (float4 *)e->rbQ.p, (float4 *)e->rbV.p, (float4 *)e->rbW.p, (float4 *)e->rbOldX.p, (float4 *)e->rbLastX.p,
-               (float4 *)e->rbOldQ.p, (float4 *)e->rbLastQ.p, (const float4 *)e->rbI.p, (const float4 *)e->rbIinv.p, e->nRb};
+    auto launched = [&](int kind) { L++; return log ? log->mark(s, kind) : 0; };
     for (unsigned sub = 0; sub < e->subSteps; sub++) {
-        if (e->nRb) { CK(launch_particles(e, s, k_rb_integrate, e->nRb, rb, h, e->g[0], e->g[1], e->g[2])); L++; }
-        if (n) {
-            CK(launch_particles(e, s, k_integrate, n, (float4 *)e->pos.p, (float4 *)e->vel.p, (float4 *)e->oldp.p, (float4 *)e->lastp.p, n, h, e->g[0], e->g[1], e->g[2], track_last(e)));
-            L++;
+        if (e->nRb) { CK(launch_step_kernel(k_rb_integrate, nblk(e->nRb, 256), 256, s, pdl, rb, h, e->g[0], e->g[1], e->g[2])); CKE(launched(kLaunchIntegrate)); }
+        if (n) {  // trackLast = 1: lastX is part of the reference's particle state
+            CK(launch_step_kernel(k_integrate, nblk(n, 256), 256, s, pdl, (float4 *)e->pos.p, (float4 *)e->vel.p, (float4 *)e->oldp.p, (float4 *)e->lastp.p, n, h, e->g[0], e->g[1], e->g[2], 1));
+            CKE(launched(kLaunchIntegrate));
         }
         for (unsigned it = 0; it < e->maxIter; it++)
             for (size_t b0 = 0; b0 < e->buckets.size();) {
                 size_t b1 = b0 + 1;
                 while (b1 < e->buckets.size() && e->buckets[b1].colour == e->buckets[b0].colour) b1++;
-                CKE(launch_colour(e, b0, b1, h, it == 0, s, &L));
+                CKE(launch_colour(e, b0, b1, h, it == 0, s, log, &L));
                 b0 = b1;
             }
         if (n) {
-            CK(launch_particles(e, s, k_velocity, n, (const float4 *)e->pos.p, (float4 *)e->vel.p, (const float4 *)e->oldp.p, (const float4 *)e->lastp.p, n, invH, e->velMethod));
-            L++;
+            CK(launch_step_kernel(k_velocity, nblk(n, 256), 256, s, pdl, (const float4 *)e->pos.p, (float4 *)e->vel.p, (const float4 *)e->oldp.p, (const float4 *)e->lastp.p, n, invH, e->velMethod));
+            CKE(launched(kLaunchVelocity));
         }
-        if (e->nRb) { CK(launch_particles(e, s, k_rb_velocity, e->nRb, rb, invH, (float)(2.0 / (double)h), e->velMethod)); L++; }
+        if (e->nRb) { CK(launch_step_kernel(k_rb_velocity, nblk(e->nRb, 256), 256, s, pdl, rb, invH, (float)(2.0 / (double)h), e->velMethod)); CKE(launched(kLaunchVelocity)); }
     }
     *launches = L;
     return 0;
@@ -1561,23 +1545,19 @@ static int enqueue_step_resident(pbd_engine *e, cudaStream_t s, unsigned long lo
     {   // L2 prefetch of the operand runs pays when the constraint stream of a sweep does not stay in L2 anyway (above ~0.38 x the L2).
         // H100 80GB HBM3 (400 W, 50 MB L2), prefetch off / on: cfg2 (192 MB per sweep) 2.28 / 2.08 ms, cfg5 (48 MB) 1.246 / 1.216 ms,
         // 300x300 cloth (below the threshold) 1.015 / 1.016 ms.
-        static const char *g = getenv("PBD_B200_L2PREFETCH");
         double streamBytes = 0.0;
         for (int t = 0; t < PBD_NUM_TYPES; t++) {
             const TypeShape sh = type_shape(t);
             streamBytes += (double)e->dev[t].count * (4.0 * sh.nBodies + 16.0 * sh.nGeoV + 4.0 * sh.nGeoS + (sh.xpbd ? 4.0 : 0.0));
         }
-        ra.l2Prefetch = g ? atoi(g) : (streamBytes > 0.38 * (double)e->l2Bytes ? 1 : 0);
-        static const char *pm = getenv("PBD_B200_POLL");
-        ra.relaxedPoll = pm ? atoi(pm) : 0;
+        ra.l2Prefetch = streamBytes > 0.38 * (double)e->l2Bytes ? 1 : 0;
     }
     ra.h = h; ra.invH = (float)(1.0 / (double)h); ra.twoInvH = (float)(2.0 / (double)h); ra.gx = e->g[0]; ra.gy = e->g[1]; ra.gz = e->g[2];
     ra.secondOrder = e->velMethod;
     ra.xCounter = (unsigned long long *)e->dXCounter.p;
     ra.xBase = e->xBase;
     e->xBase += (unsigned long long)e->subSteps * (e->xArriveInt[0] + (unsigned long long)e->maxIter * e->xArriveCol[0]);
-    ra.rb = RbState{(float4 *)e->rbX.p, (float4 *)e->rbQ.p, (float4 *)e->rbV.p, (float4 *)e->rbW.p, (float4 *)e->rbOldX.p, (float4 *)e->rbLastX.p,
-                    (float4 *)e->rbOldQ.p, (float4 *)e->rbLastQ.p, (const float4 *)e->rbI.p, (const float4 *)e->rbIinv.p, e->nRb};
+    ra.rb = rb_state(e);
     for (int t = 0; t < PBD_NUM_TYPES; t++) ra.types[t] = e->dev[t].arrays;
     *launches = 1;
     ra.trace = nullptr; ra.tracePhases = 0;
@@ -1622,21 +1602,12 @@ static int enqueue_step_jacobi(pbd_engine *e, cudaStream_t s, unsigned long long
                 const unsigned cnt = e->dev[t].count;
                 if (!cnt) continue;
                 const TypeArrays &a = e->dev[t].arrays;
-                const unsigned grid = nblk(cnt, 128);
-                const int iz = (it == 0);
-#define JB(T, V) k_project_jacobi<T, V><<<grid, 128, 0, s>>>(pos, delta, a, cnt, h, iz)
-                switch (t) {
-                case PBD_DISTANCE: JB(PBD_DISTANCE, 0); break; case PBD_DISTANCE_XPBD: JB(PBD_DISTANCE_XPBD, 0); break;
-                case PBD_DIHEDRAL: JB(PBD_DIHEDRAL, 0); break;
-                case PBD_ISOBENDING: if (a.variant) JB(PBD_ISOBENDING, 1); else JB(PBD_ISOBENDING, 0); break;
-                case PBD_ISOBENDING_XPBD: if (a.variant) JB(PBD_ISOBENDING_XPBD, 1); else JB(PBD_ISOBENDING_XPBD, 0); break;
-                case PBD_FEMTRIANGLE: JB(PBD_FEMTRIANGLE, 0); break; case PBD_STRAINTRIANGLE: JB(PBD_STRAINTRIANGLE, 0); break;
-                case PBD_VOLUME: JB(PBD_VOLUME, 0); break; case PBD_VOLUME_XPBD: JB(PBD_VOLUME_XPBD, 0); break;
-                case PBD_FEMTET: JB(PBD_FEMTET, 0); break; case PBD_FEMTET_XPBD: JB(PBD_FEMTET_XPBD, 0); break;
-                case PBD_STRAINTET: JB(PBD_STRAINTET, 0); break; case PBD_SHAPEMATCHING: JB(PBD_SHAPEMATCHING, 0); break;
-                default: break;
-                }
-#undef JB
+                CKE(with_project_type(t, a.variant, [&](auto T, auto V) -> int {
+                    constexpr int TT = decltype(T)::value, VAR = decltype(V)::value;
+                    if constexpr (TT < PBD_BALLJOINT)  // the joints are refused above
+                        k_project_jacobi<TT, VAR><<<nblk(cnt, 128), 128, 0, s>>>(pos, delta, a, cnt, h, it == 0);
+                    return 0;
+                }));
                 L++;
             }
             k_jacobi_apply<<<nblk(n, 256), 256, 0, s>>>((float4 *)e->pos.p, delta, n); L++;
@@ -1940,54 +1911,25 @@ extern "C" int pbd_profile_step(pbd_engine *e, float *msPerType, float *msIntegr
     if (e->active == PBD_MODE_RESIDENT || e->active == PBD_MODE_JACOBI || e->mode == PBD_MODE_AUTO) return fail("pbd_profile_step: per-bucket launches do not exist in this mode (select PBD_MODE_GRAPH or PBD_MODE_LAUNCH first)");
     CKE(use(e)); CKE(flatten(e));
     CK(cudaStreamSynchronize(e->stream));
-    // One event between every pair of consecutive launches, all recorded in stream order without host synchronisation
-    // (a host sync per launch would time the idle-launch latency, not the kernel); read back after one final sync.
-    const size_t nLaunch = (size_t)e->subSteps * (4 + (size_t)e->maxIter * e->buckets.size());
-    RbState rb{(float4 *)e->rbX.p, (float4 *)e->rbQ.p, (float4 *)e->rbV.p, (float4 *)e->rbW.p, (float4 *)e->rbOldX.p, (float4 *)e->rbLastX.p,
-               (float4 *)e->rbOldQ.p, (float4 *)e->rbLastQ.p, (const float4 *)e->rbI.p, (const float4 *)e->rbIinv.p, e->nRb};
-    std::vector<cudaEvent_t> ev(nLaunch + 1);
-    for (auto &x : ev) CK(cudaEventCreate(&x));
-    std::vector<int> what(nLaunch);  // >= 0: type, -1 integrate, -2 velocity
-    const float h = e->dt / (float)e->subSteps;
-    const float invH = (float)(1.0 / (double)h);
-    const unsigned n = e->n;
-    const bool pdl = e->usePDL;
-    e->usePDL = false;  // serialise: each kernel's duration must be its own
-    size_t k = 0;
-    int rc = 0;
-    CK(cudaEventRecord(ev[0], e->stream));
-    for (unsigned sub = 0; sub < e->subSteps && !rc; sub++) {
-        if (e->nRb) { k_rb_integrate<<<nblk(e->nRb, 32), 32, 0, e->stream>>>(rb, h, e->g[0], e->g[1], e->g[2]); what[k] = -1; cudaEventRecord(ev[++k], e->stream); }
-        if (n) {
-            k_integrate<<<nblk(n, 256), 256, 0, e->stream>>>((float4 *)e->pos.p, (float4 *)e->vel.p, (float4 *)e->oldp.p, (float4 *)e->lastp.p, n, h, e->g[0], e->g[1], e->g[2], track_last(e));
-            what[k] = -1; cudaEventRecord(ev[++k], e->stream);
-        }
-        for (unsigned it = 0; it < e->maxIter && !rc; it++)
-            for (const Bucket &bk : e->buckets) {
-                rc = launch_bucket(e, bk, h, it == 0, e->stream);
-                if (rc) break;
-                what[k] = bk.type; cudaEventRecord(ev[++k], e->stream);
-            }
-        if (n && !rc) {
-            k_velocity<<<nblk(n, 256), 256, 0, e->stream>>>((const float4 *)e->pos.p, (float4 *)e->vel.p, (const float4 *)e->oldp.p, (const float4 *)e->lastp.p, n, invH, e->velMethod);
-            what[k] = -2; cudaEventRecord(ev[++k], e->stream);
-        }
-        if (e->nRb && !rc) { k_rb_velocity<<<nblk(e->nRb, 32), 32, 0, e->stream>>>(rb, invH, (float)(2.0 / (double)h), e->velMethod); what[k] = -2; cudaEventRecord(ev[++k], e->stream); }
-    }
-    e->usePDL = pdl;
-    cudaError_t se = cudaStreamSynchronize(e->stream);
+    // One event after every launch, all recorded in stream order without host synchronisation (a host sync per launch would time
+    // the idle-launch latency, not the kernel); read back after one final sync.
+    LaunchLog log;
+    CKE(log.mark(e->stream, kLaunchStart));
+    unsigned long long L = 0;
+    const int rc = enqueue_step_launches(e, e->stream, &L, &log);
+    const cudaError_t se = cudaStreamSynchronize(e->stream);
     if (msPerType) for (int t = 0; t < PBD_NUM_TYPES; t++) msPerType[t] = 0.0f;
     if (launchesPerType) for (int t = 0; t < PBD_NUM_TYPES; t++) launchesPerType[t] = 0;
     float mi = 0.0f, mv = 0.0f;
     if (!rc && se == cudaSuccess)
-        for (size_t i = 0; i < k; i++) {
+        for (size_t i = 1; i < log.ev.size(); i++) {
             float ms = 0.0f;
-            cudaEventElapsedTime(&ms, ev[i], ev[i + 1]);
-            if (what[i] == -1) mi += ms;
-            else if (what[i] == -2) mv += ms;
-            else { if (msPerType) msPerType[what[i]] += ms; if (launchesPerType) launchesPerType[what[i]]++; }
+            cudaEventElapsedTime(&ms, log.ev[i - 1], log.ev[i]);
+            const int what = log.what[i];
+            if (what == kLaunchIntegrate) mi += ms;
+            else if (what == kLaunchVelocity) mv += ms;
+            else { if (msPerType) msPerType[what] += ms; if (launchesPerType) launchesPerType[what]++; }
         }
-    for (auto &x : ev) cudaEventDestroy(x);
     if (rc) return rc;
     if (se != cudaSuccess) return fail("pbd_profile_step: %s", cudaGetErrorString(se));
     if (msIntegrate) *msIntegrate = mi;

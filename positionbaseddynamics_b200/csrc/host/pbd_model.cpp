@@ -76,8 +76,10 @@ struct FlatEdgeMap {
 };
 }  // namespace
 
-// OpenMP team of the host-side model build (capped: GPU hosts expose far more hardware threads than pay off here)
-static int model_threads() {
+// OpenMP team of the host-side model build and of the engine's flatten.  GPU hosts expose far more hardware threads (128 here)
+// than a process may actually use (measured: a 128-thread team made flatten 9x slower than the serial code, 8-16 threads 3x
+// faster), so the team is capped at 8, or at PBD_B200_HOST_THREADS.
+int host_threads() {
     static const int n = [] { const char *g = getenv("PBD_B200_HOST_THREADS"); const int want = g ? atoi(g) : 8; return std::max(1, std::min(want, omp_get_max_threads())); }();
     return n;
 }
@@ -87,7 +89,7 @@ static int model_threads() {
 // pair, position), the first of every run creates the edge, the edge's index is the rank of that creating position.
 // exclusive prefix sum of flags[0..count) into pos[0..count] (pos[count] = total), two passes over per-thread chunks
 static void parallel_prefix(const unsigned char *flags, size_t count, unsigned int *pos) {
-    const int T = std::max(1, model_threads());
+    const int T = std::max(1, host_threads());
     std::vector<size_t> chunkSum((size_t)T + 1, 0);
     #pragma omp parallel num_threads(T)
     {
@@ -126,7 +128,7 @@ void IndexedFaceMesh::buildNeighbors() {
         struct Half { uint64_t key; unsigned int pos; };
         std::unique_ptr<Half[]> hbuf(new Half[nH]);  // uninitialised: filled from all threads
         Half *h = hbuf.get();
-        const int threads = model_threads();
+        const int threads = host_threads();
         #pragma omp parallel for schedule(static) num_threads(threads)
         for (long long p = 0; p < (long long)nH; p++) {
             const unsigned int f = (unsigned int)(p / 3), j = (unsigned int)(p % 3);
@@ -155,7 +157,7 @@ void IndexedFaceMesh::buildNeighbors() {
         }
     }
     int open = 0;
-    #pragma omp parallel for schedule(static) num_threads(model_threads()) reduction(| : open)
+    #pragma omp parallel for schedule(static) num_threads(host_threads()) reduction(| : open)
     for (long long i = 0; i < (long long)m_edges.size(); i++) open |= (m_edges[i].m_face[1] == 0xffffffffu) ? 1 : 0;
     m_closed = !open;
 }
@@ -288,11 +290,11 @@ void SimulationModel::addRegularTriangleModel(int width, int height, const Vecto
     const Real dy = scale[1] / (Real)(height - 1);
     const Real dx = scale[0] / (Real)(width - 1);
     std::vector<Vector3r> points((size_t)width * height);
-    #pragma omp parallel for schedule(static) num_threads(model_threads())
+    #pragma omp parallel for schedule(static) num_threads(host_threads())
     for (int i = 0; i < height; i++)
         for (int j = 0; j < width; j++) points[(size_t)i * width + j] = rotTrans(rotation, Vector3r(dx * j, dy * i, 0.0f), translation);
     PodVector<unsigned int> indices((size_t)6 * (height - 1) * (width - 1));
-    #pragma omp parallel for schedule(static) num_threads(model_threads())
+    #pragma omp parallel for schedule(static) num_threads(host_threads())
     for (int i = 0; i < height - 1; i++)
         for (int j = 0; j < width - 1; j++) {
             const unsigned int helper = (i % 2 == j % 2) ? 1u : 0u;
@@ -457,12 +459,12 @@ static void push_bulk(TypeStore &s, PodVector<ConstraintRef> &order, int type, s
     const int nb = pbd_num_bodies(type), np = pbd_num_params(type);
     std::unique_ptr<unsigned char[]> flag(new unsigned char[count + 1]);
     std::unique_ptr<unsigned int[]> pos(new unsigned int[count + 1]);
-    #pragma omp parallel for schedule(static) num_threads(model_threads())
+    #pragma omp parallel for schedule(static) num_threads(host_threads())
     for (long long i = 0; i < (long long)count; i++) flag[i] = accept((size_t)i) ? 1 : 0;  // cheap topological test
     parallel_prefix(flag.get(), count, pos.get());
     const size_t add = pos[count], base = s.ids.size(), obase = order.size();
     s.ids.resize(base + add); s.bodies.resize((base + add) * nb); s.params.resize((base + add) * np); order.resize(obase + add);  // uninitialised: filled below
-    #pragma omp parallel for schedule(static) num_threads(model_threads())
+    #pragma omp parallel for schedule(static) num_threads(host_threads())
     for (long long i = 0; i < (long long)count; i++) {
         if (!flag[i]) continue;
         const size_t k = pos[i];
@@ -837,18 +839,17 @@ bool TimeStepController::uploadModel(SimulationModel &model) {
         }
         // Colour groups (TimeStepController.cpp:256 -> SimulationModel::initConstraintGroups).  When the model has not been coloured yet the
         // engine does it on the GPU (pbd_color_first_fit_device: the same greedy first fit, identical groups) and the result is mirrored
-        // into the model, so getConstraintGroups() shows what is simulated; PBD_B200_HOST_COLOURING=1 keeps the host colouring.
+        // into the model, so getConstraintGroups() shows what is simulated; the host colouring is the fallback.
         lap("constraints (pbd_add_constraints)");
-        static const bool hostColouring = [] { const char *g = getenv("PBD_B200_HOST_COLOURING"); return g && atoi(g) != 0; }();
         bool coloured = false;
-        if (!model.m_groupsInitialized && !hostColouring && model.numConstraints() > 0 && pbd_color_first_fit_device(m_engine, nullptr, nullptr) == 0) {
+        if (!model.m_groupsInitialized && model.numConstraints() > 0 && pbd_color_first_fit_device(m_engine, nullptr, nullptr) == 0) {
             unsigned int ng = 0;
             if (pbd_get_num_groups(m_engine, &ng) == 0) {
                 std::vector<unsigned int> off(ng + 1), ids(model.numConstraints());
                 if (pbd_get_groups(m_engine, off.data(), ids.data()) == 0) {
                     SimulationModel::ConstraintGroupVector &groups = model.getConstraintGroups();
                     groups.assign(ng, std::vector<unsigned int>());
-                    #pragma omp parallel for schedule(dynamic, 1) num_threads(model_threads())
+                    #pragma omp parallel for schedule(dynamic, 1) num_threads(host_threads())
                     for (long long g = 0; g < (long long)ng; g++) groups[g].assign(ids.begin() + off[g], ids.begin() + off[g + 1]);
                     model.m_groupsInitialized = true;
                     coloured = true;

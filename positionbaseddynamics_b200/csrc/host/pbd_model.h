@@ -316,6 +316,9 @@ private:
     Real m_contactStiffnessParticleRigidBody = static_cast<Real>(100.0);
 };
 
+// OpenMP team size of the host-side model build and of the engine's flatten (capped; PBD_B200_HOST_THREADS sets the cap)
+int host_threads();
+
 // Greedy first-fit colouring shared by SimulationModel::initConstraintGroups and pbd_color_first_fit: constraint c uses
 // bodies[bodyOff[c] .. bodyOff[c+1]); returns per-constraint colour and the number of colours.
 unsigned int firstFitColouring(unsigned int numBodies, unsigned int numConstraints, const unsigned int *bodyOff,

@@ -1,10 +1,8 @@
 // positionbaseddynamics_b200/csrc/kernels.cuh
 //
 // sm_90a kernels of the PBD/XPBD step.  One thread projects one constraint: it loads the constraint's particle
-// indices (coalesced), gathers the particle float4s straight from L2 (ld.global.cg -- within one colour every
-// particle is touched by at most one constraint, so there is no L1 reuse to win and, in the persistent kernel,
-// L1 must not serve stale lines across colour phases), runs the projection in registers and scatters the float4s
-// back (st.global.cg).  Colours guarantee disjoint particle sets, so no atomics.
+// indices (coalesced), gathers the particle float4s through L1 (plain ld.global, see ldp), runs the projection in
+// registers and scatters the float4s back (st.global.cg).  Colours guarantee disjoint particle sets, so no atomics.
 //
 //   k_integrate   : TimeStepController.cpp:112-118 + TimeIntegration::semiImplicitEuler (TimeIntegration.cpp:7-19);
 //                   gravity is a uniform (TimeStep::clearAccelerations sets a = g for every dynamic particle, TimeStep.cpp:28-62)
@@ -31,12 +29,9 @@ __device__ __forceinline__ void pdl_wait_after(unsigned a, float b) {
     asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %0, %1;\n\t@p griddepcontrol.wait;\n\t@!p griddepcontrol.wait;\n\t}" :: "r"(a), "r"(__float_as_uint(b)) : "memory");
 }
 
-// Particle gather flavour (template parameter CA of the kernels):
-//   CA = false: ld.global.cg -- L2 only.
-//   CA = true : ld.global.ca -- through L1, so the 2-4 gathers of one constraint and of neighbouring threads that fall
-//               into the same 32 B sector / 128 B line are served once.  Safe because L1 is invalidated at every kernel
-//               boundary and, in the persistent kernel, by the gpu-scope fence on the acquire side of the grid barrier.
-template <bool CA> __device__ __forceinline__ float4 ldp(const float4 *p) { return CA ? *p : __ldcg(p); }
+// Particle gather of the per-bucket kernels: through L1, so the 2-4 gathers of one constraint and of neighbouring threads
+// that fall into the same 32 B sector / 128 B line are served once.  Safe because L1 is invalidated at every kernel boundary.
+__device__ __forceinline__ float4 ldp(const float4 *p) { return *p; }
 __device__ __forceinline__ void stp(float4 *p, const float4 &v) { if (v.w != 0.0f) __stcg(p, v); }  // static particles never move
 
 __device__ __forceinline__ float matv(const TypeArrays &a, int slot, unsigned i) {
@@ -84,11 +79,11 @@ __device__ __forceinline__ Streamed load_streamed(const TypeArrays &a, unsigned 
 //   GlobalAcc : the float4 array in global memory (L2-resident), index = device slot
 //   ClusterAcc (resident.cuh): bit 31 set -> slot in the shared-memory tile of a CTA of the executing cluster (DSMEM), else global
 // handle(idx) resolves the address once; ld / st take the handle (a particle is read and written through the same one)
-template <bool CA> struct GlobalAcc {
+struct GlobalAcc {
     typedef float4 *Handle;
     float4 *pos;
     __device__ __forceinline__ Handle handle(unsigned idx) const { return pos + idx; }
-    __device__ __forceinline__ float4 ld(Handle h) const { return ldp<CA>(h); }
+    __device__ __forceinline__ float4 ld(Handle h) const { return ldp(h); }
     __device__ __forceinline__ void st(Handle h, const float4 &v) const { stp(h, v); }
 };
 
@@ -166,9 +161,9 @@ __device__ __forceinline__ void project_streamed_acc(const Acc &acc, const TypeA
     if (NB >= 4) acc.st(h3, p3);
 }
 
-template <int T, bool CA, int VAR = -1>
+template <int T, int VAR = -1>
 __device__ __forceinline__ void project_streamed(float4 *pos, const TypeArrays &a, unsigned i, const Streamed &s, float dt, bool iterZero) {
-    project_streamed_acc<T, GlobalAcc<CA>, VAR>(GlobalAcc<CA>{pos}, a, i, s, dt, iterZero);
+    project_streamed_acc<T, GlobalAcc, VAR>(GlobalAcc{pos}, a, i, s, dt, iterZero);
 }
 
 #ifndef PBD_PROJECT_THREADS
@@ -176,7 +171,7 @@ __device__ __forceinline__ void project_streamed(float4 *pos, const TypeArrays &
 #endif
 constexpr int kProjectThreads = PBD_PROJECT_THREADS;
 
-template <int T, bool CA, int VAR>
+template <int T, int VAR>
 __global__ void __launch_bounds__(kProjectThreads) k_project(float4 *pos, TypeArrays a, unsigned first,
                                                              unsigned count, float dt, int iterZero) {
     pdl_launch_dependents();
@@ -184,7 +179,7 @@ __global__ void __launch_bounds__(kProjectThreads) k_project(float4 *pos, TypeAr
     if (i >= count) return;  // an exited thread counts as having passed the dependency
     const Streamed s = load_streamed<T>(a, first + i);
     pdl_wait_after(s.b.x ^ s.b.y, s.g0.x + s.g1.x + s.s0 + s.s1);
-    project_streamed<T, CA, VAR>(pos, a, first + i, s, dt, iterZero != 0);
+    project_streamed<T, VAR>(pos, a, first + i, s, dt, iterZero != 0);
 }
 
 // ---- Jacobi comparison path (north_star: "a Jacobi path uses atomicAdd for comparison") -------------------------------------------
@@ -234,7 +229,6 @@ struct MultiArgs {
     TypeArrays arrays[kMultiSegments];
 };
 
-template <bool CA>
 __global__ void __launch_bounds__(kProjectThreads) k_project_multi(float4 *pos, const __grid_constant__ MultiArgs m, float dt, int iterZero) {
     pdl_launch_dependents();
     int s = 0;
@@ -246,7 +240,7 @@ __global__ void __launch_bounds__(kProjectThreads) k_project_multi(float4 *pos, 
     const TypeArrays &a = m.arrays[s];
     const unsigned ci = m.first[s] + i;
 #define PM(T) case T: { const Streamed st = load_streamed<T>(a, ci); pdl_wait_after(st.b.x ^ st.b.y, st.g0.x + st.g1.x + st.s0 + st.s1); \
-                        project_streamed<T, CA>(pos, a, ci, st, dt, iterZero != 0); } break;
+                        project_streamed<T>(pos, a, ci, st, dt, iterZero != 0); } break;
     switch (m.type[s]) {
         PM(PBD_DISTANCE) PM(PBD_DISTANCE_XPBD) PM(PBD_DIHEDRAL) PM(PBD_ISOBENDING) PM(PBD_ISOBENDING_XPBD) PM(PBD_FEMTRIANGLE)
         PM(PBD_STRAINTRIANGLE) PM(PBD_VOLUME) PM(PBD_VOLUME_XPBD) PM(PBD_FEMTET) PM(PBD_FEMTET_XPBD) PM(PBD_STRAINTET) PM(PBD_SHAPEMATCHING) PM(PBD_BALLJOINT) PM(PBD_RB_PARTICLE_BALLJOINT)

@@ -100,7 +100,6 @@ struct ResidentArgs {
     unsigned xThreads;            // the last xThreads threads of every CTA run the X items (and nothing else); 0 when there is one cluster
     unsigned clusterSize;         // CTAs per cluster (1: the colour barrier is a plain __syncthreads)
     int l2Prefetch;               // prefetch the next colour's operand runs into L2 (scenes whose constraint stream exceeds L2)
-    int relaxedPoll;              // X warps poll the counter with relaxed loads + back-off and fence once (else: acquire loads)
     float h, invH, twoInvH, gx, gy, gz;
     int secondOrder;
     unsigned long long *xCounter; // monotone arrival counter of the X items (global memory)
@@ -120,11 +119,6 @@ __device__ __forceinline__ unsigned smem_u32(const void *p) { return (unsigned)_
 __device__ __forceinline__ unsigned long long ld_acquire_u64(const unsigned long long *p) {
     unsigned long long v;
     asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ unsigned long long ld_relaxed_u64(const unsigned long long *p) {
-    unsigned long long v;
-    asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
     return v;
 }
 __device__ __forceinline__ void red_release_add_u64(unsigned long long *p, unsigned long long v) {
@@ -216,7 +210,7 @@ template <int T>
 __device__ __forceinline__ void l2_prefetch_run(const TypeArrays &a, unsigned first, unsigned n, unsigned lane) {
     constexpr bool two = (T == PBD_DISTANCE || T == PBD_DISTANCE_XPBD || T == PBD_BALLJOINT || T == PBD_RB_PARTICLE_BALLJOINT);
     constexpr bool tri = (T == PBD_FEMTRIANGLE || T == PBD_STRAINTRIANGLE);
-    const TypeShape sh = type_shape_dev(T);
+    const TypeShape sh = type_shape(T);
     if (lane == 0) {
         if (two) l2_prefetch_bytes(a.idx2 + first, (size_t)n * 8u);
         else if (tri) l2_prefetch_bytes(a.idx3[0] + first, (size_t)n * 4u);
@@ -335,15 +329,9 @@ __device__ __forceinline__ void velocity_particle(const ResidentArgs &A, unsigne
 //   arrive: after the X warps' stores -- barrier (orders them before thread 0), then thread 0 publishes with red.release.gpu
 //           (the fence is cumulative over what the barrier ordered: the cooperative-groups grid.sync pattern).
 __device__ __forceinline__ void x_bar(unsigned xThreads) { asm volatile("bar.sync 1, %0;" :: "r"(xThreads) : "memory"); }
-__device__ __forceinline__ void x_wait(const unsigned long long *counter, unsigned long long target, unsigned xtid, unsigned xThreads, int relaxedPoll) {
-    if (xtid == 0) {
-        if (relaxedPoll) {
-            while (ld_relaxed_u64(counter) < target) __nanosleep(20);
-            asm volatile("fence.acq_rel.gpu;" ::: "memory");
-        } else {
-            while (ld_acquire_u64(counter) < target) { }
-        }
-    }
+__device__ __forceinline__ void x_wait(const unsigned long long *counter, unsigned long long target, unsigned xtid, unsigned xThreads) {
+    if (xtid == 0)
+        while (ld_acquire_u64(counter) < target) { }
     x_bar(xThreads);
 }
 __device__ __forceinline__ void x_arrive(unsigned long long *counter, unsigned xtid, unsigned xThreads) {
@@ -445,7 +433,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_step_resident(const __grid_const
                     bool mine = false;  // CTA-uniform: does this CTA own an X item of this colour?
                     for (unsigned bi = b0; bi < b1; bi++) mine = mine || (runs[bi].nX != 0u);
                     if (mine) {
-                        x_wait(A.xCounter, xTarget, xtid, XT, A.relaxedPoll);
+                        x_wait(A.xCounter, xTarget, xtid, XT);
 #pragma unroll 1
                         for (unsigned bi = b0; bi < b1; bi++) run_items<MASK, false>(A, accX, runs[bi].type, runs[bi].firstX, runs[bi].nX, iterZero, xtid, XT, pre.bucket == bi, pre);
                         x_arrive(A.xCounter, xtid, XT);
@@ -476,7 +464,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_step_resident(const __grid_const
 
         // ---- epilogue: velocity update (own particles only; the global-homed ones need the last colour's X items of every cluster)
         if (isX) {
-            if (nGl) x_wait(A.xCounter, xTarget, xtid, XT, A.relaxedPoll);
+            if (nGl) x_wait(A.xCounter, xTarget, xtid, XT);
             for (unsigned i = xtid; i < nGl; i += XT) velocity_particle(A, t0 + nSm + i, __ldcg(A.pos + t0 + nSm + i));
         } else {
             for (unsigned i = threadIdx.x; i < nSm; i += RT) velocity_particle(A, t0 + i, tile[tile_swizzle(i)]);

@@ -1,7 +1,8 @@
 """Development aid: time to the first step of cfg2 from nothing (C++ host model -> engine), one fresh model per execution mode.
 Run on the GPU box: [PBD_B200_VERBOSE=1] python tools/flatten_time.py [size]"""
-import sys, time
-sys.path.insert(0, '/root/repo'); sys.path.insert(0, '/root/repo/tests')
+import os, sys, time
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
 import numpy as np, scenes
 from positionbaseddynamics_b200 import _capi
 from positionbaseddynamics_b200.model import HostModel

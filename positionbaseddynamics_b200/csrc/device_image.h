@@ -50,30 +50,31 @@ struct Bucket {
     unsigned colour;  // index of the reference colour group
 };
 
-// static per-type shape of the image
-struct TypeShape { int nBodies, nParams, nGeoV, nGeoS, nMat; bool xpbd; };
+// static per-type shape of the image.  nStreamV: the leading float4 geometry arrays that load_streamed (kernels.cuh) fetches
+// ahead of the dependency on the previous colour phase; a projection reads any further ones itself.
+struct TypeShape { int nBodies, nParams, nGeoV, nStreamV, nGeoS, nMat; bool xpbd; };
 
 #if defined(__CUDACC__)
 __host__ __device__
 #endif
-inline TypeShape type_shape(int t) {
+constexpr TypeShape type_shape(int t) {
     switch (t) {
-    case PBD_DISTANCE:        return {2, 2, 0, 1, 1, false};
-    case PBD_DISTANCE_XPBD:   return {2, 2, 0, 1, 1, true};
-    case PBD_DIHEDRAL:        return {4, 2, 0, 1, 1, false};
-    case PBD_ISOBENDING:      return {4, 17, 4, 0, 1, false};  // nGeoV: 1 (rank-1) or 4 (full Q), decided at flatten
-    case PBD_ISOBENDING_XPBD: return {4, 17, 4, 0, 1, true};
-    case PBD_FEMTRIANGLE:     return {3, 10, 1, 1, 5, false};
-    case PBD_STRAINTRIANGLE:  return {3, 9, 1, 0, 5, false};
-    case PBD_VOLUME:          return {4, 2, 0, 1, 1, false};
-    case PBD_VOLUME_XPBD:     return {4, 2, 0, 1, 1, true};
-    case PBD_FEMTET:          return {4, 12, 2, 2, 2, false};
-    case PBD_FEMTET_XPBD:     return {4, 12, 2, 2, 2, true};
-    case PBD_STRAINTET:       return {4, 13, 2, 1, 4, false};
-    case PBD_SHAPEMATCHING:   return {4, 24, 6, 0, 1, false};
-    case PBD_BALLJOINT:       return {2, 12, 2, 0, 0, false};
-    case PBD_RB_PARTICLE_BALLJOINT: return {2, 6, 1, 0, 0, false};
-    default:                  return {0, 0, 0, 0, 0, false};
+    case PBD_DISTANCE:        return {2, 2, 0, 0, 1, 1, false};
+    case PBD_DISTANCE_XPBD:   return {2, 2, 0, 0, 1, 1, true};
+    case PBD_DIHEDRAL:        return {4, 2, 0, 0, 1, 1, false};
+    case PBD_ISOBENDING:      return {4, 17, 4, 1, 0, 1, false};  // nGeoV: 1 (rank-1) or 4 (full Q), decided at flatten
+    case PBD_ISOBENDING_XPBD: return {4, 17, 4, 1, 0, 1, true};
+    case PBD_FEMTRIANGLE:     return {3, 10, 1, 1, 1, 5, false};
+    case PBD_STRAINTRIANGLE:  return {3, 9, 1, 1, 0, 5, false};
+    case PBD_VOLUME:          return {4, 2, 0, 0, 1, 1, false};
+    case PBD_VOLUME_XPBD:     return {4, 2, 0, 0, 1, 1, true};
+    case PBD_FEMTET:          return {4, 12, 2, 2, 2, 2, false};
+    case PBD_FEMTET_XPBD:     return {4, 12, 2, 2, 2, 2, true};
+    case PBD_STRAINTET:       return {4, 13, 2, 2, 1, 4, false};
+    case PBD_SHAPEMATCHING:   return {4, 24, 6, 0, 0, 1, false};
+    case PBD_BALLJOINT:       return {2, 12, 2, 2, 0, 0, false};
+    case PBD_RB_PARTICLE_BALLJOINT: return {2, 6, 1, 1, 0, 0, false};
+    default:                  return {0, 0, 0, 0, 0, 0, false};
     }
 }
 

@@ -1400,15 +1400,11 @@ static cudaError_t launch_step_kernel(void (*kernel)(KArgs...), unsigned grid, u
 // (constraint type, layout variant) -> f(T, VAR): the compile-time arguments of the k_project / k_project_jacobi instantiation
 template <int V> using IntC = std::integral_constant<int, V>;
 template <class F> static int with_project_type(int type, int variant, F &&f) {
-    switch (type) {
-    case PBD_ISOBENDING: return variant ? f(IntC<PBD_ISOBENDING>{}, IntC<1>{}) : f(IntC<PBD_ISOBENDING>{}, IntC<0>{});
-    case PBD_ISOBENDING_XPBD: return variant ? f(IntC<PBD_ISOBENDING_XPBD>{}, IntC<1>{}) : f(IntC<PBD_ISOBENDING_XPBD>{}, IntC<0>{});
-#define PT(T) case T: return f(IntC<T>{}, IntC<0>{});
-    PT(PBD_DISTANCE) PT(PBD_DISTANCE_XPBD) PT(PBD_DIHEDRAL) PT(PBD_FEMTRIANGLE) PT(PBD_STRAINTRIANGLE) PT(PBD_VOLUME) PT(PBD_VOLUME_XPBD)
-    PT(PBD_FEMTET) PT(PBD_FEMTET_XPBD) PT(PBD_STRAINTET) PT(PBD_SHAPEMATCHING) PT(PBD_BALLJOINT) PT(PBD_RB_PARTICLE_BALLJOINT)
-#undef PT
-    default: return fail("no kernel for constraint type %d", type);
-    }
+    PBD_FOR_TYPE(kMaskAll, type,
+        if constexpr (T == PBD_ISOBENDING || T == PBD_ISOBENDING_XPBD)
+            if (variant) return f(IntC<T>{}, IntC<1>{});
+        return f(IntC<T>{}, IntC<0>{});)
+    return fail("no kernel for constraint type %d", type);
 }
 
 static int launch_bucket(pbd_engine *e, const Bucket &b, float h, int iterZero, cudaStream_t s, bool pdl) {
@@ -1490,8 +1486,8 @@ static int enqueue_step_launches(pbd_engine *e, cudaStream_t s, unsigned long lo
     auto launched = [&](int kind) { L++; return log ? log->mark(s, kind) : 0; };
     for (unsigned sub = 0; sub < e->subSteps; sub++) {
         if (e->nRb) { CK(launch_step_kernel(k_rb_integrate, nblk(e->nRb, 256), 256, s, pdl, rb, h, e->g[0], e->g[1], e->g[2])); CKE(launched(kLaunchIntegrate)); }
-        if (n) {  // trackLast = 1: lastX is part of the reference's particle state
-            CK(launch_step_kernel(k_integrate, nblk(n, 256), 256, s, pdl, (float4 *)e->pos.p, (float4 *)e->vel.p, (float4 *)e->oldp.p, (float4 *)e->lastp.p, n, h, e->g[0], e->g[1], e->g[2], 1));
+        if (n) {
+            CK(launch_step_kernel(k_integrate, nblk(n, 256), 256, s, pdl, (float4 *)e->pos.p, (float4 *)e->vel.p, (float4 *)e->oldp.p, (float4 *)e->lastp.p, n, h, e->g[0], e->g[1], e->g[2]));
             CKE(launched(kLaunchIntegrate));
         }
         for (unsigned it = 0; it < e->maxIter; it++)
@@ -1596,7 +1592,7 @@ static int enqueue_step_jacobi(pbd_engine *e, cudaStream_t s, unsigned long long
     const float4 *pos = (const float4 *)e->pos.p; float4 *delta = (float4 *)e->jacobiDelta.p;
     unsigned long long L = 0;
     for (unsigned sub = 0; sub < e->subSteps; sub++) {
-        k_integrate<<<nblk(n, 256), 256, 0, s>>>((float4 *)e->pos.p, (float4 *)e->vel.p, (float4 *)e->oldp.p, (float4 *)e->lastp.p, n, h, e->g[0], e->g[1], e->g[2], 1); L++;
+        k_integrate<<<nblk(n, 256), 256, 0, s>>>((float4 *)e->pos.p, (float4 *)e->vel.p, (float4 *)e->oldp.p, (float4 *)e->lastp.p, n, h, e->g[0], e->g[1], e->g[2]); L++;
         for (unsigned it = 0; it < e->maxIter; it++) {
             for (int t = 0; t < PBD_BALLJOINT; t++) {
                 const unsigned cnt = e->dev[t].count;

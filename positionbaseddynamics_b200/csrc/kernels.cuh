@@ -41,37 +41,32 @@ __device__ __forceinline__ float xpbd_alpha(float k, float dt) { return (k != 0.
 
 // What a constraint streams from HBM before it touches any particle: indices + per-constraint constants.  These never
 // change during a step, so they can be fetched ahead of the dependency on the previous colour phase (before the PDL
-// wait in k_project, before the grid barrier in the persistent kernel).
+// wait in k_project, before the colour barrier in k_step_resident).
 struct Streamed {
     uint4 b;        // particle indices (x,y[,z[,w]])
-    float4 g0, g1;  // float4 geometry (Kp / invRestMat rows)
+    float4 g0, g1;  // float4 geometry (Kp / invRestMat rows / joint connectors)
     float s0, s1;   // scalar geometry (rest length / angle / volume / area / invRestMat(2,2))
 };
 
+// the indices, the first nStreamV float4 and all nGeoS scalar geometry arrays of type T (type_shape)
 template <int T>
 __device__ __forceinline__ Streamed load_streamed(const TypeArrays &a, unsigned i) {
+    constexpr TypeShape sh = type_shape(T);
+    static_assert(sh.nStreamV <= 2 && sh.nGeoS <= 2, "Streamed holds two float4 and two scalar geometry values");
     Streamed s;
     s.g0 = make_float4(0.f, 0.f, 0.f, 0.f); s.g1 = s.g0; s.s0 = 0.0f; s.s1 = 0.0f;
-    if (T == PBD_BALLJOINT || T == PBD_RB_PARTICLE_BALLJOINT) {
+    if (sh.nBodies == 2) {
         const uint2 b = __ldg(a.idx2 + i);
         s.b = make_uint4(b.x, b.y, 0u, 0u);
-        s.g0 = __ldg(a.gv[0] + i);
-        if (T == PBD_BALLJOINT) s.g1 = __ldg(a.gv[1] + i);
-    } else if (T == PBD_DISTANCE || T == PBD_DISTANCE_XPBD) {
-        const uint2 b = __ldg(a.idx2 + i);
-        s.b = make_uint4(b.x, b.y, 0u, 0u);
-        s.s0 = __ldg(a.gs[0] + i);
-    } else if (T == PBD_FEMTRIANGLE || T == PBD_STRAINTRIANGLE) {
+    } else if (sh.nBodies == 3) {
         s.b = make_uint4(__ldg(a.idx3[0] + i), __ldg(a.idx3[1] + i), __ldg(a.idx3[2] + i), 0u);
-        s.g0 = __ldg(a.gv[0] + i);
-        if (T == PBD_FEMTRIANGLE) s.s0 = __ldg(a.gs[0] + i);
     } else {
         s.b = __ldg(a.idx4 + i);
-        if (T == PBD_DIHEDRAL || T == PBD_VOLUME || T == PBD_VOLUME_XPBD) s.s0 = __ldg(a.gs[0] + i);
-        if (T == PBD_ISOBENDING || T == PBD_ISOBENDING_XPBD) s.g0 = __ldg(a.gv[0] + i);
-        if (T == PBD_FEMTET || T == PBD_FEMTET_XPBD || T == PBD_STRAINTET) { s.g0 = __ldg(a.gv[0] + i); s.g1 = __ldg(a.gv[1] + i); s.s0 = __ldg(a.gs[0] + i); }
-        if (T == PBD_FEMTET || T == PBD_FEMTET_XPBD) s.s1 = __ldg(a.gs[1] + i);
     }
+    if (sh.nStreamV >= 1) s.g0 = __ldg(a.gv[0] + i);
+    if (sh.nStreamV >= 2) s.g1 = __ldg(a.gv[1] + i);
+    if (sh.nGeoS >= 1) s.s0 = __ldg(a.gs[0] + i);
+    if (sh.nGeoS >= 2) s.s1 = __ldg(a.gs[1] + i);
     return s;
 }
 
@@ -112,8 +107,8 @@ template <int T, class Acc, int VAR = -1>
 __device__ __forceinline__ void project_streamed_acc(const Acc &acc, const TypeArrays &a, unsigned i, const Streamed &s, float dt,
                                                      bool iterZero, bool lambdaGiven = false, float lambdaValue = 0.0f) {
     if (T == PBD_BALLJOINT || T == PBD_RB_PARTICLE_BALLJOINT) { project_joint<T>(acc, a, s); return; }
-    constexpr bool XPBD = (T == PBD_DISTANCE_XPBD || T == PBD_VOLUME_XPBD || T == PBD_ISOBENDING_XPBD || T == PBD_FEMTET_XPBD);
-    constexpr int NB = (T == PBD_DISTANCE || T == PBD_DISTANCE_XPBD) ? 2 : ((T == PBD_FEMTRIANGLE || T == PBD_STRAINTRIANGLE) ? 3 : 4);
+    constexpr bool XPBD = type_shape(T).xpbd;
+    constexpr int NB = type_shape(T).nBodies;
     const typename Acc::Handle h0 = acc.handle(s.b.x), h1 = acc.handle(s.b.y), h2 = acc.handle(NB >= 3 ? s.b.z : s.b.x), h3 = acc.handle(NB >= 4 ? s.b.w : s.b.x);
     float4 p0 = acc.ld(h0), p1 = acc.ld(h1), p2, p3;
     if (NB >= 3) p2 = acc.ld(h2);
@@ -166,10 +161,35 @@ __device__ __forceinline__ void project_streamed(float4 *pos, const TypeArrays &
     project_streamed_acc<T, GlobalAcc, VAR>(GlobalAcc{pos}, a, i, s, dt, iterZero);
 }
 
-#ifndef PBD_PROJECT_THREADS
-#define PBD_PROJECT_THREADS 256
-#endif
-constexpr int kProjectThreads = PBD_PROJECT_THREADS;
+// Sets of constraint types, one bit per type.  k_step_resident (resident.cuh) is instantiated per mask, the leanest that
+// covers the model: the everything-kernel is 20k instructions and 226 registers, and every colour phase jumps through it.
+constexpr unsigned type_bit(int t) { return 1u << t; }
+constexpr unsigned kMaskClothXPBD = type_bit(PBD_DISTANCE_XPBD) | type_bit(PBD_ISOBENDING_XPBD);
+constexpr unsigned kMaskCloth = kMaskClothXPBD | type_bit(PBD_DISTANCE) | type_bit(PBD_ISOBENDING);
+constexpr unsigned kMaskLight = type_bit(PBD_DISTANCE) | type_bit(PBD_DISTANCE_XPBD) | type_bit(PBD_DIHEDRAL) | type_bit(PBD_ISOBENDING) |
+                                type_bit(PBD_ISOBENDING_XPBD) | type_bit(PBD_VOLUME) | type_bit(PBD_VOLUME_XPBD) | type_bit(PBD_FEMTRIANGLE);
+// FEM solids (cfg3): tets with FEM / volume constraints; and cloth + FEM solids + the coupling joints (cfg4)
+constexpr unsigned kMaskFem = type_bit(PBD_FEMTET) | type_bit(PBD_FEMTET_XPBD) | type_bit(PBD_VOLUME) | type_bit(PBD_VOLUME_XPBD);
+constexpr unsigned kMaskSolid = kMaskCloth | kMaskFem | type_bit(PBD_FEMTRIANGLE) | type_bit(PBD_BALLJOINT) | type_bit(PBD_RB_PARTICLE_BALLJOINT);
+constexpr unsigned kMaskAll = (1u << PBD_NUM_TYPES) - 1u;
+
+// The one list of all constraint types: dispatch a statement on the runtime type, restricted to the types of MASK (T is a
+// constant inside the statement; a type outside the mask does nothing).
+#define PBD_CASE_TYPE(MASK, TT, ...) case TT: if constexpr ((MASK) & type_bit(TT)) { constexpr int T = TT; __VA_ARGS__ } break;
+#define PBD_FOR_TYPE(MASK, type, ...)                                                                                              \
+    switch (type) {                                                                                                                \
+        PBD_CASE_TYPE(MASK, PBD_DISTANCE, __VA_ARGS__) PBD_CASE_TYPE(MASK, PBD_DISTANCE_XPBD, __VA_ARGS__)                         \
+        PBD_CASE_TYPE(MASK, PBD_DIHEDRAL, __VA_ARGS__) PBD_CASE_TYPE(MASK, PBD_ISOBENDING, __VA_ARGS__)                            \
+        PBD_CASE_TYPE(MASK, PBD_ISOBENDING_XPBD, __VA_ARGS__) PBD_CASE_TYPE(MASK, PBD_FEMTRIANGLE, __VA_ARGS__)                    \
+        PBD_CASE_TYPE(MASK, PBD_STRAINTRIANGLE, __VA_ARGS__) PBD_CASE_TYPE(MASK, PBD_VOLUME, __VA_ARGS__)                          \
+        PBD_CASE_TYPE(MASK, PBD_VOLUME_XPBD, __VA_ARGS__) PBD_CASE_TYPE(MASK, PBD_FEMTET, __VA_ARGS__)                             \
+        PBD_CASE_TYPE(MASK, PBD_FEMTET_XPBD, __VA_ARGS__) PBD_CASE_TYPE(MASK, PBD_STRAINTET, __VA_ARGS__)                          \
+        PBD_CASE_TYPE(MASK, PBD_SHAPEMATCHING, __VA_ARGS__) PBD_CASE_TYPE(MASK, PBD_BALLJOINT, __VA_ARGS__)                        \
+        PBD_CASE_TYPE(MASK, PBD_RB_PARTICLE_BALLJOINT, __VA_ARGS__)                                                                \
+    default: break;                                                                                                                \
+    }
+
+constexpr int kProjectThreads = 256;
 
 template <int T, int VAR>
 __global__ void __launch_bounds__(kProjectThreads) k_project(float4 *pos, TypeArrays a, unsigned first,
@@ -239,31 +259,47 @@ __global__ void __launch_bounds__(kProjectThreads) k_project_multi(float4 *pos, 
     if (i >= m.count[s]) return;
     const TypeArrays &a = m.arrays[s];
     const unsigned ci = m.first[s] + i;
-#define PM(T) case T: { const Streamed st = load_streamed<T>(a, ci); pdl_wait_after(st.b.x ^ st.b.y, st.g0.x + st.g1.x + st.s0 + st.s1); \
-                        project_streamed<T>(pos, a, ci, st, dt, iterZero != 0); } break;
-    switch (m.type[s]) {
-        PM(PBD_DISTANCE) PM(PBD_DISTANCE_XPBD) PM(PBD_DIHEDRAL) PM(PBD_ISOBENDING) PM(PBD_ISOBENDING_XPBD) PM(PBD_FEMTRIANGLE)
-        PM(PBD_STRAINTRIANGLE) PM(PBD_VOLUME) PM(PBD_VOLUME_XPBD) PM(PBD_FEMTET) PM(PBD_FEMTET_XPBD) PM(PBD_STRAINTET) PM(PBD_SHAPEMATCHING) PM(PBD_BALLJOINT) PM(PBD_RB_PARTICLE_BALLJOINT)
-    default: break;
+    PBD_FOR_TYPE(kMaskAll, m.type[s],
+        const Streamed st = load_streamed<T>(a, ci);
+        pdl_wait_after(st.b.x ^ st.b.y, st.g0.x + st.g1.x + st.s0 + st.s1);
+        project_streamed<T>(pos, a, ci, st, dt, iterZero != 0);)
+}
+
+// The particle updates of a substep, shared by every execution mode and by the linear part of the rigid bodies, so that the modes
+// agree bit for bit.  Arithmetic only: each caller loads and stores with the cache hints of its own memory layout.
+// TimeIntegration::semiImplicitEuler (TimeIntegration.cpp:7-19) of a point with mass: v += g h; x += v h
+__device__ __forceinline__ void semi_implicit_euler(float4 &x, float4 &v, float h, float gx, float gy, float gz) {
+    v.x = fmaf(gx, h, v.x); v.y = fmaf(gy, h, v.y); v.z = fmaf(gz, h, v.z);
+    x.x = fmaf(v.x, h, x.x); x.y = fmaf(v.y, h, x.y); x.z = fmaf(v.z, h, x.z);
+}
+// TimeIntegration::velocityUpdateFirstOrder / SecondOrder (TimeIntegration.cpp:42-51, 69-79): v.xyz = (1/h)(x - oldX)  or
+// (1/h)(1.5 x - 2 oldX + 0.5 lastX); lastX() loads lastX, second order only
+template <class LastX>
+__device__ __forceinline__ void velocity_update(float4 &v, const float4 &x, const float4 &o, float invH, int secondOrder, LastX lastX) {
+    if (!secondOrder) {
+        v.x = invH * (x.x - o.x); v.y = invH * (x.y - o.y); v.z = invH * (x.z - o.z);
+    } else {
+        const float4 l = lastX();
+        v.x = invH * (1.5f * x.x - 2.0f * o.x + 0.5f * l.x);
+        v.y = invH * (1.5f * x.y - 2.0f * o.y + 0.5f * l.y);
+        v.z = invH * (1.5f * x.z - 2.0f * o.z + 0.5f * l.z);
     }
-#undef PM
 }
 
 // lastX = oldX; oldX = x; if (mass != 0) { v += g h; x += v h }
 __global__ void __launch_bounds__(256) k_integrate(float4 *__restrict__ pos, float4 *__restrict__ vel,
                                                    float4 *__restrict__ oldp, float4 *__restrict__ lastp, unsigned n,
-                                                   float h, float gx, float gy, float gz, int trackLast) {
+                                                   float h, float gx, float gy, float gz) {
     pdl_launch_dependents();
     const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     pdl_wait();
     float4 x = __ldcg(pos + i);
-    if (trackLast) __stcs(lastp + i, __ldcs(oldp + i));
+    __stcs(lastp + i, __ldcs(oldp + i));
     __stcg(oldp + i, x);
     float4 v = __ldcs(vel + i);
     if (v.w != 0.0f) {  // v.w carries the mass (TimeIntegration.cpp:14 tests mass != 0)
-        v.x = fmaf(gx, h, v.x); v.y = fmaf(gy, h, v.y); v.z = fmaf(gz, h, v.z);
-        x.x = fmaf(v.x, h, x.x); x.y = fmaf(v.y, h, x.y); x.z = fmaf(v.z, h, x.z);
+        semi_implicit_euler(x, v, h, gx, gy, gz);
         __stcs(vel + i, v);
         __stcg(pos + i, x);
     }
@@ -280,8 +316,7 @@ __device__ __forceinline__ void rb_integrate_body(const RbState &r, unsigned i, 
     r.lastX[i] = r.oldX[i]; r.oldX[i] = X;
     r.lastQ[i] = r.oldQ[i]; r.oldQ[i] = Q;
     if (V.w != 0.0f) {  // V.w = mass
-        V.x = fmaf(gx, h, V.x); V.y = fmaf(gy, h, V.y); V.z = fmaf(gz, h, V.z);
-        X.x = fmaf(V.x, h, X.x); X.y = fmaf(V.y, h, X.y); X.z = fmaf(V.z, h, X.z);
+        semi_implicit_euler(X, V, h, gx, gy, gz);
         const M3 R = qmatrix(Q);
         const float4 I = r.I[i], Ii = r.Iinv[i];
         const M3 Iw = world_tensor(R, mk(I.x, I.y, I.z)), Jw = world_tensor(R, mk(Ii.x, Ii.y, Ii.z));
@@ -299,11 +334,7 @@ __device__ __forceinline__ void rb_velocity_body(const RbState &r, unsigned i, f
     float4 V = r.V[i];
     if (V.w == 0.0f) return;
     const float4 X = __ldcg(r.X + i), Q = __ldcg(r.Q + i), o = r.oldX[i], oq = r.oldQ[i];
-    if (!secondOrder) { V.x = invH * (X.x - o.x); V.y = invH * (X.y - o.y); V.z = invH * (X.z - o.z); }
-    else {
-        const float4 l = r.lastX[i];
-        V.x = invH * (1.5f * X.x - 2.0f * o.x + 0.5f * l.x); V.y = invH * (1.5f * X.y - 2.0f * o.y + 0.5f * l.y); V.z = invH * (1.5f * X.z - 2.0f * o.z + 0.5f * l.z);
-    }
+    velocity_update(V, X, o, invH, secondOrder, [&] { return r.lastX[i]; });
     const float4 rel = qmul(Q, make_float4(-oq.x, -oq.y, -oq.z, oq.w));
     float4 W = r.W[i];
     W.x = rel.x * twoInvH; W.y = rel.y * twoInvH; W.z = rel.z * twoInvH;
@@ -337,18 +368,10 @@ __global__ void __launch_bounds__(256) k_velocity(const float4 *__restrict__ pos
     const float4 x = __ldcg(pos + i);
     if (x.w == 0.0f) return;  // invMass == 0  <=>  mass == 0 (ParticleData::setMass keeps them consistent)
     const float4 o = __ldcg(oldp + i);
-    float vx, vy, vz;
-    if (!secondOrder) {
-        vx = invH * (x.x - o.x); vy = invH * (x.y - o.y); vz = invH * (x.z - o.z);
-    } else {
-        const float4 l = __ldcs(lastp + i);
-        vx = invH * (1.5f * x.x - 2.0f * o.x + 0.5f * l.x);
-        vy = invH * (1.5f * x.y - 2.0f * o.y + 0.5f * l.y);
-        vz = invH * (1.5f * x.z - 2.0f * o.z + 0.5f * l.z);
-    }
+    float4 v;
+    velocity_update(v, x, o, invH, secondOrder, [&] { return __ldcs(lastp + i); });
     // keep the mass in .w: re-read only that lane's .w would cost a full sector anyway, so read-modify-write the float4
-    float4 v = __ldcs(vel + i);
-    v.x = vx; v.y = vy; v.z = vz;
+    v.w = __ldcs(vel + i).w;
     __stcs(vel + i, v);
 }
 

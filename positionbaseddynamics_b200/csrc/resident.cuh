@@ -56,37 +56,6 @@ __host__ __device__ inline size_t resident_smem_bytes(unsigned tileCap, unsigned
     return (size_t)tileCap * sizeof(float4) + (size_t)nBuckets * sizeof(RunEntry) + (size_t)(2u * nColours + 2u) * sizeof(unsigned);
 }
 
-#ifdef PBD_NO_DEEP
-constexpr bool kDeepPipeline = false;
-#else
-constexpr bool kDeepPipeline = true;
-#endif
-constexpr unsigned type_bit(int t) { return 1u << t; }
-constexpr unsigned kMaskClothXPBD = type_bit(PBD_DISTANCE_XPBD) | type_bit(PBD_ISOBENDING_XPBD);
-constexpr unsigned kMaskCloth = kMaskClothXPBD | type_bit(PBD_DISTANCE) | type_bit(PBD_ISOBENDING);
-constexpr unsigned kMaskLight = type_bit(PBD_DISTANCE) | type_bit(PBD_DISTANCE_XPBD) | type_bit(PBD_DIHEDRAL) | type_bit(PBD_ISOBENDING) |
-                                type_bit(PBD_ISOBENDING_XPBD) | type_bit(PBD_VOLUME) | type_bit(PBD_VOLUME_XPBD) | type_bit(PBD_FEMTRIANGLE);
-// FEM solids (cfg3): tets with FEM / volume constraints; and cloth + FEM solids + the coupling joints (cfg4).  Lean instantiations
-// matter: the everything-kernel is 20k instructions and 226 registers, and every colour phase jumps through it.
-constexpr unsigned kMaskFem = type_bit(PBD_FEMTET) | type_bit(PBD_FEMTET_XPBD) | type_bit(PBD_VOLUME) | type_bit(PBD_VOLUME_XPBD);
-constexpr unsigned kMaskSolid = kMaskCloth | kMaskFem | type_bit(PBD_FEMTRIANGLE) | type_bit(PBD_BALLJOINT) | type_bit(PBD_RB_PARTICLE_BALLJOINT);
-constexpr unsigned kMaskAll = (1u << PBD_NUM_TYPES) - 1u;
-
-// dispatch a statement on the runtime type, restricted to the compiled-in mask (T is a constant inside the statement)
-#define PBD_CASE_TYPE(MASK, TT, ...) case TT: if constexpr ((MASK) & type_bit(TT)) { constexpr int T = TT; __VA_ARGS__ } break;
-#define PBD_FOR_TYPE(MASK, type, ...)                                                                                              \
-    switch (type) {                                                                                                                \
-        PBD_CASE_TYPE(MASK, PBD_DISTANCE, __VA_ARGS__) PBD_CASE_TYPE(MASK, PBD_DISTANCE_XPBD, __VA_ARGS__)                         \
-        PBD_CASE_TYPE(MASK, PBD_DIHEDRAL, __VA_ARGS__) PBD_CASE_TYPE(MASK, PBD_ISOBENDING, __VA_ARGS__)                            \
-        PBD_CASE_TYPE(MASK, PBD_ISOBENDING_XPBD, __VA_ARGS__) PBD_CASE_TYPE(MASK, PBD_FEMTRIANGLE, __VA_ARGS__)                    \
-        PBD_CASE_TYPE(MASK, PBD_STRAINTRIANGLE, __VA_ARGS__) PBD_CASE_TYPE(MASK, PBD_VOLUME, __VA_ARGS__)                          \
-        PBD_CASE_TYPE(MASK, PBD_VOLUME_XPBD, __VA_ARGS__) PBD_CASE_TYPE(MASK, PBD_FEMTET, __VA_ARGS__)                             \
-        PBD_CASE_TYPE(MASK, PBD_FEMTET_XPBD, __VA_ARGS__) PBD_CASE_TYPE(MASK, PBD_STRAINTET, __VA_ARGS__)                          \
-        PBD_CASE_TYPE(MASK, PBD_SHAPEMATCHING, __VA_ARGS__) PBD_CASE_TYPE(MASK, PBD_BALLJOINT, __VA_ARGS__)                        \
-        PBD_CASE_TYPE(MASK, PBD_RB_PARTICLE_BALLJOINT, __VA_ARGS__)                                                                \
-    default: break;                                                                                                                \
-    }
-
 struct ResidentArgs {
     float4 *pos, *vel, *oldp, *lastp;
     const Bucket *buckets;        // colour after colour
@@ -205,18 +174,17 @@ __device__ __forceinline__ void l2_prefetch_bytes(const void *p, size_t bytes) {
         a += chunk;
     }
 }
-// the streamed arrays of one type (mirror of load_streamed): array k of items [first, first + n), one array per calling lane
+// the per-constraint arrays of one type (indices, every geometry array, multipliers): array k of items [first, first + n), one array
+// per calling lane
 template <int T>
 __device__ __forceinline__ void l2_prefetch_run(const TypeArrays &a, unsigned first, unsigned n, unsigned lane) {
-    constexpr bool two = (T == PBD_DISTANCE || T == PBD_DISTANCE_XPBD || T == PBD_BALLJOINT || T == PBD_RB_PARTICLE_BALLJOINT);
-    constexpr bool tri = (T == PBD_FEMTRIANGLE || T == PBD_STRAINTRIANGLE);
-    const TypeShape sh = type_shape(T);
+    constexpr TypeShape sh = type_shape(T);
     if (lane == 0) {
-        if (two) l2_prefetch_bytes(a.idx2 + first, (size_t)n * 8u);
-        else if (tri) l2_prefetch_bytes(a.idx3[0] + first, (size_t)n * 4u);
+        if (sh.nBodies == 2) l2_prefetch_bytes(a.idx2 + first, (size_t)n * 8u);
+        else if (sh.nBodies == 3) l2_prefetch_bytes(a.idx3[0] + first, (size_t)n * 4u);
         else l2_prefetch_bytes(a.idx4 + first, (size_t)n * 16u);
     } else if (lane <= 2) {
-        if (tri) l2_prefetch_bytes(a.idx3[lane] + first, (size_t)n * 4u);
+        if (sh.nBodies == 3) l2_prefetch_bytes(a.idx3[lane] + first, (size_t)n * 4u);
     } else if (lane < 3 + (unsigned)kMaxGeoV) {
         const unsigned k = lane - 3u;
         if ((int)k < sh.nGeoV && a.gv[k]) l2_prefetch_bytes(a.gv[k] + first, (size_t)n * 16u);
@@ -233,7 +201,6 @@ constexpr unsigned kPrefetchLanes = 3u + (unsigned)kMaxGeoV + (unsigned)kMaxGeoS
 // the XPBD multiplier (last written by this very thread one sweep ago), so that after the barrier only the gathers remain.
 struct Prefetched { Streamed s; float lam; unsigned bucket; };
 
-template <int T> __device__ __forceinline__ constexpr bool is_xpbd() { return T == PBD_DISTANCE_XPBD || T == PBD_VOLUME_XPBD || T == PBD_ISOBENDING_XPBD || T == PBD_FEMTET_XPBD; }
 // types whose item loop keeps the next item's operands in flight (the register-heavy projections would spill with a second operand set)
 template <int T> __device__ __forceinline__ constexpr bool is_pipelined() {
     return T == PBD_DISTANCE || T == PBD_DISTANCE_XPBD || T == PBD_ISOBENDING || T == PBD_ISOBENDING_XPBD || T == PBD_VOLUME || T == PBD_VOLUME_XPBD || T == PBD_FEMTRIANGLE || T == PBD_DIHEDRAL;
@@ -248,7 +215,7 @@ __device__ __forceinline__ void prefetch_first(const ResidentArgs &A, const RunE
     if (tid >= n) return;
     PBD_FOR_TYPE(MASK, r.type,
         pre.s = load_streamed<T>(A.types[T], first + tid);
-        if (is_xpbd<T>() && !iterZero) pre.lam = __ldcg(A.types[T].lambda + first + tid);
+        if (type_shape(T).xpbd && !iterZero) pre.lam = __ldcg(A.types[T].lambda + first + tid);
         pre.bucket = bi;)
 }
 
@@ -262,7 +229,7 @@ __device__ __forceinline__ void run_items(const ResidentArgs &A, const Acc &acc,
         unsigned i = tid;
         if (DEEP && is_pipelined2<T>()) {
             if (i < n) {
-                auto fetch = [&](unsigned k, Streamed &sx, float &lx) { sx = load_streamed<T>(ta, first + k); if (is_xpbd<T>() && !iterZero) lx = __ldcg(ta.lambda + first + k); };
+                auto fetch = [&](unsigned k, Streamed &sx, float &lx) { sx = load_streamed<T>(ta, first + k); if (type_shape(T).xpbd && !iterZero) lx = __ldcg(ta.lambda + first + k); };
                 Streamed s0, s1, s2; float l0 = 0.0f, l1 = 0.0f, l2 = 0.0f;
                 if (usePre) { s0 = pre.s; l0 = pre.lam; } else fetch(i, s0, l0);
                 bool h1 = i + stride < n;
@@ -281,16 +248,16 @@ __device__ __forceinline__ void run_items(const ResidentArgs &A, const Acc &acc,
         if (i < n) {
             Streamed cur; float lam = 0.0f;
             if (usePre) { cur = pre.s; lam = pre.lam; }
-            else { cur = load_streamed<T>(ta, first + i); if (is_xpbd<T>() && !iterZero) lam = __ldcg(ta.lambda + first + i); }
+            else { cur = load_streamed<T>(ta, first + i); if (type_shape(T).xpbd && !iterZero) lam = __ldcg(ta.lambda + first + i); }
             _Pragma("unroll 1")
             for (;;) {
                 const unsigned j = i + stride;
                 const bool more = j < n;
                 Streamed nxt; float lamN = 0.0f;
-                if (is_pipelined<T>() && more) { nxt = load_streamed<T>(ta, first + j); if (is_xpbd<T>() && !iterZero) lamN = __ldcg(ta.lambda + first + j); }
+                if (is_pipelined<T>() && more) { nxt = load_streamed<T>(ta, first + j); if (type_shape(T).xpbd && !iterZero) lamN = __ldcg(ta.lambda + first + j); }
                 project_streamed_acc<T, Acc, 0>(acc, ta, first + i, cur, A.h, iterZero, true, lam);  // variant 0 only: flatten refuses the full-Q bending layout in this mode
                 if (!more) break;
-                if (!is_pipelined<T>()) { nxt = load_streamed<T>(ta, first + j); if (is_xpbd<T>() && !iterZero) lamN = __ldcg(ta.lambda + first + j); }
+                if (!is_pipelined<T>()) { nxt = load_streamed<T>(ta, first + j); if (type_shape(T).xpbd && !iterZero) lamN = __ldcg(ta.lambda + first + j); }
                 cur = nxt; lam = lamN; i = j;
             }
         })
@@ -302,24 +269,16 @@ __device__ __forceinline__ bool integrate_particle(const ResidentArgs &A, unsign
     __stcs(A.oldp + slot, x);
     float4 v = __ldcs(A.vel + slot);
     if (v.w == 0.0f) return false;  // v.w carries the mass
-    v.x = fmaf(A.gx, A.h, v.x); v.y = fmaf(A.gy, A.h, v.y); v.z = fmaf(A.gz, A.h, v.z);
-    x.x = fmaf(v.x, A.h, x.x); x.y = fmaf(v.y, A.h, x.y); x.z = fmaf(v.z, A.h, x.z);
+    semi_implicit_euler(x, v, A.h, A.gx, A.gy, A.gz);
     __stcs(A.vel + slot, v);
     return true;
 }
-// TimeIntegration::velocityUpdateFirstOrder / SecondOrder (TimeIntegration.cpp:42-51, 69-79)
+// velocity update of one particle whose position is `x` (TimeIntegration.cpp:42-51, 69-79)
 __device__ __forceinline__ void velocity_particle(const ResidentArgs &A, unsigned slot, const float4 &x) {
     if (x.w == 0.0f) return;
     const float4 o = __ldcs(A.oldp + slot);
     float4 v = __ldcs(A.vel + slot);
-    if (!A.secondOrder) {
-        v.x = A.invH * (x.x - o.x); v.y = A.invH * (x.y - o.y); v.z = A.invH * (x.z - o.z);
-    } else {
-        const float4 l = __ldcs(A.lastp + slot);
-        v.x = A.invH * (1.5f * x.x - 2.0f * o.x + 0.5f * l.x);
-        v.y = A.invH * (1.5f * x.y - 2.0f * o.y + 0.5f * l.y);
-        v.z = A.invH * (1.5f * x.z - 2.0f * o.z + 0.5f * l.z);
-    }
+    velocity_update(v, x, o, A.invH, A.secondOrder, [&] { return __ldcs(A.lastp + slot); });
     __stcs(A.vel + slot, v);
 }
 
@@ -444,7 +403,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_step_resident(const __grid_const
 #pragma unroll 1
                     for (unsigned bi = b0; bi < b1; bi++) {
                         const unsigned rot = runs[bi].rotR;  // 0 for the first bucket of a colour (the one prefetch_first serves)
-                        run_items<MASK, kDeepPipeline && SINGLE && MASK == kMaskClothXPBD>(A, accR, runs[bi].type, runs[bi].firstR, runs[bi].nR, iterZero,
+                        run_items<MASK, SINGLE && MASK == kMaskClothXPBD>(A, accR, runs[bi].type, runs[bi].firstR, runs[bi].nR, iterZero,
                                                                            threadIdx.x >= rot ? threadIdx.x - rot : threadIdx.x + RT - rot, RT, pre.bucket == bi, pre);
                     }
                 }

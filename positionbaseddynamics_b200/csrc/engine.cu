@@ -138,9 +138,8 @@ struct pbd_engine {
     // resident mode (resident.cuh): G clusters x C CTAs = nTiles tiles, block size and type mask of the instantiation
     unsigned resG = 0, resC = 0, nTiles = 0, resThreads = 0, resMask = 0, resColours = 0, resTileCap = 0, resXThreads = 0;
     bool resChecked = false;              // co-residency of the clusters verified for the current image
-    DevBuf dColourStart, dTileOff, dTileStart, dTileSmem, dXArrive, dXCounter;
-    unsigned long long xBase = 0, xPerStep = 0;  // arrival counter of the X items: value at the next launch, arrivals per substep-sweep unit
-    std::vector<unsigned long long> xArriveInt, xArriveCol;  // per-launch bookkeeping of the X counter (host copy of dXArrive)
+    DevBuf dColourStart, dTileOff, dTileStart, dTileSmem, dXNbr, dXMask, dXFlags;
+    unsigned long long xLaunch = 0;       // resident launches so far: the high word of the X arrival flags
 };
 
 static int use(pbd_engine *e) { CK(cudaSetDevice(e->device)); return 0; }
@@ -191,7 +190,7 @@ extern "C" int pbd_destroy(pbd_engine *e) {
     cudaStreamSynchronize(e->stream);
     drop_graph(e);
     for (auto *b : {&e->pos, &e->vel, &e->oldp, &e->lastp, &e->pos0, &e->stage, &e->stage2, &e->massStage, &e->jacobiDelta, &e->dSlot, &e->dSlotOld, &e->relayoutTmp,
-                    &e->dPColliders, &e->dRColliders, &e->dRangeStart, &e->dContacts, &e->dContactCount, &e->dColourStart, &e->dTileOff, &e->dTileStart, &e->dTileSmem, &e->dXArrive, &e->dXCounter, &e->dBuckets, &e->dTrace,
+                    &e->dPColliders, &e->dRColliders, &e->dRangeStart, &e->dContacts, &e->dContactCount, &e->dColourStart, &e->dTileOff, &e->dTileStart, &e->dTileSmem, &e->dXNbr, &e->dXMask, &e->dXFlags, &e->dBuckets, &e->dTrace,
                     &e->rbX, &e->rbQ, &e->rbV, &e->rbW, &e->rbOldX, &e->rbLastX, &e->rbOldQ, &e->rbLastQ, &e->rbI, &e->rbIinv}) b->release();
     for (auto &d : e->dev) {
         for (auto &b : d.idx) b.release();
@@ -1295,8 +1294,12 @@ static int pack_type(pbd_engine *e, int t, const std::vector<unsigned> &order, b
     return 0;
 }
 
-// resident mode: colour ranges of the bucket table, the per-tile runs and the arrival counts of the X items
-static int build_phase_tables(pbd_engine *e, const ResidentPlan &pl, const std::vector<unsigned> &tileOff) {
+// resident mode: colour ranges of the bucket table, the per-tile runs, and who waits for whom in the X flag protocol.  Tile j is a
+// neighbour of tile i when an X item of i and an X item of j touch the same global-homed particle, or an X item of one of them touches
+// a particle homed in the other: exactly the tiles whose global-memory accesses i's X items and i's global-homed particles have to be
+// ordered with.  xMask[i][0] bit k: neighbour k has global-homed particles (arrives in the integration phase); xMask[i][1 + c] bit k:
+// neighbour k has X items in colour c.
+static int build_phase_tables(pbd_engine *e, const ResidentPlan &pl, const std::vector<unsigned> &tileOff, const std::vector<unsigned> (&order)[PBD_NUM_TYPES]) {
     const unsigned T = e->nTiles;
     std::vector<unsigned> colourStart;
     for (size_t i = 0; i < e->buckets.size(); i++)
@@ -1304,38 +1307,80 @@ static int build_phase_tables(pbd_engine *e, const ResidentPlan &pl, const std::
     e->resColours = (unsigned)colourStart.size();
     colourStart.push_back((unsigned)e->buckets.size());
     if (tileOff.size() != e->buckets.size() * (2 * (size_t)T + 1)) return fail("flatten: internal error (tile runs)");
-    // arrivals on the X counter: one per CTA that owns X work in the phase -- integration phase (global-homed particles), then every colour
-    std::vector<unsigned> xArrive(1 + e->resColours, 0u);
-    for (unsigned t = 0; t < T; t++) xArrive[0] += (pl.tileStart[t + 1] - pl.tileStart[t] - pl.tileSmem[t]) ? 1u : 0u;
-    for (unsigned c = 0; c < e->resColours; c++)
-        for (unsigned t = 0; t < T; t++) {
-            unsigned any = 0;
-            for (unsigned bi = colourStart[c]; bi < colourStart[c + 1]; bi++) {
-                const unsigned *off = &tileOff[(size_t)bi * (2 * T + 1) + 2 * t];
-                any |= (off[1] - off[0]);
+    const unsigned nC = e->resColours;
+    auto run = [&](size_t bi, unsigned t) { return &tileOff[bi * (2 * (size_t)T + 1) + 2 * t]; };  // [0] X items .. [1] others .. [2]
+    // (global-homed particle, tile) pairs: its home tile and every tile that executes an X item touching it
+    std::vector<std::pair<unsigned, unsigned>> touch;
+    for (unsigned i = 0; i < e->n; i++) if (pl.homedGlobal[i]) touch.emplace_back(i, pl.tileOf[i]);
+    for (size_t bi = 0; bi < e->buckets.size(); bi++) {
+        const Bucket &b = e->buckets[bi];
+        const int nb = type_shape(b.type).nBodies;
+        for (unsigned t = 0; t < T; t++)
+            for (unsigned k = run(bi, t)[0]; k < run(bi, t)[1]; k++) {
+                const unsigned *bod = &e->host[b.type].bodies[(size_t)order[b.type][b.first + k] * nb];
+                for (int j = 0; j < nb; j++) if (!is_rb_body(b.type, j) && pl.homedGlobal[bod[j]]) touch.emplace_back(bod[j], t);
             }
-            xArrive[1 + c] += any ? 1u : 0u;
+    }
+    std::sort(touch.begin(), touch.end());
+    touch.erase(std::unique(touch.begin(), touch.end()), touch.end());
+    std::vector<unsigned char> adj((size_t)T * T, 0);
+    for (size_t lo = 0, hi; lo < touch.size(); lo = hi) {
+        for (hi = lo + 1; hi < touch.size() && touch[hi].first == touch[lo].first; hi++) {}
+        for (size_t a = lo; a < hi; a++)
+            for (size_t c = lo; c < hi; c++)
+                if (touch[a].second != touch[c].second) adj[(size_t)touch[a].second * T + touch[c].second] = 1;
+    }
+    std::vector<unsigned char> hasX((size_t)T * (1 + nC), 0);  // [tile][phase]: the tile arrives in the phase
+    for (unsigned t = 0; t < T; t++) {
+        hasX[(size_t)t * (1 + nC)] = (pl.tileStart[t + 1] - pl.tileStart[t] - pl.tileSmem[t]) != 0;
+        for (unsigned c = 0; c < nC; c++)
+            for (unsigned bi = colourStart[c]; bi < colourStart[c + 1]; bi++) hasX[(size_t)t * (1 + nC) + 1 + c] |= run(bi, t)[1] != run(bi, t)[0];
+    }
+    std::vector<unsigned> nbr((size_t)T * kMaxXNeighbours), mask((size_t)T * (1 + nC), 0u), nNbr(T, 0u);
+    for (unsigned i = 0; i < T; i++) {
+        for (unsigned k = 0; k < kMaxXNeighbours; k++) nbr[(size_t)i * kMaxXNeighbours + k] = i;  // unused lanes: never polled (mask bit 0)
+        for (unsigned j = 0; j < T; j++) {
+            if (!adj[(size_t)i * T + j]) continue;
+            if (nNbr[i] == kMaxXNeighbours)
+                return fail("resident mode: tile %u shares global-homed particles with more than %u other tiles (the constraints reach too far "
+                            "across the scene for the resident mode; use PBD_MODE_GRAPH)", i, kMaxXNeighbours);
+            const unsigned k = nNbr[i]++;
+            nbr[(size_t)i * kMaxXNeighbours + k] = j;
+            for (unsigned p = 0; p <= nC; p++) mask[(size_t)i * (1 + nC) + p] |= (unsigned)hasX[(size_t)j * (1 + nC) + p] << k;
         }
-    unsigned long long perSweep = 0;
-    for (unsigned c = 0; c < e->resColours; c++) perSweep += xArrive[1 + c];
-    e->xArriveInt.assign(1, xArrive[0]); e->xArriveCol.assign(1, perSweep);
+    }
     CKE(upload_vec(e->dColourStart, colourStart, e->stream));
     CKE(upload_vec(e->dTileOff, tileOff, e->stream));
-    CKE(upload_vec(e->dXArrive, xArrive, e->stream));
-    CKE(e->dXCounter.alloc(256));
-    CK(cudaMemsetAsync(e->dXCounter.p, 0, 256, e->stream));
-    e->xBase = 0;
+    CKE(upload_vec(e->dXNbr, nbr, e->stream));
+    CKE(upload_vec(e->dXMask, mask, e->stream));
+    CKE(e->dXFlags.alloc((size_t)T * kXFlagStride * sizeof(unsigned long long)));
+    CK(cudaMemsetAsync(e->dXFlags.p, 0, e->dXFlags.bytes, e->stream));
     if (verbose()) {
         unsigned long long xItems = 0, mxRun = 0;
-        for (size_t bi = 0; bi < e->buckets.size(); bi++)
+        std::vector<unsigned long long> perTile(T, 0);  // items a tile executes over one sweep
+        unsigned long long lockstep = 0;                // ... and the sum over the colours of the largest tile's items of the colour
+        for (unsigned c = 0; c < nC; c++) {
+            unsigned long long mx = 0;
             for (unsigned t = 0; t < T; t++) {
-                const unsigned *off = &tileOff[bi * (2 * (size_t)T + 1) + 2 * t];
-                xItems += off[1] - off[0];
-                mxRun = std::max<unsigned long long>(mxRun, off[2] - off[0]);
+                unsigned long long items = 0;
+                for (unsigned bi = colourStart[c]; bi < colourStart[c + 1]; bi++) {
+                    xItems += run(bi, t)[1] - run(bi, t)[0];
+                    items += run(bi, t)[2] - run(bi, t)[0];
+                    mxRun = std::max<unsigned long long>(mxRun, run(bi, t)[2] - run(bi, t)[0]);
+                }
+                perTile[t] += items; mx = std::max(mx, items);
             }
-        fprintf(stderr, "[pbd_b200] resident: %u colours, %zu buckets, %.2f %% X items, largest run of a tile in a bucket %llu (mean %.0f), X arrivals per sweep %llu\n",
-                e->resColours, e->buckets.size(), 100.0 * xItems / std::max(1u, e->numConstraints), mxRun,
-                (double)e->numConstraints / std::max<size_t>(1, e->buckets.size()) / T, perSweep);
+            lockstep += mx;
+        }
+        std::vector<unsigned> hist(kMaxXNeighbours + 1, 0u);
+        for (unsigned t = 0; t < T; t++) hist[nNbr[t]]++;
+        fprintf(stderr, "[pbd_b200] resident: %u colours, %zu buckets, %.2f %% X items, largest run of a tile in a bucket %llu (mean %.0f)\n",
+                nC, e->buckets.size(), 100.0 * xItems / std::max(1u, e->numConstraints), mxRun, (double)e->numConstraints / std::max<size_t>(1, e->buckets.size()) / T);
+        fprintf(stderr, "[pbd_b200] resident: X neighbours per tile (count x tiles):");
+        for (unsigned k = 0; k <= kMaxXNeighbours; k++) if (hist[k]) fprintf(stderr, " %u x %u", k, hist[k]);
+        const unsigned long long mxTile = T ? *std::max_element(perTile.begin(), perTile.end()) : 0;
+        fprintf(stderr, "\n[pbd_b200] resident: items per sweep, sum over colours of the largest tile %llu, largest tile over all colours %llu (lockstep penalty %.2f %%)\n",
+                lockstep, mxTile, mxTile ? 100.0 * ((double)lockstep / mxTile - 1.0) : 0.0);
     }
     return 0;
 }
@@ -1362,7 +1407,7 @@ static int flatten_image(pbd_engine *e) {
     for (int t = 0; t < PBD_NUM_TYPES; t++) CKE(pack_type(e, t, order[t], tiled, pl, lap));
     lap("SoA arrays + upload");
     CKE(upload_vec(e->dBuckets, e->buckets, e->stream));
-    if (tiled) CKE(build_phase_tables(e, pl, tileOff));
+    if (tiled) CKE(build_phase_tables(e, pl, tileOff, order));
     CK(cudaStreamSynchronize(e->stream));
     lap("phase tables");
     e->stats.num_constraints = e->numConstraints;
@@ -1535,7 +1580,8 @@ static int enqueue_step_resident(pbd_engine *e, cudaStream_t s, unsigned long lo
     ra.pos = (float4 *)e->pos.p; ra.vel = (float4 *)e->vel.p; ra.oldp = (float4 *)e->oldp.p; ra.lastp = (float4 *)e->lastp.p;
     ra.buckets = (const Bucket *)e->dBuckets.p;
     ra.colourStart = (const unsigned *)e->dColourStart.p; ra.tileOff = (const unsigned *)e->dTileOff.p;
-    ra.tileStart = (const unsigned *)e->dTileStart.p; ra.tileSmem = (const unsigned *)e->dTileSmem.p; ra.xArrive = (const unsigned *)e->dXArrive.p;
+    ra.tileStart = (const unsigned *)e->dTileStart.p; ra.tileSmem = (const unsigned *)e->dTileSmem.p;
+    ra.xNbr = (const unsigned *)e->dXNbr.p; ra.xMask = (const unsigned *)e->dXMask.p;
     ra.nBuckets = (unsigned)e->buckets.size(); ra.nColours = e->resColours; ra.nTiles = e->nTiles; ra.subSteps = e->subSteps; ra.maxIter = e->maxIter;
     ra.tileCap = e->resTileCap; ra.xThreads = e->resXThreads; ra.clusterSize = e->resC;
     {   // L2 prefetch of the operand runs pays when the constraint stream of a sweep does not stay in L2 anyway (above ~0.38 x the L2).
@@ -1550,9 +1596,8 @@ static int enqueue_step_resident(pbd_engine *e, cudaStream_t s, unsigned long lo
     }
     ra.h = h; ra.invH = (float)(1.0 / (double)h); ra.twoInvH = (float)(2.0 / (double)h); ra.gx = e->g[0]; ra.gy = e->g[1]; ra.gz = e->g[2];
     ra.secondOrder = e->velMethod;
-    ra.xCounter = (unsigned long long *)e->dXCounter.p;
-    ra.xBase = e->xBase;
-    e->xBase += (unsigned long long)e->subSteps * (e->xArriveInt[0] + (unsigned long long)e->maxIter * e->xArriveCol[0]);
+    ra.xFlags = (unsigned long long *)e->dXFlags.p;
+    ra.xLaunch = (++e->xLaunch) << 32;  // above every flag value of the earlier launches, whatever subSteps / maxIter they ran with
     ra.rb = rb_state(e);
     for (int t = 0; t < PBD_NUM_TYPES; t++) ra.types[t] = e->dev[t].arrays;
     *launches = 1;
@@ -1560,7 +1605,7 @@ static int enqueue_step_resident(pbd_engine *e, cudaStream_t s, unsigned long lo
     static const char *tracePath = getenv("PBD_B200_TRACE");  // development aid: dump per-phase timelines of one step (tools/trace_resident.py)
     const unsigned kTracePhases = 256;
     if (tracePath) {
-        CKE(e->dTrace.alloc((size_t)kTracePhases * e->nTiles * 4 * sizeof(unsigned long long)));
+        CKE(e->dTrace.alloc((size_t)kTracePhases * e->nTiles * kTraceSlots * sizeof(unsigned long long)));
         CK(cudaMemsetAsync(e->dTrace.p, 0, e->dTrace.bytes, s));
         ra.trace = (unsigned long long *)e->dTrace.p; ra.tracePhases = kTracePhases;
     }
@@ -1569,7 +1614,7 @@ static int enqueue_step_resident(pbd_engine *e, cudaStream_t s, unsigned long lo
         ~TraceDump() {
             if (!path) return;
             cudaStreamSynchronize(s);
-            std::vector<unsigned long long> h((size_t)phases * e->nTiles * 4);
+            std::vector<unsigned long long> h((size_t)phases * e->nTiles * kTraceSlots);
             cudaMemcpy(h.data(), e->dTrace.p, h.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost);
             if (FILE *f = fopen(path, "wb")) { fwrite(h.data(), sizeof(unsigned long long), h.size(), f); fclose(f); }
         }

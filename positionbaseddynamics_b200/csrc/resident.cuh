@@ -13,10 +13,13 @@
 //     so inside a cluster a colour phase ends with the hardware cluster barrier (barrier.cluster) instead of a
 //     grid-wide atomic barrier or a kernel boundary;
 //   * only particles touched by a constraint that spans two clusters stay in global memory ("global-homed").  The constraints
-//     touching them ("X items") are run by dedicated warps of every CTA, which order themselves across clusters through one
-//     monotone arrival counter: red.release.gpu after their X items of phase p, ld.acquire.gpu spin before their X items of
-//     phase p+1.  The round trip overlaps the shared-memory work the other warps do in the meantime; those never touch the
-//     counter.  A scene that fits one cluster (G = 1) has no X items.
+//     touching them ("X items") are run by dedicated warps of every CTA, which order themselves across CTAs through per-CTA
+//     arrival flags: after its X items of phase p a CTA publishes its arrival count with st.release.gpu on its own flag, and
+//     before its X items of phase p+1 it spins (ld.acquire.gpu, one lane per neighbour) on the flags of its NEIGHBOURS only --
+//     the CTAs whose X items share a global-homed particle with its own, or touch one it is the home of (flatten time, at most
+//     32).  A phase is thus no grid-wide barrier: a CTA waits for the few tiles around it, not for the slowest of all.  The
+//     round trip overlaps the shared-memory work the other warps do in the meantime; those never touch the flags.  A scene that
+//     fits one cluster (G = 1) has no X items.
 //   Two regimes are used (engine.cu:choose_resident_shape): ONE cluster of up to 16 CTAs for scenes whose colour phases are small
 //   (cfg1 / cfg3 / cfg4), and G = #SMs clusters of ONE CTA for big scenes (cfg2 / cfg5: 132 independent CTAs on an H100; the SINGLE
 //   instantiations: plain LDS / STS, __syncthreads).
@@ -48,12 +51,18 @@ constexpr size_t kMaxDynamicSmem = 227u * 1024u;  // what a CTA may opt in to on
 // quarter-warp; the swizzle spreads such strides over all eight.
 __host__ __device__ __forceinline__ unsigned tile_swizzle(unsigned s) { return s ^ ((s >> 3) & 7u); }
 constexpr int kMaxClusterCtas = 16;   // non-portable cluster size (opt-in attribute), one GPC
-// Dynamic shared memory of a CTA: [tile: tileCap float4][run table: nBuckets x RunEntry][xArrive: 1 + nColours][colourStart: nColours + 1]
+// Dynamic shared memory of a CTA: [tile: tileCap float4][run table: nBuckets x RunEntry][xMask: 1 + nColours][colourStart: nColours + 1]
+// [xNbr: kMaxXNeighbours]
 // this CTA's two runs of one bucket (absolute indices into the type's arrays); rotR: where the run of shared-memory items starts in the
 // colour's concatenated item sequence, modulo the number of threads that share it (the buckets of one colour go to different threads)
 struct RunEntry { int type; unsigned firstX, nX, firstR, nR, rotR, pad0, pad1; };
+constexpr unsigned kMaxXNeighbours = 32;  // one lane of the first X warp per neighbour
+constexpr unsigned kXFlagStride = 16;     // unsigned long longs: every CTA's arrival flag on its own 128-byte line
+// PBD_B200_TRACE record per (phase, CTA): [0] phase start, [1] X items done, [2] other items done + colour arrive issued,
+// [3] colour wait returned, [4] X wait returned (0 where the CTA has no X items in the phase); tools/trace_resident.py
+constexpr unsigned kTraceSlots = 5;
 __host__ __device__ inline size_t resident_smem_bytes(unsigned tileCap, unsigned nBuckets, unsigned nColours) {
-    return (size_t)tileCap * sizeof(float4) + (size_t)nBuckets * sizeof(RunEntry) + (size_t)(2u * nColours + 2u) * sizeof(unsigned);
+    return (size_t)tileCap * sizeof(float4) + (size_t)nBuckets * sizeof(RunEntry) + (size_t)(2u * nColours + 2u + kMaxXNeighbours) * sizeof(unsigned);
 }
 
 struct ResidentArgs {
@@ -63,7 +72,8 @@ struct ResidentArgs {
     const unsigned *tileOff;      // [nBuckets][2 nTiles + 1], relative to the bucket's `first`: tile t = [2t] X items.. [2t+1] others.. [2t+2]
     const unsigned *tileStart;    // [nTiles + 1] device slots: tile t owns [tileStart[t], tileStart[t+1])
     const unsigned *tileSmem;     // [nTiles] leading slots of the tile that live in shared memory; the rest is global-homed
-    const unsigned *xArrive;      // [1 + nColours] counter arrivals (CTAs that own X work) of the integration phase and of every colour
+    const unsigned *xNbr;         // [nTiles][kMaxXNeighbours] neighbours of every CTA (the CTAs whose X items it has to wait for)
+    const unsigned *xMask;        // [nTiles][1 + nColours] bit k: neighbour k arrives in the integration phase / in colour c
     unsigned nBuckets, nColours, nTiles, subSteps, maxIter;
     unsigned tileCap;             // float4 slots reserved for the tile in every CTA's shared memory (>= the largest tileSmem)
     unsigned xThreads;            // the last xThreads threads of every CTA run the X items (and nothing else); 0 when there is one cluster
@@ -71,10 +81,10 @@ struct ResidentArgs {
     int l2Prefetch;               // prefetch the next colour's operand runs into L2 (scenes whose constraint stream exceeds L2)
     float h, invH, twoInvH, gx, gy, gz;
     int secondOrder;
-    unsigned long long *xCounter; // monotone arrival counter of the X items (global memory)
-    unsigned long long xBase;     // its value when this launch starts
+    unsigned long long *xFlags;   // [nTiles][kXFlagStride] arrival flag of every CTA: (launch ordinal << 32) | arrivals in this launch
+    unsigned long long xLaunch;   // this launch's ordinal << 32 (the host counts resident launches: flags stay monotone across launches)
     RbState rb;                   // rigid bodies coupled through joints (global memory; single-cluster scenes only)
-    unsigned long long *trace;    // development aid (PBD_B200_TRACE): globaltimer per (phase, CTA)
+    unsigned long long *trace;    // development aid (PBD_B200_TRACE): globaltimer per (phase, CTA, kTraceSlots)
     unsigned tracePhases;
     TypeArrays types[PBD_NUM_TYPES];
 };
@@ -90,8 +100,8 @@ __device__ __forceinline__ unsigned long long ld_acquire_u64(const unsigned long
     asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
     return v;
 }
-__device__ __forceinline__ void red_release_add_u64(unsigned long long *p, unsigned long long v) {
-    asm volatile("red.release.gpu.global.add.u64 [%0], %1;" :: "l"(p), "l"(v) : "memory");
+__device__ __forceinline__ void st_release_u64(unsigned long long *p, unsigned long long v) {
+    asm volatile("st.release.gpu.global.u64 [%0], %1;" :: "l"(p), "l"(v) : "memory");
 }
 __device__ __forceinline__ unsigned long long globaltimer_ns() {
     unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t;
@@ -282,20 +292,21 @@ __device__ __forceinline__ void velocity_particle(const ResidentArgs &A, unsigne
     __stcs(A.vel + slot, v);
 }
 
-// X warps of a CTA act as one party of the counter protocol (one arrival and one poller per CTA and colour instead of one per warp: the
-// counter is ONE L2 address).  Named barrier 1 synchronises the CTA's XT threads (whole warps); its first thread talks to the counter.
-//   wait  : thread 0 spins until every arrival of the earlier phases is visible (ld.acquire.gpu), then releases its CTA's X warps;
-//   arrive: after the X warps' stores -- barrier (orders them before thread 0), then thread 0 publishes with red.release.gpu
-//           (the fence is cumulative over what the barrier ordered: the cooperative-groups grid.sync pattern).
+// X warps of a CTA act as one party of the flag protocol (one arrival per CTA and phase, one poller per neighbour).  Named barrier 1
+// synchronises the CTA's XT threads (whole warps).
+//   wait  : lane k of the first X warp spins until neighbour k's flag shows every arrival of the earlier phases this CTA depends on
+//           (ld.acquire.gpu; `target` = launch ordinal | arrivals, `spin` false when there is none), then the barrier releases the X warps;
+//   arrive: after the X warps' stores -- barrier (orders them before the first X thread), then that thread publishes its CTA's arrival
+//           count with st.release.gpu (the fence is cumulative over what the barrier ordered: the cooperative-groups grid.sync pattern).
 __device__ __forceinline__ void x_bar(unsigned xThreads) { asm volatile("bar.sync 1, %0;" :: "r"(xThreads) : "memory"); }
-__device__ __forceinline__ void x_wait(const unsigned long long *counter, unsigned long long target, unsigned xtid, unsigned xThreads) {
-    if (xtid == 0)
-        while (ld_acquire_u64(counter) < target) { }
+__device__ __forceinline__ void x_wait(const unsigned long long *peer, unsigned long long target, bool spin, unsigned xThreads) {
+    if (spin)
+        while (ld_acquire_u64(peer) < target) { }
     x_bar(xThreads);
 }
-__device__ __forceinline__ void x_arrive(unsigned long long *counter, unsigned xtid, unsigned xThreads) {
+__device__ __forceinline__ void x_arrive(unsigned long long *flag, unsigned long long value, unsigned xtid, unsigned xThreads) {
     x_bar(xThreads);
-    if (xtid == 0) red_release_add_u64(counter, 1ull);
+    if (xtid == 0) st_release_u64(flag, value);
 }
 
 // colour barrier of the cluster: arrive (publishes this thread's shared-memory stores), then wait; one CTA: a block barrier
@@ -306,8 +317,9 @@ template <unsigned MASK, int THREADS, bool SINGLE>
 __global__ void __launch_bounds__(THREADS, 1) k_step_resident(const __grid_constant__ ResidentArgs A) {
     extern __shared__ float4 tile[];
     RunEntry *runs = reinterpret_cast<RunEntry *>(tile + A.tileCap);
-    unsigned *sArrive = reinterpret_cast<unsigned *>(runs + A.nBuckets);  // [1 + nColours]
-    unsigned *sColour = sArrive + 1 + A.nColours;                         // [nColours + 1]
+    unsigned *sMask = reinterpret_cast<unsigned *>(runs + A.nBuckets);  // [1 + nColours]
+    unsigned *sColour = sMask + 1 + A.nColours;                         // [nColours + 1]
+    unsigned *sNbr = sColour + 1 + A.nColours;                          // [kMaxXNeighbours]
     const unsigned cta = blockIdx.x;  // tile id = cluster * C + rank (1-D grid, cluster dimension C)
     const unsigned t0 = __ldg(A.tileStart + cta), nSm = __ldg(A.tileSmem + cta), nAll = __ldg(A.tileStart + cta + 1) - t0;
     const unsigned nGl = nAll - nSm;
@@ -322,11 +334,19 @@ __global__ void __launch_bounds__(THREADS, 1) k_step_resident(const __grid_const
     XAcc accX; RAcc accR;
     if constexpr (SINGLE) { accX.pos = A.pos; accX.tile = tile; accR.tile = tile; }
     else { accX.pos = A.pos; accX.tileBase = smem_u32(tile); accR.tileBase = smem_u32(tile); }
-    unsigned long long xTarget = A.xBase;  // counter value once every arrival of the phases before the current one is in
+    // flag protocol (X threads only): lane k of the first X warp counts the arrivals of neighbour k up to the current phase
+    unsigned xNeed = 0, xArrivals = 0;  // ... and every X thread this CTA's own
+    unsigned long long *const xFlag = A.xFlags + (size_t)cta * kXFlagStride;
+    const bool xLane = isX && xtid < kMaxXNeighbours;
+    auto x_count = [&](unsigned p) { if (xLane) xNeed += (sMask[p] >> xtid) & 1u; };  // after phase p (0: integration, 1 + c: colour c)
+    auto x_publish = [&]() { x_arrive(xFlag, A.xLaunch | ++xArrivals, xtid, XT); };
+    auto x_peer = [&]() { return A.xFlags + (size_t)sNbr[xtid & (kMaxXNeighbours - 1u)] * kXFlagStride; };  // neighbour xtid's flag
     unsigned phase = 0;
     auto stamp = [&](unsigned k) {
-        if (A.trace && phase < A.tracePhases && (threadIdx.x == 0 || (k == 1 && threadIdx.x == RT))) A.trace[((size_t)phase * gridDim.x + cta) * 4 + k] = globaltimer_ns();
+        if (A.trace && phase < A.tracePhases && (threadIdx.x == 0 || ((k == 1 || k == 4) && threadIdx.x == RT)))
+            A.trace[((size_t)phase * gridDim.x + cta) * kTraceSlots + k] = globaltimer_ns();
     };
+    auto x_sync = [&]() { x_wait(x_peer(), A.xLaunch | xNeed, xLane && xNeed != 0u, XT); stamp(4); };
 
     // ---- once per launch: the tile and this CTA's view of the phase structure go to shared memory (after a cluster barrier L1 is
     // invalid, so anything read per phase from global memory would cost an L2 round trip on the critical path of every colour)
@@ -338,7 +358,8 @@ __global__ void __launch_bounds__(THREADS, 1) k_step_resident(const __grid_const
         RunEntry r; r.type = b.type; r.firstX = b.first + o0; r.nX = o1 - o0; r.firstR = b.first + o1; r.nR = o2 - o1; r.rotR = r.pad0 = r.pad1 = 0u;
         runs[bi] = r;
     }
-    for (unsigned i = threadIdx.x; i < 1u + A.nColours; i += THREADS) { sArrive[i] = __ldg(A.xArrive + i); sColour[i] = __ldg(A.colourStart + i); }
+    for (unsigned i = threadIdx.x; i < 1u + A.nColours; i += THREADS) { sMask[i] = __ldg(A.xMask + (size_t)cta * (1u + A.nColours) + i); sColour[i] = __ldg(A.colourStart + i); }
+    if (threadIdx.x < kMaxXNeighbours) sNbr[threadIdx.x] = __ldg(A.xNbr + (size_t)cta * kMaxXNeighbours + threadIdx.x);
     __syncthreads();
     for (unsigned c = threadIdx.x; c < A.nColours; c += THREADS) {  // rotations: bucket k of a colour starts where bucket k-1 ended
         unsigned accR = 0;
@@ -359,7 +380,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_step_resident(const __grid_const
                 float4 x = __ldcg(A.pos + t0 + nSm + i);
                 if (integrate_particle(A, t0 + nSm + i, x)) __stcg(A.pos + t0 + nSm + i, x);
             }
-            if (nGl) x_arrive(A.xCounter, xtid, XT);
+            if (nGl) x_publish();
             stamp(1);
         } else {
             for (unsigned i = threadIdx.x; i < nSm; i += RT) {
@@ -368,7 +389,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_step_resident(const __grid_const
             }
             if (A.rb.n && cta == 0 && threadIdx.x < A.rb.n) rb_integrate_body(A.rb, threadIdx.x, A.h, A.gx, A.gy, A.gz);
         }
-        xTarget += sArrive[0];
+        x_count(0);
         colour_arrive(single);
         if (A.nColours) prefetch_first<MASK>(A, runs[sColour[0]], sColour[0], true, isX ? xtid : threadIdx.x, isX, pre);
         stamp(2); colour_wait(single); stamp(3);
@@ -388,14 +409,14 @@ __global__ void __launch_bounds__(THREADS, 1) k_step_resident(const __grid_const
                     }
                 }
                 if (isX) {
-                    // X items of every bucket of the colour: they touch global-homed particles and are ordered across clusters by the counter
+                    // X items of every bucket of the colour: they touch global-homed particles and are ordered across CTAs by the flags
                     bool mine = false;  // CTA-uniform: does this CTA own an X item of this colour?
                     for (unsigned bi = b0; bi < b1; bi++) mine = mine || (runs[bi].nX != 0u);
                     if (mine) {
-                        x_wait(A.xCounter, xTarget, xtid, XT);
+                        x_sync();
 #pragma unroll 1
                         for (unsigned bi = b0; bi < b1; bi++) run_items<MASK, false>(A, accX, runs[bi].type, runs[bi].firstX, runs[bi].nX, iterZero, xtid, XT, pre.bucket == bi, pre);
-                        x_arrive(A.xCounter, xtid, XT);
+                        x_publish();
                     }
                     stamp(1);
                 } else {
@@ -407,7 +428,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_step_resident(const __grid_const
                                                                            threadIdx.x >= rot ? threadIdx.x - rot : threadIdx.x + RT - rot, RT, pre.bucket == bi, pre);
                     }
                 }
-                xTarget += sArrive[1 + c];
+                x_count(1u + c);
                 colour_arrive(single);
                 {   // this thread's first item of the next colour streams in while the CTAs synchronise
                     const bool lastColour = (c + 1 == A.nColours);
@@ -421,9 +442,9 @@ __global__ void __launch_bounds__(THREADS, 1) k_step_resident(const __grid_const
             }
         }
 
-        // ---- epilogue: velocity update (own particles only; the global-homed ones need the last colour's X items of every cluster)
+        // ---- epilogue: velocity update (own particles only; the global-homed ones need the last X items of every neighbour)
         if (isX) {
-            if (nGl) x_wait(A.xCounter, xTarget, xtid, XT);
+            if (nGl) x_wait(x_peer(), A.xLaunch | xNeed, xLane && xNeed != 0u, XT);
             for (unsigned i = xtid; i < nGl; i += XT) velocity_particle(A, t0 + nSm + i, __ldcg(A.pos + t0 + nSm + i));
         } else {
             for (unsigned i = threadIdx.x; i < nSm; i += RT) velocity_particle(A, t0 + i, tile[tile_swizzle(i)]);

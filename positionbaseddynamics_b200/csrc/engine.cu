@@ -1381,6 +1381,19 @@ static int build_phase_tables(pbd_engine *e, const ResidentPlan &pl, const std::
         const unsigned long long mxTile = T ? *std::max_element(perTile.begin(), perTile.end()) : 0;
         fprintf(stderr, "\n[pbd_b200] resident: items per sweep, sum over colours of the largest tile %llu, largest tile over all colours %llu (lockstep penalty %.2f %%)\n",
                 lockstep, mxTile, mxTile ? 100.0 * ((double)lockstep / mxTile - 1.0) : 0.0);
+        // the constraint stream of one sweep as this image streams it from DRAM: the 32-bit indices, the per-constraint geometry and
+        // material arrays, the multipliers (read and written)
+        double idxBytes = 0, constBytes = 0;
+        for (const Bucket &b : e->buckets) {
+            const TypeArrays &a = e->dev[b.type].arrays;
+            double perItem = a.lambda ? 8.0 : 0.0;
+            for (int k = 0; k < kMaxGeoV; k++) perItem += a.gv[k] ? 16.0 : 0.0;
+            for (int k = 0; k < kMaxGeoS; k++) perItem += a.gs[k] ? 4.0 : 0.0;
+            for (int k = 0; k < kMaxMat; k++) perItem += a.mat[k] ? 4.0 : 0.0;
+            idxBytes += b.count * 4.0 * type_shape(b.type).nBodies; constBytes += b.count * perItem;
+        }
+        fprintf(stderr, "[pbd_b200] resident: constraint stream per sweep %.1f MB: indices %.1f MB, constants and multipliers %.1f MB\n",
+                (idxBytes + constBytes) * 1e-6, idxBytes * 1e-6, constBytes * 1e-6);
     }
     return 0;
 }

@@ -401,12 +401,15 @@ __global__ void __launch_bounds__(THREADS, 1) k_step_resident(const __grid_const
             for (unsigned c = 0; c < A.nColours; c++) {
                 const unsigned b0 = sColour[c], b1 = sColour[c + 1];
                 stamp(0);
-                if (A.l2Prefetch && threadIdx.x < kPrefetchLanes) {  // the next colour's operand runs of this CTA start travelling DRAM -> L2 now
+                if (A.l2Prefetch && !isX && (threadIdx.x & 31u) == 0u) {  // the next colour's operand runs of this CTA start travelling DRAM -> L2 now
+                    // one array per R warp (lane 0): the colour barrier waits for the slowest warp, and the arrays issued by the lanes of
+                    // one warp would go one divergent path after the other; the X warps stay free for their cross-tile chain
                     const unsigned cn = (c + 1 == A.nColours) ? 0u : c + 1u;
-                    for (unsigned bi = sColour[cn]; bi < sColour[cn + 1]; bi++) {
-                        const RunEntry r = runs[bi];
-                        PBD_FOR_TYPE(MASK, r.type, l2_prefetch_run<T>(A.types[T], r.firstX, r.nX + r.nR, threadIdx.x);)
-                    }
+                    for (unsigned k = threadIdx.x >> 5; k < kPrefetchLanes; k += RT >> 5)
+                        for (unsigned bi = sColour[cn]; bi < sColour[cn + 1]; bi++) {
+                            const RunEntry r = runs[bi];
+                            PBD_FOR_TYPE(MASK, r.type, l2_prefetch_run<T>(A.types[T], r.firstX, r.nX + r.nR, k);)
+                        }
                 }
                 if (isX) {
                     // X items of every bucket of the colour: they touch global-homed particles and are ordered across CTAs by the flags

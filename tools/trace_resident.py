@@ -1,6 +1,8 @@
 """Development aid: summarise the per-phase timeline k_step_resident dumps with PBD_B200_TRACE=<file> (globaltimer, ns).
 Record per (phase, CTA): [0] phase start, [1] X items done, [2] other items done + cluster arrive issued, [3] cluster wait returned,
-[4] X wait returned (0 where the CTA has no X items in the phase: the integration phase, or no X item of its own in the colour)."""
+[4] X wait returned (0 where the CTA has no X items in the phase: the integration phase, or no X item of its own in the colour).
+Stamps 0, 2 and 3 are written by thread 0 (it runs shared-memory items, "R items"), stamps 1 and 4 by the first X thread: the two run
+concurrently, so the R side of a phase is [2] - [0], and [2] - [1] is how long the R side runs on after the X warps have published."""
 import sys
 import numpy as np
 
@@ -11,12 +13,12 @@ valid = (a[:, :, 0] > 0).all(axis=1) & (a[:, :, 3] > 0).all(axis=1)
 a = a[valid]
 print("phases recorded:", len(a), "CTAs:", ctas)
 t0 = a[0, :, 0].min()
-x = a[:, :, 1] - a[:, :, 0]; r = a[:, :, 2] - a[:, :, 1]; w = a[:, :, 3] - a[:, :, 2]
+x = a[:, :, 1] - a[:, :, 0]; r = a[:, :, 2] - a[:, :, 0]; tail = a[:, :, 2] - a[:, :, 1]; w = a[:, :, 3] - a[:, :, 2]
 has_xw = a[:, :, 4] > 0
 xw = np.where(has_xw, a[:, :, 4] - a[:, :, 0], np.nan)  # phase start -> X wait returned
 period = np.diff(a[:, :, 0].min(axis=1))
 print("phase period (first CTA start to next phase's first CTA start): mean %.0f ns, median %.0f, p95 %.0f" % (period.mean(), np.median(period), np.percentile(period, 95)))
-for name, v in (("X items (incl. wait)", x), ("other items + arrive", r), ("cluster wait", w)):
+for name, v in (("X items (incl. wait)", x), ("R items (thread 0)", r), ("R tail after X publish", tail), ("cluster wait", w)):
     print("%-22s per CTA: mean %.0f ns, median %.0f, p95 %.0f, max-over-CTAs mean %.0f" % (name, v.mean(), np.median(v), np.percentile(v, 95), v.max(axis=1).mean()))
 if has_xw.any():
     v = xw[has_xw]

@@ -122,8 +122,6 @@ int pbd_set_params(pbd_engine *e, float dt, unsigned subSteps, unsigned maxIter,
                    const float gravity[3]);
 int pbd_set_mode(pbd_engine *e, int mode);
 int pbd_get_mode(pbd_engine *e, int *requested, int *active);  /* active = the mode the current image runs in (resolved at the first step) */
-/* sort constraints inside each (colour,type) bucket by their lowest particle index (order inside a colour is free). */
-int pbd_set_bucket_sort(pbd_engine *e, int enable);
 
 /* nSteps x TimeStepController::step, asynchronous on the engine's stream. */
 int pbd_step(pbd_engine *e, unsigned nSteps);

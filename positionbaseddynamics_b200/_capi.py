@@ -23,7 +23,7 @@ MODE_GRAPH, MODE_RESIDENT, MODE_LAUNCH, MODE_JACOBI, MODE_AUTO = 0, 1, 2, 3, 4
 SYMBOLS = ["pbd_last_error", "pbd_device_count", "pbd_create", "pbd_destroy", "pbd_set_particles", "pbd_set_attr",
            "pbd_get_attr", "pbd_set_masses", "pbd_set_rigid_bodies", "pbd_get_rigid_bodies", "pbd_clear_constraints", "pbd_add_constraints", "pbd_num_bodies",
            "pbd_num_params", "pbd_set_groups", "pbd_color_first_fit", "pbd_color_first_fit_device", "pbd_pin_host", "pbd_unpin_host", "pbd_get_num_groups", "pbd_get_groups",
-           "pbd_set_params", "pbd_set_mode", "pbd_get_mode", "pbd_set_bucket_sort", "pbd_step", "pbd_sync", "pbd_step_host", "pbd_step_host_async", "pbd_step_host_wait",
+           "pbd_set_params", "pbd_set_mode", "pbd_get_mode", "pbd_step", "pbd_sync", "pbd_step_host", "pbd_step_host_async", "pbd_step_host_wait",
            "pbd_get_lambdas", "pbd_get_stats", "pbd_profile_step",
            "pbd_set_colliders", "pbd_set_contact_params", "pbd_record_contacts", "pbd_get_contacts"]
 
@@ -89,7 +89,6 @@ def lib():
         _lib.pbd_set_params.argtypes = [C.c_void_p, C.c_float, C.c_uint, C.c_uint, C.c_int, C.c_void_p]
         _lib.pbd_set_mode.argtypes = [C.c_void_p, C.c_int]
         _lib.pbd_get_mode.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int)]
-        _lib.pbd_set_bucket_sort.argtypes = [C.c_void_p, C.c_int]
         _lib.pbd_step.argtypes = [C.c_void_p, C.c_uint]
         _lib.pbd_step_host.argtypes = [C.c_void_p, C.c_uint, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         _lib.pbd_step_host_async.argtypes = [C.c_void_p, C.c_uint, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -247,9 +246,6 @@ class Engine:
         r, a = C.c_int(0), C.c_int(0)
         _ck(lib().pbd_get_mode(self._h, C.byref(r), C.byref(a)))
         return r.value, a.value
-
-    def set_bucket_sort(self, enable):
-        _ck(lib().pbd_set_bucket_sort(self._h, int(bool(enable))))
 
     def step(self, n=1):
         _ck(lib().pbd_step(self._h, int(n)))

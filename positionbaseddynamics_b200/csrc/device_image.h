@@ -101,4 +101,42 @@ inline double algorithmic_bytes(int t, int isoVariant) {
     }
 }
 
+// Sets of constraint types, one bit per type.  k_step_resident (resident.cuh) is instantiated per mask, the leanest that
+// covers the model: the everything-kernel is 20k instructions and 226 registers, and every colour phase jumps through it.
+constexpr unsigned type_bit(int t) { return 1u << t; }
+constexpr unsigned kMaskClothXPBD = type_bit(PBD_DISTANCE_XPBD) | type_bit(PBD_ISOBENDING_XPBD);
+constexpr unsigned kMaskCloth = kMaskClothXPBD | type_bit(PBD_DISTANCE) | type_bit(PBD_ISOBENDING);
+constexpr unsigned kMaskLight = type_bit(PBD_DISTANCE) | type_bit(PBD_DISTANCE_XPBD) | type_bit(PBD_DIHEDRAL) | type_bit(PBD_ISOBENDING) |
+                                type_bit(PBD_ISOBENDING_XPBD) | type_bit(PBD_VOLUME) | type_bit(PBD_VOLUME_XPBD) | type_bit(PBD_FEMTRIANGLE);
+// FEM solids (cfg3): tets with FEM / volume constraints; and cloth + FEM solids + the coupling joints (cfg4)
+constexpr unsigned kMaskFem = type_bit(PBD_FEMTET) | type_bit(PBD_FEMTET_XPBD) | type_bit(PBD_VOLUME) | type_bit(PBD_VOLUME_XPBD);
+constexpr unsigned kMaskSolid = kMaskCloth | kMaskFem | type_bit(PBD_FEMTRIANGLE) | type_bit(PBD_BALLJOINT) | type_bit(PBD_RB_PARTICLE_BALLJOINT);
+constexpr unsigned kMaskAll = (1u << PBD_NUM_TYPES) - 1u;
+
+// Block size of the resident instantiation of a type mask: the largest it compiles for without spilling (cloth 96 registers,
+// light 128, everything 236).
+constexpr unsigned resident_threads(unsigned mask) { return mask == kMaskClothXPBD ? 640u : (mask == kMaskAll ? 256u : 512u); }
+
+// ---- the resident image (resident.cuh) ---------------------------------------------------------------------------------------
+// Index encoding: bit 31 set -> shared memory: bits 30..27 = CTA rank inside the executing cluster, bits 26..0 = slot inside that
+// CTA's tile;  bit 31 clear -> device slot in the global float4 array.
+constexpr unsigned kSmemFlag = 0x80000000u;
+constexpr unsigned kRankShift = 27u;
+constexpr unsigned kLocalMask = (1u << kRankShift) - 1u;
+constexpr size_t kMaxDynamicSmem = 227u * 1024u;  // what a CTA may opt in to on sm_90
+// Bank swizzle of a tile: slot s lives at tile[s ^ ((s >> 3) & 7)] (a permutation inside every aligned 64-slot block; tileCap is a
+// multiple of 64).  One colour's constraints touch slots 2 or 3 apart, i.e. only half of the eight 16-byte bank groups per
+// quarter-warp; the swizzle spreads such strides over all eight.
+__host__ __device__ __forceinline__ unsigned tile_swizzle(unsigned s) { return s ^ ((s >> 3) & 7u); }
+constexpr int kMaxClusterCtas = 16;   // non-portable cluster size (opt-in attribute), one GPC
+// Dynamic shared memory of a CTA: [tile: tileCap float4][run table: nBuckets x RunEntry][xMask: 1 + nColours][colourStart: nColours + 1]
+// [xNbr: kMaxXNeighbours]
+// this CTA's two runs of one bucket (absolute indices into the type's arrays); rotR: where the run of shared-memory items starts in the
+// colour's concatenated item sequence, modulo the number of threads that share it (the buckets of one colour go to different threads)
+struct RunEntry { int type; unsigned firstX, nX, firstR, nR, rotR, pad0, pad1; };
+constexpr unsigned kMaxXNeighbours = 32;  // one lane of the first X warp per neighbour
+__host__ __device__ inline size_t resident_smem_bytes(unsigned tileCap, unsigned nBuckets, unsigned nColours) {
+    return (size_t)tileCap * sizeof(float4) + (size_t)nBuckets * sizeof(RunEntry) + (size_t)(2u * nColours + 2u + kMaxXNeighbours) * sizeof(unsigned);
+}
+
 }  // namespace pbdk

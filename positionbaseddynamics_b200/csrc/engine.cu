@@ -1,7 +1,7 @@
 // positionbaseddynamics_b200/csrc/engine.cu
 //
 // Host side of the H100 PBD/XPBD engine behind the C ABI of include/pbd_b200.h:
-//   * flattening of a constraint list + the reference's colour groups into (colour,type) buckets of SoA arrays,
+//   * the device image: colour groups (device colouring), the image planned by host/image_plan.cpp, and its upload,
 //   * the step driver that replaces TimeStepController::step (Simulation/TimeStepController.cpp:75-241) for
 //     particle constraints: per substep  integrate -> maxIterations x (colour by colour, bucket by bucket) -> velocity update,
 //     executed as plain launches, as a replayed CUDA graph, or as one cluster launch with the positions resident in
@@ -12,7 +12,6 @@
 #include <cstdio>
 #include <cstring>
 #include <cstdlib>
-#include <numeric>
 #include <string>
 #include <vector>
 #include "kernels.cuh"
@@ -21,17 +20,12 @@
 #include "contacts.cuh"
 #include <cub/cub.cuh>
 #include <omp.h>
-#include <parallel/algorithm>  // libstdc++ parallel mode (OpenMP): the per-bucket sorts of flatten
-#include "host/pbd_model.h"
+#include "host/image_plan.h"
 
 using namespace pbdk;
 using pbd_b200::host_threads;
-
-// PBD_B200_VERBOSE: flatten and the resident planner report their stages and timings on stderr
-static bool verbose() {
-    static const bool v = getenv("PBD_B200_VERBOSE") != nullptr;
-    return v;
-}
+using pbd_b200::verbose;
+using pbd_b200::is_rb_body;
 
 // ------------------------------------------------------------------------------------------------------------
 // error plumbing
@@ -52,14 +46,14 @@ extern "C" const char *pbd_last_error(void) { return g_err.c_str(); }
 // engine state
 // ------------------------------------------------------------------------------------------------------------
 using pbd_b200::PodVector;        // std::vector whose resize() does not zero (filled from all threads right after)
-struct HostType {                 // constraints of one type as handed in through pbd_add_constraints
-    PodVector<unsigned> ids;      // insertion index in the reference's m_constraints
-    PodVector<unsigned> bodies;   // nBodies per constraint
-    PodVector<float> params;      // nParams per constraint (reference layout)
-};
+using pbd_b200::TypeStore;        // constraints of one type as handed in through pbd_add_constraints (ids: insertion index)
 
-struct DevBuf {
+struct DevBuf {                   // one device allocation, freed with its owner
     void *p = nullptr; size_t bytes = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf &) = delete;
+    DevBuf &operator=(const DevBuf &) = delete;
+    ~DevBuf() { release(); }
     int alloc(size_t b) {
         if (b <= bytes && p) return 0;
         if (p) cudaFree(p);
@@ -75,7 +69,7 @@ struct DevBuf {
 
 struct DevType {
     DevBuf idx[3], gv[kMaxGeoV], gs[kMaxGeoS], mat[kMaxMat], lambda;
-    std::vector<unsigned> order;  // position in the device arrays -> insertion id
+    PodVector<unsigned> order;    // position in the device arrays -> insertion id
     unsigned count = 0;
     TypeArrays arrays{};
 };
@@ -93,7 +87,7 @@ struct pbd_engine {
     unsigned nRb = 0;
     DevBuf rbX, rbQ, rbV, rbW, rbOldX, rbLastX, rbOldQ, rbLastQ, rbI, rbIinv;
     // constraints (host copy, insertion order) and groups
-    HostType host[PBD_NUM_TYPES];
+    TypeStore host[PBD_NUM_TYPES];
     unsigned numConstraints = 0;
     std::vector<unsigned> groupOff, groupIds;
     bool groupsSet = false;
@@ -102,7 +96,6 @@ struct pbd_engine {
     std::vector<Bucket> buckets;
     DevBuf dBuckets, dTrace;
     bool imageDirty = true;
-    bool sortBuckets = true;
     // parameters
     float dt = 0.005f; unsigned subSteps = 5, maxIter = 1; int velMethod = 0; float g[3] = {0.f, -9.81f, 0.f};
     int mode = PBD_MODE_AUTO;             // requested (pbd_set_mode)
@@ -125,7 +118,6 @@ struct pbd_engine {
     } pipe;
     // contact path (contacts.cuh): colliders, parameters, optional record of the last step's contacts
     std::vector<float> rbMass;
-    std::vector<int> scratchInt;
     std::vector<ParticleCollider> pColliders;
     std::vector<RigidCollider> rColliders;
     DevBuf dPColliders, dRColliders, dRangeStart, dContacts, dContactCount;
@@ -134,9 +126,8 @@ struct pbd_engine {
     bool timingPending = false;
     std::vector<unsigned> slot;          // host particle index -> device slot (formula layouts or the tile-major permutation)
     DevBuf dSlot, dSlotOld, relayoutTmp;
-    bool slotIsTiled = false;
-    // resident mode (resident.cuh): G clusters x C CTAs = nTiles tiles, block size and type mask of the instantiation
-    unsigned resG = 0, resC = 0, nTiles = 0, resThreads = 0, resMask = 0, resColours = 0, resTileCap = 0, resXThreads = 0;
+    // resident mode (resident.cuh): the launch shape of the current image
+    pbd_b200::ResidentShape res;
     bool resChecked = false;              // co-residency of the clusters verified for the current image
     DevBuf dColourStart, dTileOff, dTileStart, dTileSmem, dXNbr, dXMask, dXFlags;
     unsigned long long xLaunch = 0;       // resident launches so far: the high word of the X arrival flags
@@ -189,28 +180,16 @@ extern "C" int pbd_destroy(pbd_engine *e) {
     cudaSetDevice(e->device);
     cudaStreamSynchronize(e->stream);
     drop_graph(e);
-    for (auto *b : {&e->pos, &e->vel, &e->oldp, &e->lastp, &e->pos0, &e->stage, &e->stage2, &e->massStage, &e->jacobiDelta, &e->dSlot, &e->dSlotOld, &e->relayoutTmp,
-                    &e->dPColliders, &e->dRColliders, &e->dRangeStart, &e->dContacts, &e->dContactCount, &e->dColourStart, &e->dTileOff, &e->dTileStart, &e->dTileSmem, &e->dXNbr, &e->dXMask, &e->dXFlags, &e->dBuckets, &e->dTrace,
-                    &e->rbX, &e->rbQ, &e->rbV, &e->rbW, &e->rbOldX, &e->rbLastX, &e->rbOldQ, &e->rbLastQ, &e->rbI, &e->rbIinv}) b->release();
-    for (auto &d : e->dev) {
-        for (auto &b : d.idx) b.release();
-        for (auto &b : d.gv) b.release();
-        for (auto &b : d.gs) b.release();
-        for (auto &b : d.mat) b.release();
-        d.lambda.release();
-    }
     if (e->evStart) cudaEventDestroy(e->evStart);
     if (e->evStop) cudaEventDestroy(e->evStop);
     if (e->pipe.ready) {
         cudaStreamSynchronize(e->pipe.up); cudaStreamSynchronize(e->pipe.down);
-        for (int s = 0; s < 2; s++) {
-            for (auto *b : {&e->pipe.inX[s], &e->pipe.inV[s], &e->pipe.outX[s], &e->pipe.outV[s]}) b->release();
+        for (int s = 0; s < 2; s++)
             for (cudaEvent_t ev : {e->pipe.uploaded[s], e->pipe.consumed[s], e->pipe.produced[s], e->pipe.downloaded[s]}) cudaEventDestroy(ev);
-        }
         cudaStreamDestroy(e->pipe.up); cudaStreamDestroy(e->pipe.down);
     }
     if (e->ownsStream) cudaStreamDestroy(e->stream);
-    delete e;
+    delete e;  // the DevBufs free the device memory (on the device selected above)
     return 0;
 }
 
@@ -235,10 +214,6 @@ static int upload_slot_map(pbd_engine *e) {
     CKE(e->dSlot.alloc((size_t)e->n * sizeof(unsigned)));
     CK(cudaMemcpy(e->dSlot.p, e->slot.data(), (size_t)e->n * sizeof(unsigned), cudaMemcpyHostToDevice));
     return 0;
-}
-static void formula_slot_map(pbd_engine *e, std::vector<unsigned> &m) {
-    m.resize(e->n);
-    for (unsigned i = 0; i < e->n; i++) m[i] = particle_slot(i, e->n);
 }
 // move every particle array from the current slot map to `newSlot`
 static int relayout(pbd_engine *e, const std::vector<unsigned> &newSlot) {
@@ -289,7 +264,8 @@ extern "C" int pbd_set_particles(pbd_engine *e, unsigned n, const float *x, cons
     CKE(e->stage.alloc((size_t)n * 3 * sizeof(float)));
     CKE(e->massStage.alloc((size_t)n * sizeof(float)));
     drop_graph(e);  // buffers may have moved
-    formula_slot_map(e, e->slot); e->slotIsTiled = false; e->imageDirty = true;
+    e->slot.resize(n); e->imageDirty = true;
+    for (unsigned i = 0; i < n; i++) e->slot[i] = particle_slot(i, n);
     if (n == 0) return 0;
     CKE(upload_slot_map(e));
     CK(cudaMemsetAsync(e->vel.p, 0, b4, e->stream));
@@ -399,34 +375,17 @@ extern "C" int pbd_clear_constraints(pbd_engine *e) {
     return 0;
 }
 
-// body k of a constraint of this type is a rigid body (else a particle)
-static bool is_rb_body(int type, int k) { return type == PBD_BALLJOINT || (type == PBD_RB_PARTICLE_BALLJOINT && k == 0); }
-
-// Body indices of `count` constraints of one type against the engine's particle and rigid-body counts, all threads (millions of
-// indices for a big cloth).  Returns the position in `bodies` of the last index out of range, or -1.
-static long long bad_body_index(const pbd_engine *e, int type, const unsigned *bodies, size_t count) {
-    const int nb = type_shape(type).nBodies;
-    long long badAt = -1;
-    #pragma omp parallel for schedule(static) num_threads(host_threads()) reduction(max : badAt) if (count * nb > 100000)
-    for (long long c = 0; c < (long long)count; c++)
-        for (int k = 0; k < nb; k++) {
-            const long long i = c * nb + k;
-            if (bodies[i] >= (is_rb_body(type, k) ? e->nRb : e->n)) badAt = std::max(badAt, i);
-        }
-    return badAt;
-}
-
 extern "C" int pbd_add_constraints(pbd_engine *e, int type, unsigned count, const unsigned *bodies, const float *params, const unsigned *ids) {
     if (!e) return fail("null engine");
     if (type < 0 || type >= PBD_NUM_TYPES) return fail("pbd_add_constraints: unknown constraint type %d", type);
     if (count && (!bodies || !params)) return fail("pbd_add_constraints: null arrays");
     const TypeShape s = type_shape(type);
-    const long long badAt = bad_body_index(e, type, bodies, count);
+    const long long badAt = pbd_b200::bad_body_index(type, bodies, count, e->n, e->nRb);
     if (badAt >= 0) {
         if (is_rb_body(type, (int)(badAt % s.nBodies))) return fail("pbd_add_constraints: rigid-body index %u out of range (%u bodies; call pbd_set_rigid_bodies first)", bodies[badAt], e->nRb);
         return fail("pbd_add_constraints: particle index %u out of range (n=%u)", bodies[badAt], e->n);
     }
-    HostType &h = e->host[type];
+    TypeStore &h = e->host[type];
     {
         const size_t b0 = h.ids.size();
         h.ids.resize(b0 + count); h.bodies.resize((b0 + count) * s.nBodies); h.params.resize((b0 + count) * s.nParams);  // uninitialised, filled below
@@ -443,29 +402,6 @@ extern "C" int pbd_add_constraints(pbd_engine *e, int type, unsigned count, cons
     e->groupsSet = false;  // any add invalidates the groups (SimulationModel: m_groupsInitialized = false)
     e->imageDirty = true; e->autoNoResident = false;
     return 0;
-}
-
-// insertion id -> (type, local index); verifies that the ids form a permutation of 0..N-1
-static int build_id_map(pbd_engine *e, std::vector<std::pair<int, unsigned>> &map) {
-    const unsigned N = e->numConstraints;
-    map.resize(N);
-    std::vector<int> &seenType = e->scratchInt; seenType.resize(N);
-    #pragma omp parallel for schedule(static) num_threads(host_threads())
-    for (long long i = 0; i < (long long)N; i++) seenType[i] = -1;
-    for (int t = 0; t < PBD_NUM_TYPES; t++) {
-        const HostType &h = e->host[t];
-        long long bad = -1; int dup = 0;
-        #pragma omp parallel for schedule(static) num_threads(host_threads()) reduction(max : bad) reduction(| : dup) if (h.ids.size() > 50000)
-        for (long long i = 0; i < (long long)h.ids.size(); i++) {
-            const unsigned id = h.ids[i];
-            if (id >= N) { bad = std::max(bad, (long long)id); continue; }
-            if (__atomic_exchange_n(&seenType[id], t, __ATOMIC_RELAXED) != -1) { dup = 1; bad = std::max(bad, (long long)id); continue; }
-            map[id] = std::make_pair(t, (unsigned)i);
-        }
-        if (bad >= 0 && !dup) return fail("constraint id %u out of range (N=%u)", (unsigned)bad, N);
-        if (dup) return fail("constraint id %u used twice", (unsigned)bad);
-    }
-    return 0;  // N ids, all below N, none twice: a permutation
 }
 
 extern "C" int pbd_set_groups(pbd_engine *e, unsigned nGroups, const unsigned *offsets, const unsigned *ids) {
@@ -492,7 +428,8 @@ extern "C" int pbd_set_groups(pbd_engine *e, unsigned nGroups, const unsigned *o
 // insertion-ordered CSR of the constraint bodies (the colouring's input)
 static int build_id_csr(pbd_engine *e, std::vector<unsigned> &off, std::vector<unsigned> &bodies) {
     std::vector<std::pair<int, unsigned>> map;
-    CKE(build_id_map(e, map));
+    const std::string err = pbd_b200::build_id_map(e->host, e->numConstraints, map);
+    if (!err.empty()) return fail("%s", err.c_str());
     const unsigned N = e->numConstraints;
     off.resize((size_t)N + 1);
     // off = exclusive prefix sum of the body counts (chunked two-pass scan), then every constraint copies its bodies
@@ -582,7 +519,6 @@ extern "C" int pbd_color_first_fit_device(pbd_engine *e, float *ms, unsigned *wa
     struct View { void *p = nullptr; };
     View dOff, dBody, dBody4, dNext4, dKeys, dVals, dKeysS, dValsS, dIndeg, dColour, dA, dB, dCnt, dTmp;
     DevBuf dAll, dUsed;
-    struct Release { std::vector<DevBuf *> b; ~Release() { for (auto *x : b) x->release(); } } rel{{&dAll, &dUsed}};
     {
         struct Want { View *v; size_t bytes; } want[] = {{&dOff, ((size_t)N + 1) * sizeof(unsigned)}, {&dBody, (size_t)M * sizeof(unsigned)}, {&dKeys, (size_t)M * sizeof(unsigned)},
             {&dVals, (size_t)M * sizeof(unsigned)}, {&dKeysS, (size_t)M * sizeof(unsigned)}, {&dValsS, (size_t)M * sizeof(unsigned)}, {&dBody4, (size_t)N * sizeof(uint4)},
@@ -681,90 +617,17 @@ extern "C" int pbd_get_mode(pbd_engine *e, int *requested, int *active) {
     if (active) *active = e->active;
     return 0;
 }
-extern "C" int pbd_set_bucket_sort(pbd_engine *e, int enable) {
-    if (!e) return fail("null engine");
-    e->sortBuckets = enable != 0; e->imageDirty = true;
-    return 0;
-}
 
 // ------------------------------------------------------------------------------------------------------------
-// flattening: constraints + colour groups -> per-type SoA arrays ordered bucket by bucket
+// the device image: planned on the host (host/image_plan.cpp), uploaded here
 // ------------------------------------------------------------------------------------------------------------
-// Q (row-major 4x4, solver order) = -Kp Kp^T ?  Returns true and Kp when the rank-one negative-semidefinite form of
-// init_IsometricBendingConstraint (PositionBasedDynamics.cpp:169-180) reproduces Q to fp32 accuracy.
-static bool factor_rank1(const float *Q, float Kp[4]) {
-    int piv = 0; float best = 0.0f, maxAbs = 0.0f;
-    for (int j = 0; j < 4; j++) { if (-Q[5 * j] > best) { best = -Q[5 * j]; piv = j; } }
-    for (int i = 0; i < 16; i++) maxAbs = std::max(maxAbs, std::fabs(Q[i]));
-    if (maxAbs == 0.0f) { Kp[0] = Kp[1] = Kp[2] = Kp[3] = 0.0f; return true; }
-    if (!(best > 0.0f)) return false;
-    const double kp = std::sqrt((double)best);
-    double K[4];
-    for (int k = 0; k < 4; k++) K[k] = -(double)Q[4 * piv + k] / kp;
-    for (int j = 0; j < 4; j++)
-        for (int k = 0; k < 4; k++)
-            if (std::fabs((double)Q[4 * j + k] + K[j] * K[k]) > 1e-5 * (double)maxAbs) return false;
-    for (int k = 0; k < 4; k++) Kp[k] = (float)K[k];
-    return true;
-}
-
-
-// Resident mode (resident.cuh): the particles are partitioned into G cluster regions x C tiles by recursive coordinate
-// bisection of the rest positions; the device arrays are permuted to tile-major order.
-static void bisect(std::vector<unsigned> &idx, size_t lo, size_t hi, unsigned t0, unsigned nt, const std::vector<float4> &x, std::vector<unsigned> &tileOf) {
-    if (nt == 1) { for (size_t i = lo; i < hi; i++) tileOf[idx[i]] = t0; return; }
-    float mn[3] = {3.4e38f, 3.4e38f, 3.4e38f}, mx[3] = {-3.4e38f, -3.4e38f, -3.4e38f};
-    for (size_t i = lo; i < hi; i++) {
-        const float4 &p = x[idx[i]];
-        const float c[3] = {p.x, p.y, p.z};
-        for (int k = 0; k < 3; k++) { mn[k] = std::min(mn[k], c[k]); mx[k] = std::max(mx[k], c[k]); }
-    }
-    int ax = 0;
-    for (int k = 1; k < 3; k++) if (mx[k] - mn[k] > mx[ax] - mn[ax]) ax = k;
-    const unsigned ntL = nt / 2;
-    const size_t mid = lo + (size_t)((double)(hi - lo) * ntL / nt);
-    auto key = [&](unsigned i) { const float4 &p = x[i]; return ax == 0 ? p.x : (ax == 1 ? p.y : p.z); };
-    std::nth_element(idx.begin() + lo, idx.begin() + mid, idx.begin() + hi, [&](unsigned a, unsigned b) { const float ka = key(a), kb = key(b); return ka < kb || (ka == kb && a < b); });
-    // the two halves are independent: run them as tasks while they are big enough to pay for it
-    #pragma omp task shared(idx, x, tileOf) if (hi - lo > 65536)
-    bisect(idx, lo, mid, t0, ntL, x, tileOf);
-    bisect(idx, mid, hi, t0 + ntL, nt - ntL, x, tileOf);
-    #pragma omp taskwait
-}
-
-struct ResidentPlan {
-    std::vector<unsigned> tileOf;             // host particle -> tile (cluster = tile / C, rank = tile % C)
-    std::vector<unsigned> tileStart, tileSmem;
-    std::vector<unsigned char> homedGlobal;   // host particle lives in global memory (touched by a constraint that spans clusters)
-};
-
-// Executing tile of a constraint: the tile that holds most of its shared-memory particles (ties: the lowest tile); none -> the tile of
-// its first particle (0 for a joint between rigid bodies).  *touchesGlobal: one of its particles is global-homed.
-static inline unsigned exec_tile(int t, const unsigned *b, int nb, const std::vector<unsigned> &tileOf, const std::vector<unsigned char> &homedGlobal, bool *touchesGlobal) {
-    bool x = false;
-    unsigned best = 0xffffffffu, bestCnt = 0, first = 0xffffffffu;
-    for (int k = 0; k < nb; k++) {
-        if (is_rb_body(t, k)) continue;
-        if (first == 0xffffffffu) first = tileOf[b[k]];
-        if (homedGlobal[b[k]]) { x = true; continue; }
-        unsigned cnt = 0;
-        for (int j = 0; j < nb; j++) cnt += (!is_rb_body(t, j) && !homedGlobal[b[j]] && tileOf[b[j]] == tileOf[b[k]]);
-        if (cnt > bestCnt || (cnt == bestCnt && tileOf[b[k]] < best)) { best = tileOf[b[k]]; bestCnt = cnt; }
-    }
-    *touchesGlobal = x;
-    return (best != 0xffffffffu) ? best : (first != 0xffffffffu ? first : 0u);
-}
-
-// Block size of the resident instantiation of a type mask: the largest it compiles for without spilling (cloth 96 registers,
-// light 128, everything 236).
-constexpr unsigned resident_threads(unsigned mask) { return mask == kMaskClothXPBD ? 640u : (mask == kMaskAll ? 256u : 512u); }
 template <unsigned M, class F> static int resident_kernel(bool single, F &&f) {
     return single ? f(k_step_resident<M, resident_threads(M), true>) : f(k_step_resident<M, resident_threads(M), false>);
 }
-// the compiled instantiations of k_step_resident: F(kernel pointer) for the engine's type mask, one CTA per cluster or not
-template <class F> static int with_resident_kernel(const pbd_engine *e, unsigned C, F &&f) {
+// the compiled instantiations of k_step_resident: F(kernel pointer) for a type mask, one CTA per cluster or not
+template <class F> static int with_resident_kernel(unsigned mask, unsigned C, F &&f) {
     const bool single = (C == 1);
-    switch (e->resMask) {
+    switch (mask) {
     case kMaskClothXPBD: return resident_kernel<kMaskClothXPBD>(single, f);
     case kMaskCloth: return resident_kernel<kMaskCloth>(single, f);
     case kMaskLight: return resident_kernel<kMaskLight>(single, f);
@@ -774,155 +637,26 @@ template <class F> static int with_resident_kernel(const pbd_engine *e, unsigned
     }
 }
 
-static void resident_launch_config(const pbd_engine *e, unsigned C, unsigned grid, size_t smem, cudaStream_t s, cudaLaunchConfig_t &cfg, cudaLaunchAttribute *attr) {
+static void resident_launch_config(unsigned mask, unsigned C, unsigned grid, size_t smem, cudaStream_t s, cudaLaunchConfig_t &cfg, cudaLaunchAttribute *attr) {
     cfg = cudaLaunchConfig_t{};
-    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(e->resThreads); cfg.dynamicSmemBytes = smem; cfg.stream = s;
+    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(resident_threads(mask)); cfg.dynamicSmemBytes = smem; cfg.stream = s;
     attr[0].id = cudaLaunchAttributeClusterDimension;
     attr[0].val.clusterDim.x = C; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr; cfg.numAttrs = 1;
 }
 
-// how many clusters of C CTAs (one CTA per SM, `smem` bytes each) the device keeps resident at the same time
-static int resident_max_clusters(const pbd_engine *e, unsigned C, size_t smem, int *out) {
-    return with_resident_kernel(e, C, [&](auto kernel) -> int {
+// how many clusters of C CTAs (one CTA per SM, `smem` bytes each) of the instantiation for `mask` the device keeps resident at the same time
+static int resident_max_clusters(const pbd_engine *e, unsigned mask, unsigned C, size_t smem, int *out) {
+    return with_resident_kernel(mask, C, [&](auto kernel) -> int {
         CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynamicSmem));
         CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
         cudaLaunchConfig_t cfg; cudaLaunchAttribute attr[1];
-        resident_launch_config(e, C, C, smem, e->stream, cfg, attr);
+        resident_launch_config(mask, C, C, smem, e->stream, cfg, attr);
         cudaError_t err = cudaOccupancyMaxActiveClusters(out, kernel, &cfg);
         if (err != cudaSuccess) { cudaGetLastError(); *out = 0; }
         return 0;
     });
 }
-
-// shape of the launch: type mask / block size of the instantiation, clusters x CTAs per cluster
-static int choose_resident_shape(pbd_engine *e) {
-    unsigned present = 0, nTypes = 0;
-    for (int t = 0; t < PBD_NUM_TYPES; t++) if (!e->host[t].ids.empty()) { present |= 1u << t; nTypes++; }
-    e->resMask = kMaskAll;
-    for (unsigned m : {kMaskClothXPBD, kMaskCloth, kMaskFem, kMaskLight, kMaskSolid})  // the leanest instantiation that covers the model
-        if ((present & ~m) == 0) { e->resMask = m; break; }
-    e->resThreads = resident_threads(e->resMask);
-    const unsigned nGroups = (unsigned)std::max<size_t>(e->groupOff.size(), 2) - 1;
-    const unsigned perPhase = e->numConstraints / std::max(1u, nGroups);
-    // particles a tile can hold: what is left of the CTA's shared memory after the phase tables (bound: one bucket per colour and type)
-    const size_t tables = resident_smem_bytes(0u, nGroups * std::max(1u, nTypes), nGroups);
-    if (tables + 1024 * sizeof(float4) > kMaxDynamicSmem) return fail("resident mode: %u colour groups need %zu bytes of phase tables (use PBD_MODE_GRAPH)", nGroups, tables);
-    const unsigned cap = (unsigned)(0.97 * (double)((kMaxDynamicSmem - tables) / sizeof(float4)));  // bisection splits counts evenly; slack for rounding
-    unsigned G = 1, C = 1;
-    if (e->n <= (unsigned)kMaxClusterCtas * cap && perPhase <= (unsigned)kMaxClusterCtas * 1024u) {
-        // one cluster: enough CTAs that a colour phase is about one item per thread, and that the tiles fit
-        while (C < (unsigned)kMaxClusterCtas && (perPhase > C * 256u || e->n > C * cap)) C *= 2;
-    } else {
-        // Too big for one cluster: one independent CTA per SM (clusters of 1).  Larger clusters have fewer X items but idle SMs (a
-        // cluster must fit a GPC) and a colour barrier that waits for the slowest of C CTAs; with C = 1 the colour barrier is a
-        // __syncthreads.
-        int mc = 0;
-        CKE(resident_max_clusters(e, 1u, kMaxDynamicSmem, &mc));
-        if (mc < 1) return fail("resident mode: a CTA with %zu bytes of shared memory is not schedulable on this device", kMaxDynamicSmem);
-        C = 1; G = (unsigned)std::min(mc, e->smCount);
-    }
-    if (const char *g = getenv("PBD_B200_CLUSTERS")) {  // development knob "GxC"
-        unsigned gg = 0, cc = 0;
-        if (sscanf(g, "%ux%u", &gg, &cc) == 2 && gg >= 1 && cc >= 1 && cc <= (unsigned)kMaxClusterCtas && (cc & (cc - 1)) == 0) { G = gg; C = cc; }
-    }
-    if ((unsigned long long)G * C * cap < e->n)
-        return fail("resident mode: %u particles do not fit %u x %u tiles of %u (use PBD_MODE_GRAPH)", e->n, G, C, cap);
-    // (bodies without joints -- e.g. the static colliders of the contact path -- are integrated by CTA 0 and touch no constraint)
-    if (G > 1 && (!e->host[PBD_BALLJOINT].ids.empty() || !e->host[PBD_RB_PARTICLE_BALLJOINT].ids.empty()))
-        return fail("resident mode: rigid-body coupling is supported for scenes that fit one cluster (use PBD_MODE_GRAPH)");
-    e->resG = G; e->resC = C; e->nTiles = G * C;
-    e->resXThreads = (G > 1) ? 128u : 0u;  // refined in prepare_resident once the share of X items is known
-    return 0;
-}
-
-static int prepare_resident(pbd_engine *e, ResidentPlan &pl) {
-    CKE(choose_resident_shape(e));
-    const unsigned n = e->n, G = e->resG, C = e->resC, T = e->nTiles;
-    pl.tileOf.assign(n, 0); pl.homedGlobal.assign(n, 0); pl.tileStart.assign(T + 1, 0); pl.tileSmem.assign(T, 0);
-    if (n) {
-        // rest positions by host index
-        std::vector<float4> raw(n), x(n);
-        CK(cudaStreamSynchronize(e->stream));
-        CK(cudaMemcpy(raw.data(), e->pos0.p, (size_t)n * sizeof(float4), cudaMemcpyDeviceToHost));
-        for (unsigned i = 0; i < n; i++) x[i] = raw[e->slot[i]];
-        std::vector<unsigned> idx(n), region(n);
-        for (unsigned i = 0; i < n; i++) idx[i] = i;
-        #pragma omp parallel num_threads(host_threads())
-        #pragma omp single
-        bisect(idx, 0, n, 0, G, x, region);  // cluster regions; idx is now grouped region by region
-        size_t lo = 0;
-        for (unsigned g = 0; g < G; g++) {
-            size_t hi = lo;
-            while (hi < n && region[idx[hi]] == g) hi++;
-            if (C == 1) { for (size_t i = lo; i < hi; i++) pl.tileOf[idx[i]] = g; }
-            else {
-                #pragma omp parallel num_threads(host_threads())
-                #pragma omp single
-                bisect(idx, lo, hi, g * C, C, x, pl.tileOf);
-            }
-            lo = hi;
-        }
-        // global-homed = touched by a constraint whose particles lie in more than one cluster
-        if (G > 1)
-            for (int t = 0; t < PBD_NUM_TYPES; t++) {
-                const HostType &h = e->host[t];
-                const int nb = type_shape(t).nBodies;
-                unsigned char *hg = pl.homedGlobal.data();
-                #pragma omp parallel for schedule(static) num_threads(host_threads())
-                for (long long c = 0; c < (long long)h.ids.size(); c++) {
-                    const unsigned *b = &h.bodies[(size_t)c * nb];
-                    bool spans = false;
-                    for (int k = 1; k < nb; k++) spans |= (pl.tileOf[b[k]] / C != pl.tileOf[b[0]] / C);
-                    if (spans) for (int k = 0; k < nb; k++) hg[b[k]] = 1;  // every writer stores the same byte
-                }
-            }
-        // threads of a CTA dedicated to the X items: in proportion to their share, times 3.1 because an X item waits for L2 where
-        // the others read shared memory.  The factor is carried over from an earlier GPU; on an H100 80GB HBM3 (400 W) cfg2 is flat in
-        // it: 160 / 192 / 224 / 256 X threads -> 2.07 / 2.05 / 2.09 / 2.11 ms, within the run-to-run spread.
-        if (G > 1) {
-            unsigned long long xItems = 0;
-            for (int t = 0; t < PBD_NUM_TYPES; t++) {
-                const HostType &h = e->host[t];
-                const int nb = type_shape(t).nBodies;
-                #pragma omp parallel for schedule(static) num_threads(host_threads()) reduction(+ : xItems)
-                for (long long c = 0; c < (long long)h.ids.size(); c++) {
-                    bool x = false;
-                    for (int k = 0; k < nb; k++) x |= (!is_rb_body(t, k) && pl.homedGlobal[h.bodies[(size_t)c * nb + k]]);
-                    xItems += x;
-                }
-            }
-            const double share = (double)xItems / std::max(1u, e->numConstraints);
-            unsigned xt = ((unsigned)(e->resThreads * share * 3.1) + 31u) & ~31u;
-            e->resXThreads = std::max(64u, std::min(xt, (e->resThreads / 2u) & ~31u));
-        }
-        // tile-major slots: shared-memory particles first (host order), global-homed behind them
-        std::vector<unsigned> cntS(T, 0), cntG(T, 0);
-        for (unsigned i = 0; i < n; i++) (pl.homedGlobal[i] ? cntG : cntS)[pl.tileOf[i]]++;
-        for (unsigned t = 0; t < T; t++) {
-            pl.tileStart[t + 1] = pl.tileStart[t] + cntS[t] + cntG[t];
-            pl.tileSmem[t] = cntS[t];
-        }
-        std::vector<unsigned> curS(T), curG(T), newSlot(n);
-        for (unsigned t = 0; t < T; t++) { curS[t] = pl.tileStart[t]; curG[t] = pl.tileStart[t] + cntS[t]; }
-        for (unsigned i = 0; i < n; i++) newSlot[i] = pl.homedGlobal[i] ? curG[pl.tileOf[i]]++ : curS[pl.tileOf[i]]++;
-        CKE(relayout(e, newSlot));
-        if (verbose()) {
-            unsigned long long nGl = 0;
-            for (unsigned i = 0; i < n; i++) nGl += pl.homedGlobal[i];
-            fprintf(stderr, "[pbd_b200] resident: %u clusters x %u CTAs, %u threads (%u for X items), %u particles, %.2f %% global-homed, max tile %u\n", G, C, e->resThreads, e->resXThreads, n,
-                    100.0 * nGl / n, *std::max_element(cntS.begin(), cntS.end()));
-        }
-    }
-    e->slotIsTiled = true;
-    e->resTileCap = 64u;  // multiple of 64: the bank swizzle permutes inside aligned 64-slot blocks
-    for (unsigned t = 0; t < T; t++) e->resTileCap = std::max(e->resTileCap, (pl.tileSmem[t] + 63u) & ~63u);
-    e->resChecked = false;
-    CKE(upload_vec(e->dTileStart, pl.tileStart, e->stream));
-    CKE(upload_vec(e->dTileSmem, pl.tileSmem, e->stream));
-    return 0;
-}
-
 static int flatten_image(pbd_engine *e);
 // PBD_MODE_AUTO: the resident mode where it is the faster exact mode -- models made of cloth and FEM / volume constraints with at
 // least kAutoResidentMinParticles particles (cfg2, cfg3, cfg5); small models (cfg1), mixed models with rigid coupling and the heavy
@@ -948,17 +682,6 @@ static int flatten(pbd_engine *e) {
     }
     return rc;
 }
-// ---- the stages of flatten_image -----------------------------------------------------------------------------------------------
-// stage timings on stderr (PBD_B200_VERBOSE)
-struct Lap {
-    double prev = omp_get_wtime();
-    void operator()(const char *what) {
-        if (!verbose()) return;
-        const double t = omp_get_wtime();
-        fprintf(stderr, "[pbd_b200] flatten: %-34s %.3f s\n", what, t - prev);
-        prev = t;
-    }
-};
 
 // colour groups when none were given: the reference-order-preserving first fit on the GPU (colouring.cuh), the host version as the fallback
 static int colour_if_needed(pbd_engine *e) {
@@ -968,461 +691,80 @@ static int colour_if_needed(pbd_engine *e) {
     return 0;
 }
 
-// the particle / rigid-body counts may have shrunk since the constraints were added (pbd_set_particles, pbd_set_rigid_bodies)
-static int validate_bodies(const pbd_engine *e) {
-    for (int t = 0; t < PBD_NUM_TYPES; t++) {
-        const HostType &h = e->host[t];
-        const long long badAt = bad_body_index(e, t, h.bodies.data(), h.ids.size());
-        if (badAt < 0) continue;
-        const bool isRb = is_rb_body(t, (int)(badAt % type_shape(t).nBodies));
-        return fail("constraint of type %d refers to %s %u, but the engine holds %u: re-add the constraints after shrinking the model", t,
-                    isRb ? "rigid body" : "particle", h.bodies[badAt], isRb ? e->nRb : e->n);
-    }
-    return 0;
-}
-
-// particle placement: tile-major for the resident mode, the formula layout otherwise
-static int place_particles(pbd_engine *e, bool tiled, ResidentPlan &pl) {
-    if (tiled) return prepare_resident(e, pl);
-    if (e->slotIsTiled) {
-        std::vector<unsigned> m;
-        formula_slot_map(e, m);
-        CKE(relayout(e, m));
-        e->slotIsTiled = false;
-    }
-    return 0;
-}
-
-typedef std::pair<unsigned long long, unsigned> KeyedItem;  // (sort key, local host index of the constraint)
-struct Wavefronts { double before = 0, after = 0, requests = 0; };
-
-// Shared-memory bank groups of one run of a resident tile.  The eight lanes of a quarter-warp (eight consecutive items of the run) read
-// operand k of their items with one LDS.128; it takes as many wavefronts as the fullest 16-byte bank group (slot & 7 after the swizzle).
-// Greedy re-ordering: each group of eight is filled with the items, out of the next `kWindow` unused ones, that add the fewest
-// collisions over all operands.  The order inside a colour is free; results are bit-identical.  H100 80GB HBM3 (400 W), without / with
-// the fill: cfg2 2.14 / 2.08 ms, cfg5 1.221 / 1.216 ms, cfg3 7.81 / 7.69 ms (bank group taken inside the CTA that holds the particle).
-// With `wf`: the wavefronts of the run's quarter-warp gathers before and after, and their number.
-static void bank_group_fill(KeyedItem *run, size_t cnt, int t, const pbd_engine *e, const ResidentPlan &pl, Wavefronts *wf) {
-    constexpr int kWindow = 64;
-    const int nb = type_shape(t).nBodies, nk = std::min(nb, 4);
-    const unsigned *bod = e->host[t].bodies.data();
-    std::vector<unsigned char> bg(cnt * 4, 0);
-    for (size_t i = 0; i < cnt; i++) {
-        const unsigned *b = bod + (size_t)run[i].second * nb;
-        for (int k = 0; k < nk; k++) bg[i * 4 + k] = (unsigned char)(tile_swizzle(e->slot[b[k]] - pl.tileStart[pl.tileOf[b[k]]]) & 7u);  // bank group inside the CTA that holds the particle
-    }
-    // greedy fill from a sliding pool of the next kWindow unused items (kept in run order)
-    std::vector<unsigned> out; out.reserve(cnt);
-    unsigned pool[kWindow]; int nPool = 0; size_t head = 0;
-    while (out.size() < cnt) {
-        unsigned char load[4][8] = {};
-        for (int j = 0; j < 8 && out.size() < cnt; j++) {
-            while (nPool < kWindow && head < cnt) pool[nPool++] = (unsigned)head++;
-            int best = 0, bestCost = 1 << 30;
-            for (int c = 0; c < nPool; c++) {
-                const unsigned char *g4 = &bg[(size_t)pool[c] * 4];
-                int cost = 0;
-                for (int k = 0; k < nk; k++) cost += load[k][g4[k]];
-                if (cost < bestCost) { bestCost = cost; best = c; if (!cost) break; }
-            }
-            const unsigned pick = pool[best];
-            for (int c = best; c + 1 < nPool; c++) pool[c] = pool[c + 1];
-            nPool--;
-            out.push_back(pick);
-            for (int k = 0; k < nk; k++) load[k][bg[(size_t)pick * 4 + k]]++;
-        }
-    }
-    if (wf) {
-        auto wavefronts = [&](const std::vector<unsigned> &ord) {
-            double w = 0;
-            for (size_t g8 = 0; g8 + 8 <= cnt; g8 += 8)
-                for (int k = 0; k < nk; k++) {
-                    unsigned char c8[8] = {0, 0, 0, 0, 0, 0, 0, 0}; unsigned mx = 0;
-                    for (int j = 0; j < 8; j++) mx = std::max<unsigned>(mx, ++c8[bg[ord[g8 + j] * 4 + k]]);
-                    w += mx;
-                }
-            return w;
-        };
-        std::vector<unsigned> asSorted(cnt);
-        std::iota(asSorted.begin(), asSorted.end(), 0u);
-        wf->before += wavefronts(asSorted); wf->after += wavefronts(out); wf->requests += (double)(cnt / 8) * nk;
-    }
-    const std::vector<KeyedItem> sorted(run, run + cnt);
-    for (size_t i = 0; i < cnt; i++) run[i] = sorted[out[i]];
-}
-
-// The items (local host indices) of the bucket (colour g, type t), re-ordered.  The order inside a colour is free: sorted by lowest
-// particle slot for gather locality (joints keep their order); resident: major key = executing tile, then the X items (touching a
-// global-homed particle) before the others, the shared-memory runs bank-group filled, and the runs of every tile appended to tileOff:
-// [2 tile] X items, [2 tile + 1] the others.
-static void sort_bucket(const pbd_engine *e, unsigned g, int t, std::vector<unsigned> &items, bool tiled, const ResidentPlan &pl, std::vector<unsigned> &tileOff) {
-    const bool joint = (t == PBD_BALLJOINT || t == PBD_RB_PARTICLE_BALLJOINT);
-    const int nb = type_shape(t).nBodies;
-    const unsigned *bod = e->host[t].bodies.data();
-    std::vector<KeyedItem> keyed(items.size());
-    #pragma omp parallel for schedule(static) num_threads(host_threads())
-    for (long long i = 0; i < (long long)items.size(); i++) {
-        const unsigned *b = bod + (size_t)items[i] * nb;
-        unsigned mn = 0xffffffffu;
-        for (int k = 0; k < nb; k++) if (!is_rb_body(t, k)) mn = std::min(mn, e->slot[b[k]]);
-        if (joint) mn = (unsigned)i;
-        // resident: run = executing tile and kind (X items first) in key bits 51 and up.  Ordering a run by kind of element as well
-        // (constraints with the same slot offsets between their particles first) made no difference on an H100 80GB HBM3 (700 W):
-        // cfg3 7.66 / 7.62 ms, cfg4 0.625 / 0.625 ms with / without.
-        unsigned long long run = 0;
-        if (tiled) {
-            bool x = false;
-            const unsigned exec = exec_tile(t, b, nb, pl.tileOf, pl.homedGlobal, &x);
-            run = 2ull * exec + (x ? 0u : 1u);
-        }
-        keyed[i] = std::make_pair((run << 51) | mn, items[i]);
-    }
-    __gnu_parallel::stable_sort(keyed.begin(), keyed.end(), [](const KeyedItem &a, const KeyedItem &b) { return a.first < b.first; },
-                                __gnu_parallel::default_parallel_tag(host_threads()));
-    if (tiled && !joint) {
-        std::vector<size_t> runStart;
-        for (size_t i = 0; i < keyed.size(); i++) if (i == 0 || (keyed[i].first >> 51) != (keyed[i - 1].first >> 51)) runStart.push_back(i);
-        runStart.push_back(keyed.size());
-        double before = 0, after = 0, requests = 0;
-        const long long nRuns = (long long)runStart.size() - 1;
-        #pragma omp parallel for schedule(dynamic, 1) num_threads(host_threads()) reduction(+ : before, after, requests)
-        for (long long r = 0; r < nRuns; r++) {
-            const size_t lo = runStart[r], cnt = runStart[r + 1] - lo;
-            if (!((keyed[lo].first >> 51) & 1ull) || cnt < 16) continue;  // X runs gather from global memory: left alone
-            Wavefronts w;
-            bank_group_fill(&keyed[lo], cnt, t, e, pl, verbose() ? &w : nullptr);
-            before += w.before; after += w.after; requests += w.requests;
-        }
-        if (verbose() && requests > 0) fprintf(stderr, "[pbd_b200] flatten:   colour %u type %d: %.2f wavefronts per quarter-warp gather as sorted, %.2f after the bank-group fill\n", g, t,
-                                               before / requests, after / requests);
-    }
-    #pragma omp parallel for schedule(static) num_threads(host_threads())
-    for (long long i = 0; i < (long long)keyed.size(); i++) items[i] = keyed[i].second;
-    if (tiled) {
-        const size_t base = tileOff.size();
-        tileOff.resize(base + 2 * e->nTiles + 1, 0u);
-        for (size_t i = 0; i < keyed.size(); i++) tileOff[base + (keyed[i].first >> 51) + 1]++;
-        for (unsigned k = 0; k < 2 * e->nTiles; k++) tileOff[base + k + 1] += tileOff[base + k];
-    }
-}
-
-// every colour group split by type into (colour, type) buckets; order[t]: device position -> local host index
-static void order_buckets(pbd_engine *e, const std::vector<std::pair<int, unsigned>> &map, bool tiled, const ResidentPlan &pl,
-                          std::vector<unsigned> (&order)[PBD_NUM_TYPES], std::vector<unsigned> &tileOff) {
-    const unsigned nGroups = (unsigned)e->groupOff.size() - 1;
-    e->buckets.clear();
-    std::vector<unsigned> items[PBD_NUM_TYPES];
-    for (unsigned g = 0; g < nGroups; g++) {
-        for (auto &v : items) v.clear();
-        for (unsigned i = e->groupOff[g]; i < e->groupOff[g + 1]; i++) {
-            const auto &m = map[e->groupIds[i]];
-            items[m.first].push_back(m.second);
-        }
-        for (int t = 0; t < PBD_NUM_TYPES; t++) {
-            if (items[t].empty()) continue;
-            const bool joint = (t == PBD_BALLJOINT || t == PBD_RB_PARTICLE_BALLJOINT);
-            if ((e->sortBuckets && !joint) || tiled) sort_bucket(e, g, t, items[t], tiled, pl, tileOff);
-            Bucket b; b.type = t; b.first = (unsigned)order[t].size(); b.count = (unsigned)items[t].size(); b.colour = g;
-            e->buckets.push_back(b);
-            order[t].insert(order[t].end(), items[t].begin(), items[t].end());
-        }
-    }
-}
-
-// Debug-grade safety: inside a colour no particle may be used twice (race freedom by construction, SURVEY.md section 5).  Particles
-// and rigid bodies are stamped in separate index spaces (the reference's colouring shares one, which only ever over-separates; a body
-// really used twice in a colour would be a race here).
-static int check_colouring(const pbd_engine *e, const std::vector<unsigned> (&order)[PBD_NUM_TYPES]) {
-    std::vector<unsigned> stamp((size_t)e->n + e->nRb, 0xffffffffu);
-    for (const Bucket &b : e->buckets) {  // colour after colour
-        const unsigned g = b.colour;
-        const int nb = type_shape(b.type).nBodies;
-        long long bad = -1;  // items of a bucket in parallel: the stamp of a slot is exchanged atomically
-        #pragma omp parallel for schedule(static) num_threads(host_threads()) reduction(max : bad) if (b.count > 20000)
-        for (long long i = 0; i < (long long)b.count; i++) {
-            const unsigned *bd = &e->host[b.type].bodies[(size_t)order[b.type][b.first + i] * nb];
-            for (int k = 0; k < nb; k++) {
-                const size_t slot = is_rb_body(b.type, k) ? (size_t)e->n + bd[k] : bd[k];
-                if (__atomic_exchange_n(&stamp[slot], g, __ATOMIC_RELAXED) == g) bad = std::max(bad, (long long)slot);
-            }
-        }
-        if (bad >= 0) {
-            const bool isRb = (size_t)bad >= e->n;
-            return fail("colour group %u uses %s %u twice: the groups are not a valid colouring", g, isRb ? "rigid body" : "particle", (unsigned)(isRb ? bad - e->n : bad));
-        }
-    }
-    return 0;
-}
-
-// Parameter columns (include/pbd_b200.h) of a type's SoA arrays: float4 geometry array k = columns gv[k][0..3], scalar geometry
-// array k = column gs[k], material slot k = column mat[k]; -1 = zero-filled component, or no such array / slot.
-struct PackColumns { signed char gv[kMaxGeoV][4], gs[kMaxGeoS], mat[kMaxMat]; };
-static PackColumns pack_columns(int t) {
-    PackColumns p;
-    memset(&p, -1, sizeof(p));
-    auto gv = [&](int k, int c0, int c1, int c2, int c3) { p.gv[k][0] = c0; p.gv[k][1] = c1; p.gv[k][2] = c2; p.gv[k][3] = c3; };
-    auto mat = [&](int first, int count) { for (int k = 0; k < count; k++) p.mat[k] = first + k; };
-    switch (t) {
-    case PBD_DISTANCE: case PBD_DISTANCE_XPBD: case PBD_DIHEDRAL: case PBD_VOLUME: case PBD_VOLUME_XPBD: p.gs[0] = 0; mat(1, 1); break;
-    case PBD_ISOBENDING: case PBD_ISOBENDING_XPBD: for (int r = 0; r < 4; r++) gv(r, 1 + 4 * r, 2 + 4 * r, 3 + 4 * r, 4 + 4 * r); mat(0, 1); break;  // full Q (see pack_type)
-    case PBD_FEMTRIANGLE: p.gs[0] = 0; gv(0, 1, 2, 3, 4); mat(5, 5); break;
-    case PBD_STRAINTRIANGLE: gv(0, 0, 1, 2, 3); mat(4, 5); break;
-    case PBD_FEMTET: case PBD_FEMTET_XPBD: gv(0, 1, 2, 3, 4); gv(1, 5, 6, 7, 8); p.gs[0] = 9; p.gs[1] = 0; mat(10, 2); break;
-    case PBD_STRAINTET: gv(0, 0, 1, 2, 3); gv(1, 4, 5, 6, 7); p.gs[0] = 8; mat(9, 4); break;
-    // local connectors (jointInfo columns 0 [and 1]); the global columns are recomputed per solve
-    case PBD_BALLJOINT: gv(0, 0, 1, 2, -1); gv(1, 3, 4, 5, -1); break;
-    case PBD_RB_PARTICLE_BALLJOINT: gv(0, 0, 1, 2, -1); break;
-    // restCm | x0[0..3] packed in 3 float4 | w | numClusters ; stiffness is the material slot
-    case PBD_SHAPEMATCHING: gv(0, 1, 2, 3, -1); for (int k = 1; k < 6; k++) gv(k, 4 * k, 4 * k + 1, 4 * k + 2, 4 * k + 3); mat(0, 1); break;
-    }
-    return p;
-}
-
-// build and upload the SoA arrays of type t in device order (order: device position -> local host index)
-static int pack_type(pbd_engine *e, int t, const std::vector<unsigned> &order, bool tiled, const ResidentPlan &pl, Lap &lap) {
+// one type's planned arrays to the device, and its TypeArrays pointed at them
+static int upload_type(pbd_engine *e, int t, pbd_b200::TypePlan &p) {
     DevType &d = e->dev[t];
-    const HostType &h = e->host[t];
-    const TypeShape s = type_shape(t);
-    const unsigned cnt = (unsigned)order.size();
+    const unsigned cnt = (unsigned)p.order.size();
     d.count = cnt;
     e->stats.constraints_per_type[t] = cnt;
     d.arrays = TypeArrays{};
-    d.order.resize(cnt);
+    d.order.swap(p.order);
     if (cnt == 0) return 0;
-    #pragma omp parallel for schedule(static) num_threads(host_threads())
-    for (long long i = 0; i < (long long)cnt; i++) d.order[i] = h.ids[order[i]];
-    auto P = [&](unsigned i, int k) { return h.params[(size_t)order[i] * s.nParams + k]; };
-    auto B = [&](unsigned i, int k) {
-        const unsigned raw = h.bodies[(size_t)order[i] * s.nBodies + k];
-        if (is_rb_body(t, k)) return raw;
-        if (tiled && !pl.homedGlobal[raw]) {  // lives in the shared memory of CTA (tile % C) of the executing cluster
-            const unsigned tl = pl.tileOf[raw];
-            return kSmemFlag | ((tl % e->resC) << kRankShift) | tile_swizzle(e->slot[raw] - pl.tileStart[tl]);
-        }
-        return e->slot[raw];
-    };
-
-    if (verbose()) fprintf(stderr, "[pbd_b200] flatten:   type %d (%u constraints)\n", t, cnt);
-    lap("  order ids");
-    // indices
-    if (s.nBodies == 2) {
-        PodVector<uint2> v(cnt);
-        #pragma omp parallel for schedule(static) num_threads(host_threads())
-        for (long long i = 0; i < (long long)cnt; i++) v[i] = make_uint2(B(i, 0), B(i, 1));
-        CKE(upload_vec(d.idx[0], v, e->stream)); d.arrays.idx2 = (const uint2 *)d.idx[0].p;
-    } else if (s.nBodies == 4) {
-        PodVector<uint4> v(cnt);
-        #pragma omp parallel for schedule(static) num_threads(host_threads())
-        for (long long i = 0; i < (long long)cnt; i++) v[i] = make_uint4(B(i, 0), B(i, 1), B(i, 2), B(i, 3));
-        CKE(upload_vec(d.idx[0], v, e->stream)); d.arrays.idx4 = (const uint4 *)d.idx[0].p;
-    } else {
-        for (int k = 0; k < 3; k++) {
-            PodVector<unsigned> v(cnt);
-            #pragma omp parallel for schedule(static) num_threads(host_threads())
-            for (long long i = 0; i < (long long)cnt; i++) v[i] = B(i, k);
-            CKE(upload_vec(d.idx[k], v, e->stream)); d.arrays.idx3[k] = (const unsigned *)d.idx[k].p;
-        }
-    }
-
-    lap("  indices (remap + upload)");
-    // geometry: the parameter columns of the table, with two exceptions
-    const PackColumns pc = pack_columns(t);
-    PodVector<float4> gv[kMaxGeoV]; PodVector<float> gs[kMaxGeoS];
-    bool fromColumns = true;
-    if (t == PBD_ISOBENDING || t == PBD_ISOBENDING_XPBD) {
-        // the rank-one form Q = -Kp Kp^T of init_IsometricBendingConstraint: gv[0] = Kp; a user-modified Q anywhere in this type:
-        // the literal 4x4 evaluation (variant 1) for the whole type, Q row by row from the columns of the table
-        gv[0].resize(cnt);
-        int notRank1 = 0;
-        #pragma omp parallel for schedule(static) num_threads(host_threads()) reduction(| : notRank1)
-        for (long long i = 0; i < (long long)cnt; i++) {
-            float Q[16], Kp[4] = {0.f, 0.f, 0.f, 0.f};
-            for (int k = 0; k < 16; k++) Q[k] = P((unsigned)i, 1 + k);
-            if (!factor_rank1(Q, Kp)) notRank1 |= 1;
-            gv[0][i] = make_float4(Kp[0], Kp[1], Kp[2], Kp[3]);
-        }
-        if (notRank1 && tiled) return fail("resident mode: IsometricBending with a user-modified Q matrix (not of the rank-one form) is evaluated by the per-bucket kernels only (use PBD_MODE_GRAPH)");
-        d.arrays.variant = notRank1 ? 1 : 0;
-        fromColumns = notRank1 != 0;
-    }
-    if (t == PBD_SHAPEMATCHING)
-        for (unsigned i = 0; i < cnt; i++)
-            for (int k = 20; k < 24; k++) if (!(P(i, k) >= 1.0f)) return fail("ShapeMatching constraint: numClusters must be >= 1");
-    auto col = [&](unsigned i, int c) { return c < 0 ? 0.0f : P(i, c); };
-    for (int k = 0; k < kMaxGeoV && fromColumns; k++) {
-        const signed char *c = pc.gv[k];
-        if (c[0] < 0 && c[1] < 0 && c[2] < 0 && c[3] < 0) continue;
-        gv[k].resize(cnt);
-        #pragma omp parallel for schedule(static) num_threads(host_threads())
-        for (long long i = 0; i < (long long)cnt; i++) gv[k][i] = make_float4(col(i, c[0]), col(i, c[1]), col(i, c[2]), col(i, c[3]));
-    }
-    for (int k = 0; k < kMaxGeoS; k++) {
-        if (pc.gs[k] < 0) continue;
-        gs[k].resize(cnt);
-        #pragma omp parallel for schedule(static) num_threads(host_threads())
-        for (long long i = 0; i < (long long)cnt; i++) gs[k][i] = P(i, pc.gs[k]);
-    }
-    if (t == PBD_BALLJOINT || t == PBD_RB_PARTICLE_BALLJOINT) {
-        d.arrays.rbX = (float4 *)e->rbX.p; d.arrays.rbQ = (float4 *)e->rbQ.p; d.arrays.rbIinv = (const float4 *)e->rbIinv.p;
-    }
-    lap("  geometry (host fill)");
-    for (int k = 0; k < kMaxGeoV; k++) if (!gv[k].empty()) { CKE(upload_vec(d.gv[k], gv[k], e->stream)); d.arrays.gv[k] = (const float4 *)d.gv[k].p; }
-    for (int k = 0; k < kMaxGeoS; k++) if (!gs[k].empty()) { CKE(upload_vec(d.gs[k], gs[k], e->stream)); d.arrays.gs[k] = (const float *)d.gs[k].p; }
-    lap("  geometry (upload)");
-    // material parameters: one uniform per type when every constraint agrees, else a per-constraint array
+    TypeArrays &a = d.arrays;
+    if (!p.idx2.empty()) { CKE(upload_vec(d.idx[0], p.idx2, e->stream)); a.idx2 = (const uint2 *)d.idx[0].p; }
+    if (!p.idx4.empty()) { CKE(upload_vec(d.idx[0], p.idx4, e->stream)); a.idx4 = (const uint4 *)d.idx[0].p; }
+    for (int k = 0; k < 3; k++) if (!p.idx3[k].empty()) { CKE(upload_vec(d.idx[k], p.idx3[k], e->stream)); a.idx3[k] = (const unsigned *)d.idx[k].p; }
+    for (int k = 0; k < kMaxGeoV; k++) if (!p.gv[k].empty()) { CKE(upload_vec(d.gv[k], p.gv[k], e->stream)); a.gv[k] = (const float4 *)d.gv[k].p; }
+    for (int k = 0; k < kMaxGeoS; k++) if (!p.gs[k].empty()) { CKE(upload_vec(d.gs[k], p.gs[k], e->stream)); a.gs[k] = (const float *)d.gs[k].p; }
     for (int k = 0; k < kMaxMat; k++) {
-        const int c = pc.mat[k];
-        if (c < 0) continue;
-        const float first = P(0, c);
-        int differs = 0;
-        #pragma omp parallel for schedule(static) num_threads(host_threads()) reduction(| : differs) if (cnt > 100000)
-        for (long long i = 1; i < (long long)cnt; i++) differs |= (P((unsigned)i, c) != first) ? 1 : 0;
-        d.arrays.matU[k] = first;
-        if (differs) {
-            PodVector<float> v(cnt);
-            #pragma omp parallel for schedule(static) num_threads(host_threads())
-            for (long long i = 0; i < (long long)cnt; i++) v[i] = P(i, c);
-            CKE(upload_vec(d.mat[k], v, e->stream)); d.arrays.mat[k] = (const float *)d.mat[k].p;
-        }
+        a.matU[k] = p.matU[k];
+        if (!p.mat[k].empty()) { CKE(upload_vec(d.mat[k], p.mat[k], e->stream)); a.mat[k] = (const float *)d.mat[k].p; }
     }
-    if (s.xpbd) {
+    a.variant = p.variant;
+    if (t == PBD_BALLJOINT || t == PBD_RB_PARTICLE_BALLJOINT) {
+        a.rbX = (float4 *)e->rbX.p; a.rbQ = (float4 *)e->rbQ.p; a.rbIinv = (const float4 *)e->rbIinv.p;
+    }
+    if (type_shape(t).xpbd) {
         CKE(d.lambda.alloc((size_t)cnt * sizeof(float) + 16));  // + 16 like the other streamed arrays: the L2 prefetch of a run rounds its end up to 16 bytes
         CK(cudaMemsetAsync(d.lambda.p, 0, (size_t)cnt * sizeof(float), e->stream));
-        d.arrays.lambda = (float *)d.lambda.p;
-    }
-    lap("  material + multipliers");
-    return 0;
-}
-
-// resident mode: colour ranges of the bucket table, the per-tile runs, and who waits for whom in the X flag protocol.  Tile j is a
-// neighbour of tile i when an X item of i and an X item of j touch the same global-homed particle, or an X item of one of them touches
-// a particle homed in the other: exactly the tiles whose global-memory accesses i's X items and i's global-homed particles have to be
-// ordered with.  xMask[i][0] bit k: neighbour k has global-homed particles (arrives in the integration phase); xMask[i][1 + c] bit k:
-// neighbour k has X items in colour c.
-static int build_phase_tables(pbd_engine *e, const ResidentPlan &pl, const std::vector<unsigned> &tileOff, const std::vector<unsigned> (&order)[PBD_NUM_TYPES]) {
-    const unsigned T = e->nTiles;
-    std::vector<unsigned> colourStart;
-    for (size_t i = 0; i < e->buckets.size(); i++)
-        if (i == 0 || e->buckets[i].colour != e->buckets[i - 1].colour) colourStart.push_back((unsigned)i);
-    e->resColours = (unsigned)colourStart.size();
-    colourStart.push_back((unsigned)e->buckets.size());
-    if (tileOff.size() != e->buckets.size() * (2 * (size_t)T + 1)) return fail("flatten: internal error (tile runs)");
-    const unsigned nC = e->resColours;
-    auto run = [&](size_t bi, unsigned t) { return &tileOff[bi * (2 * (size_t)T + 1) + 2 * t]; };  // [0] X items .. [1] others .. [2]
-    // (global-homed particle, tile) pairs: its home tile and every tile that executes an X item touching it
-    std::vector<std::pair<unsigned, unsigned>> touch;
-    for (unsigned i = 0; i < e->n; i++) if (pl.homedGlobal[i]) touch.emplace_back(i, pl.tileOf[i]);
-    for (size_t bi = 0; bi < e->buckets.size(); bi++) {
-        const Bucket &b = e->buckets[bi];
-        const int nb = type_shape(b.type).nBodies;
-        for (unsigned t = 0; t < T; t++)
-            for (unsigned k = run(bi, t)[0]; k < run(bi, t)[1]; k++) {
-                const unsigned *bod = &e->host[b.type].bodies[(size_t)order[b.type][b.first + k] * nb];
-                for (int j = 0; j < nb; j++) if (!is_rb_body(b.type, j) && pl.homedGlobal[bod[j]]) touch.emplace_back(bod[j], t);
-            }
-    }
-    std::sort(touch.begin(), touch.end());
-    touch.erase(std::unique(touch.begin(), touch.end()), touch.end());
-    std::vector<unsigned char> adj((size_t)T * T, 0);
-    for (size_t lo = 0, hi; lo < touch.size(); lo = hi) {
-        for (hi = lo + 1; hi < touch.size() && touch[hi].first == touch[lo].first; hi++) {}
-        for (size_t a = lo; a < hi; a++)
-            for (size_t c = lo; c < hi; c++)
-                if (touch[a].second != touch[c].second) adj[(size_t)touch[a].second * T + touch[c].second] = 1;
-    }
-    std::vector<unsigned char> hasX((size_t)T * (1 + nC), 0);  // [tile][phase]: the tile arrives in the phase
-    for (unsigned t = 0; t < T; t++) {
-        hasX[(size_t)t * (1 + nC)] = (pl.tileStart[t + 1] - pl.tileStart[t] - pl.tileSmem[t]) != 0;
-        for (unsigned c = 0; c < nC; c++)
-            for (unsigned bi = colourStart[c]; bi < colourStart[c + 1]; bi++) hasX[(size_t)t * (1 + nC) + 1 + c] |= run(bi, t)[1] != run(bi, t)[0];
-    }
-    std::vector<unsigned> nbr((size_t)T * kMaxXNeighbours), mask((size_t)T * (1 + nC), 0u), nNbr(T, 0u);
-    for (unsigned i = 0; i < T; i++) {
-        for (unsigned k = 0; k < kMaxXNeighbours; k++) nbr[(size_t)i * kMaxXNeighbours + k] = i;  // unused lanes: never polled (mask bit 0)
-        for (unsigned j = 0; j < T; j++) {
-            if (!adj[(size_t)i * T + j]) continue;
-            if (nNbr[i] == kMaxXNeighbours)
-                return fail("resident mode: tile %u shares global-homed particles with more than %u other tiles (the constraints reach too far "
-                            "across the scene for the resident mode; use PBD_MODE_GRAPH)", i, kMaxXNeighbours);
-            const unsigned k = nNbr[i]++;
-            nbr[(size_t)i * kMaxXNeighbours + k] = j;
-            for (unsigned p = 0; p <= nC; p++) mask[(size_t)i * (1 + nC) + p] |= (unsigned)hasX[(size_t)j * (1 + nC) + p] << k;
-        }
-    }
-    CKE(upload_vec(e->dColourStart, colourStart, e->stream));
-    CKE(upload_vec(e->dTileOff, tileOff, e->stream));
-    CKE(upload_vec(e->dXNbr, nbr, e->stream));
-    CKE(upload_vec(e->dXMask, mask, e->stream));
-    CKE(e->dXFlags.alloc((size_t)T * kXFlagStride * sizeof(unsigned long long)));
-    CK(cudaMemsetAsync(e->dXFlags.p, 0, e->dXFlags.bytes, e->stream));
-    if (verbose()) {
-        unsigned long long xItems = 0, mxRun = 0;
-        std::vector<unsigned long long> perTile(T, 0);  // items a tile executes over one sweep
-        unsigned long long lockstep = 0;                // ... and the sum over the colours of the largest tile's items of the colour
-        for (unsigned c = 0; c < nC; c++) {
-            unsigned long long mx = 0;
-            for (unsigned t = 0; t < T; t++) {
-                unsigned long long items = 0;
-                for (unsigned bi = colourStart[c]; bi < colourStart[c + 1]; bi++) {
-                    xItems += run(bi, t)[1] - run(bi, t)[0];
-                    items += run(bi, t)[2] - run(bi, t)[0];
-                    mxRun = std::max<unsigned long long>(mxRun, run(bi, t)[2] - run(bi, t)[0]);
-                }
-                perTile[t] += items; mx = std::max(mx, items);
-            }
-            lockstep += mx;
-        }
-        std::vector<unsigned> hist(kMaxXNeighbours + 1, 0u);
-        for (unsigned t = 0; t < T; t++) hist[nNbr[t]]++;
-        fprintf(stderr, "[pbd_b200] resident: %u colours, %zu buckets, %.2f %% X items, largest run of a tile in a bucket %llu (mean %.0f)\n",
-                nC, e->buckets.size(), 100.0 * xItems / std::max(1u, e->numConstraints), mxRun, (double)e->numConstraints / std::max<size_t>(1, e->buckets.size()) / T);
-        fprintf(stderr, "[pbd_b200] resident: X neighbours per tile (count x tiles):");
-        for (unsigned k = 0; k <= kMaxXNeighbours; k++) if (hist[k]) fprintf(stderr, " %u x %u", k, hist[k]);
-        const unsigned long long mxTile = T ? *std::max_element(perTile.begin(), perTile.end()) : 0;
-        fprintf(stderr, "\n[pbd_b200] resident: items per sweep, sum over colours of the largest tile %llu, largest tile over all colours %llu (lockstep penalty %.2f %%)\n",
-                lockstep, mxTile, mxTile ? 100.0 * ((double)lockstep / mxTile - 1.0) : 0.0);
-        // the constraint stream of one sweep as this image streams it from DRAM: the 32-bit indices, the per-constraint geometry and
-        // material arrays, the multipliers (read and written)
-        double idxBytes = 0, constBytes = 0;
-        for (const Bucket &b : e->buckets) {
-            const TypeArrays &a = e->dev[b.type].arrays;
-            double perItem = a.lambda ? 8.0 : 0.0;
-            for (int k = 0; k < kMaxGeoV; k++) perItem += a.gv[k] ? 16.0 : 0.0;
-            for (int k = 0; k < kMaxGeoS; k++) perItem += a.gs[k] ? 4.0 : 0.0;
-            for (int k = 0; k < kMaxMat; k++) perItem += a.mat[k] ? 4.0 : 0.0;
-            idxBytes += b.count * 4.0 * type_shape(b.type).nBodies; constBytes += b.count * perItem;
-        }
-        fprintf(stderr, "[pbd_b200] resident: constraint stream per sweep %.1f MB: indices %.1f MB, constants and multipliers %.1f MB\n",
-                (idxBytes + constBytes) * 1e-6, idxBytes * 1e-6, constBytes * 1e-6);
+        a.lambda = (float *)d.lambda.p;
     }
     return 0;
 }
 
-// constraints + colour groups -> the device image of the active mode
+// constraints + colour groups -> the device image of the active mode: the planner's inputs gathered, the plan uploaded
 static int flatten_image(pbd_engine *e) {
     if (!e->imageDirty) return 0;
     CKE(use(e));
-    Lap lap;
+    pbd_b200::Lap lap;
     CKE(colour_if_needed(e));
     drop_graph(e);
-    CKE(validate_bodies(e));
-    std::vector<std::pair<int, unsigned>> map;
-    CKE(build_id_map(e, map));
     const bool tiled = (e->active == PBD_MODE_RESIDENT);
-    ResidentPlan pl;
-    CKE(place_particles(e, tiled, pl));
-    lap("colouring + validation + placement");
-    std::vector<unsigned> order[PBD_NUM_TYPES], tileOff;
-    order_buckets(e, map, tiled, pl, order, tileOff);
-    lap("bucket ordering");
-    CKE(check_colouring(e, order));
-    lap("colouring validity check");
-    for (int t = 0; t < PBD_NUM_TYPES; t++) CKE(pack_type(e, t, order[t], tiled, pl, lap));
-    lap("SoA arrays + upload");
+    std::vector<float4> x0;  // resident: rest positions by host index
+    if (tiled && e->n) {
+        std::vector<float4> raw(e->n);
+        CK(cudaStreamSynchronize(e->stream));
+        CK(cudaMemcpy(raw.data(), e->pos0.p, (size_t)e->n * sizeof(float4), cudaMemcpyDeviceToHost));
+        x0.resize(e->n);
+        for (unsigned i = 0; i < e->n; i++) x0[i] = raw[e->slot[i]];
+    }
+    lap("colouring + rest positions");
+    pbd_b200::PlanInput in{e->host, e->numConstraints, e->n, e->nRb, &e->groupOff, &e->groupIds, tiled, x0.data(), 0u, 0u, e->smCount, nullptr};
+    if (const char *g = getenv("PBD_B200_CLUSTERS")) {  // development knob "GxC"
+        unsigned gg = 0, cc = 0;
+        if (sscanf(g, "%ux%u", &gg, &cc) == 2 && gg >= 1 && cc >= 1 && cc <= (unsigned)kMaxClusterCtas && (cc & (cc - 1)) == 0) { in.forcedG = gg; in.forcedC = cc; }
+    }
+    in.maxClusters = [&](unsigned mask) { int mc = 0; return resident_max_clusters(e, mask, 1u, kMaxDynamicSmem, &mc) ? 0 : mc; };
+    pbd_b200::ImagePlan plan;
+    const std::string err = pbd_b200::plan_image(in, plan);
+    if (!err.empty()) return fail("%s", err.c_str());
+    CKE(relayout(e, plan.slot));
+    for (int t = 0; t < PBD_NUM_TYPES; t++) CKE(upload_type(e, t, plan.types[t]));
+    e->buckets.swap(plan.buckets);
     CKE(upload_vec(e->dBuckets, e->buckets, e->stream));
-    if (tiled) CKE(build_phase_tables(e, pl, tileOff, order));
+    if (tiled) {
+        e->res = plan.res; e->resChecked = false;
+        CKE(upload_vec(e->dTileStart, plan.tileStart, e->stream));
+        CKE(upload_vec(e->dTileSmem, plan.tileSmem, e->stream));
+        CKE(upload_vec(e->dColourStart, plan.colourStart, e->stream));
+        CKE(upload_vec(e->dTileOff, plan.tileOff, e->stream));
+        CKE(upload_vec(e->dXNbr, plan.xNbr, e->stream));
+        CKE(upload_vec(e->dXMask, plan.xMask, e->stream));
+        CKE(e->dXFlags.alloc((size_t)e->res.G * e->res.C * kXFlagStride * sizeof(unsigned long long)));
+        CK(cudaMemsetAsync(e->dXFlags.p, 0, e->dXFlags.bytes, e->stream));
+    }
     CK(cudaStreamSynchronize(e->stream));
-    lap("phase tables");
+    lap("relayout + upload");
     e->stats.num_constraints = e->numConstraints;
     e->stats.num_groups = (unsigned)e->groupOff.size() - 1;
     e->stats.num_buckets = (unsigned)e->buckets.size();
@@ -1565,23 +907,24 @@ static int enqueue_step_launches(pbd_engine *e, cudaStream_t s, unsigned long lo
     return 0;
 }
 
-// One step as one launch of k_step_resident: grid = nTiles CTAs in clusters of resC, one CTA per SM, all co-resident
+// One step as one launch of k_step_resident: grid = G x C CTAs in clusters of C, one CTA per SM, all co-resident
 // (the X items of different clusters wait for each other).
 static int launch_resident(pbd_engine *e, cudaStream_t s, ResidentArgs &ra) {
     const size_t smem = resident_smem_bytes(ra.tileCap, ra.nBuckets, ra.nColours);
     if (smem > kMaxDynamicSmem) return fail("resident mode: a CTA needs %zu bytes of shared memory (tile of %u particles + phase tables), %zu available", smem, ra.tileCap, kMaxDynamicSmem);
-    if (e->resG > 1 && !e->resChecked) {
+    const pbd_b200::ResidentShape &r = e->res;
+    if (r.G > 1 && !e->resChecked) {
         int mc = 0;
-        CKE(resident_max_clusters(e, e->resC, smem, &mc));
-        if ((unsigned)mc < e->resG)
-            return fail("resident mode: the device runs %d clusters of %u CTAs at a time, the scene needs %u co-resident", mc, e->resC, e->resG);
+        CKE(resident_max_clusters(e, r.mask, r.C, smem, &mc));
+        if ((unsigned)mc < r.G)
+            return fail("resident mode: the device runs %d clusters of %u CTAs at a time, the scene needs %u co-resident", mc, r.C, r.G);
         e->resChecked = true;
     }
-    return with_resident_kernel(e, e->resC, [&](auto kernel) -> int {
+    return with_resident_kernel(r.mask, r.C, [&](auto kernel) -> int {
         CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynamicSmem));
-        if (e->resC > 8) CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+        if (r.C > 8) CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
         cudaLaunchConfig_t cfg; cudaLaunchAttribute attr[1];
-        resident_launch_config(e, e->resC, e->nTiles, smem, s, cfg, attr);
+        resident_launch_config(r.mask, r.C, r.G * r.C, smem, s, cfg, attr);
         CK(cudaLaunchKernelEx(&cfg, kernel, ra));
         return 0;
     });
@@ -1595,8 +938,8 @@ static int enqueue_step_resident(pbd_engine *e, cudaStream_t s, unsigned long lo
     ra.colourStart = (const unsigned *)e->dColourStart.p; ra.tileOff = (const unsigned *)e->dTileOff.p;
     ra.tileStart = (const unsigned *)e->dTileStart.p; ra.tileSmem = (const unsigned *)e->dTileSmem.p;
     ra.xNbr = (const unsigned *)e->dXNbr.p; ra.xMask = (const unsigned *)e->dXMask.p;
-    ra.nBuckets = (unsigned)e->buckets.size(); ra.nColours = e->resColours; ra.nTiles = e->nTiles; ra.subSteps = e->subSteps; ra.maxIter = e->maxIter;
-    ra.tileCap = e->resTileCap; ra.xThreads = e->resXThreads; ra.clusterSize = e->resC;
+    ra.nBuckets = (unsigned)e->buckets.size(); ra.nColours = e->res.nColours; ra.nTiles = e->res.G * e->res.C; ra.subSteps = e->subSteps; ra.maxIter = e->maxIter;
+    ra.tileCap = e->res.tileCap; ra.xThreads = e->res.xThreads; ra.clusterSize = e->res.C;
     {   // L2 prefetch of the operand runs pays when the constraint stream of a sweep does not stay in L2 anyway (above ~0.38 x the L2).
         // H100 80GB HBM3 (400 W, 50 MB L2), prefetch off / on: cfg2 (192 MB per sweep) 2.28 / 2.08 ms, cfg5 (48 MB) 1.246 / 1.216 ms,
         // 300x300 cloth (below the threshold) 1.015 / 1.016 ms.
@@ -1618,20 +961,20 @@ static int enqueue_step_resident(pbd_engine *e, cudaStream_t s, unsigned long lo
     static const char *tracePath = getenv("PBD_B200_TRACE");  // development aid: dump per-phase timelines of one step (tools/trace_resident.py)
     const unsigned kTracePhases = 256;
     if (tracePath) {
-        CKE(e->dTrace.alloc((size_t)kTracePhases * e->nTiles * kTraceSlots * sizeof(unsigned long long)));
+        CKE(e->dTrace.alloc((size_t)kTracePhases * ra.nTiles * kTraceSlots * sizeof(unsigned long long)));
         CK(cudaMemsetAsync(e->dTrace.p, 0, e->dTrace.bytes, s));
         ra.trace = (unsigned long long *)e->dTrace.p; ra.tracePhases = kTracePhases;
     }
     struct TraceDump {  // runs after the launch below has been enqueued (scope exit)
-        pbd_engine *e; cudaStream_t s; const char *path; unsigned phases;
+        pbd_engine *e; cudaStream_t s; const char *path; size_t words;
         ~TraceDump() {
             if (!path) return;
             cudaStreamSynchronize(s);
-            std::vector<unsigned long long> h((size_t)phases * e->nTiles * kTraceSlots);
+            std::vector<unsigned long long> h(words);
             cudaMemcpy(h.data(), e->dTrace.p, h.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost);
             if (FILE *f = fopen(path, "wb")) { fwrite(h.data(), sizeof(unsigned long long), h.size(), f); fclose(f); }
         }
-    } dump{e, s, tracePath, kTracePhases};
+    } dump{e, s, tracePath, (size_t)kTracePhases * ra.nTiles * kTraceSlots};
     return launch_resident(e, s, ra);
 }
 

@@ -1,0 +1,685 @@
+// positionbaseddynamics_b200/csrc/host/image_plan.cpp
+//
+// The image planner (image_plan.h): a constraint list + the reference's colour groups -> (colour,type) buckets of SoA arrays; for the
+// resident mode (resident.cuh) also the tiling of the particles, the per-tile runs and the X-neighbour tables.  No CUDA API call.
+#include "image_plan.h"
+#include <algorithm>
+#include <cmath>
+#include <cstdarg>
+#include <cstdio>
+#include <cstdlib>
+#include <cstring>
+#include <numeric>
+#include <omp.h>
+#include <parallel/algorithm>  // libstdc++ parallel mode (OpenMP): the per-bucket sorts
+
+namespace pbd_b200 {
+using namespace pbdk;
+
+bool verbose() {
+    static const bool v = getenv("PBD_B200_VERBOSE") != nullptr;
+    return v;
+}
+Lap::Lap() : prev(omp_get_wtime()) {}
+void Lap::operator()(const char *what) {
+    if (!verbose()) return;
+    const double t = omp_get_wtime();
+    fprintf(stderr, "[pbd_b200] flatten: %-34s %.3f s\n", what, t - prev);
+    prev = t;
+}
+
+static std::string fmt(const char *f, ...) {
+    char buf[1024];
+    va_list ap; va_start(ap, f); vsnprintf(buf, sizeof(buf), f, ap); va_end(ap);
+    return buf;
+}
+
+long long bad_body_index(int type, const unsigned *bodies, size_t count, unsigned n, unsigned nRb) {
+    const int nb = type_shape(type).nBodies;
+    long long badAt = -1;
+    #pragma omp parallel for schedule(static) num_threads(host_threads()) reduction(max : badAt) if (count * nb > 100000)
+    for (long long c = 0; c < (long long)count; c++)
+        for (int k = 0; k < nb; k++) {
+            const long long i = c * nb + k;
+            if (bodies[i] >= (is_rb_body(type, k) ? nRb : n)) badAt = std::max(badAt, i);
+        }
+    return badAt;
+}
+
+std::string build_id_map(const TypeStore *store, unsigned N, std::vector<std::pair<int, unsigned>> &map) {
+    map.resize(N);
+    PodVector<int> seenType(N);
+    #pragma omp parallel for schedule(static) num_threads(host_threads())
+    for (long long i = 0; i < (long long)N; i++) seenType[i] = -1;
+    for (int t = 0; t < PBD_NUM_TYPES; t++) {
+        const TypeStore &h = store[t];
+        long long bad = -1; int dup = 0;
+        #pragma omp parallel for schedule(static) num_threads(host_threads()) reduction(max : bad) reduction(| : dup) if (h.ids.size() > 50000)
+        for (long long i = 0; i < (long long)h.ids.size(); i++) {
+            const unsigned id = h.ids[i];
+            if (id >= N) { bad = std::max(bad, (long long)id); continue; }
+            if (__atomic_exchange_n(&seenType[id], t, __ATOMIC_RELAXED) != -1) { dup = 1; bad = std::max(bad, (long long)id); continue; }
+            map[id] = std::make_pair(t, (unsigned)i);
+        }
+        if (bad >= 0 && !dup) return fmt("constraint id %u out of range (N=%u)", (unsigned)bad, N);
+        if (dup) return fmt("constraint id %u used twice", (unsigned)bad);
+    }
+    return "";  // N ids, all below N, none twice: a permutation
+}
+
+// the particle / rigid-body counts may have shrunk since the constraints were added (pbd_set_particles, pbd_set_rigid_bodies)
+static std::string validate_bodies(const PlanInput &in) {
+    for (int t = 0; t < PBD_NUM_TYPES; t++) {
+        const TypeStore &h = in.store[t];
+        const long long badAt = bad_body_index(t, h.bodies.data(), h.ids.size(), in.n, in.nRb);
+        if (badAt < 0) continue;
+        const bool isRb = is_rb_body(t, (int)(badAt % type_shape(t).nBodies));
+        return fmt("constraint of type %d refers to %s %u, but the engine holds %u: re-add the constraints after shrinking the model", t,
+                   isRb ? "rigid body" : "particle", h.bodies[badAt], isRb ? in.nRb : in.n);
+    }
+    return "";
+}
+
+// Q (row-major 4x4, solver order) = -Kp Kp^T ?  Returns true and Kp when the rank-one negative-semidefinite form of
+// init_IsometricBendingConstraint (PositionBasedDynamics.cpp:169-180) reproduces Q to fp32 accuracy.
+static bool factor_rank1(const float *Q, float Kp[4]) {
+    int piv = 0; float best = 0.0f, maxAbs = 0.0f;
+    for (int j = 0; j < 4; j++) { if (-Q[5 * j] > best) { best = -Q[5 * j]; piv = j; } }
+    for (int i = 0; i < 16; i++) maxAbs = std::max(maxAbs, std::fabs(Q[i]));
+    if (maxAbs == 0.0f) { Kp[0] = Kp[1] = Kp[2] = Kp[3] = 0.0f; return true; }
+    if (!(best > 0.0f)) return false;
+    const double kp = std::sqrt((double)best);
+    double K[4];
+    for (int k = 0; k < 4; k++) K[k] = -(double)Q[4 * piv + k] / kp;
+    for (int j = 0; j < 4; j++)
+        for (int k = 0; k < 4; k++)
+            if (std::fabs((double)Q[4 * j + k] + K[j] * K[k]) > 1e-5 * (double)maxAbs) return false;
+    for (int k = 0; k < 4; k++) Kp[k] = (float)K[k];
+    return true;
+}
+
+// The planner's state: its input, the plan being built, and for the resident mode where every host particle lives.
+struct Ctx {
+    const PlanInput &in;
+    ImagePlan &out;
+    std::vector<unsigned> tileOf;             // host particle -> tile (cluster = tile / C, rank = tile % C)
+    std::vector<unsigned char> homedGlobal;   // host particle lives in global memory (touched by a constraint that spans clusters)
+    unsigned nTiles() const { return out.res.G * out.res.C; }
+};
+
+// Resident mode (resident.cuh): the particles are partitioned into G cluster regions x C tiles by recursive coordinate
+// bisection of the rest positions; the device arrays are permuted to tile-major order.
+static void bisect(std::vector<unsigned> &idx, size_t lo, size_t hi, unsigned t0, unsigned nt, const float4 *x, std::vector<unsigned> &tileOf) {
+    if (nt == 1) { for (size_t i = lo; i < hi; i++) tileOf[idx[i]] = t0; return; }
+    float mn[3] = {3.4e38f, 3.4e38f, 3.4e38f}, mx[3] = {-3.4e38f, -3.4e38f, -3.4e38f};
+    for (size_t i = lo; i < hi; i++) {
+        const float4 &p = x[idx[i]];
+        const float c[3] = {p.x, p.y, p.z};
+        for (int k = 0; k < 3; k++) { mn[k] = std::min(mn[k], c[k]); mx[k] = std::max(mx[k], c[k]); }
+    }
+    int ax = 0;
+    for (int k = 1; k < 3; k++) if (mx[k] - mn[k] > mx[ax] - mn[ax]) ax = k;
+    const unsigned ntL = nt / 2;
+    const size_t mid = lo + (size_t)((double)(hi - lo) * ntL / nt);
+    auto key = [&](unsigned i) { const float4 &p = x[i]; return ax == 0 ? p.x : (ax == 1 ? p.y : p.z); };
+    std::nth_element(idx.begin() + lo, idx.begin() + mid, idx.begin() + hi, [&](unsigned a, unsigned b) { const float ka = key(a), kb = key(b); return ka < kb || (ka == kb && a < b); });
+    // the two halves are independent: run them as tasks while they are big enough to pay for it
+    #pragma omp task shared(idx, x, tileOf) if (hi - lo > 65536)
+    bisect(idx, lo, mid, t0, ntL, x, tileOf);
+    bisect(idx, mid, hi, t0 + ntL, nt - ntL, x, tileOf);
+    #pragma omp taskwait
+}
+
+// Executing tile of a constraint: the tile that holds most of its shared-memory particles (ties: the lowest tile); none -> the tile of
+// its first particle (0 for a joint between rigid bodies).  *touchesGlobal: one of its particles is global-homed.
+static inline unsigned exec_tile(int t, const unsigned *b, int nb, const std::vector<unsigned> &tileOf, const std::vector<unsigned char> &homedGlobal, bool *touchesGlobal) {
+    bool x = false;
+    unsigned best = 0xffffffffu, bestCnt = 0, first = 0xffffffffu;
+    for (int k = 0; k < nb; k++) {
+        if (is_rb_body(t, k)) continue;
+        if (first == 0xffffffffu) first = tileOf[b[k]];
+        if (homedGlobal[b[k]]) { x = true; continue; }
+        unsigned cnt = 0;
+        for (int j = 0; j < nb; j++) cnt += (!is_rb_body(t, j) && !homedGlobal[b[j]] && tileOf[b[j]] == tileOf[b[k]]);
+        if (cnt > bestCnt || (cnt == bestCnt && tileOf[b[k]] < best)) { best = tileOf[b[k]]; bestCnt = cnt; }
+    }
+    *touchesGlobal = x;
+    return (best != 0xffffffffu) ? best : (first != 0xffffffffu ? first : 0u);
+}
+
+// shape of the launch: type mask / block size of the instantiation, clusters x CTAs per cluster
+static std::string choose_resident_shape(const PlanInput &in, ResidentShape &r) {
+    unsigned present = 0, nTypes = 0;
+    for (int t = 0; t < PBD_NUM_TYPES; t++) if (!in.store[t].ids.empty()) { present |= 1u << t; nTypes++; }
+    r.mask = kMaskAll;
+    for (unsigned m : {kMaskClothXPBD, kMaskCloth, kMaskFem, kMaskLight, kMaskSolid})  // the leanest instantiation that covers the model
+        if ((present & ~m) == 0) { r.mask = m; break; }
+    r.threads = resident_threads(r.mask);
+    const unsigned nGroups = (unsigned)std::max<size_t>(in.groupOff->size(), 2) - 1;
+    const unsigned perPhase = in.numConstraints / std::max(1u, nGroups);
+    // particles a tile can hold: what is left of the CTA's shared memory after the phase tables (bound: one bucket per colour and type)
+    const size_t tables = resident_smem_bytes(0u, nGroups * std::max(1u, nTypes), nGroups);
+    if (tables + 1024 * sizeof(float4) > kMaxDynamicSmem) return fmt("resident mode: %u colour groups need %zu bytes of phase tables (use PBD_MODE_GRAPH)", nGroups, tables);
+    const unsigned cap = (unsigned)(0.97 * (double)((kMaxDynamicSmem - tables) / sizeof(float4)));  // bisection splits counts evenly; slack for rounding
+    unsigned G = 1, C = 1;
+    if (in.n <= (unsigned)kMaxClusterCtas * cap && perPhase <= (unsigned)kMaxClusterCtas * 1024u) {
+        // one cluster: enough CTAs that a colour phase is about one item per thread, and that the tiles fit
+        while (C < (unsigned)kMaxClusterCtas && (perPhase > C * 256u || in.n > C * cap)) C *= 2;
+    } else {
+        // Too big for one cluster: one independent CTA per SM (clusters of 1).  Larger clusters have fewer X items but idle SMs (a
+        // cluster must fit a GPC) and a colour barrier that waits for the slowest of C CTAs; with C = 1 the colour barrier is a
+        // __syncthreads.
+        const int mc = in.maxClusters(r.mask);
+        if (mc < 1) return fmt("resident mode: a CTA with %zu bytes of shared memory is not schedulable on this device", kMaxDynamicSmem);
+        C = 1; G = (unsigned)std::min(mc, in.smCount);
+    }
+    if (in.forcedG) { G = in.forcedG; C = in.forcedC; }
+    if ((unsigned long long)G * C * cap < in.n)
+        return fmt("resident mode: %u particles do not fit %u x %u tiles of %u (use PBD_MODE_GRAPH)", in.n, G, C, cap);
+    // (bodies without joints -- e.g. the static colliders of the contact path -- are integrated by CTA 0 and touch no constraint)
+    if (G > 1 && (!in.store[PBD_BALLJOINT].ids.empty() || !in.store[PBD_RB_PARTICLE_BALLJOINT].ids.empty()))
+        return "resident mode: rigid-body coupling is supported for scenes that fit one cluster (use PBD_MODE_GRAPH)";
+    r.G = G; r.C = C;
+    r.xThreads = (G > 1) ? 128u : 0u;  // refined in place_in_tiles once the share of X items is known
+    return "";
+}
+
+static std::string place_in_tiles(Ctx &c) {
+    const PlanInput &in = c.in;
+    ImagePlan &pl = c.out;
+    const std::string err = choose_resident_shape(in, pl.res);
+    if (!err.empty()) return err;
+    const unsigned n = in.n, G = pl.res.G, C = pl.res.C, T = c.nTiles();
+    c.tileOf.assign(n, 0); c.homedGlobal.assign(n, 0); pl.tileStart.assign(T + 1, 0); pl.tileSmem.assign(T, 0);
+    if (n) {
+        const float4 *x = in.x0;  // rest positions by host index
+        std::vector<unsigned> idx(n), region(n);
+        for (unsigned i = 0; i < n; i++) idx[i] = i;
+        #pragma omp parallel num_threads(host_threads())
+        #pragma omp single
+        bisect(idx, 0, n, 0, G, x, region);  // cluster regions; idx is now grouped region by region
+        size_t lo = 0;
+        for (unsigned g = 0; g < G; g++) {
+            size_t hi = lo;
+            while (hi < n && region[idx[hi]] == g) hi++;
+            if (C == 1) { for (size_t i = lo; i < hi; i++) c.tileOf[idx[i]] = g; }
+            else {
+                #pragma omp parallel num_threads(host_threads())
+                #pragma omp single
+                bisect(idx, lo, hi, g * C, C, x, c.tileOf);
+            }
+            lo = hi;
+        }
+        // global-homed = touched by a constraint whose particles lie in more than one cluster
+        if (G > 1)
+            for (int t = 0; t < PBD_NUM_TYPES; t++) {
+                const TypeStore &h = in.store[t];
+                const int nb = type_shape(t).nBodies;
+                unsigned char *hg = c.homedGlobal.data();
+                #pragma omp parallel for schedule(static) num_threads(host_threads())
+                for (long long k0 = 0; k0 < (long long)h.ids.size(); k0++) {
+                    const unsigned *b = &h.bodies[(size_t)k0 * nb];
+                    bool spans = false;
+                    for (int k = 1; k < nb; k++) spans |= (c.tileOf[b[k]] / C != c.tileOf[b[0]] / C);
+                    if (spans) for (int k = 0; k < nb; k++) hg[b[k]] = 1;  // every writer stores the same byte
+                }
+            }
+        // threads of a CTA dedicated to the X items: in proportion to their share, times 3.1 because an X item waits for L2 where
+        // the others read shared memory.  The factor is carried over from an earlier GPU; on an H100 80GB HBM3 (400 W) cfg2 is flat in
+        // it: 160 / 192 / 224 / 256 X threads -> 2.07 / 2.05 / 2.09 / 2.11 ms, within the run-to-run spread.
+        if (G > 1) {
+            unsigned long long xItems = 0;
+            for (int t = 0; t < PBD_NUM_TYPES; t++) {
+                const TypeStore &h = in.store[t];
+                const int nb = type_shape(t).nBodies;
+                #pragma omp parallel for schedule(static) num_threads(host_threads()) reduction(+ : xItems)
+                for (long long k0 = 0; k0 < (long long)h.ids.size(); k0++) {
+                    bool x = false;
+                    for (int k = 0; k < nb; k++) x |= (!is_rb_body(t, k) && c.homedGlobal[h.bodies[(size_t)k0 * nb + k]]);
+                    xItems += x;
+                }
+            }
+            const double share = (double)xItems / std::max(1u, in.numConstraints);
+            unsigned xt = ((unsigned)(pl.res.threads * share * 3.1) + 31u) & ~31u;
+            pl.res.xThreads = std::max(64u, std::min(xt, (pl.res.threads / 2u) & ~31u));
+        }
+        // tile-major slots: shared-memory particles first (host order), global-homed behind them
+        std::vector<unsigned> cntS(T, 0), cntG(T, 0);
+        for (unsigned i = 0; i < n; i++) (c.homedGlobal[i] ? cntG : cntS)[c.tileOf[i]]++;
+        for (unsigned t = 0; t < T; t++) {
+            pl.tileStart[t + 1] = pl.tileStart[t] + cntS[t] + cntG[t];
+            pl.tileSmem[t] = cntS[t];
+        }
+        std::vector<unsigned> curS(T), curG(T);
+        for (unsigned t = 0; t < T; t++) { curS[t] = pl.tileStart[t]; curG[t] = pl.tileStart[t] + cntS[t]; }
+        pl.slot.resize(n);
+        for (unsigned i = 0; i < n; i++) pl.slot[i] = c.homedGlobal[i] ? curG[c.tileOf[i]]++ : curS[c.tileOf[i]]++;
+        if (verbose()) {
+            unsigned long long nGl = 0;
+            for (unsigned i = 0; i < n; i++) nGl += c.homedGlobal[i];
+            fprintf(stderr, "[pbd_b200] resident: %u clusters x %u CTAs, %u threads (%u for X items), %u particles, %.2f %% global-homed, max tile %u\n", G, C, pl.res.threads, pl.res.xThreads, n,
+                    100.0 * nGl / n, *std::max_element(cntS.begin(), cntS.end()));
+        }
+    }
+    pl.res.tileCap = 64u;  // multiple of 64: the bank swizzle permutes inside aligned 64-slot blocks
+    for (unsigned t = 0; t < T; t++) pl.res.tileCap = std::max(pl.res.tileCap, (pl.tileSmem[t] + 63u) & ~63u);
+    return "";
+}
+
+typedef std::pair<unsigned long long, unsigned> KeyedItem;  // (sort key, local host index of the constraint)
+struct Wavefronts { double before = 0, after = 0, requests = 0; };
+
+// Shared-memory bank groups of one run of a resident tile.  The eight lanes of a quarter-warp (eight consecutive items of the run) read
+// operand k of their items with one LDS.128; it takes as many wavefronts as the fullest 16-byte bank group (slot & 7 after the swizzle).
+// Greedy re-ordering: each group of eight is filled with the items, out of the next `kWindow` unused ones, that add the fewest
+// collisions over all operands.  The order inside a colour is free; results are bit-identical.  H100 80GB HBM3 (400 W), without / with
+// the fill: cfg2 2.14 / 2.08 ms, cfg5 1.221 / 1.216 ms, cfg3 7.81 / 7.69 ms (bank group taken inside the CTA that holds the particle).
+// With `wf`: the wavefronts of the run's quarter-warp gathers before and after, and their number.
+static void bank_group_fill(KeyedItem *run, size_t cnt, int t, const Ctx &c, Wavefronts *wf) {
+    constexpr int kWindow = 64;
+    const int nb = type_shape(t).nBodies, nk = std::min(nb, 4);
+    const unsigned *bod = c.in.store[t].bodies.data();
+    std::vector<unsigned char> bg(cnt * 4, 0);
+    for (size_t i = 0; i < cnt; i++) {
+        const unsigned *b = bod + (size_t)run[i].second * nb;
+        for (int k = 0; k < nk; k++) bg[i * 4 + k] = (unsigned char)(tile_swizzle(c.out.slot[b[k]] - c.out.tileStart[c.tileOf[b[k]]]) & 7u);  // bank group inside the CTA that holds the particle
+    }
+    // greedy fill from a sliding pool of the next kWindow unused items (kept in run order)
+    std::vector<unsigned> out; out.reserve(cnt);
+    unsigned pool[kWindow]; int nPool = 0; size_t head = 0;
+    while (out.size() < cnt) {
+        unsigned char load[4][8] = {};
+        for (int j = 0; j < 8 && out.size() < cnt; j++) {
+            while (nPool < kWindow && head < cnt) pool[nPool++] = (unsigned)head++;
+            int best = 0, bestCost = 1 << 30;
+            for (int p = 0; p < nPool; p++) {
+                const unsigned char *g4 = &bg[(size_t)pool[p] * 4];
+                int cost = 0;
+                for (int k = 0; k < nk; k++) cost += load[k][g4[k]];
+                if (cost < bestCost) { bestCost = cost; best = p; if (!cost) break; }
+            }
+            const unsigned pick = pool[best];
+            for (int p = best; p + 1 < nPool; p++) pool[p] = pool[p + 1];
+            nPool--;
+            out.push_back(pick);
+            for (int k = 0; k < nk; k++) load[k][bg[(size_t)pick * 4 + k]]++;
+        }
+    }
+    if (wf) {
+        auto wavefronts = [&](const std::vector<unsigned> &ord) {
+            double w = 0;
+            for (size_t g8 = 0; g8 + 8 <= cnt; g8 += 8)
+                for (int k = 0; k < nk; k++) {
+                    unsigned char c8[8] = {0, 0, 0, 0, 0, 0, 0, 0}; unsigned mx = 0;
+                    for (int j = 0; j < 8; j++) mx = std::max<unsigned>(mx, ++c8[bg[ord[g8 + j] * 4 + k]]);
+                    w += mx;
+                }
+            return w;
+        };
+        std::vector<unsigned> asSorted(cnt);
+        std::iota(asSorted.begin(), asSorted.end(), 0u);
+        wf->before += wavefronts(asSorted); wf->after += wavefronts(out); wf->requests += (double)(cnt / 8) * nk;
+    }
+    const std::vector<KeyedItem> sorted(run, run + cnt);
+    for (size_t i = 0; i < cnt; i++) run[i] = sorted[out[i]];
+}
+
+// The items (local host indices) of the bucket (colour g, type t), re-ordered.  The order inside a colour is free: sorted by lowest
+// particle slot for gather locality (joints keep their order); resident: major key = executing tile, then the X items (touching a
+// global-homed particle) before the others, the shared-memory runs bank-group filled, and the runs of every tile appended to tileOff:
+// [2 tile] X items, [2 tile + 1] the others.
+static void sort_bucket(const Ctx &c, unsigned g, int t, std::vector<unsigned> &items, std::vector<unsigned> &tileOff) {
+    const bool tiled = c.in.tiled;
+    const bool joint = (t == PBD_BALLJOINT || t == PBD_RB_PARTICLE_BALLJOINT);
+    const int nb = type_shape(t).nBodies;
+    const unsigned *bod = c.in.store[t].bodies.data();
+    std::vector<KeyedItem> keyed(items.size());
+    #pragma omp parallel for schedule(static) num_threads(host_threads())
+    for (long long i = 0; i < (long long)items.size(); i++) {
+        const unsigned *b = bod + (size_t)items[i] * nb;
+        unsigned mn = 0xffffffffu;
+        for (int k = 0; k < nb; k++) if (!is_rb_body(t, k)) mn = std::min(mn, c.out.slot[b[k]]);
+        if (joint) mn = (unsigned)i;
+        // resident: run = executing tile and kind (X items first) in key bits 51 and up.  Ordering a run by kind of element as well
+        // (constraints with the same slot offsets between their particles first) made no difference on an H100 80GB HBM3 (700 W):
+        // cfg3 7.66 / 7.62 ms, cfg4 0.625 / 0.625 ms with / without.
+        unsigned long long run = 0;
+        if (tiled) {
+            bool x = false;
+            const unsigned exec = exec_tile(t, b, nb, c.tileOf, c.homedGlobal, &x);
+            run = 2ull * exec + (x ? 0u : 1u);
+        }
+        keyed[i] = std::make_pair((run << 51) | mn, items[i]);
+    }
+    __gnu_parallel::stable_sort(keyed.begin(), keyed.end(), [](const KeyedItem &a, const KeyedItem &b) { return a.first < b.first; },
+                                __gnu_parallel::default_parallel_tag(host_threads()));
+    if (tiled && !joint) {
+        std::vector<size_t> runStart;
+        for (size_t i = 0; i < keyed.size(); i++) if (i == 0 || (keyed[i].first >> 51) != (keyed[i - 1].first >> 51)) runStart.push_back(i);
+        runStart.push_back(keyed.size());
+        double before = 0, after = 0, requests = 0;
+        const long long nRuns = (long long)runStart.size() - 1;
+        #pragma omp parallel for schedule(dynamic, 1) num_threads(host_threads()) reduction(+ : before, after, requests)
+        for (long long r = 0; r < nRuns; r++) {
+            const size_t lo = runStart[r], cnt = runStart[r + 1] - lo;
+            if (!((keyed[lo].first >> 51) & 1ull) || cnt < 16) continue;  // X runs gather from global memory: left alone
+            Wavefronts w;
+            bank_group_fill(&keyed[lo], cnt, t, c, verbose() ? &w : nullptr);
+            before += w.before; after += w.after; requests += w.requests;
+        }
+        if (verbose() && requests > 0) fprintf(stderr, "[pbd_b200] flatten:   colour %u type %d: %.2f wavefronts per quarter-warp gather as sorted, %.2f after the bank-group fill\n", g, t,
+                                               before / requests, after / requests);
+    }
+    #pragma omp parallel for schedule(static) num_threads(host_threads())
+    for (long long i = 0; i < (long long)keyed.size(); i++) items[i] = keyed[i].second;
+    if (tiled) {
+        const size_t base = tileOff.size();
+        tileOff.resize(base + 2 * c.nTiles() + 1, 0u);
+        for (size_t i = 0; i < keyed.size(); i++) tileOff[base + (keyed[i].first >> 51) + 1]++;
+        for (unsigned k = 0; k < 2 * c.nTiles(); k++) tileOff[base + k + 1] += tileOff[base + k];
+    }
+}
+
+// every colour group split by type into (colour, type) buckets; order[t]: device position -> local host index
+static void order_buckets(Ctx &c, const std::vector<std::pair<int, unsigned>> &map, std::vector<unsigned> (&order)[PBD_NUM_TYPES]) {
+    const std::vector<unsigned> &groupOff = *c.in.groupOff, &groupIds = *c.in.groupIds;
+    const unsigned nGroups = (unsigned)groupOff.size() - 1;
+    c.out.buckets.clear();
+    std::vector<unsigned> items[PBD_NUM_TYPES];
+    for (unsigned g = 0; g < nGroups; g++) {
+        for (auto &v : items) v.clear();
+        for (unsigned i = groupOff[g]; i < groupOff[g + 1]; i++) {
+            const auto &m = map[groupIds[i]];
+            items[m.first].push_back(m.second);
+        }
+        for (int t = 0; t < PBD_NUM_TYPES; t++) {
+            if (items[t].empty()) continue;
+            const bool joint = (t == PBD_BALLJOINT || t == PBD_RB_PARTICLE_BALLJOINT);
+            if (!joint || c.in.tiled) sort_bucket(c, g, t, items[t], c.out.tileOff);
+            Bucket b; b.type = t; b.first = (unsigned)order[t].size(); b.count = (unsigned)items[t].size(); b.colour = g;
+            c.out.buckets.push_back(b);
+            order[t].insert(order[t].end(), items[t].begin(), items[t].end());
+        }
+    }
+}
+
+// Debug-grade safety: inside a colour no particle may be used twice (race freedom by construction, SURVEY.md section 5).  Particles
+// and rigid bodies are stamped in separate index spaces (the reference's colouring shares one, which only ever over-separates; a body
+// really used twice in a colour would be a race here).
+static std::string check_colouring(const Ctx &c, const std::vector<unsigned> (&order)[PBD_NUM_TYPES]) {
+    const unsigned n = c.in.n;
+    std::vector<unsigned> stamp((size_t)n + c.in.nRb, 0xffffffffu);
+    for (const Bucket &b : c.out.buckets) {  // colour after colour
+        const unsigned g = b.colour;
+        const int nb = type_shape(b.type).nBodies;
+        long long bad = -1;  // items of a bucket in parallel: the stamp of a slot is exchanged atomically
+        #pragma omp parallel for schedule(static) num_threads(host_threads()) reduction(max : bad) if (b.count > 20000)
+        for (long long i = 0; i < (long long)b.count; i++) {
+            const unsigned *bd = &c.in.store[b.type].bodies[(size_t)order[b.type][b.first + i] * nb];
+            for (int k = 0; k < nb; k++) {
+                const size_t slot = is_rb_body(b.type, k) ? (size_t)n + bd[k] : bd[k];
+                if (__atomic_exchange_n(&stamp[slot], g, __ATOMIC_RELAXED) == g) bad = std::max(bad, (long long)slot);
+            }
+        }
+        if (bad >= 0) {
+            const bool isRb = (size_t)bad >= n;
+            return fmt("colour group %u uses %s %u twice: the groups are not a valid colouring", g, isRb ? "rigid body" : "particle", (unsigned)(isRb ? bad - n : bad));
+        }
+    }
+    return "";
+}
+
+// Parameter columns (include/pbd_b200.h) of a type's SoA arrays: float4 geometry array k = columns gv[k][0..3], scalar geometry
+// array k = column gs[k], material slot k = column mat[k]; -1 = zero-filled component, or no such array / slot.
+struct PackColumns { signed char gv[kMaxGeoV][4], gs[kMaxGeoS], mat[kMaxMat]; };
+static PackColumns pack_columns(int t) {
+    PackColumns p;
+    memset(&p, -1, sizeof(p));
+    auto gv = [&](int k, int c0, int c1, int c2, int c3) { p.gv[k][0] = c0; p.gv[k][1] = c1; p.gv[k][2] = c2; p.gv[k][3] = c3; };
+    auto mat = [&](int first, int count) { for (int k = 0; k < count; k++) p.mat[k] = first + k; };
+    switch (t) {
+    case PBD_DISTANCE: case PBD_DISTANCE_XPBD: case PBD_DIHEDRAL: case PBD_VOLUME: case PBD_VOLUME_XPBD: p.gs[0] = 0; mat(1, 1); break;
+    case PBD_ISOBENDING: case PBD_ISOBENDING_XPBD: for (int r = 0; r < 4; r++) gv(r, 1 + 4 * r, 2 + 4 * r, 3 + 4 * r, 4 + 4 * r); mat(0, 1); break;  // full Q (see pack_type)
+    case PBD_FEMTRIANGLE: p.gs[0] = 0; gv(0, 1, 2, 3, 4); mat(5, 5); break;
+    case PBD_STRAINTRIANGLE: gv(0, 0, 1, 2, 3); mat(4, 5); break;
+    case PBD_FEMTET: case PBD_FEMTET_XPBD: gv(0, 1, 2, 3, 4); gv(1, 5, 6, 7, 8); p.gs[0] = 9; p.gs[1] = 0; mat(10, 2); break;
+    case PBD_STRAINTET: gv(0, 0, 1, 2, 3); gv(1, 4, 5, 6, 7); p.gs[0] = 8; mat(9, 4); break;
+    // local connectors (jointInfo columns 0 [and 1]); the global columns are recomputed per solve
+    case PBD_BALLJOINT: gv(0, 0, 1, 2, -1); gv(1, 3, 4, 5, -1); break;
+    case PBD_RB_PARTICLE_BALLJOINT: gv(0, 0, 1, 2, -1); break;
+    // restCm | x0[0..3] packed in 3 float4 | w | numClusters ; stiffness is the material slot
+    case PBD_SHAPEMATCHING: gv(0, 1, 2, 3, -1); for (int k = 1; k < 6; k++) gv(k, 4 * k, 4 * k + 1, 4 * k + 2, 4 * k + 3); mat(0, 1); break;
+    }
+    return p;
+}
+
+// the SoA arrays of type t in device order (order: device position -> local host index)
+static std::string pack_type(Ctx &c, int t, const std::vector<unsigned> &order, Lap &lap) {
+    TypePlan &d = c.out.types[t];
+    const TypeStore &h = c.in.store[t];
+    const TypeShape s = type_shape(t);
+    const unsigned cnt = (unsigned)order.size();
+    const bool tiled = c.in.tiled;
+    d.order.resize(cnt);
+    if (cnt == 0) return "";
+    #pragma omp parallel for schedule(static) num_threads(host_threads())
+    for (long long i = 0; i < (long long)cnt; i++) d.order[i] = h.ids[order[i]];
+    auto P = [&](unsigned i, int k) { return h.params[(size_t)order[i] * s.nParams + k]; };
+    auto B = [&](unsigned i, int k) {
+        const unsigned raw = h.bodies[(size_t)order[i] * s.nBodies + k];
+        if (is_rb_body(t, k)) return raw;
+        if (tiled && !c.homedGlobal[raw]) {  // lives in the shared memory of CTA (tile % C) of the executing cluster
+            const unsigned tl = c.tileOf[raw];
+            return kSmemFlag | ((tl % c.out.res.C) << kRankShift) | tile_swizzle(c.out.slot[raw] - c.out.tileStart[tl]);
+        }
+        return c.out.slot[raw];
+    };
+
+    if (verbose()) fprintf(stderr, "[pbd_b200] flatten:   type %d (%u constraints)\n", t, cnt);
+    lap("  order ids");
+    // indices
+    if (s.nBodies == 2) {
+        d.idx2.resize(cnt);
+        #pragma omp parallel for schedule(static) num_threads(host_threads())
+        for (long long i = 0; i < (long long)cnt; i++) d.idx2[i] = make_uint2(B(i, 0), B(i, 1));
+    } else if (s.nBodies == 4) {
+        d.idx4.resize(cnt);
+        #pragma omp parallel for schedule(static) num_threads(host_threads())
+        for (long long i = 0; i < (long long)cnt; i++) d.idx4[i] = make_uint4(B(i, 0), B(i, 1), B(i, 2), B(i, 3));
+    } else {
+        for (int k = 0; k < 3; k++) {
+            d.idx3[k].resize(cnt);
+            #pragma omp parallel for schedule(static) num_threads(host_threads())
+            for (long long i = 0; i < (long long)cnt; i++) d.idx3[k][i] = B(i, k);
+        }
+    }
+
+    lap("  indices");
+    // geometry: the parameter columns of the table, with two exceptions
+    const PackColumns pc = pack_columns(t);
+    bool fromColumns = true;
+    if (t == PBD_ISOBENDING || t == PBD_ISOBENDING_XPBD) {
+        // the rank-one form Q = -Kp Kp^T of init_IsometricBendingConstraint: gv[0] = Kp; a user-modified Q anywhere in this type:
+        // the literal 4x4 evaluation (variant 1) for the whole type, Q row by row from the columns of the table
+        d.gv[0].resize(cnt);
+        int notRank1 = 0;
+        #pragma omp parallel for schedule(static) num_threads(host_threads()) reduction(| : notRank1)
+        for (long long i = 0; i < (long long)cnt; i++) {
+            float Q[16], Kp[4] = {0.f, 0.f, 0.f, 0.f};
+            for (int k = 0; k < 16; k++) Q[k] = P((unsigned)i, 1 + k);
+            if (!factor_rank1(Q, Kp)) notRank1 |= 1;
+            d.gv[0][i] = make_float4(Kp[0], Kp[1], Kp[2], Kp[3]);
+        }
+        if (notRank1 && tiled) return "resident mode: IsometricBending with a user-modified Q matrix (not of the rank-one form) is evaluated by the per-bucket kernels only (use PBD_MODE_GRAPH)";
+        d.variant = notRank1 ? 1 : 0;
+        fromColumns = notRank1 != 0;
+    }
+    if (t == PBD_SHAPEMATCHING)
+        for (unsigned i = 0; i < cnt; i++)
+            for (int k = 20; k < 24; k++) if (!(P(i, k) >= 1.0f)) return "ShapeMatching constraint: numClusters must be >= 1";
+    auto col = [&](unsigned i, int k) { return k < 0 ? 0.0f : P(i, k); };
+    for (int k = 0; k < kMaxGeoV && fromColumns; k++) {
+        const signed char *cc = pc.gv[k];
+        if (cc[0] < 0 && cc[1] < 0 && cc[2] < 0 && cc[3] < 0) continue;
+        d.gv[k].resize(cnt);
+        #pragma omp parallel for schedule(static) num_threads(host_threads())
+        for (long long i = 0; i < (long long)cnt; i++) d.gv[k][i] = make_float4(col(i, cc[0]), col(i, cc[1]), col(i, cc[2]), col(i, cc[3]));
+    }
+    for (int k = 0; k < kMaxGeoS; k++) {
+        if (pc.gs[k] < 0) continue;
+        d.gs[k].resize(cnt);
+        #pragma omp parallel for schedule(static) num_threads(host_threads())
+        for (long long i = 0; i < (long long)cnt; i++) d.gs[k][i] = P(i, pc.gs[k]);
+    }
+    lap("  geometry");
+    // material parameters: one uniform per type when every constraint agrees, else a per-constraint array
+    for (int k = 0; k < kMaxMat; k++) {
+        const int cm = pc.mat[k];
+        if (cm < 0) continue;
+        const float first = P(0, cm);
+        int differs = 0;
+        #pragma omp parallel for schedule(static) num_threads(host_threads()) reduction(| : differs) if (cnt > 100000)
+        for (long long i = 1; i < (long long)cnt; i++) differs |= (P((unsigned)i, cm) != first) ? 1 : 0;
+        d.matU[k] = first;
+        if (differs) {
+            d.mat[k].resize(cnt);
+            #pragma omp parallel for schedule(static) num_threads(host_threads())
+            for (long long i = 0; i < (long long)cnt; i++) d.mat[k][i] = P(i, cm);
+        }
+    }
+    lap("  material");
+    return "";
+}
+
+// resident mode: colour ranges of the bucket table, the per-tile runs, and who waits for whom in the X flag protocol.  Tile j is a
+// neighbour of tile i when an X item of i and an X item of j touch the same global-homed particle, or an X item of one of them touches
+// a particle homed in the other: exactly the tiles whose global-memory accesses i's X items and i's global-homed particles have to be
+// ordered with.  xMask[i][0] bit k: neighbour k has global-homed particles (arrives in the integration phase); xMask[i][1 + c] bit k:
+// neighbour k has X items in colour c.
+static std::string build_phase_tables(Ctx &c, const std::vector<unsigned> (&order)[PBD_NUM_TYPES]) {
+    ImagePlan &pl = c.out;
+    const std::vector<Bucket> &buckets = pl.buckets;
+    const std::vector<unsigned> &tileOff = pl.tileOff;
+    const unsigned T = c.nTiles();
+    std::vector<unsigned> &colourStart = pl.colourStart;
+    colourStart.clear();
+    for (size_t i = 0; i < buckets.size(); i++)
+        if (i == 0 || buckets[i].colour != buckets[i - 1].colour) colourStart.push_back((unsigned)i);
+    pl.res.nColours = (unsigned)colourStart.size();
+    colourStart.push_back((unsigned)buckets.size());
+    if (tileOff.size() != buckets.size() * (2 * (size_t)T + 1)) return "flatten: internal error (tile runs)";
+    const unsigned nC = pl.res.nColours;
+    auto run = [&](size_t bi, unsigned t) { return &tileOff[bi * (2 * (size_t)T + 1) + 2 * t]; };  // [0] X items .. [1] others .. [2]
+    // (global-homed particle, tile) pairs: its home tile and every tile that executes an X item touching it
+    std::vector<std::pair<unsigned, unsigned>> touch;
+    for (unsigned i = 0; i < c.in.n; i++) if (c.homedGlobal[i]) touch.emplace_back(i, c.tileOf[i]);
+    for (size_t bi = 0; bi < buckets.size(); bi++) {
+        const Bucket &b = buckets[bi];
+        const int nb = type_shape(b.type).nBodies;
+        for (unsigned t = 0; t < T; t++)
+            for (unsigned k = run(bi, t)[0]; k < run(bi, t)[1]; k++) {
+                const unsigned *bod = &c.in.store[b.type].bodies[(size_t)order[b.type][b.first + k] * nb];
+                for (int j = 0; j < nb; j++) if (!is_rb_body(b.type, j) && c.homedGlobal[bod[j]]) touch.emplace_back(bod[j], t);
+            }
+    }
+    std::sort(touch.begin(), touch.end());
+    touch.erase(std::unique(touch.begin(), touch.end()), touch.end());
+    std::vector<unsigned char> adj((size_t)T * T, 0);
+    for (size_t lo = 0, hi; lo < touch.size(); lo = hi) {
+        for (hi = lo + 1; hi < touch.size() && touch[hi].first == touch[lo].first; hi++) {}
+        for (size_t a = lo; a < hi; a++)
+            for (size_t cc = lo; cc < hi; cc++)
+                if (touch[a].second != touch[cc].second) adj[(size_t)touch[a].second * T + touch[cc].second] = 1;
+    }
+    std::vector<unsigned char> hasX((size_t)T * (1 + nC), 0);  // [tile][phase]: the tile arrives in the phase
+    for (unsigned t = 0; t < T; t++) {
+        hasX[(size_t)t * (1 + nC)] = (pl.tileStart[t + 1] - pl.tileStart[t] - pl.tileSmem[t]) != 0;
+        for (unsigned cl = 0; cl < nC; cl++)
+            for (unsigned bi = colourStart[cl]; bi < colourStart[cl + 1]; bi++) hasX[(size_t)t * (1 + nC) + 1 + cl] |= run(bi, t)[1] != run(bi, t)[0];
+    }
+    std::vector<unsigned> &nbr = pl.xNbr, &mask = pl.xMask, nNbr(T, 0u);
+    nbr.assign((size_t)T * kMaxXNeighbours, 0u); mask.assign((size_t)T * (1 + nC), 0u);
+    for (unsigned i = 0; i < T; i++) {
+        for (unsigned k = 0; k < kMaxXNeighbours; k++) nbr[(size_t)i * kMaxXNeighbours + k] = i;  // unused lanes: never polled (mask bit 0)
+        for (unsigned j = 0; j < T; j++) {
+            if (!adj[(size_t)i * T + j]) continue;
+            if (nNbr[i] == kMaxXNeighbours)
+                return fmt("resident mode: tile %u shares global-homed particles with more than %u other tiles (the constraints reach too far "
+                           "across the scene for the resident mode; use PBD_MODE_GRAPH)", i, kMaxXNeighbours);
+            const unsigned k = nNbr[i]++;
+            nbr[(size_t)i * kMaxXNeighbours + k] = j;
+            for (unsigned p = 0; p <= nC; p++) mask[(size_t)i * (1 + nC) + p] |= (unsigned)hasX[(size_t)j * (1 + nC) + p] << k;
+        }
+    }
+    if (verbose()) {
+        const unsigned numConstraints = c.in.numConstraints;
+        unsigned long long xItems = 0, mxRun = 0;
+        std::vector<unsigned long long> perTile(T, 0);  // items a tile executes over one sweep
+        unsigned long long lockstep = 0;                // ... and the sum over the colours of the largest tile's items of the colour
+        for (unsigned cl = 0; cl < nC; cl++) {
+            unsigned long long mx = 0;
+            for (unsigned t = 0; t < T; t++) {
+                unsigned long long items = 0;
+                for (unsigned bi = colourStart[cl]; bi < colourStart[cl + 1]; bi++) {
+                    xItems += run(bi, t)[1] - run(bi, t)[0];
+                    items += run(bi, t)[2] - run(bi, t)[0];
+                    mxRun = std::max<unsigned long long>(mxRun, run(bi, t)[2] - run(bi, t)[0]);
+                }
+                perTile[t] += items; mx = std::max(mx, items);
+            }
+            lockstep += mx;
+        }
+        std::vector<unsigned> hist(kMaxXNeighbours + 1, 0u);
+        for (unsigned t = 0; t < T; t++) hist[nNbr[t]]++;
+        fprintf(stderr, "[pbd_b200] resident: %u colours, %zu buckets, %.2f %% X items, largest run of a tile in a bucket %llu (mean %.0f)\n",
+                nC, buckets.size(), 100.0 * xItems / std::max(1u, numConstraints), mxRun, (double)numConstraints / std::max<size_t>(1, buckets.size()) / T);
+        fprintf(stderr, "[pbd_b200] resident: X neighbours per tile (count x tiles):");
+        for (unsigned k = 0; k <= kMaxXNeighbours; k++) if (hist[k]) fprintf(stderr, " %u x %u", k, hist[k]);
+        const unsigned long long mxTile = T ? *std::max_element(perTile.begin(), perTile.end()) : 0;
+        fprintf(stderr, "\n[pbd_b200] resident: items per sweep, sum over colours of the largest tile %llu, largest tile over all colours %llu (lockstep penalty %.2f %%)\n",
+                lockstep, mxTile, mxTile ? 100.0 * ((double)lockstep / mxTile - 1.0) : 0.0);
+        // the constraint stream of one sweep as this image streams it from DRAM: the 32-bit indices, the per-constraint geometry and
+        // material arrays, the multipliers (read and written)
+        double idxBytes = 0, constBytes = 0;
+        for (const Bucket &b : buckets) {
+            const TypePlan &a = pl.types[b.type];
+            double perItem = type_shape(b.type).xpbd ? 8.0 : 0.0;
+            for (int k = 0; k < kMaxGeoV; k++) perItem += !a.gv[k].empty() ? 16.0 : 0.0;
+            for (int k = 0; k < kMaxGeoS; k++) perItem += !a.gs[k].empty() ? 4.0 : 0.0;
+            for (int k = 0; k < kMaxMat; k++) perItem += !a.mat[k].empty() ? 4.0 : 0.0;
+            idxBytes += b.count * 4.0 * type_shape(b.type).nBodies; constBytes += b.count * perItem;
+        }
+        fprintf(stderr, "[pbd_b200] resident: constraint stream per sweep %.1f MB: indices %.1f MB, constants and multipliers %.1f MB\n",
+                (idxBytes + constBytes) * 1e-6, idxBytes * 1e-6, constBytes * 1e-6);
+    }
+    return "";
+}
+
+std::string plan_image(const PlanInput &in, ImagePlan &out) {
+    Lap lap;
+    std::vector<std::pair<int, unsigned>> map;
+    std::string err = validate_bodies(in);
+    if (err.empty()) err = build_id_map(in.store, in.numConstraints, map);
+    if (!err.empty()) return err;
+    Ctx c{in, out, {}, {}};
+    if (in.tiled) {
+        if (!(err = place_in_tiles(c)).empty()) return err;
+    } else {
+        out.slot.resize(in.n);
+        for (unsigned i = 0; i < in.n; i++) out.slot[i] = particle_slot(i, in.n);
+    }
+    lap("validation + placement");
+    std::vector<unsigned> order[PBD_NUM_TYPES];
+    order_buckets(c, map, order);
+    lap("bucket ordering");
+    if (!(err = check_colouring(c, order)).empty()) return err;
+    lap("colouring validity check");
+    for (int t = 0; t < PBD_NUM_TYPES; t++)
+        if (!(err = pack_type(c, t, order[t], lap)).empty()) return err;
+    lap("SoA arrays");
+    if (in.tiled && !(err = build_phase_tables(c, order)).empty()) return err;
+    lap("phase tables");
+    return "";
+}
+
+}  // namespace pbd_b200

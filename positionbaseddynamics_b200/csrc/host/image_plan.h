@@ -1,0 +1,70 @@
+// positionbaseddynamics_b200/csrc/host/image_plan.h
+//
+// The planner of the device image: constraints + colour groups (+ rest positions for the resident mode) -> every array the
+// engine uploads, in host memory.  Host-only C++ (no CUDA API call): the engine gathers its inputs, plans, and uploads the
+// result (engine.cu:flatten_image); the CPU tests run the same code on scenes of their own (tests/test_image_plan.py).
+#pragma once
+#include <functional>
+#include <string>
+#include <utility>
+#include <vector>
+#include "../device_image.h"
+#include "pbd_model.h"
+
+namespace pbd_b200 {
+
+// PBD_B200_VERBOSE: flatten and the resident planner report their stages and timings on stderr
+bool verbose();
+// stage timings on stderr (PBD_B200_VERBOSE)
+struct Lap {
+    double prev;
+    Lap();
+    void operator()(const char *what);
+};
+
+// body k of a constraint of this type is a rigid body (else a particle)
+inline bool is_rb_body(int type, int k) { return type == PBD_BALLJOINT || (type == PBD_RB_PARTICLE_BALLJOINT && k == 0); }
+// Body indices of `count` constraints of one type against the particle and rigid-body counts, all threads.  Returns the position in
+// `bodies` of the last index out of range, or -1.
+long long bad_body_index(int type, const unsigned *bodies, size_t count, unsigned n, unsigned nRb);
+// insertion id -> (type, local index) of the N constraints in store[PBD_NUM_TYPES]; "" or why the ids are not a permutation of 0..N-1
+std::string build_id_map(const TypeStore *store, unsigned N, std::vector<std::pair<int, unsigned>> &map);
+
+// What the planner needs to know about the model and, for the resident mode, about the device.
+struct PlanInput {
+    const TypeStore *store;                        // [PBD_NUM_TYPES] constraints by type, as added
+    unsigned numConstraints, n, nRb;
+    const std::vector<unsigned> *groupOff, *groupIds;  // the colour groups (CSR over insertion ids)
+    bool tiled;                                    // the resident mode's image
+    const float4 *x0;                              // tiled: rest positions by host index
+    unsigned forcedG, forcedC;                     // tiled: G x C clusters x CTAs (PBD_B200_CLUSTERS), 0 = chosen from the model
+    int smCount;
+    std::function<int(unsigned mask)> maxClusters; // tiled: clusters of one CTA with kMaxDynamicSmem the device keeps co-resident
+};
+
+// One constraint type's arrays in device order (the host side of pbdk::TypeArrays).
+struct TypePlan {
+    PodVector<unsigned> order;                     // device position -> insertion id
+    PodVector<uint2> idx2; PodVector<uint4> idx4; PodVector<unsigned> idx3[3];
+    PodVector<float4> gv[pbdk::kMaxGeoV];
+    PodVector<float> gs[pbdk::kMaxGeoS], mat[pbdk::kMaxMat];  // mat[k] empty: every constraint has matU[k]
+    float matU[pbdk::kMaxMat] = {};
+    int variant = 0;
+};
+
+// Launch shape of a resident image: G clusters x C CTAs (one tile each), block size and type mask of the instantiation.
+struct ResidentShape { unsigned G = 0, C = 0, threads = 0, xThreads = 0, mask = 0, tileCap = 0, nColours = 0; };
+
+struct ImagePlan {
+    std::vector<unsigned> slot;                    // host particle index -> device slot
+    std::vector<pbdk::Bucket> buckets;             // colour after colour
+    TypePlan types[PBD_NUM_TYPES];
+    // resident only (resident.cuh: ResidentArgs)
+    ResidentShape res;
+    std::vector<unsigned> colourStart, tileOff, tileStart, tileSmem, xNbr, xMask;
+};
+
+// Plans the image of `in` into `out`; returns "" or why the model cannot be flattened (for this mode).
+std::string plan_image(const PlanInput &in, ImagePlan &out);
+
+}  // namespace pbd_b200

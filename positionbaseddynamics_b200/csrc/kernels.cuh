@@ -161,18 +161,6 @@ __device__ __forceinline__ void project_streamed(float4 *pos, const TypeArrays &
     project_streamed_acc<T, GlobalAcc, VAR>(GlobalAcc{pos}, a, i, s, dt, iterZero);
 }
 
-// Sets of constraint types, one bit per type.  k_step_resident (resident.cuh) is instantiated per mask, the leanest that
-// covers the model: the everything-kernel is 20k instructions and 226 registers, and every colour phase jumps through it.
-constexpr unsigned type_bit(int t) { return 1u << t; }
-constexpr unsigned kMaskClothXPBD = type_bit(PBD_DISTANCE_XPBD) | type_bit(PBD_ISOBENDING_XPBD);
-constexpr unsigned kMaskCloth = kMaskClothXPBD | type_bit(PBD_DISTANCE) | type_bit(PBD_ISOBENDING);
-constexpr unsigned kMaskLight = type_bit(PBD_DISTANCE) | type_bit(PBD_DISTANCE_XPBD) | type_bit(PBD_DIHEDRAL) | type_bit(PBD_ISOBENDING) |
-                                type_bit(PBD_ISOBENDING_XPBD) | type_bit(PBD_VOLUME) | type_bit(PBD_VOLUME_XPBD) | type_bit(PBD_FEMTRIANGLE);
-// FEM solids (cfg3): tets with FEM / volume constraints; and cloth + FEM solids + the coupling joints (cfg4)
-constexpr unsigned kMaskFem = type_bit(PBD_FEMTET) | type_bit(PBD_FEMTET_XPBD) | type_bit(PBD_VOLUME) | type_bit(PBD_VOLUME_XPBD);
-constexpr unsigned kMaskSolid = kMaskCloth | kMaskFem | type_bit(PBD_FEMTRIANGLE) | type_bit(PBD_BALLJOINT) | type_bit(PBD_RB_PARTICLE_BALLJOINT);
-constexpr unsigned kMaskAll = (1u << PBD_NUM_TYPES) - 1u;
-
 // The one list of all constraint types: dispatch a statement on the runtime type, restricted to the types of MASK (T is a
 // constant inside the statement; a type outside the mask does nothing).
 #define PBD_CASE_TYPE(MASK, TT, ...) case TT: if constexpr ((MASK) & type_bit(TT)) { constexpr int T = TT; __VA_ARGS__ } break;

@@ -20,19 +20,18 @@
 //     32).  A phase is thus no grid-wide barrier: a CTA waits for the few tiles around it, not for the slowest of all.  The
 //     round trip overlaps the shared-memory work the other warps do in the meantime; those never touch the flags.  A scene that
 //     fits one cluster (G = 1) has no X items.
-//   Two regimes are used (engine.cu:choose_resident_shape): ONE cluster of up to 16 CTAs for scenes whose colour phases are small
+//   Two regimes are used (host/image_plan.cpp:choose_resident_shape): ONE cluster of up to 16 CTAs for scenes whose colour phases are small
 //   (cfg1 / cfg3 / cfg4), and G = #SMs clusters of ONE CTA for big scenes (cfg2 / cfg5: 132 independent CTAs on an H100; the SINGLE
 //   instantiations: plain LDS / STS, __syncthreads).
 //   The order of the items inside a tile's run is chosen at flatten time so that the lanes of a quarter-warp hit distinct 16-byte
-//   bank groups (engine.cu, "bank-group fill").
+//   bank groups (host/image_plan.cpp:bank_group_fill).
 //
 // Exactness.  Colour phases are kept: inside a colour no two constraints share a particle (checked at flatten time),
 // across colours every constraint reads exactly what the reference's sequential sweep would have produced, whichever CTA
 // executes it.  The projection code is the one the per-bucket kernels inline (project_streamed_acc), compiled with
 // -fmad=false + explicit fmaf, so the result is bit-identical to the graph / launch modes (tested).
 //
-// Index encoding (flatten time): bit 31 set -> shared memory: bits 30..27 = CTA rank inside the executing cluster, bits
-// 26..0 = slot inside that CTA's tile;  bit 31 clear -> device slot in the global float4 array.
+// Index encoding: device_image.h (kSmemFlag).
 // Constraint order inside a (colour,type) bucket: by executing tile, inside a tile the X items (touching a global-homed
 // particle) first; tileOff[bucket][2t], [2t+1], [2t+2] delimit the two runs of tile t (relative to the bucket's `first`).
 #pragma once
@@ -42,28 +41,11 @@
 
 namespace pbdk {
 
-constexpr unsigned kSmemFlag = 0x80000000u;
-constexpr unsigned kRankShift = 27u;
-constexpr unsigned kLocalMask = (1u << kRankShift) - 1u;
-constexpr size_t kMaxDynamicSmem = 227u * 1024u;  // what a CTA may opt in to on sm_90
-// Bank swizzle of a tile: slot s lives at tile[s ^ ((s >> 3) & 7)] (a permutation inside every aligned 64-slot block; tileCap is a
-// multiple of 64).  One colour's constraints touch slots 2 or 3 apart, i.e. only half of the eight 16-byte bank groups per
-// quarter-warp; the swizzle spreads such strides over all eight.
-__host__ __device__ __forceinline__ unsigned tile_swizzle(unsigned s) { return s ^ ((s >> 3) & 7u); }
-constexpr int kMaxClusterCtas = 16;   // non-portable cluster size (opt-in attribute), one GPC
-// Dynamic shared memory of a CTA: [tile: tileCap float4][run table: nBuckets x RunEntry][xMask: 1 + nColours][colourStart: nColours + 1]
-// [xNbr: kMaxXNeighbours]
-// this CTA's two runs of one bucket (absolute indices into the type's arrays); rotR: where the run of shared-memory items starts in the
-// colour's concatenated item sequence, modulo the number of threads that share it (the buckets of one colour go to different threads)
-struct RunEntry { int type; unsigned firstX, nX, firstR, nR, rotR, pad0, pad1; };
-constexpr unsigned kMaxXNeighbours = 32;  // one lane of the first X warp per neighbour
+// (the index encoding, tile swizzle, run table and shared-memory layout of the image are defined in device_image.h)
 constexpr unsigned kXFlagStride = 16;     // unsigned long longs: every CTA's arrival flag on its own 128-byte line
 // PBD_B200_TRACE record per (phase, CTA): [0] phase start, [1] X items done, [2] other items done + colour arrive issued,
 // [3] colour wait returned, [4] X wait returned (0 where the CTA has no X items in the phase); tools/trace_resident.py
 constexpr unsigned kTraceSlots = 5;
-__host__ __device__ inline size_t resident_smem_bytes(unsigned tileCap, unsigned nBuckets, unsigned nColours) {
-    return (size_t)tileCap * sizeof(float4) + (size_t)nBuckets * sizeof(RunEntry) + (size_t)(2u * nColours + 2u + kMaxXNeighbours) * sizeof(unsigned);
-}
 
 struct ResidentArgs {
     float4 *pos, *vel, *oldp, *lastp;

@@ -60,8 +60,8 @@ enum pbd_solver_mode {
     PBD_MODE_LAUNCH = 2,     /* plain stream launches (debug / per-kernel profiling) */
     PBD_MODE_JACOBI = 3,     /* comparison path, NOT the reference's algorithm: colours ignored, one launch per type and sweep, corrections
                                 accumulated with float4 atomicAdd and averaged per particle (rigid-body joints are not supported) */
-    PBD_MODE_AUTO = 4        /* default: RESIDENT where it is the faster exact mode (cloth and FEM models of >= 40,000 particles that fit), else GRAPH; both produce
-                                the same bits, so the choice is invisible in the results (pbd_get_mode reports it) */
+    PBD_MODE_AUTO = 4        /* default: RESIDENT where it is the faster exact mode (cloth and FEM models of >= 40,000 particles), else GRAPH, and GRAPH for a model
+                                RESIDENT refuses (decided when the model is flattened); both produce the same bits (pbd_get_mode reports the choice) */
 };
 
 typedef struct pbd_stats {

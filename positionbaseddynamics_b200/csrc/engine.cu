@@ -99,7 +99,7 @@ struct pbd_engine {
     // parameters
     float dt = 0.005f; unsigned subSteps = 5, maxIter = 1; int velMethod = 0; float g[3] = {0.f, -9.81f, 0.f};
     int mode = PBD_MODE_AUTO;             // requested (pbd_set_mode)
-    int active = PBD_MODE_GRAPH;          // what the current image runs in: == mode, or the resolution of PBD_MODE_AUTO
+    int active = PBD_MODE_GRAPH;          // what the current image runs in: == mode, or the resolution of PBD_MODE_AUTO (image_plan.h)
     bool autoNoResident = false;          // PBD_MODE_AUTO: the resident mode was tried for this model and refused
     // graph cache
     cudaGraphExec_t graphExec = nullptr;
@@ -128,7 +128,6 @@ struct pbd_engine {
     DevBuf dSlot, dSlotOld, relayoutTmp;
     // resident mode (resident.cuh): the launch shape of the current image
     pbd_b200::ResidentShape res;
-    bool resChecked = false;              // co-residency of the clusters verified for the current image
     DevBuf dColourStart, dTileOff, dTileStart, dTileSmem, dXNbr, dXMask, dXFlags;
     unsigned long long xLaunch = 0;       // resident launches so far: the high word of the X arrival flags
 };
@@ -604,10 +603,10 @@ extern "C" int pbd_set_mode(pbd_engine *e, int mode) {
     if (!e) return fail("null engine");
     if (mode != PBD_MODE_GRAPH && mode != PBD_MODE_RESIDENT && mode != PBD_MODE_LAUNCH && mode != PBD_MODE_JACOBI && mode != PBD_MODE_AUTO) return fail("unknown solver mode %d", mode);
     if (mode == e->mode) return 0;
-    // the resident image encodes indices differently; with AUTO on either side the resolution may change
-    if (mode == PBD_MODE_AUTO || e->mode == PBD_MODE_AUTO || (mode == PBD_MODE_RESIDENT) != (e->active == PBD_MODE_RESIDENT)) e->imageDirty = true;
-    e->mode = mode; e->autoNoResident = false;
-    if (mode != PBD_MODE_AUTO) e->active = mode;
+    // only the resident image is laid out differently: the others run the image they share
+    const int active = pbd_b200::preferred_mode(mode, e->host, e->n, e->numConstraints, false);
+    if ((active == PBD_MODE_RESIDENT) != (e->active == PBD_MODE_RESIDENT)) e->imageDirty = true;
+    e->mode = mode; e->active = active; e->autoNoResident = false;
     drop_graph(e);
     return 0;
 }
@@ -657,32 +656,6 @@ static int resident_max_clusters(const pbd_engine *e, unsigned mask, unsigned C,
         return 0;
     });
 }
-static int flatten_image(pbd_engine *e);
-// PBD_MODE_AUTO: the resident mode where it is the faster exact mode -- models made of cloth and FEM / volume constraints with at
-// least kAutoResidentMinParticles particles (cfg2, cfg3, cfg5); small models (cfg1), mixed models with rigid coupling and the heavy
-// solver families (cfg4) stay in graph mode -- falling back to the graph mode when the resident mode refuses the model.
-// Measured on an H100 80GB HBM3 (SXM, 400 W, 1980 MHz), XPBD cloth 1 x 20, ms per step graph / resident: 100x100 0.66 / 0.79,
-// 200x200 0.93 / 0.92, 300x300 1.20 / 1.02; cfg1 (50x50) 0.129 / 0.183; cfg3 (44,541 particles) 8.03 / 7.69.
-constexpr unsigned kAutoResidentMinParticles = 40000;
-static bool auto_prefers_resident(const pbd_engine *e) {
-    if (e->autoNoResident || e->numConstraints == 0 || e->n < kAutoResidentMinParticles) return false;
-    unsigned present = 0;
-    for (int t = 0; t < PBD_NUM_TYPES; t++) if (!e->host[t].ids.empty()) present |= 1u << t;
-    return (present & ~(kMaskCloth | kMaskFem)) == 0 || (present & ~kMaskLight) == 0;
-}
-static int flatten(pbd_engine *e) {
-    if (!e->imageDirty) return 0;
-    if (e->mode != PBD_MODE_AUTO) { e->active = e->mode; return flatten_image(e); }
-    e->active = auto_prefers_resident(e) ? PBD_MODE_RESIDENT : PBD_MODE_GRAPH;
-    int rc = flatten_image(e);
-    if (rc && e->active == PBD_MODE_RESIDENT) {  // refused (does not fit, user-modified bending Q, ...): the graph mode takes every model
-        if (verbose()) fprintf(stderr, "[pbd_b200] auto mode: resident refused (%s), using the graph mode\n", g_err.c_str());
-        e->autoNoResident = true; e->active = PBD_MODE_GRAPH; e->imageDirty = true;
-        rc = flatten_image(e);
-    }
-    return rc;
-}
-
 // colour groups when none were given: the reference-order-preserving first fit on the GPU (colouring.cuh), the host version as the fallback
 static int colour_if_needed(pbd_engine *e) {
     if (e->groupsSet) return 0;
@@ -722,16 +695,16 @@ static int upload_type(pbd_engine *e, int t, pbd_b200::TypePlan &p) {
     return 0;
 }
 
-// constraints + colour groups -> the device image of the active mode: the planner's inputs gathered, the plan uploaded
-static int flatten_image(pbd_engine *e) {
+// constraints + colour groups -> the device image of the requested mode (the planner resolves PBD_MODE_AUTO): the planner's inputs
+// gathered, the plan uploaded
+static int flatten(pbd_engine *e) {
     if (!e->imageDirty) return 0;
     CKE(use(e));
     pbd_b200::Lap lap;
     CKE(colour_if_needed(e));
     drop_graph(e);
-    const bool tiled = (e->active == PBD_MODE_RESIDENT);
     std::vector<float4> x0;  // resident: rest positions by host index
-    if (tiled && e->n) {
+    if (pbd_b200::preferred_mode(e->mode, e->host, e->n, e->numConstraints, e->autoNoResident) == PBD_MODE_RESIDENT && e->n) {
         std::vector<float4> raw(e->n);
         CK(cudaStreamSynchronize(e->stream));
         CK(cudaMemcpy(raw.data(), e->pos0.p, (size_t)e->n * sizeof(float4), cudaMemcpyDeviceToHost));
@@ -739,21 +712,26 @@ static int flatten_image(pbd_engine *e) {
         for (unsigned i = 0; i < e->n; i++) x0[i] = raw[e->slot[i]];
     }
     lap("colouring + rest positions");
-    pbd_b200::PlanInput in{e->host, e->numConstraints, e->n, e->nRb, &e->groupOff, &e->groupIds, tiled, x0.data(), 0u, 0u, e->smCount, nullptr};
+    pbd_b200::PlanInput in{e->host, e->numConstraints, e->n, e->nRb, &e->groupOff, &e->groupIds, e->mode, x0.data(), 0u, 0u, e->smCount, nullptr, e->autoNoResident};
     if (const char *g = getenv("PBD_B200_CLUSTERS")) {  // development knob "GxC"
         unsigned gg = 0, cc = 0;
         if (sscanf(g, "%ux%u", &gg, &cc) == 2 && gg >= 1 && cc >= 1 && cc <= (unsigned)kMaxClusterCtas && (cc & (cc - 1)) == 0) { in.forcedG = gg; in.forcedC = cc; }
     }
-    in.maxClusters = [&](unsigned mask) { int mc = 0; return resident_max_clusters(e, mask, 1u, kMaxDynamicSmem, &mc) ? 0 : mc; };
+    in.maxClusters = [&](unsigned mask, unsigned C, size_t smem) { int mc = 0; return resident_max_clusters(e, mask, C, smem, &mc) ? 0 : mc; };
     pbd_b200::ImagePlan plan;
     const std::string err = pbd_b200::plan_image(in, plan);
+    if (!plan.residentRefusal.empty()) {
+        if (verbose()) fprintf(stderr, "[pbd_b200] auto mode: resident refused (%s), using the graph mode\n", plan.residentRefusal.c_str());
+        e->autoNoResident = true;
+    }
     if (!err.empty()) return fail("%s", err.c_str());
+    e->active = plan.mode;
     CKE(relayout(e, plan.slot));
     for (int t = 0; t < PBD_NUM_TYPES; t++) CKE(upload_type(e, t, plan.types[t]));
     e->buckets.swap(plan.buckets);
     CKE(upload_vec(e->dBuckets, e->buckets, e->stream));
-    if (tiled) {
-        e->res = plan.res; e->resChecked = false;
+    if (plan.mode == PBD_MODE_RESIDENT) {
+        e->res = plan.res;
         CKE(upload_vec(e->dTileStart, plan.tileStart, e->stream));
         CKE(upload_vec(e->dTileSmem, plan.tileSmem, e->stream));
         CKE(upload_vec(e->dColourStart, plan.colourStart, e->stream));
@@ -908,28 +886,7 @@ static int enqueue_step_launches(pbd_engine *e, cudaStream_t s, unsigned long lo
 }
 
 // One step as one launch of k_step_resident: grid = G x C CTAs in clusters of C, one CTA per SM, all co-resident
-// (the X items of different clusters wait for each other).
-static int launch_resident(pbd_engine *e, cudaStream_t s, ResidentArgs &ra) {
-    const size_t smem = resident_smem_bytes(ra.tileCap, ra.nBuckets, ra.nColours);
-    if (smem > kMaxDynamicSmem) return fail("resident mode: a CTA needs %zu bytes of shared memory (tile of %u particles + phase tables), %zu available", smem, ra.tileCap, kMaxDynamicSmem);
-    const pbd_b200::ResidentShape &r = e->res;
-    if (r.G > 1 && !e->resChecked) {
-        int mc = 0;
-        CKE(resident_max_clusters(e, r.mask, r.C, smem, &mc));
-        if ((unsigned)mc < r.G)
-            return fail("resident mode: the device runs %d clusters of %u CTAs at a time, the scene needs %u co-resident", mc, r.C, r.G);
-        e->resChecked = true;
-    }
-    return with_resident_kernel(r.mask, r.C, [&](auto kernel) -> int {
-        CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynamicSmem));
-        if (r.C > 8) CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
-        cudaLaunchConfig_t cfg; cudaLaunchAttribute attr[1];
-        resident_launch_config(r.mask, r.C, r.G * r.C, smem, s, cfg, attr);
-        CK(cudaLaunchKernelEx(&cfg, kernel, ra));
-        return 0;
-    });
-}
-
+// (the X items of different clusters wait for each other; the planner admitted the image only if the device keeps them so).
 static int enqueue_step_resident(pbd_engine *e, cudaStream_t s, unsigned long long *launches) {
     const float h = e->dt / (float)e->subSteps;
     ResidentArgs ra;
@@ -975,7 +932,15 @@ static int enqueue_step_resident(pbd_engine *e, cudaStream_t s, unsigned long lo
             if (FILE *f = fopen(path, "wb")) { fwrite(h.data(), sizeof(unsigned long long), h.size(), f); fclose(f); }
         }
     } dump{e, s, tracePath, (size_t)kTracePhases * ra.nTiles * kTraceSlots};
-    return launch_resident(e, s, ra);
+    const pbd_b200::ResidentShape &r = e->res;
+    return with_resident_kernel(r.mask, r.C, [&](auto kernel) -> int {
+        CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynamicSmem));
+        if (r.C > 8) CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+        cudaLaunchConfig_t cfg; cudaLaunchAttribute attr[1];
+        resident_launch_config(r.mask, r.C, r.G * r.C, r.smem, s, cfg, attr);
+        CK(cudaLaunchKernelEx(&cfg, kernel, ra));
+        return 0;
+    });
 }
 
 // Jacobi comparison path (kernels.cuh): per sweep one launch per type over all its constraints + the averaging pass
@@ -1106,7 +1071,7 @@ static int enqueue_contacts(pbd_engine *e, cudaStream_t s, unsigned long long *l
     return 0;
 }
 
-static int ensure_graph(pbd_engine *e, unsigned long long *launchesPerStep) {
+static int ensure_graph(pbd_engine *e) {
     if (e->graphValid) return 0;
     cudaGraph_t graph = nullptr;
     CK(cudaStreamBeginCapture(e->stream, cudaStreamCaptureModeThreadLocal));
@@ -1119,7 +1084,7 @@ static int ensure_graph(pbd_engine *e, unsigned long long *launchesPerStep) {
     cudaGraphDestroy(graph);
     if (err != cudaSuccess) return fail("cudaGraphInstantiate -> %s", cudaGetErrorString(err));
     e->graphValid = true;
-    *launchesPerStep = L;
+    e->graphLaunches = L;
     return 0;
 }
 
@@ -1130,27 +1095,10 @@ extern "C" int pbd_step(pbd_engine *e, unsigned nSteps) {
     CK(cudaEventRecord(e->evStart, e->stream));
     for (unsigned s = 0; s < nSteps; s++) {
         unsigned long long L = 0;
-        if (e->active == PBD_MODE_LAUNCH) {
-            CKE(enqueue_step_launches(e, e->stream, &L));
-        } else if (e->active == PBD_MODE_RESIDENT) {
-            int rc = enqueue_step_resident(e, e->stream, &L);
-            if (rc && e->mode == PBD_MODE_AUTO) {  // e.g. the clusters cannot be co-resident on this device: run the step in graph mode instead
-                e->autoNoResident = true; e->imageDirty = true;
-                CKE(flatten(e));
-                unsigned long long LL = 0;
-                if (!e->graphValid) { CKE(ensure_graph(e, &LL)); e->graphLaunches = LL; }
-                CK(cudaGraphLaunch(e->graphExec, e->stream));
-                L = e->graphLaunches; rc = 0;
-            }
-            CKE(rc);
-        } else if (e->active == PBD_MODE_JACOBI) {
-            CKE(enqueue_step_jacobi(e, e->stream, &L));
-        } else {
-            unsigned long long LL = 0;
-            if (!e->graphValid) { CKE(ensure_graph(e, &LL)); e->graphLaunches = LL; }
-            CK(cudaGraphLaunch(e->graphExec, e->stream));
-            L = e->graphLaunches;
-        }
+        if (e->active == PBD_MODE_LAUNCH) CKE(enqueue_step_launches(e, e->stream, &L));
+        else if (e->active == PBD_MODE_RESIDENT) CKE(enqueue_step_resident(e, e->stream, &L));
+        else if (e->active == PBD_MODE_JACOBI) CKE(enqueue_step_jacobi(e, e->stream, &L));
+        else { CKE(ensure_graph(e)); CK(cudaGraphLaunch(e->graphExec, e->stream)); L = e->graphLaunches; }
         CKE(enqueue_contacts(e, e->stream, &L));
         e->stats.kernel_launches += L;
         e->stats.steps++;

@@ -102,6 +102,7 @@ static bool factor_rank1(const float *Q, float Kp[4]) {
 struct Ctx {
     const PlanInput &in;
     ImagePlan &out;
+    bool tiled;                               // the resident mode's image
     std::vector<unsigned> tileOf;             // host particle -> tile (cluster = tile / C, rank = tile % C)
     std::vector<unsigned char> homedGlobal;   // host particle lives in global memory (touched by a constraint that spans clusters)
     unsigned nTiles() const { return out.res.G * out.res.C; }
@@ -169,7 +170,7 @@ static std::string choose_resident_shape(const PlanInput &in, ResidentShape &r) 
         // Too big for one cluster: one independent CTA per SM (clusters of 1).  Larger clusters have fewer X items but idle SMs (a
         // cluster must fit a GPC) and a colour barrier that waits for the slowest of C CTAs; with C = 1 the colour barrier is a
         // __syncthreads.
-        const int mc = in.maxClusters(r.mask);
+        const int mc = in.maxClusters(r.mask, 1u, kMaxDynamicSmem);
         if (mc < 1) return fmt("resident mode: a CTA with %zu bytes of shared memory is not schedulable on this device", kMaxDynamicSmem);
         C = 1; G = (unsigned)std::min(mc, in.smCount);
     }
@@ -329,7 +330,7 @@ static void bank_group_fill(KeyedItem *run, size_t cnt, int t, const Ctx &c, Wav
 // global-homed particle) before the others, the shared-memory runs bank-group filled, and the runs of every tile appended to tileOff:
 // [2 tile] X items, [2 tile + 1] the others.
 static void sort_bucket(const Ctx &c, unsigned g, int t, std::vector<unsigned> &items, std::vector<unsigned> &tileOff) {
-    const bool tiled = c.in.tiled;
+    const bool tiled = c.tiled;
     const bool joint = (t == PBD_BALLJOINT || t == PBD_RB_PARTICLE_BALLJOINT);
     const int nb = type_shape(t).nBodies;
     const unsigned *bod = c.in.store[t].bodies.data();
@@ -395,7 +396,7 @@ static void order_buckets(Ctx &c, const std::vector<std::pair<int, unsigned>> &m
         for (int t = 0; t < PBD_NUM_TYPES; t++) {
             if (items[t].empty()) continue;
             const bool joint = (t == PBD_BALLJOINT || t == PBD_RB_PARTICLE_BALLJOINT);
-            if (!joint || c.in.tiled) sort_bucket(c, g, t, items[t], c.out.tileOff);
+            if (!joint || c.tiled) sort_bucket(c, g, t, items[t], c.out.tileOff);
             Bucket b; b.type = t; b.first = (unsigned)order[t].size(); b.count = (unsigned)items[t].size(); b.colour = g;
             c.out.buckets.push_back(b);
             order[t].insert(order[t].end(), items[t].begin(), items[t].end());
@@ -459,7 +460,7 @@ static std::string pack_type(Ctx &c, int t, const std::vector<unsigned> &order, 
     const TypeStore &h = c.in.store[t];
     const TypeShape s = type_shape(t);
     const unsigned cnt = (unsigned)order.size();
-    const bool tiled = c.in.tiled;
+    const bool tiled = c.tiled;
     d.order.resize(cnt);
     if (cnt == 0) return "";
     #pragma omp parallel for schedule(static) num_threads(host_threads())
@@ -655,14 +656,29 @@ static std::string build_phase_tables(Ctx &c, const std::vector<unsigned> (&orde
     return "";
 }
 
-std::string plan_image(const PlanInput &in, ImagePlan &out) {
+// PBD_MODE_AUTO: the resident mode where it is the faster exact mode -- models made of cloth and FEM / volume constraints with at
+// least kAutoResidentMinParticles particles (cfg2, cfg3, cfg5); small models (cfg1), mixed models with rigid coupling and the heavy
+// solver families (cfg4) stay in graph mode, and so does a model the resident mode has refused.
+// Measured on an H100 80GB HBM3 (SXM, 400 W, 1980 MHz), XPBD cloth 1 x 20, ms per step graph / resident: 100x100 0.66 / 0.79,
+// 200x200 0.93 / 0.92, 300x300 1.20 / 1.02; cfg1 (50x50) 0.129 / 0.183; cfg3 (44,541 particles) 8.03 / 7.69.
+constexpr unsigned kAutoResidentMinParticles = 40000;
+int preferred_mode(int requested, const TypeStore *store, unsigned n, unsigned numConstraints, bool residentRefused) {
+    if (requested != PBD_MODE_AUTO) return requested;
+    if (residentRefused || numConstraints == 0 || n < kAutoResidentMinParticles) return PBD_MODE_GRAPH;
+    unsigned present = 0;
+    for (int t = 0; t < PBD_NUM_TYPES; t++) if (!store[t].ids.empty()) present |= 1u << t;
+    return ((present & ~(kMaskCloth | kMaskFem)) == 0 || (present & ~kMaskLight) == 0) ? PBD_MODE_RESIDENT : PBD_MODE_GRAPH;
+}
+
+// the image of the resident mode (tiled) or of the others
+static std::string plan_mode(const PlanInput &in, bool tiled, ImagePlan &out) {
     Lap lap;
     std::vector<std::pair<int, unsigned>> map;
     std::string err = validate_bodies(in);
     if (err.empty()) err = build_id_map(in.store, in.numConstraints, map);
     if (!err.empty()) return err;
-    Ctx c{in, out, {}, {}};
-    if (in.tiled) {
+    Ctx c{in, out, tiled, {}, {}};
+    if (tiled) {
         if (!(err = place_in_tiles(c)).empty()) return err;
     } else {
         out.slot.resize(in.n);
@@ -677,9 +693,26 @@ std::string plan_image(const PlanInput &in, ImagePlan &out) {
     for (int t = 0; t < PBD_NUM_TYPES; t++)
         if (!(err = pack_type(c, t, order[t], lap)).empty()) return err;
     lap("SoA arrays");
-    if (in.tiled && !(err = build_phase_tables(c, order)).empty()) return err;
+    if (tiled && !(err = build_phase_tables(c, order)).empty()) return err;
     lap("phase tables");
-    return "";
+    if (!tiled) return "";
+    // admitted when every CTA gets its shared memory and all G x C are co-resident (the X items of different clusters wait for each other)
+    ResidentShape &r = out.res;
+    r.smem = resident_smem_bytes(r.tileCap, (unsigned)out.buckets.size(), r.nColours);
+    if (r.smem > kMaxDynamicSmem)
+        return fmt("resident mode: a CTA needs %zu bytes of shared memory (tile of %u particles + phase tables), %zu available", r.smem, r.tileCap, kMaxDynamicSmem);
+    const int mc = in.maxClusters(r.mask, r.C, r.smem);
+    return (unsigned)mc < r.G ? fmt("resident mode: the device runs %d clusters of %u CTAs at a time, the scene needs %u co-resident", mc, r.C, r.G) : "";
+}
+
+std::string plan_image(const PlanInput &in, ImagePlan &out) {
+    out.mode = preferred_mode(in.mode, in.store, in.n, in.numConstraints, in.residentRefused);
+    const std::string err = plan_mode(in, out.mode == PBD_MODE_RESIDENT, out);
+    if (err.empty() || in.mode != PBD_MODE_AUTO || out.mode != PBD_MODE_RESIDENT) return err;
+    // AUTO, and the resident mode refused the model (does not fit, user-modified bending Q, ...): the graph image, planned from scratch
+    out = ImagePlan{};
+    out.residentRefusal = err;
+    return plan_mode(in, false, out);
 }
 
 }  // namespace pbd_b200

@@ -2,10 +2,11 @@
 //
 // The planner of the device image: constraints + colour groups (+ rest positions for the resident mode) -> every array the
 // engine uploads, in host memory.  Host-only C++ (no CUDA API call): the engine gathers its inputs, plans, and uploads the
-// result (engine.cu:flatten_image); the CPU tests run the same code on scenes of their own (tests/test_image_plan.py).
+// result (engine.cu:flatten); the CPU tests run the same code on scenes of their own (tests/test_image_plan.py).
 #pragma once
 #include <functional>
 #include <string>
+#include <type_traits>
 #include <utility>
 #include <vector>
 #include "../device_image.h"
@@ -30,16 +31,26 @@ long long bad_body_index(int type, const unsigned *bodies, size_t count, unsigne
 // insertion id -> (type, local index) of the N constraints in store[PBD_NUM_TYPES]; "" or why the ids are not a permutation of 0..N-1
 std::string build_id_map(const TypeStore *store, unsigned N, std::vector<std::pair<int, unsigned>> &map);
 
+// The mode an image is planned for: `requested`, or for PBD_MODE_AUTO the resident mode where it is faster and not refused yet, else graph.
+int preferred_mode(int requested, const TypeStore *store, unsigned n, unsigned numConstraints, bool residentRefused);
+
+// Clusters of C CTAs with `smem` bytes each the device keeps co-resident; a query of the type mask alone answers for every cluster shape.
+struct ClusterQuery : std::function<int(unsigned mask, unsigned C, size_t smem)> {
+    using function::function;
+    template <class F, class = std::enable_if_t<std::is_invocable_r_v<int, F, unsigned>>> ClusterQuery(F f) : function([f](unsigned m, unsigned, size_t) { return f(m); }) {}
+};
+
 // What the planner needs to know about the model and, for the resident mode, about the device.
 struct PlanInput {
     const TypeStore *store;                        // [PBD_NUM_TYPES] constraints by type, as added
     unsigned numConstraints, n, nRb;
     const std::vector<unsigned> *groupOff, *groupIds;  // the colour groups (CSR over insertion ids)
-    bool tiled;                                    // the resident mode's image
-    const float4 *x0;                              // tiled: rest positions by host index
-    unsigned forcedG, forcedC;                     // tiled: G x C clusters x CTAs (PBD_B200_CLUSTERS), 0 = chosen from the model
+    int mode;                                      // the requested pbd_solver_mode (PBD_MODE_GRAPH = 0, PBD_MODE_RESIDENT = 1, ...)
+    const float4 *x0;                              // resident: rest positions by host index
+    unsigned forcedG, forcedC;                     // resident: G x C clusters x CTAs (PBD_B200_CLUSTERS), 0 = chosen from the model
     int smCount;
-    std::function<int(unsigned mask)> maxClusters; // tiled: clusters of one CTA with kMaxDynamicSmem the device keeps co-resident
+    ClusterQuery maxClusters;                      // resident: what the device keeps co-resident
+    bool residentRefused = false;                  // PBD_MODE_AUTO: the resident mode refused this model before
 };
 
 // One constraint type's arrays in device order (the host side of pbdk::TypeArrays).
@@ -52,10 +63,12 @@ struct TypePlan {
     int variant = 0;
 };
 
-// Launch shape of a resident image: G clusters x C CTAs (one tile each), block size and type mask of the instantiation.
-struct ResidentShape { unsigned G = 0, C = 0, threads = 0, xThreads = 0, mask = 0, tileCap = 0, nColours = 0; };
+// Launch shape of a resident image: G clusters x C CTAs (one tile each), block size and type mask of the instantiation, smem per CTA.
+struct ResidentShape { unsigned G = 0, C = 0, threads = 0, xThreads = 0, mask = 0, tileCap = 0, nColours = 0; size_t smem = 0; };
 
 struct ImagePlan {
+    int mode = PBD_MODE_GRAPH;                     // what the image runs in: the requested mode, PBD_MODE_AUTO resolved
+    std::string residentRefusal;                   // PBD_MODE_AUTO fell back to the graph mode: why the resident mode refused the model
     std::vector<unsigned> slot;                    // host particle index -> device slot
     std::vector<pbdk::Bucket> buckets;             // colour after colour
     TypePlan types[PBD_NUM_TYPES];
@@ -64,7 +77,7 @@ struct ImagePlan {
     std::vector<unsigned> colourStart, tileOff, tileStart, tileSmem, xNbr, xMask;
 };
 
-// Plans the image of `in` into `out`; returns "" or why the model cannot be flattened (for this mode).
+// Plans the image of `in` into `out`; returns "" or why the model cannot be flattened (for this mode and, resident, this device).
 std::string plan_image(const PlanInput &in, ImagePlan &out);
 
 }  // namespace pbd_b200

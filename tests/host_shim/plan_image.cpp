@@ -1,9 +1,10 @@
 // TEST INFRASTRUCTURE: runs the image planner of libpbd_b200.so (csrc/host/image_plan.h) on a model read from a file and writes every
 // array of the plan to another, for tests/test_image_plan.py.  Needs no GPU: the co-residency query answers a constant from the input.
 //   plan_image <input> <output>
-// input : u32 n, nRb, numConstraints, tiled, forcedG, forcedC, smCount, maxClusters, nGroups; u32 groupOff[nGroups + 1];
+// input : u32 n, nRb, numConstraints, mode, residentRefused, forcedG, forcedC, smCount, maxClusters, nGroups; u32 groupOff[nGroups + 1];
 //         u32 groupIds[numConstraints]; float4 x0[n]; per type: u32 count, u32 ids[count], u32 bodies[count nBodies], f32 params[count nParams]
-// output: records of (char name[32], u64 bytes, bytes of data); "error" first, the plan's arrays after it when it is empty
+// output: records of (char name[32], u64 bytes, bytes of data); "error" and "residentRefusal" first, the plan's mode and arrays after
+//         them when the error is empty
 #include "host/image_plan.h"
 #include <cstdint>
 #include <cstdio>
@@ -27,7 +28,8 @@ template <class V> static void put(const char *name, int t, int k, const V &v) {
 
 int main(int argc, char **argv) {
     if (argc != 3 || !(fin = fopen(argv[1], "rb")) || !(fout = fopen(argv[2], "wb"))) { fprintf(stderr, "usage: plan_image <input> <output>\n"); return 2; }
-    const unsigned n = get1(), nRb = get1(), N = get1(), tiled = get1(), G = get1(), C = get1(), smCount = get1(), maxClusters = get1(), nGroups = get1();
+    const unsigned n = get1(), nRb = get1(), N = get1(), mode = get1(), refused = get1(), G = get1(), C = get1(), smCount = get1(), maxClusters = get1(),
+                   nGroups = get1();
     std::vector<unsigned> groupOff(nGroups + 1), groupIds(N);
     get(groupOff.data(), groupOff.size()); get(groupIds.data(), N);
     std::vector<float4> x0(n);
@@ -40,11 +42,14 @@ int main(int argc, char **argv) {
         h.ids.resize(cnt); h.bodies.resize((size_t)cnt * s.nBodies); h.params.resize((size_t)cnt * s.nParams);
         get(h.ids.data(), h.ids.size()); get(h.bodies.data(), h.bodies.size()); get(h.params.data(), h.params.size());
     }
-    const PlanInput in{store, N, n, nRb, &groupOff, &groupIds, tiled != 0, x0.data(), G, C, (int)smCount, [=](unsigned) { return (int)maxClusters; }};
+    const PlanInput in{store, N, n, nRb, &groupOff, &groupIds, (int)mode, x0.data(), G, C, (int)smCount, [=](unsigned) { return (int)maxClusters; },
+                       refused != 0};
     ImagePlan p;
     const std::string err = plan_image(in, p);
     put("error", err);
+    put("residentRefusal", p.residentRefusal);
     if (err.empty()) {
+        put("mode", std::vector<int>{p.mode});
         put("slot", p.slot);
         put("buckets", p.buckets);
         for (int t = 0; t < PBD_NUM_TYPES; t++) {
@@ -59,6 +64,7 @@ int main(int argc, char **argv) {
         }
         const ResidentShape &r = p.res;
         put("res", std::vector<unsigned>{r.G, r.C, r.threads, r.xThreads, r.mask, r.tileCap, r.nColours});
+        put("smem", std::vector<uint64_t>{r.smem});
         put("colourStart", p.colourStart); put("tileOff", p.tileOff); put("tileStart", p.tileStart); put("tileSmem", p.tileSmem);
         put("xNbr", p.xNbr); put("xMask", p.xMask);
     }

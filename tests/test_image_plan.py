@@ -19,6 +19,7 @@ XPBD = {1, 4, 8, 10}
 ISOBENDING, BALLJOINT, RB_PARTICLE_BALLJOINT = (3, 4), 13, 14
 SMEM_FLAG, RANK_SHIFT = 0x80000000, 27
 MAX_SMEM, MAX_NBR = 227 * 1024, 32
+GRAPH, RESIDENT, LAUNCH, JACOBI, AUTO = range(5)  # pbd_solver_mode
 # Parameter columns of the SoA arrays (the layout of include/pbd_b200.h): float4 geometry arrays (-1: zero), scalar arrays, material slots
 _C4 = lambda *cs: [tuple(range(c, c + 4)) for c in cs]
 COLUMNS = {0: ([], [0], [1]), 1: ([], [0], [1]), 2: ([], [0], [1]), 7: ([], [0], [1]), 8: ([], [0], [1]),
@@ -73,9 +74,10 @@ class Scene:
         return col
 
 
-def plan(driver, tmp_path, sc, tiled, shape=(0, 0), threads=None, tag="p"):
+def plan(driver, tmp_path, sc, mode, shape=(0, 0), threads=None, tag="p", refused=False, max_clusters=132):
+    """The plan of `sc` in `mode` on a device of 132 SMs that keeps `max_clusters` clusters of any shape co-resident."""
     x0 = np.zeros((sc.n, 4), np.float32); x0[:, :3] = sc.x0
-    head = [sc.n, sc.nrb, sc.N, int(tiled), shape[0], shape[1], 132, 132, len(sc.off) - 1]
+    head = [sc.n, sc.nrb, sc.N, mode, int(refused), shape[0], shape[1], 132, max_clusters, len(sc.off) - 1]
     parts = [np.asarray(head, np.uint32), sc.off, sc.ids, x0]
     for ids, b, p in sc.store:
         parts += [np.asarray([len(ids)], np.uint32), ids, b, p]
@@ -100,6 +102,17 @@ def u32(p, k):
     return np.frombuffer(p[k], np.uint32)
 
 
+def mode_of(p):
+    assert p["error"] == b""
+    return int(np.frombuffer(p["mode"], np.int32)[0])
+
+
+def same_image(a, b, *skip):
+    """The plans `a` and `b` are byte-identical, apart from the refusal and the records in `skip`."""
+    drop = {"raw", "residentRefusal"} | set(skip)
+    return {k: v for k, v in a.items() if k not in drop} == {k: v for k, v in b.items() if k not in drop}
+
+
 def indices(p, t, cnt):
     if NB[t] == 2:
         return u32(p, "idx2_%d" % t).reshape(cnt, 2)
@@ -111,6 +124,7 @@ def indices(p, t, cnt):
 def check_plan(sc, p, tiled):
     """Every invariant of the plan `p` of scene `sc`; returns (G, C)."""
     assert p["error"] == b""
+    assert (mode_of(p) == RESIDENT) == tiled
     n = sc.n
     slot = u32(p, "slot")
     assert np.array_equal(np.sort(slot), np.arange(n))                        # a permutation
@@ -118,6 +132,7 @@ def check_plan(sc, p, tiled):
     buckets = np.frombuffer(p["buckets"], np.int32).reshape(-1, 4)          # type, first, count, colour
     G, C, threads, xthreads, mask, tile_cap, n_col = (int(v) for v in u32(p, "res"))
     T = G * C
+    smem = int(np.frombuffer(p["smem"], np.uint64)[0])
     colour = sc.colour_of()
 
     # buckets: colour after colour, each exactly its colour group's constraints of its type, no body twice in a colour
@@ -149,6 +164,8 @@ def check_plan(sc, p, tiled):
         assert len(tstart) == T + 1 and tstart[0] == 0 and tstart[-1] == n and (np.diff(tstart) >= 0).all()
         assert (tsmem <= np.diff(tstart)).all() and (tsmem <= tile_cap).all() and tile_cap % 64 == 0
         assert tile_cap * 16 + len(buckets) * 32 + (2 * n_col + 2 + MAX_NBR) * 4 <= MAX_SMEM
+        assert smem == tile_cap * 16 + len(buckets) * 32 + (2 * n_col + 2 + MAX_NBR) * 4  # what the kernel lays out
+        assert 16 * tile_cap <= smem <= MAX_SMEM
         ptile = np.searchsorted(tstart, slot, "right") - 1                   # tile of every host particle
         homed_global = (slot - tstart[ptile]) >= tsmem[ptile]
         assert n_col == len(np.unique(buckets[:, 3]))
@@ -242,6 +259,8 @@ def check_plan(sc, p, tiled):
                     bit = (int(xmask[i, ph]) >> k) & 1
                     assert bit == (k < len(got) and has_x[got[k], ph]), (i, ph, k)
         assert all(i in want[j] for i in range(T) for j in want[i])
+    else:
+        assert smem == 0
     return G, C
 
 
@@ -265,13 +284,55 @@ def test_plan_invariants(driver, tmp_path, build, shape):
     sc = Scene.of(build)
     tiled = shape != "graph"
     G, C = (int(v) for v in shape.split("x")) if tiled else (0, 0)
-    got = check_plan(sc, plan(driver, tmp_path, sc, tiled, (G, C)), tiled)
+    got = check_plan(sc, plan(driver, tmp_path, sc, RESIDENT if tiled else GRAPH, (G, C)), tiled)
     if tiled:
         assert got == (G, C)
 
 
+def test_auto_mode_resolution(driver, tmp_path):
+    """PBD_MODE_AUTO: the resident image for a cloth of at least 40,000 particles, the graph image for a smaller cloth and for rigid
+    coupling.  The explicit modes get what they ask for; graph, launch and Jacobi share one image."""
+    big = Scene.of(cloth(210))
+    p = plan(driver, tmp_path, big, AUTO)
+    assert mode_of(p) == RESIDENT and p["residentRefusal"] == b""
+    check_plan(big, p, True)
+    assert same_image(p, plan(driver, tmp_path, big, RESIDENT, tag="r"))
+    graph = plan(driver, tmp_path, big, GRAPH, tag="g")
+    check_plan(big, graph, False)
+    for mode in (LAUNCH, JACOBI):
+        q = plan(driver, tmp_path, big, mode, tag="m%d" % mode)
+        assert mode_of(q) == mode and same_image(q, graph, "mode")
+    for build in (cloth(40), rig):
+        sc = Scene.of(build)
+        q = plan(driver, tmp_path, sc, AUTO, tag="a")
+        assert mode_of(q) == GRAPH and q["residentRefusal"] == b""
+        assert same_image(q, plan(driver, tmp_path, sc, GRAPH, tag="g"))
+
+
+def test_too_few_coresident_clusters(driver, tmp_path):
+    """A device that keeps 8 clusters co-resident refuses 37 of them: an error under PBD_MODE_RESIDENT, the graph image under AUTO."""
+    sc = Scene.of(cloth(210))
+    assert sc.n >= 40000
+    p = plan(driver, tmp_path, sc, RESIDENT, (37, 1), max_clusters=8, tag="r")
+    assert p["error"] == b"resident mode: the device runs 8 clusters of 1 CTAs at a time, the scene needs 37 co-resident"
+    q = plan(driver, tmp_path, sc, AUTO, (37, 1), max_clusters=8, tag="a")
+    assert mode_of(q) == GRAPH and q["residentRefusal"] == p["error"]
+    assert same_image(q, plan(driver, tmp_path, sc, GRAPH, (37, 1), max_clusters=8, tag="g"))
+
+
+def test_auto_mode_does_not_retry_a_refused_model(driver, tmp_path):
+    """Once the resident mode has refused a model, AUTO plans the graph image without trying it again (a device without co-resident
+    clusters would refuse it once more)."""
+    sc = Scene.of(cloth(210))
+    assert b"the device runs 0 clusters" in plan(driver, tmp_path, sc, AUTO, max_clusters=0)["residentRefusal"]
+    p = plan(driver, tmp_path, sc, AUTO, refused=True, max_clusters=0, tag="a")
+    assert mode_of(p) == GRAPH and p["residentRefusal"] == b""
+    assert same_image(p, plan(driver, tmp_path, sc, GRAPH, tag="g"))
+
+
 def test_long_range_scene_is_refused(driver, tmp_path):
-    """The random long-range distance constraints of test_gpu_resident_neighbours.py in 64 independent tiles."""
+    """The random long-range distance constraints of test_gpu_resident_neighbours.py in 64 independent tiles: refused by the resident
+    mode, planned in graph mode under AUTO."""
     from positionbaseddynamics_b200.model import first_fit_colouring
     rng = np.random.default_rng(7)
     side = 200
@@ -287,8 +348,11 @@ def test_long_range_scene_is_refused(driver, tmp_path):
     bodies = np.zeros((N, 4), np.uint32); bodies[:, :2] = pairs
     params = np.zeros((N, 24), np.float32); params[:, 0] = rest; params[:, 1] = 1.0e4
     sc = Scene(side * side, 0, np.full(N, 1), bodies, params, off, ids, x)
-    p = plan(driver, tmp_path, sc, True, (64, 1))
+    p = plan(driver, tmp_path, sc, RESIDENT, (64, 1))
     assert b"more than 32 other tiles" in p["error"]
+    q = plan(driver, tmp_path, sc, AUTO, (64, 1), tag="a")
+    assert mode_of(q) == GRAPH and b"more than 32 other tiles" in q["residentRefusal"]
+    assert same_image(q, plan(driver, tmp_path, sc, GRAPH, (64, 1), tag="g"))
 
 
 def test_modified_bending_q(driver, tmp_path):
@@ -296,8 +360,20 @@ def test_modified_bending_q(driver, tmp_path):
     sc = Scene.of(lambda m: scenes.cloth(m, 20, 20, cloth_method=1, bending_method=2))
     ids, b, prm = sc.store[3]
     prm[5, 1:17] += np.eye(4, dtype=np.float32).reshape(-1) * 0.5
-    assert b"user-modified Q" in plan(driver, tmp_path, sc, True, (1, 1))["error"]
-    p = plan(driver, tmp_path, sc, False)
+    assert b"user-modified Q" in plan(driver, tmp_path, sc, RESIDENT, (1, 1))["error"]
+    p = plan(driver, tmp_path, sc, GRAPH)
+    assert int(np.frombuffer(p["variant3"], np.int32)[0]) == 1
+    check_plan(sc, p, False)
+
+
+def test_modified_bending_q_under_auto(driver, tmp_path):
+    """The same in a cloth big enough for AUTO to try the resident mode: refused, and planned in graph mode instead."""
+    sc = Scene.of(lambda m: scenes.cloth(m, 200, 200, cloth_method=1, bending_method=2))
+    assert sc.n >= 40000
+    ids, b, prm = sc.store[3]
+    prm[5, 1:17] += np.eye(4, dtype=np.float32).reshape(-1) * 0.5
+    p = plan(driver, tmp_path, sc, AUTO)
+    assert mode_of(p) == GRAPH and b"user-modified Q" in p["residentRefusal"]
     assert int(np.frombuffer(p["variant3"], np.int32)[0]) == 1
     check_plan(sc, p, False)
 
@@ -305,6 +381,6 @@ def test_modified_bending_q(driver, tmp_path):
 def test_plan_is_deterministic(driver, tmp_path):
     """Byte-identical plans with one host thread and with four (each in a process of its own: the thread count is read once)."""
     sc = Scene.of(cloth(300))
-    one = plan(driver, tmp_path, sc, True, (37, 1), threads=1, tag="t1")
-    four = plan(driver, tmp_path, sc, True, (37, 1), threads=4, tag="t4")
+    one = plan(driver, tmp_path, sc, RESIDENT, (37, 1), threads=1, tag="t1")
+    four = plan(driver, tmp_path, sc, RESIDENT, (37, 1), threads=4, tag="t4")
     assert one["error"] == b"" and one["raw"] == four["raw"]

@@ -60,7 +60,8 @@ enum pbd_solver_mode {
     PBD_MODE_LAUNCH = 2,     /* plain stream launches (debug / per-kernel profiling) */
     PBD_MODE_JACOBI = 3,     /* comparison path, NOT the reference's algorithm: colours ignored, one launch per type and sweep, corrections
                                 accumulated with float4 atomicAdd and averaged per particle (rigid-body joints are not supported) */
-    PBD_MODE_AUTO = 4        /* default: RESIDENT where it is the faster exact mode (cloth and FEM models of >= 40,000 particles), else GRAPH, and GRAPH for a model
+    PBD_MODE_AUTO = 4        /* default: RESIDENT where it is the faster exact mode (cloth and FEM models of >= 40,000 particles, or batches of >= 32 replicas
+                                of them -- 64 for FEMTriangle / Dihedral / Volume models, pbd_set_replicas), else GRAPH, and GRAPH for a model
                                 RESIDENT refuses (decided when the model is flattened); both produce the same bits (pbd_get_mode reports the choice) */
 };
 
@@ -176,6 +177,23 @@ int pbd_set_contact_params(pbd_engine *e, float tolerance, float stiffness, unsi
  * (particle, body) and the number found (which may exceed what was kept) */
 int pbd_record_contacts(pbd_engine *e, unsigned capacity);
 int pbd_get_contacts(pbd_engine *e, pbd_contact *out, unsigned capacity, unsigned *count);
+
+/* ---- Replica batch: K independent copies of one model's state stepped together on one device ---------------------------------
+ * One engine holds one model (particles, constraints, groups, parameters) and K copies of its state; one pbd_step advances all K,
+ * and replica r advances bit for bit as an engine of its own started from replica r's state would, in every mode.  The constraint
+ * image is shared by the replicas and uploaded once.
+ *  - Calls that DEFINE the model describe one replica: pbd_set_particles (n, and it sets EVERY replica to the given state),
+ *    pbd_add_constraints, the colour groups, pbd_set_params.
+ *  - Calls that MOVE state take the whole batch, replica after replica: pbd_set_attr / pbd_get_attr (K*n*3 floats), pbd_set_masses
+ *    (K*n: each replica may pin other particles), pbd_step_host / pbd_step_host_async (K*n*3 per array), pbd_get_lambdas (K*count
+ *    multipliers, `ids` count insertion ids).  Constraint parameters are shared.
+ *  - pbd_get_stats: projections and bytes_per_step count every replica; num_particles and num_constraints are per replica.
+ *  - K > 1 is refused with rigid bodies or joints, with colliders and in PBD_MODE_JACOBI.  PBD_MODE_RESIDENT runs one cluster of CTAs
+ *    per replica and refuses a replica that does not fit one cluster; PBD_MODE_AUTO then runs the graph mode.
+ * pbd_set_replicas: 1 <= K <= 65535 and K*n < 2^31.  Every replica starts as a copy of replica 0's current state (x, v, x0, oldX,
+ * lastX, masses), the XPBD multipliers at zero, and the image is planned again.  At K = 1 every call behaves as for one scene. */
+int pbd_set_replicas(pbd_engine *e, unsigned K);
+int pbd_get_replicas(pbd_engine *e, unsigned *K);
 
 int pbd_get_lambdas(pbd_engine *e, int type, float *dst, unsigned *ids); /* debug: per-type XPBD multipliers + insertion ids */
 int pbd_get_stats(pbd_engine *e, pbd_stats *out);

@@ -24,7 +24,7 @@ SYMBOLS = ["pbd_last_error", "pbd_device_count", "pbd_create", "pbd_destroy", "p
            "pbd_get_attr", "pbd_set_masses", "pbd_set_rigid_bodies", "pbd_get_rigid_bodies", "pbd_clear_constraints", "pbd_add_constraints", "pbd_num_bodies",
            "pbd_num_params", "pbd_set_groups", "pbd_color_first_fit", "pbd_color_first_fit_device", "pbd_pin_host", "pbd_unpin_host", "pbd_get_num_groups", "pbd_get_groups",
            "pbd_set_params", "pbd_set_mode", "pbd_get_mode", "pbd_step", "pbd_sync", "pbd_step_host", "pbd_step_host_async", "pbd_step_host_wait",
-           "pbd_get_lambdas", "pbd_get_stats", "pbd_profile_step",
+           "pbd_get_lambdas", "pbd_get_stats", "pbd_profile_step", "pbd_set_replicas", "pbd_get_replicas",
            "pbd_set_colliders", "pbd_set_contact_params", "pbd_record_contacts", "pbd_get_contacts"]
 
 
@@ -100,6 +100,8 @@ def lib():
         _lib.pbd_get_lambdas.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
         _lib.pbd_get_stats.argtypes = [C.c_void_p, C.POINTER(Stats)]
         _lib.pbd_profile_step.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        _lib.pbd_set_replicas.argtypes = [C.c_void_p, C.c_uint]
+        _lib.pbd_get_replicas.argtypes = [C.c_void_p, C.POINTER(C.c_uint)]
     return _lib
 
 
@@ -131,13 +133,20 @@ def num_params(t):
 
 
 class Engine:
-    """One engine <-> one CUDA device + one stream (pbd_create / pbd_destroy)."""
+    """One engine <-> one CUDA device + one stream (pbd_create / pbd_destroy).
+
+    A replica batch (set_replicas(K), K > 1) steps K independent copies of the model's state at once: the particle state calls then
+    take and return (K, n, 3) / (K, n) arrays and lambdas() (K, count); at K = 1 the shapes are those of one scene."""
 
     def __init__(self, device=0, stream=None):
         self._h = C.c_void_p()
         _ck(lib().pbd_create(int(device), C.c_void_p(stream) if stream else None, C.byref(self._h)))
         self.n = 0
+        self.K = 1
         self._nc = 0  # constraints added so far (sizes the buffer of groups())
+
+    def _batch_shape(self, *tail):
+        return ((self.K,) if self.K > 1 else ()) + (self.n,) + tail
 
     def close(self):
         if self._h:
@@ -159,18 +168,29 @@ class Engine:
         _ck(lib().pbd_set_particles(self._h, self.n, _ptr(x), _ptr(x0), _ptr(v), _ptr(mass)))
 
     def set_attr(self, attr, a):
-        a = _f32(a).reshape(-1, 3); assert len(a) == self.n
+        a = _f32(a).reshape(-1, 3); assert len(a) == self.K * self.n
         _ck(lib().pbd_set_attr(self._h, attr, _ptr(a)))
 
     def get_attr(self, attr=ATTR_X, out=None):
         if out is None:
-            out = np.empty((self.n, 3), dtype=np.float32)
+            out = np.empty(self._batch_shape(3), dtype=np.float32)
         _ck(lib().pbd_get_attr(self._h, attr, _ptr(out)))
         return out
 
     def set_masses(self, mass):
-        mass = _f32(mass).reshape(-1); assert len(mass) == self.n
+        mass = _f32(mass).reshape(-1); assert len(mass) == self.K * self.n
         _ck(lib().pbd_set_masses(self._h, _ptr(mass)))
+
+    # replica batch ---------------------------------------------------------------------------------
+    def set_replicas(self, k):
+        """K copies of replica 0's current state (x, v, x0, oldX, lastX, masses), multipliers zero; the image is re-planned."""
+        _ck(lib().pbd_set_replicas(self._h, int(k)))
+        self.K = int(k)
+
+    def replicas(self):
+        k = C.c_uint(0)
+        _ck(lib().pbd_get_replicas(self._h, C.byref(k)))
+        return k.value
 
     # rigid bodies ----------------------------------------------------------------------------------
     def set_rigid_bodies(self, mass, x, q, inertia, v=None, omega=None):
@@ -254,6 +274,7 @@ class Engine:
         _ck(lib().pbd_sync(self._h))
 
     def step_host(self, n, x_in, v_in, x_out, v_out=None):
+        """Host arrays of K * n * 3 floats (replica after replica), or None."""
         _ck(lib().pbd_step_host(self._h, int(n), _ptr(x_in), _ptr(v_in), _ptr(x_out), _ptr(v_out)))
 
     def step_host_async(self, n, x_in, v_in, x_out, v_out=None):
@@ -281,10 +302,12 @@ class Engine:
         return [buf[i] for i in range(min(cnt.value, capacity))], cnt.value
 
     def lambdas(self, ctype):
+        """(multipliers, insertion ids): multipliers (count,), or (K, count) for a batch."""
         cnt = self.stats().constraints_per_type[ctype]
-        lam = np.zeros(max(cnt, 1), dtype=np.float32); ids = np.zeros(max(cnt, 1), dtype=np.uint32)
+        lam = np.zeros(max(self.K * cnt, 1), dtype=np.float32); ids = np.zeros(max(cnt, 1), dtype=np.uint32)
         _ck(lib().pbd_get_lambdas(self._h, ctype, _ptr(lam), _ptr(ids)))
-        return lam[:cnt], ids[:cnt]
+        lam = lam[:self.K * cnt]
+        return (lam.reshape(self.K, cnt) if self.K > 1 else lam), ids[:cnt]
 
     def stats(self, flatten=True):
         s = Stats()

@@ -114,8 +114,11 @@ constexpr unsigned kMaskSolid = kMaskCloth | kMaskFem | type_bit(PBD_FEMTRIANGLE
 constexpr unsigned kMaskAll = (1u << PBD_NUM_TYPES) - 1u;
 
 // Block size of the resident instantiation of a type mask: the largest it compiles for without spilling (cloth 96 registers,
-// light 128, everything 236).
-constexpr unsigned resident_threads(unsigned mask) { return mask == kMaskClothXPBD ? 640u : (mask == kMaskAll ? 256u : 512u); }
+// light 128, everything 236).  A replica batch's light instantiation keeps the replica loop's state as well: at 512 threads (128
+// registers) it spilled 44-64 bytes where the single-scene one spills 32-36, so it runs 384 threads (up to 168 registers).
+constexpr unsigned resident_threads(unsigned mask, bool batch = false) {
+    return mask == kMaskClothXPBD ? 640u : (mask == kMaskAll ? 256u : (batch && mask == kMaskLight ? 384u : 512u));
+}
 
 // ---- the resident image (resident.cuh) ---------------------------------------------------------------------------------------
 // Index encoding: bit 31 set -> shared memory: bits 30..27 = CTA rank inside the executing cluster, bits 26..0 = slot inside that

@@ -80,8 +80,8 @@ struct pbd_engine {
     bool ownsStream = false;
     int smCount = 132;                    // H100 SXM; read from the device in pbd_create
     size_t l2Bytes = 50u << 20;           // likewise
-    // particles
-    unsigned n = 0;
+    // particles: K replicas of n (pbd_set_replicas), replica r at device slots [r n, (r + 1) n)
+    unsigned n = 0, K = 1;
     DevBuf pos, vel, oldp, lastp, pos0, stage, stage2, massStage, jacobiDelta;
     // rigid bodies coupled through joints (SURVEY.md 8f-1): float4 arrays X(xyz,invMass) Q(x,y,z,w) V(xyz,mass) W(omega) + history + inertia
     unsigned nRb = 0;
@@ -222,9 +222,9 @@ static int relayout(pbd_engine *e, const std::vector<unsigned> &newSlot) {
     CK(cudaMemcpy(e->dSlotOld.p, e->slot.data(), nb, cudaMemcpyHostToDevice));
     e->slot = newSlot;
     CKE(upload_slot_map(e));
-    CKE(e->relayoutTmp.alloc((size_t)e->n * sizeof(float4)));
+    CKE(e->relayoutTmp.alloc((size_t)e->K * e->n * sizeof(float4)));
     for (DevBuf *b : {&e->pos, &e->vel, &e->oldp, &e->lastp, &e->pos0}) {
-        k_relayout<<<(e->n + 255) / 256, 256, 0, e->stream>>>((const float4 *)b->p, (float4 *)e->relayoutTmp.p, e->n, (const unsigned *)e->dSlotOld.p, (const unsigned *)e->dSlot.p);
+        k_relayout<<<dim3((e->n + 255) / 256, e->K), 256, 0, e->stream>>>((const float4 *)b->p, (float4 *)e->relayoutTmp.p, e->n, (const unsigned *)e->dSlotOld.p, (const unsigned *)e->dSlot.p);
         CK(cudaGetLastError());
         CK(cudaStreamSynchronize(e->stream));
         std::swap(b->p, e->relayoutTmp.p); std::swap(b->bytes, e->relayoutTmp.bytes);
@@ -232,12 +232,24 @@ static int relayout(pbd_engine *e, const std::vector<unsigned> &newSlot) {
     return 0;
 }
 
-// host AoS-3 -> staging -> float4 (keeps .w)
-static int upload3(pbd_engine *e, const float *src, float4 *dst, int keepW) {
-    const size_t bytes = (size_t)e->n * 3 * sizeof(float);
+// grid of a per-particle kernel over `replicas` replicas: blockIdx.y = replica (kernels.cuh: k_pack3 ...)
+static dim3 replica_grid(const pbd_engine *e, unsigned replicas) { return dim3(nblk(e->n, 256), replicas); }
+
+// host AoS-3 of the first `replicas` replicas -> staging -> float4 (keeps .w)
+static int upload3(pbd_engine *e, const float *src, float4 *dst, int keepW, unsigned replicas) {
+    const size_t bytes = (size_t)replicas * e->n * 3 * sizeof(float);
     CK(cudaMemcpyAsync(e->stage.p, src, bytes, cudaMemcpyHostToDevice, e->stream));
-    k_pack3<<<nblk(e->n, 256), 256, 0, e->stream>>>((const float *)e->stage.p, dst, e->n, keepW, (const unsigned *)e->dSlot.p);
+    k_pack3<<<replica_grid(e, replicas), 256, 0, e->stream>>>((const float *)e->stage.p, dst, e->n, keepW, (const unsigned *)e->dSlot.p);
     CK(cudaGetLastError());
+    return 0;
+}
+
+// masses of the first `replicas` replicas (n floats each)
+static int set_w(pbd_engine *e, const float *mass, unsigned replicas) {
+    CK(cudaMemcpyAsync(e->massStage.p, mass, (size_t)replicas * e->n * sizeof(float), cudaMemcpyHostToDevice, e->stream));
+    k_set_w<<<replica_grid(e, replicas), 256, 0, e->stream>>>((float4 *)e->pos.p, (float4 *)e->vel.p, (const float *)e->massStage.p, e->n, (const unsigned *)e->dSlot.p);
+    CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(e->stream));  // staging buffers are reused by the next call
     return 0;
 }
 
@@ -245,39 +257,84 @@ extern "C" int pbd_set_masses(pbd_engine *e, const float *mass) {
     if (!e || !mass) return fail("pbd_set_masses: null argument");
     CKE(use(e));
     if (e->n == 0) return 0;
-    CK(cudaMemcpyAsync(e->massStage.p, mass, (size_t)e->n * sizeof(float), cudaMemcpyHostToDevice, e->stream));
-    k_set_w<<<nblk(e->n, 256), 256, 0, e->stream>>>((float4 *)e->pos.p, (float4 *)e->vel.p, (const float *)e->massStage.p, e->n, (const unsigned *)e->dSlot.p);
-    CK(cudaGetLastError());
-    CK(cudaStreamSynchronize(e->stream));  // staging buffers are reused by the next call
+    return set_w(e, mass, e->K);
+}
+
+// replica 0 of a particle array copied to replicas 1 .. K-1 (doubling copies)
+static int broadcast_replica0(pbd_engine *e, DevBuf &b) {
+    const size_t one = (size_t)e->n * sizeof(float4);
+    for (size_t have = 1; have < e->K; have *= 2)
+        CK(cudaMemcpyAsync((char *)b.p + have * one, b.p, std::min(have, (size_t)e->K - have) * one, cudaMemcpyDeviceToDevice, e->stream));
     return 0;
 }
 
 extern "C" int pbd_set_particles(pbd_engine *e, unsigned n, const float *x, const float *x0, const float *v, const float *mass) {
     if (!e || (n && (!x || !mass))) return fail("pbd_set_particles: null argument");
+    const std::string why = pbd_b200::batch_refusal(e->K, n, e->mode, e->nRb, e->host);
+    if (!why.empty()) return fail("pbd_set_particles: %s", why.c_str());
     CKE(use(e));
     CK(cudaStreamSynchronize(e->stream));
     if (n != e->n) { e->imageDirty = true; drop_graph(e); }
     e->n = n;
     const size_t b4 = (size_t)n * sizeof(float4);
-    for (auto *b : {&e->pos, &e->vel, &e->oldp, &e->lastp, &e->pos0}) CKE(b->alloc(b4));
-    CKE(e->stage.alloc((size_t)n * 3 * sizeof(float)));
-    CKE(e->massStage.alloc((size_t)n * sizeof(float)));
+    for (auto *b : {&e->pos, &e->vel, &e->oldp, &e->lastp, &e->pos0}) CKE(b->alloc(b4 * e->K));
+    CKE(e->stage.alloc((size_t)e->K * n * 3 * sizeof(float)));
+    CKE(e->massStage.alloc((size_t)e->K * n * sizeof(float)));
     drop_graph(e);  // buffers may have moved
     e->slot.resize(n); e->imageDirty = true;
     for (unsigned i = 0; i < n; i++) e->slot[i] = particle_slot(i, n);
     if (n == 0) return 0;
     CKE(upload_slot_map(e));
     CK(cudaMemsetAsync(e->vel.p, 0, b4, e->stream));
-    CKE(upload3(e, x, (float4 *)e->pos.p, 0)); CK(cudaStreamSynchronize(e->stream));
-    if (v) { CKE(upload3(e, v, (float4 *)e->vel.p, 0)); CK(cudaStreamSynchronize(e->stream)); }
-    CKE(pbd_set_masses(e, mass));
+    CKE(upload3(e, x, (float4 *)e->pos.p, 0, 1)); CK(cudaStreamSynchronize(e->stream));
+    if (v) { CKE(upload3(e, v, (float4 *)e->vel.p, 0, 1)); CK(cudaStreamSynchronize(e->stream)); }
+    CKE(set_w(e, mass, 1));
     // oldX = lastX = x, x0 = x unless given (ParticleData::addVertex, ParticleData.h:127-137)
     CK(cudaMemcpyAsync(e->oldp.p, e->pos.p, b4, cudaMemcpyDeviceToDevice, e->stream));
     CK(cudaMemcpyAsync(e->lastp.p, e->pos.p, b4, cudaMemcpyDeviceToDevice, e->stream));
     CK(cudaMemcpyAsync(e->pos0.p, e->pos.p, b4, cudaMemcpyDeviceToDevice, e->stream));
-    if (x0) { CKE(upload3(e, x0, (float4 *)e->pos0.p, 1)); }
+    if (x0) { CKE(upload3(e, x0, (float4 *)e->pos0.p, 1, 1)); }
+    for (DevBuf *b : {&e->pos, &e->vel, &e->oldp, &e->lastp, &e->pos0}) CKE(broadcast_replica0(e, *b));  // every replica of a batch starts here
     CK(cudaStreamSynchronize(e->stream));
     e->stats.num_particles = n;
+    return 0;
+}
+
+// collider-based contacts run one scene per engine: the contact kernel indexes particles of one replica
+static int collider_refusal(const pbd_engine *e, unsigned K, size_t nColliders) {
+    if (K > 1 && nColliders) return fail("replica batch: colliders (pbd_set_colliders) are stepped one scene per engine (pbd_set_replicas 1)");
+    return 0;
+}
+
+extern "C" int pbd_set_replicas(pbd_engine *e, unsigned K) {
+    if (!e) return fail("null engine");
+    const std::string why = pbd_b200::batch_refusal(K, e->n, e->mode, e->nRb, e->host);
+    if (!why.empty()) return fail("pbd_set_replicas: %s", why.c_str());
+    CKE(collider_refusal(e, K, e->pColliders.size() + e->rColliders.size()));
+    CKE(use(e));
+    CK(cudaStreamSynchronize(e->stream));
+    drop_graph(e);
+    const size_t one = (size_t)e->n * sizeof(float4);
+    if (e->n)
+        for (DevBuf *b : {&e->pos, &e->vel, &e->oldp, &e->lastp, &e->pos0}) {  // replica 0 kept, the others copies of it
+            DevBuf grown;
+            CKE(grown.alloc(one * K));
+            CK(cudaMemcpyAsync(grown.p, b->p, one, cudaMemcpyDeviceToDevice, e->stream));
+            std::swap(b->p, grown.p); std::swap(b->bytes, grown.bytes);
+            CK(cudaStreamSynchronize(e->stream));  // before `grown` frees the old array
+        }
+    e->K = K;
+    for (DevBuf *b : {&e->pos, &e->vel, &e->oldp, &e->lastp, &e->pos0}) CKE(broadcast_replica0(e, *b));
+    CKE(e->stage.alloc((size_t)K * e->n * 3 * sizeof(float)));
+    CKE(e->massStage.alloc((size_t)K * e->n * sizeof(float)));
+    CK(cudaStreamSynchronize(e->stream));
+    e->imageDirty = true;  // re-planned for the batch; the multipliers of every replica start at zero
+    e->autoNoResident = false;  // whether the resident mode takes the model depends on the batch size
+    return 0;
+}
+extern "C" int pbd_get_replicas(pbd_engine *e, unsigned *K) {
+    if (!e || !K) return fail("pbd_get_replicas: null argument");
+    *K = e->K;
     return 0;
 }
 
@@ -287,7 +344,7 @@ extern "C" int pbd_set_attr(pbd_engine *e, int attr, const float *src) {
     float4 *dst = attr_buf(e, attr);
     if (!dst) return fail("pbd_set_attr: bad attribute %d", attr);
     if (e->n == 0) return 0;
-    CKE(upload3(e, src, dst, 1));
+    CKE(upload3(e, src, dst, 1, e->K));
     CK(cudaStreamSynchronize(e->stream));
     return 0;
 }
@@ -298,9 +355,9 @@ extern "C" int pbd_get_attr(pbd_engine *e, int attr, float *dst) {
     const float4 *src = attr_buf(e, attr);
     if (!src) return fail("pbd_get_attr: bad attribute %d", attr);
     if (e->n == 0) return 0;
-    k_unpack3<<<nblk(e->n, 256), 256, 0, e->stream>>>(src, (float *)e->stage.p, e->n, (const unsigned *)e->dSlot.p);
+    k_unpack3<<<replica_grid(e, e->K), 256, 0, e->stream>>>(src, (float *)e->stage.p, e->n, (const unsigned *)e->dSlot.p);
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(dst, e->stage.p, (size_t)e->n * 3 * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaMemcpyAsync(dst, e->stage.p, (size_t)e->K * e->n * 3 * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
     CK(cudaStreamSynchronize(e->stream));
     return 0;
 }
@@ -311,6 +368,8 @@ extern "C" int pbd_get_attr(pbd_engine *e, int attr, float *dst) {
 extern "C" int pbd_set_rigid_bodies(pbd_engine *e, unsigned n, const float *mass, const float *x, const float *q, const float *inertia,
                                     const float *v, const float *omega) {
     if (!e || (n && (!mass || !x || !q || !inertia))) return fail("pbd_set_rigid_bodies: null argument");
+    const std::string why = pbd_b200::batch_refusal(e->K, e->n, e->mode, n, e->host);
+    if (!why.empty()) return fail("pbd_set_rigid_bodies: %s", why.c_str());
     CKE(use(e));
     CK(cudaStreamSynchronize(e->stream));
     if (n != e->nRb) { e->imageDirty = true; e->groupsSet = e->groupsSet && n == e->nRb; }
@@ -603,8 +662,10 @@ extern "C" int pbd_set_mode(pbd_engine *e, int mode) {
     if (!e) return fail("null engine");
     if (mode != PBD_MODE_GRAPH && mode != PBD_MODE_RESIDENT && mode != PBD_MODE_LAUNCH && mode != PBD_MODE_JACOBI && mode != PBD_MODE_AUTO) return fail("unknown solver mode %d", mode);
     if (mode == e->mode) return 0;
+    const std::string why = pbd_b200::batch_refusal(e->K, e->n, mode, e->nRb, e->host);
+    if (!why.empty()) return fail("pbd_set_mode: %s", why.c_str());
     // only the resident image is laid out differently: the others run the image they share
-    const int active = pbd_b200::preferred_mode(mode, e->host, e->n, e->numConstraints, false);
+    const int active = pbd_b200::preferred_mode(mode, e->host, e->n, e->numConstraints, false, e->K);
     if ((active == PBD_MODE_RESIDENT) != (e->active == PBD_MODE_RESIDENT)) e->imageDirty = true;
     e->mode = mode; e->active = active; e->autoNoResident = false;
     drop_graph(e);
@@ -620,25 +681,28 @@ extern "C" int pbd_get_mode(pbd_engine *e, int *requested, int *active) {
 // ------------------------------------------------------------------------------------------------------------
 // the device image: planned on the host (host/image_plan.cpp), uploaded here
 // ------------------------------------------------------------------------------------------------------------
-template <unsigned M, class F> static int resident_kernel(bool single, F &&f) {
-    return single ? f(k_step_resident<M, resident_threads(M), true>) : f(k_step_resident<M, resident_threads(M), false>);
+template <unsigned M, bool BATCH, class F> static int resident_kernel(bool single, F &&f) {
+    return single ? f(k_step_resident<M, resident_threads(M, BATCH), true, BATCH>) : f(k_step_resident<M, resident_threads(M, BATCH), false, BATCH>);
 }
-// the compiled instantiations of k_step_resident: F(kernel pointer) for a type mask, one CTA per cluster or not
-template <class F> static int with_resident_kernel(unsigned mask, unsigned C, F &&f) {
+template <unsigned M, class F> static int resident_kernel(bool single, bool batch, F &&f) {
+    return batch ? resident_kernel<M, true>(single, f) : resident_kernel<M, false>(single, f);
+}
+// the compiled instantiations of k_step_resident: F(kernel pointer) for a type mask, one CTA per cluster or not, a replica batch or not
+template <class F> static int with_resident_kernel(unsigned mask, unsigned C, bool batch, F &&f) {
     const bool single = (C == 1);
     switch (mask) {
-    case kMaskClothXPBD: return resident_kernel<kMaskClothXPBD>(single, f);
-    case kMaskCloth: return resident_kernel<kMaskCloth>(single, f);
-    case kMaskLight: return resident_kernel<kMaskLight>(single, f);
-    case kMaskFem: return resident_kernel<kMaskFem>(single, f);
-    case kMaskSolid: return resident_kernel<kMaskSolid>(single, f);
-    default: return resident_kernel<kMaskAll>(single, f);
+    case kMaskClothXPBD: return resident_kernel<kMaskClothXPBD>(single, batch, f);
+    case kMaskCloth: return resident_kernel<kMaskCloth>(single, batch, f);
+    case kMaskLight: return resident_kernel<kMaskLight>(single, batch, f);
+    case kMaskFem: return resident_kernel<kMaskFem>(single, batch, f);
+    case kMaskSolid: return resident_kernel<kMaskSolid>(single, batch, f);
+    default: return resident_kernel<kMaskAll>(single, batch, f);
     }
 }
 
-static void resident_launch_config(unsigned mask, unsigned C, unsigned grid, size_t smem, cudaStream_t s, cudaLaunchConfig_t &cfg, cudaLaunchAttribute *attr) {
+static void resident_launch_config(unsigned mask, unsigned C, bool batch, unsigned grid, size_t smem, cudaStream_t s, cudaLaunchConfig_t &cfg, cudaLaunchAttribute *attr) {
     cfg = cudaLaunchConfig_t{};
-    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(resident_threads(mask)); cfg.dynamicSmemBytes = smem; cfg.stream = s;
+    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(resident_threads(mask, batch)); cfg.dynamicSmemBytes = smem; cfg.stream = s;
     attr[0].id = cudaLaunchAttributeClusterDimension;
     attr[0].val.clusterDim.x = C; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr; cfg.numAttrs = 1;
@@ -646,11 +710,11 @@ static void resident_launch_config(unsigned mask, unsigned C, unsigned grid, siz
 
 // how many clusters of C CTAs (one CTA per SM, `smem` bytes each) of the instantiation for `mask` the device keeps resident at the same time
 static int resident_max_clusters(const pbd_engine *e, unsigned mask, unsigned C, size_t smem, int *out) {
-    return with_resident_kernel(mask, C, [&](auto kernel) -> int {
+    return with_resident_kernel(mask, C, e->K > 1, [&](auto kernel) -> int {
         CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynamicSmem));
         CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
         cudaLaunchConfig_t cfg; cudaLaunchAttribute attr[1];
-        resident_launch_config(mask, C, C, smem, e->stream, cfg, attr);
+        resident_launch_config(mask, C, e->K > 1, C, smem, e->stream, cfg, attr);
         cudaError_t err = cudaOccupancyMaxActiveClusters(out, kernel, &cfg);
         if (err != cudaSuccess) { cudaGetLastError(); *out = 0; }
         return 0;
@@ -688,8 +752,9 @@ static int upload_type(pbd_engine *e, int t, pbd_b200::TypePlan &p) {
         a.rbX = (float4 *)e->rbX.p; a.rbQ = (float4 *)e->rbQ.p; a.rbIinv = (const float4 *)e->rbIinv.p;
     }
     if (type_shape(t).xpbd) {
-        CKE(d.lambda.alloc((size_t)cnt * sizeof(float) + 16));  // + 16 like the other streamed arrays: the L2 prefetch of a run rounds its end up to 16 bytes
-        CK(cudaMemsetAsync(d.lambda.p, 0, (size_t)cnt * sizeof(float), e->stream));
+        // replica r's multipliers at [r cnt, (r + 1) cnt); + 16 like the other streamed arrays: the L2 prefetch of a run rounds its end up to 16 bytes
+        CKE(d.lambda.alloc((size_t)e->K * cnt * sizeof(float) + 16));
+        CK(cudaMemsetAsync(d.lambda.p, 0, (size_t)e->K * cnt * sizeof(float), e->stream));
         a.lambda = (float *)d.lambda.p;
     }
     return 0;
@@ -704,7 +769,7 @@ static int flatten(pbd_engine *e) {
     CKE(colour_if_needed(e));
     drop_graph(e);
     std::vector<float4> x0;  // resident: rest positions by host index
-    if (pbd_b200::preferred_mode(e->mode, e->host, e->n, e->numConstraints, e->autoNoResident) == PBD_MODE_RESIDENT && e->n) {
+    if (pbd_b200::preferred_mode(e->mode, e->host, e->n, e->numConstraints, e->autoNoResident, e->K) == PBD_MODE_RESIDENT && e->n) {
         std::vector<float4> raw(e->n);
         CK(cudaStreamSynchronize(e->stream));
         CK(cudaMemcpy(raw.data(), e->pos0.p, (size_t)e->n * sizeof(float4), cudaMemcpyDeviceToHost));
@@ -712,7 +777,7 @@ static int flatten(pbd_engine *e) {
         for (unsigned i = 0; i < e->n; i++) x0[i] = raw[e->slot[i]];
     }
     lap("colouring + rest positions");
-    pbd_b200::PlanInput in{e->host, e->numConstraints, e->n, e->nRb, &e->groupOff, &e->groupIds, e->mode, x0.data(), 0u, 0u, e->smCount, nullptr, e->autoNoResident};
+    pbd_b200::PlanInput in{e->host, e->numConstraints, e->n, e->nRb, &e->groupOff, &e->groupIds, e->mode, x0.data(), 0u, 0u, e->smCount, nullptr, e->autoNoResident, e->K};
     if (const char *g = getenv("PBD_B200_CLUSTERS")) {  // development knob "GxC"
         unsigned gg = 0, cc = 0;
         if (sscanf(g, "%ux%u", &gg, &cc) == 2 && gg >= 1 && cc >= 1 && cc <= (unsigned)kMaxClusterCtas && (cc & (cc - 1)) == 0) { in.forcedG = gg; in.forcedC = cc; }
@@ -743,7 +808,7 @@ static int flatten(pbd_engine *e) {
     }
     CK(cudaStreamSynchronize(e->stream));
     lap("relayout + upload");
-    e->stats.num_constraints = e->numConstraints;
+    e->stats.num_constraints = e->numConstraints;  // per replica, like num_particles
     e->stats.num_groups = (unsigned)e->groupOff.size() - 1;
     e->stats.num_buckets = (unsigned)e->buckets.size();
     e->imageDirty = false;
@@ -765,9 +830,9 @@ static unsigned project_block(const pbd_engine *e, unsigned count) {
 // One kernel of a step.  With `pdl` the launch carries the programmatic-stream-serialization attribute, so that the whole step is one
 // programmatic dependency chain (kernels.cuh); pbd_profile_step launches without it, so that each kernel's duration is its own.
 template <typename... KArgs, typename... Args>
-static cudaError_t launch_step_kernel(void (*kernel)(KArgs...), unsigned grid, unsigned block, cudaStream_t s, bool pdl, Args... args) {
+static cudaError_t launch_step_kernel(void (*kernel)(KArgs...), dim3 grid, unsigned block, cudaStream_t s, bool pdl, Args... args) {
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(block); cfg.stream = s;
+    cfg.gridDim = grid; cfg.blockDim = dim3(block); cfg.stream = s;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
@@ -785,12 +850,15 @@ template <class F> static int with_project_type(int type, int variant, F &&f) {
     return fail("no kernel for constraint type %d", type);
 }
 
+// A batch's projection launches run replica blockIdx.y (the BATCH instantiations); their block size follows the whole batch's count.
 static int launch_bucket(pbd_engine *e, const Bucket &b, float h, int iterZero, cudaStream_t s, bool pdl) {
     const TypeArrays &a = e->dev[b.type].arrays;
-    const unsigned block = project_block(e, b.count);
+    const unsigned block = project_block(e, b.count * e->K);
+    const ReplicaStrides rs{e->n, {e->dev[b.type].count}};
     return with_project_type(b.type, a.variant, [&](auto T, auto V) -> int {
         constexpr int TT = decltype(T)::value, VAR = decltype(V)::value;
-        CK(launch_step_kernel(k_project<TT, VAR>, nblk(b.count, block), block, s, pdl, (float4 *)e->pos.p, a, b.first, b.count, h, iterZero));
+        if (e->K > 1) CK(launch_step_kernel(k_project<TT, VAR, true>, dim3(nblk(b.count, block), e->K), block, s, pdl, (float4 *)e->pos.p, a, b.first, b.count, h, iterZero, rs));
+        else CK(launch_step_kernel(k_project<TT, VAR, false>, nblk(b.count, block), block, s, pdl, (float4 *)e->pos.p, a, b.first, b.count, h, iterZero, rs));
         return 0;
     });
 }
@@ -818,6 +886,7 @@ static int launch_colour(pbd_engine *e, size_t b0, size_t b1, float h, int iterZ
     constexpr unsigned kMergeMaxConstraints = 65536;
     unsigned colourTotal = 0;
     for (size_t i = b0; i < b1; i++) colourTotal += e->buckets[i].count;
+    colourTotal *= e->K;
     if (b1 - b0 == 1 || log || colourTotal > kMergeMaxConstraints) {
         for (size_t i = b0; i < b1; i++) {
             CKE(launch_bucket(e, e->buckets[i], h, iterZero, s, !log));
@@ -829,19 +898,22 @@ static int launch_colour(pbd_engine *e, size_t b0, size_t b1, float h, int iterZ
     for (size_t c0 = b0; c0 < b1; c0 += kMultiSegments) {
         const size_t c1 = std::min(b1, c0 + (size_t)kMultiSegments);
         MultiArgs m{};
+        ReplicaStrides rs{e->n, {}};
         m.nSeg = (int)(c1 - c0);
         unsigned blocks = 0, total = 0;
         for (size_t i = c0; i < c1; i++) total += e->buckets[i].count;
-        const unsigned block = project_block(e, total);
+        const unsigned block = project_block(e, total * e->K);
         for (size_t i = c0; i < c1; i++) {
             const Bucket &b = e->buckets[i];
             const int k = (int)(i - c0);
             m.type[k] = b.type; m.first[k] = b.first; m.count[k] = b.count; m.blockStart[k] = blocks;
             m.arrays[k] = e->dev[b.type].arrays;
+            rs.nLambda[k] = e->dev[b.type].count;
             blocks += nblk(b.count, block);
         }
         for (int k = m.nSeg; k <= kMultiSegments; k++) m.blockStart[k] = blocks;
-        CK(launch_step_kernel(k_project_multi, blocks, block, s, true, (float4 *)e->pos.p, m, h, iterZero));
+        if (e->K > 1) CK(launch_step_kernel(k_project_multi<true>, dim3(blocks, e->K), block, s, true, (float4 *)e->pos.p, m, h, iterZero, rs));
+        else CK(launch_step_kernel(k_project_multi<false>, blocks, block, s, true, (float4 *)e->pos.p, m, h, iterZero, rs));
         (*launches)++;
     }
     return 0;
@@ -857,7 +929,7 @@ static RbState rb_state(const pbd_engine *e) {
 static int enqueue_step_launches(pbd_engine *e, cudaStream_t s, unsigned long long *launches, LaunchLog *log = nullptr) {
     const float h = e->dt / (float)e->subSteps;  // TimeStepController.cpp:91
     const float invH = (float)(1.0 / (double)h);
-    const unsigned n = e->n;
+    const unsigned n = e->n * e->K;  // the particle updates run over every replica's slots at once
     const bool pdl = !log;
     const RbState rb = rb_state(e);
     unsigned long long L = 0;
@@ -895,7 +967,8 @@ static int enqueue_step_resident(pbd_engine *e, cudaStream_t s, unsigned long lo
     ra.colourStart = (const unsigned *)e->dColourStart.p; ra.tileOff = (const unsigned *)e->dTileOff.p;
     ra.tileStart = (const unsigned *)e->dTileStart.p; ra.tileSmem = (const unsigned *)e->dTileSmem.p;
     ra.xNbr = (const unsigned *)e->dXNbr.p; ra.xMask = (const unsigned *)e->dXMask.p;
-    ra.nBuckets = (unsigned)e->buckets.size(); ra.nColours = e->res.nColours; ra.nTiles = e->res.G * e->res.C; ra.subSteps = e->subSteps; ra.maxIter = e->maxIter;
+    const bool batch = e->res.replicas > 1;  // the tables hold the C tiles of one replica
+    ra.nBuckets = (unsigned)e->buckets.size(); ra.nColours = e->res.nColours; ra.nTiles = batch ? e->res.C : e->res.G * e->res.C; ra.subSteps = e->subSteps; ra.maxIter = e->maxIter;
     ra.tileCap = e->res.tileCap; ra.xThreads = e->res.xThreads; ra.clusterSize = e->res.C;
     {   // L2 prefetch of the operand runs pays when the constraint stream of a sweep does not stay in L2 anyway (above ~0.38 x the L2).
         // H100 80GB HBM3 (400 W, 50 MB L2), prefetch off / on: cfg2 (192 MB per sweep) 2.28 / 2.08 ms, cfg5 (48 MB) 1.246 / 1.216 ms,
@@ -912,12 +985,13 @@ static int enqueue_step_resident(pbd_engine *e, cudaStream_t s, unsigned long lo
     ra.xFlags = (unsigned long long *)e->dXFlags.p;
     ra.xLaunch = (++e->xLaunch) << 32;  // above every flag value of the earlier launches, whatever subSteps / maxIter they ran with
     ra.rb = rb_state(e);
-    for (int t = 0; t < PBD_NUM_TYPES; t++) ra.types[t] = e->dev[t].arrays;
+    for (int t = 0; t < PBD_NUM_TYPES; t++) { ra.types[t] = e->dev[t].arrays; ra.lamCount[t] = e->dev[t].count; }
+    ra.replicas = e->res.replicas; ra.replicaStride = e->n;
     *launches = 1;
     ra.trace = nullptr; ra.tracePhases = 0;
     static const char *tracePath = getenv("PBD_B200_TRACE");  // development aid: dump per-phase timelines of one step (tools/trace_resident.py)
     const unsigned kTracePhases = 256;
-    if (tracePath) {
+    if (tracePath && !batch) {  // (a batch's clusters step different replicas through the same tiles: no per-CTA timeline to record)
         CKE(e->dTrace.alloc((size_t)kTracePhases * ra.nTiles * kTraceSlots * sizeof(unsigned long long)));
         CK(cudaMemsetAsync(e->dTrace.p, 0, e->dTrace.bytes, s));
         ra.trace = (unsigned long long *)e->dTrace.p; ra.tracePhases = kTracePhases;
@@ -931,13 +1005,13 @@ static int enqueue_step_resident(pbd_engine *e, cudaStream_t s, unsigned long lo
             cudaMemcpy(h.data(), e->dTrace.p, h.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost);
             if (FILE *f = fopen(path, "wb")) { fwrite(h.data(), sizeof(unsigned long long), h.size(), f); fclose(f); }
         }
-    } dump{e, s, tracePath, (size_t)kTracePhases * ra.nTiles * kTraceSlots};
+    } dump{e, s, batch ? nullptr : tracePath, (size_t)kTracePhases * ra.nTiles * kTraceSlots};
     const pbd_b200::ResidentShape &r = e->res;
-    return with_resident_kernel(r.mask, r.C, [&](auto kernel) -> int {
+    return with_resident_kernel(r.mask, r.C, batch, [&](auto kernel) -> int {
         CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynamicSmem));
         if (r.C > 8) CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
         cudaLaunchConfig_t cfg; cudaLaunchAttribute attr[1];
-        resident_launch_config(r.mask, r.C, r.G * r.C, r.smem, s, cfg, attr);
+        resident_launch_config(r.mask, r.C, batch, r.G * r.C, r.smem, s, cfg, attr);
         CK(cudaLaunchKernelEx(&cfg, kernel, ra));
         return 0;
     });
@@ -986,6 +1060,7 @@ static int enqueue_step_jacobi(pbd_engine *e, cudaStream_t s, unsigned long long
 // ------------------------------------------------------------------------------------------------------------
 extern "C" int pbd_set_colliders(pbd_engine *e, unsigned nP, const pbd_particle_collider *pc, unsigned nR, const pbd_rigid_collider *rc) {
     if (!e || (nP && !pc) || (nR && !rc)) return fail("pbd_set_colliders: null argument");
+    CKE(collider_refusal(e, e->K, (size_t)nP + nR));
     CKE(use(e));
     if (nR > (unsigned)kMaxRigidColliders) return fail("pbd_set_colliders: %u rigid colliders (the contact kernel keeps up to %d contacts per particle)", nR, kMaxRigidColliders);
     std::vector<ParticleCollider> P(nP);
@@ -1102,7 +1177,7 @@ extern "C" int pbd_step(pbd_engine *e, unsigned nSteps) {
         CKE(enqueue_contacts(e, e->stream, &L));
         e->stats.kernel_launches += L;
         e->stats.steps++;
-        e->stats.projections += (unsigned long long)e->numConstraints * e->subSteps * e->maxIter;
+        e->stats.projections += (unsigned long long)e->numConstraints * e->subSteps * e->maxIter * e->K;
     }
     CK(cudaEventRecord(e->evStop, e->stream));
     e->timingPending = true;
@@ -1138,27 +1213,28 @@ extern "C" int pbd_step_host(pbd_engine *e, unsigned nSteps, const float *x_in, 
     if (!e) return fail("null engine");
     CKE(use(e));
     if (e->n == 0) return pbd_step(e, nSteps);
-    const size_t bytes = (size_t)e->n * 3 * sizeof(float);
+    const size_t bytes = (size_t)e->K * e->n * 3 * sizeof(float);
+    const dim3 grid = replica_grid(e, e->K);
     // two staging areas so that x and v uploads do not serialise on a host sync
     CKE(e->stage.alloc(bytes));
     DevBuf &stage2 = e->stage2;
     CKE(stage2.alloc(bytes));
     if (x_in) {
         CK(cudaMemcpyAsync(e->stage.p, x_in, bytes, cudaMemcpyHostToDevice, e->stream));
-        k_pack3<<<nblk(e->n, 256), 256, 0, e->stream>>>((const float *)e->stage.p, (float4 *)e->pos.p, e->n, 1, (const unsigned *)e->dSlot.p);
+        k_pack3<<<grid, 256, 0, e->stream>>>((const float *)e->stage.p, (float4 *)e->pos.p, e->n, 1, (const unsigned *)e->dSlot.p);
     }
     if (v_in) {
         CK(cudaMemcpyAsync(stage2.p, v_in, bytes, cudaMemcpyHostToDevice, e->stream));
-        k_pack3<<<nblk(e->n, 256), 256, 0, e->stream>>>((const float *)stage2.p, (float4 *)e->vel.p, e->n, 1, (const unsigned *)e->dSlot.p);
+        k_pack3<<<grid, 256, 0, e->stream>>>((const float *)stage2.p, (float4 *)e->vel.p, e->n, 1, (const unsigned *)e->dSlot.p);
     }
     CK(cudaGetLastError());
     CKE(pbd_step(e, nSteps));
     if (x_out) {
-        k_unpack3<<<nblk(e->n, 256), 256, 0, e->stream>>>((const float4 *)e->pos.p, (float *)e->stage.p, e->n, (const unsigned *)e->dSlot.p);
+        k_unpack3<<<grid, 256, 0, e->stream>>>((const float4 *)e->pos.p, (float *)e->stage.p, e->n, (const unsigned *)e->dSlot.p);
         CK(cudaMemcpyAsync(x_out, e->stage.p, bytes, cudaMemcpyDeviceToHost, e->stream));
     }
     if (v_out) {
-        k_unpack3<<<nblk(e->n, 256), 256, 0, e->stream>>>((const float4 *)e->vel.p, (float *)stage2.p, e->n, (const unsigned *)e->dSlot.p);
+        k_unpack3<<<grid, 256, 0, e->stream>>>((const float4 *)e->vel.p, (float *)stage2.p, e->n, (const unsigned *)e->dSlot.p);
         CK(cudaMemcpyAsync(v_out, stage2.p, bytes, cudaMemcpyDeviceToHost, e->stream));
     }
     CK(cudaGetLastError());
@@ -1172,7 +1248,8 @@ extern "C" int pbd_step_host_async(pbd_engine *e, unsigned nSteps, const float *
     if (!e) return fail("null engine");
     CKE(use(e));
     if (e->n == 0) return pbd_step(e, nSteps);
-    const size_t bytes = (size_t)e->n * 3 * sizeof(float);
+    const size_t bytes = (size_t)e->K * e->n * 3 * sizeof(float);
+    const dim3 grid = replica_grid(e, e->K);
     auto &P = e->pipe;
     if (!P.ready) {
         CK(cudaStreamCreateWithFlags(&P.up, cudaStreamNonBlocking));
@@ -1190,16 +1267,16 @@ extern "C" int pbd_step_host_async(pbd_engine *e, unsigned nSteps, const float *
         if (v_in) { CKE(P.inV[s].alloc(bytes)); CK(cudaMemcpyAsync(P.inV[s].p, v_in, bytes, cudaMemcpyHostToDevice, P.up)); }
         CK(cudaEventRecord(P.uploaded[s], P.up));
         CK(cudaStreamWaitEvent(e->stream, P.uploaded[s], 0));
-        if (x_in) k_pack3<<<nblk(e->n, 256), 256, 0, e->stream>>>((const float *)P.inX[s].p, (float4 *)e->pos.p, e->n, 1, slot);
-        if (v_in) k_pack3<<<nblk(e->n, 256), 256, 0, e->stream>>>((const float *)P.inV[s].p, (float4 *)e->vel.p, e->n, 1, slot);
+        if (x_in) k_pack3<<<grid, 256, 0, e->stream>>>((const float *)P.inX[s].p, (float4 *)e->pos.p, e->n, 1, slot);
+        if (v_in) k_pack3<<<grid, 256, 0, e->stream>>>((const float *)P.inV[s].p, (float4 *)e->vel.p, e->n, 1, slot);
         CK(cudaGetLastError());
     }
     CK(cudaEventRecord(P.consumed[s], e->stream));
     CKE(pbd_step(e, nSteps));
     if (x_out || v_out) {
         if (reuse) CK(cudaStreamWaitEvent(e->stream, P.downloaded[s], 0));
-        if (x_out) { CKE(P.outX[s].alloc(bytes)); k_unpack3<<<nblk(e->n, 256), 256, 0, e->stream>>>((const float4 *)e->pos.p, (float *)P.outX[s].p, e->n, slot); }
-        if (v_out) { CKE(P.outV[s].alloc(bytes)); k_unpack3<<<nblk(e->n, 256), 256, 0, e->stream>>>((const float4 *)e->vel.p, (float *)P.outV[s].p, e->n, slot); }
+        if (x_out) { CKE(P.outX[s].alloc(bytes)); k_unpack3<<<grid, 256, 0, e->stream>>>((const float4 *)e->pos.p, (float *)P.outX[s].p, e->n, slot); }
+        if (v_out) { CKE(P.outV[s].alloc(bytes)); k_unpack3<<<grid, 256, 0, e->stream>>>((const float4 *)e->vel.p, (float *)P.outV[s].p, e->n, slot); }
         CK(cudaGetLastError());
         CK(cudaEventRecord(P.produced[s], e->stream));
         CK(cudaStreamWaitEvent(P.down, P.produced[s], 0));
@@ -1234,7 +1311,7 @@ extern "C" int pbd_get_lambdas(pbd_engine *e, int type, float *dst, unsigned *id
     DevType &d = e->dev[type];
     if (d.count == 0) return 0;
     CK(cudaStreamSynchronize(e->stream));
-    CK(cudaMemcpy(dst, d.lambda.p, (size_t)d.count * sizeof(float), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(dst, d.lambda.p, (size_t)e->K * d.count * sizeof(float), cudaMemcpyDeviceToHost));  // replica after replica
     if (ids) memcpy(ids, d.order.data(), (size_t)d.count * sizeof(unsigned));
     return 0;
 }
@@ -1246,7 +1323,7 @@ extern "C" int pbd_get_stats(pbd_engine *e, pbd_stats *out) {
     for (int t = 0; t < PBD_NUM_TYPES; t++) sweep += (double)e->dev[t].count * algorithmic_bytes(t, e->dev[t].arrays.variant);
     // per particle per substep: integrate 48 read + 64 write = 112, velocity update 32 read + 16 write = 48 (SURVEY.md 8d)
     const double perParticle = 112.0 + 48.0 + (e->velMethod ? 16.0 : 0.0);
-    e->stats.bytes_per_step = (sweep * e->maxIter + (double)e->n * perParticle) * e->subSteps;
+    e->stats.bytes_per_step = (sweep * e->maxIter + (double)e->n * perParticle) * e->subSteps * e->K;
     *out = e->stats;
     return 0;
 }
@@ -1280,6 +1357,6 @@ extern "C" int pbd_profile_step(pbd_engine *e, float *msPerType, float *msIntegr
     if (msIntegrate) *msIntegrate = mi;
     if (msVelocity) *msVelocity = mv;
     e->stats.steps++;
-    e->stats.projections += (unsigned long long)e->numConstraints * e->subSteps * e->maxIter;
+    e->stats.projections += (unsigned long long)e->numConstraints * e->subSteps * e->maxIter * e->K;
     return 0;
 }

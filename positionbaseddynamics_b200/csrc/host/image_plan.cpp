@@ -155,7 +155,7 @@ static std::string choose_resident_shape(const PlanInput &in, ResidentShape &r) 
     r.mask = kMaskAll;
     for (unsigned m : {kMaskClothXPBD, kMaskCloth, kMaskFem, kMaskLight, kMaskSolid})  // the leanest instantiation that covers the model
         if ((present & ~m) == 0) { r.mask = m; break; }
-    r.threads = resident_threads(r.mask);
+    r.threads = resident_threads(r.mask, in.replicas > 1);
     const unsigned nGroups = (unsigned)std::max<size_t>(in.groupOff->size(), 2) - 1;
     const unsigned perPhase = in.numConstraints / std::max(1u, nGroups);
     // particles a tile can hold: what is left of the CTA's shared memory after the phase tables (bound: one bucket per colour and type)
@@ -163,7 +163,29 @@ static std::string choose_resident_shape(const PlanInput &in, ResidentShape &r) 
     if (tables + 1024 * sizeof(float4) > kMaxDynamicSmem) return fmt("resident mode: %u colour groups need %zu bytes of phase tables (use PBD_MODE_GRAPH)", nGroups, tables);
     const unsigned cap = (unsigned)(0.97 * (double)((kMaxDynamicSmem - tables) / sizeof(float4)));  // bisection splits counts evenly; slack for rounding
     unsigned G = 1, C = 1;
-    if (in.n <= (unsigned)kMaxClusterCtas * cap && perPhase <= (unsigned)kMaxClusterCtas * 1024u) {
+    const bool oneCluster = in.n <= (unsigned)kMaxClusterCtas * cap && perPhase <= (unsigned)kMaxClusterCtas * 1024u;
+    if (in.replicas > 1) {
+        // A batch tiles one replica into one cluster of C CTAs; G clusters (plan_mode) step the replicas one after the other.  Smaller
+        // clusters run more replicas at once, larger ones step each replica faster.  C: one CTA when a replica fits one (no cluster
+        // barrier at all); else the largest C up to the single-scene choice below whose clusters the device runs all at once, else the
+        // smallest C that holds the replica.  H100 80GB HBM3 (700 W), ms per batched step (tools/bench_batch.py, C forced):
+        //   cfg1 (2,500 particles, fits one CTA), C = 1 / 2 / 4 / 8 / 16:  K = 8  0.147 / 0.193 / 0.186 / 0.185 / 0.342,
+        //        K = 132  0.151 / 0.394 / 0.923 / 1.640 / 3.270,  K = 528  0.628 / 1.600 / 3.346 / 6.572 / 13.098;
+        //   cfg3 (44,541 particles, C >= 4; the single scene takes 16), C = 4 / 8 / 16:  K = 4 (C = 16 only) 7.82,  K = 8  14.38 / 10.12 /
+        //        15.54 (16-CTA clusters: fewer than 8 at once),  K = 33  29.28 / 30.69 / 39.60,  K = 66  44.38 / 51.50 / 78.25.
+        if (!oneCluster)
+            return fmt("resident mode: a replica of %u particles (%u constraints per colour) does not fit one cluster of %d CTAs (use PBD_MODE_GRAPH)", in.n, perPhase, kMaxClusterCtas);
+        unsigned fit = 1;
+        while (in.n > fit * cap) fit *= 2;
+        C = fit;
+        if (fit > 1) {
+            unsigned solo = fit;
+            while (solo < (unsigned)kMaxClusterCtas && (perPhase > solo * 256u || in.n > solo * cap)) solo *= 2;
+            for (unsigned c = solo; c > fit; c /= 2)
+                if (in.maxClusters(r.mask, c, kMaxDynamicSmem) >= (int)in.replicas) { C = c; break; }
+        }
+        if (in.forcedC) C = in.forcedC;
+    } else if (oneCluster) {
         // one cluster: enough CTAs that a colour phase is about one item per thread, and that the tiles fit
         while (C < (unsigned)kMaxClusterCtas && (perPhase > C * 256u || in.n > C * cap)) C *= 2;
     } else {
@@ -174,7 +196,7 @@ static std::string choose_resident_shape(const PlanInput &in, ResidentShape &r) 
         if (mc < 1) return fmt("resident mode: a CTA with %zu bytes of shared memory is not schedulable on this device", kMaxDynamicSmem);
         C = 1; G = (unsigned)std::min(mc, in.smCount);
     }
-    if (in.forcedG) { G = in.forcedG; C = in.forcedC; }
+    if (in.forcedG && in.replicas == 1) { G = in.forcedG; C = in.forcedC; }
     if ((unsigned long long)G * C * cap < in.n)
         return fmt("resident mode: %u particles do not fit %u x %u tiles of %u (use PBD_MODE_GRAPH)", in.n, G, C, cap);
     // (bodies without joints -- e.g. the static colliders of the contact path -- are integrated by CTA 0 and touch no constraint)
@@ -661,13 +683,22 @@ static std::string build_phase_tables(Ctx &c, const std::vector<unsigned> (&orde
 // solver families (cfg4) stay in graph mode, and so does a model the resident mode has refused.
 // Measured on an H100 80GB HBM3 (SXM, 400 W, 1980 MHz), XPBD cloth 1 x 20, ms per step graph / resident: 100x100 0.66 / 0.79,
 // 200x200 0.93 / 0.92, 300x300 1.20 / 1.02; cfg1 (50x50) 0.129 / 0.183; cfg3 (44,541 particles) 8.03 / 7.69.
-constexpr unsigned kAutoResidentMinParticles = 40000;
-int preferred_mode(int requested, const TypeStore *store, unsigned n, unsigned numConstraints, bool residentRefused) {
+// Replica batches take the resident mode from kAutoResidentMinReplicas replicas on whatever the size of a replica, from twice as many
+// for models only the light instantiation covers (FEMTriangle, Dihedral, Volume: per replica a longer step than the cloth and FEM
+// kernels take).  H100 80GB HBM3 (SXM, 700 W), ms per batched step graph / resident (tools/bench_batch.py): cfg1 K = 8 0.146 / 0.147,
+// K = 33 0.263 / 0.147, K = 528 1.447 / 0.628; 100x100 XPBD cloth 1 x 20 K = 8 1.09 / 1.44, K = 33 2.78 / 1.45, K = 264 15.82 / 3.21;
+// cfg3 K = 4 13.42 / 7.88, K = 66 127.9 / 44.1; 100x100 FEMTriangle + Dihedral cloth 1 x 5 (light) K = 33 0.531 / 0.692, K = 66
+// 0.838 / 0.717, K = 132 1.412 / 0.745.
+constexpr unsigned kAutoResidentMinParticles = 40000, kAutoResidentMinReplicas = 32;
+int preferred_mode(int requested, const TypeStore *store, unsigned n, unsigned numConstraints, bool residentRefused, unsigned replicas) {
     if (requested != PBD_MODE_AUTO) return requested;
-    if (residentRefused || numConstraints == 0 || n < kAutoResidentMinParticles) return PBD_MODE_GRAPH;
+    if (residentRefused || numConstraints == 0) return PBD_MODE_GRAPH;
     unsigned present = 0;
     for (int t = 0; t < PBD_NUM_TYPES; t++) if (!store[t].ids.empty()) present |= 1u << t;
-    return ((present & ~(kMaskCloth | kMaskFem)) == 0 || (present & ~kMaskLight) == 0) ? PBD_MODE_RESIDENT : PBD_MODE_GRAPH;
+    const bool clothFem = (present & ~(kMaskCloth | kMaskFem)) == 0, light = (present & ~kMaskLight) == 0;
+    if (!clothFem && !light) return PBD_MODE_GRAPH;
+    if (n >= kAutoResidentMinParticles) return PBD_MODE_RESIDENT;
+    return replicas >= (clothFem ? 1u : 2u) * kAutoResidentMinReplicas ? PBD_MODE_RESIDENT : PBD_MODE_GRAPH;
 }
 
 // the image of the resident mode (tiled) or of the others
@@ -702,11 +733,31 @@ static std::string plan_mode(const PlanInput &in, bool tiled, ImagePlan &out) {
     if (r.smem > kMaxDynamicSmem)
         return fmt("resident mode: a CTA needs %zu bytes of shared memory (tile of %u particles + phase tables), %zu available", r.smem, r.tileCap, kMaxDynamicSmem);
     const int mc = in.maxClusters(r.mask, r.C, r.smem);
+    if (in.replicas > 1) {  // a batch: as many clusters as the device runs at once, up to one per replica; none waits for another
+        if (mc < 1) return fmt("resident mode: the device cannot run a cluster of %u CTAs with %zu bytes of shared memory each", r.C, r.smem);
+        r.G = std::min(in.replicas, (unsigned)mc);
+        r.replicas = in.replicas;
+        return "";
+    }
     return (unsigned)mc < r.G ? fmt("resident mode: the device runs %d clusters of %u CTAs at a time, the scene needs %u co-resident", mc, r.C, r.G) : "";
 }
 
+std::string batch_refusal(unsigned replicas, unsigned n, int mode, unsigned nRb, const TypeStore *store) {
+    if (replicas == 0) return "replica batch: at least one replica";
+    if ((unsigned long long)replicas * n >= (1ull << 31))
+        return fmt("replica batch: %u replicas of %u particles exceed 2^31 particles", replicas, n);
+    if (replicas == 1) return "";
+    if (replicas > 65535u) return fmt("replica batch: %u replicas, at most 65535 (the projection kernels run one replica per grid row)", replicas);
+    if (nRb || !store[PBD_BALLJOINT].ids.empty() || !store[PBD_RB_PARTICLE_BALLJOINT].ids.empty())
+        return "replica batch: rigid bodies and joints are stepped one scene per engine (pbd_set_replicas 1)";
+    if (mode == PBD_MODE_JACOBI) return "replica batch: PBD_MODE_JACOBI steps one scene per engine (pbd_set_replicas 1)";
+    return "";
+}
+
 std::string plan_image(const PlanInput &in, ImagePlan &out) {
-    out.mode = preferred_mode(in.mode, in.store, in.n, in.numConstraints, in.residentRefused);
+    const std::string refusal = batch_refusal(in.replicas, in.n, in.mode, in.nRb, in.store);
+    if (!refusal.empty()) return refusal;
+    out.mode = preferred_mode(in.mode, in.store, in.n, in.numConstraints, in.residentRefused, in.replicas);
     const std::string err = plan_mode(in, out.mode == PBD_MODE_RESIDENT, out);
     if (err.empty() || in.mode != PBD_MODE_AUTO || out.mode != PBD_MODE_RESIDENT) return err;
     // AUTO, and the resident mode refused the model (does not fit, user-modified bending Q, ...): the graph image, planned from scratch

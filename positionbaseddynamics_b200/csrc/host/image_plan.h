@@ -32,7 +32,8 @@ long long bad_body_index(int type, const unsigned *bodies, size_t count, unsigne
 std::string build_id_map(const TypeStore *store, unsigned N, std::vector<std::pair<int, unsigned>> &map);
 
 // The mode an image is planned for: `requested`, or for PBD_MODE_AUTO the resident mode where it is faster and not refused yet, else graph.
-int preferred_mode(int requested, const TypeStore *store, unsigned n, unsigned numConstraints, bool residentRefused);
+// `replicas`: the size of the replica batch the image serves (pbd_set_replicas).
+int preferred_mode(int requested, const TypeStore *store, unsigned n, unsigned numConstraints, bool residentRefused, unsigned replicas = 1);
 
 // Clusters of C CTAs with `smem` bytes each the device keeps co-resident; a query of the type mask alone answers for every cluster shape.
 struct ClusterQuery : std::function<int(unsigned mask, unsigned C, size_t smem)> {
@@ -51,6 +52,7 @@ struct PlanInput {
     int smCount;
     ClusterQuery maxClusters;                      // resident: what the device keeps co-resident
     bool residentRefused = false;                  // PBD_MODE_AUTO: the resident mode refused this model before
+    unsigned replicas = 1;                         // replica batch: every replica runs this one image (n, the constraints: one replica)
 };
 
 // One constraint type's arrays in device order (the host side of pbdk::TypeArrays).
@@ -64,7 +66,8 @@ struct TypePlan {
 };
 
 // Launch shape of a resident image: G clusters x C CTAs (one tile each), block size and type mask of the instantiation, smem per CTA.
-struct ResidentShape { unsigned G = 0, C = 0, threads = 0, xThreads = 0, mask = 0, tileCap = 0, nColours = 0; size_t smem = 0; };
+// A replica batch (replicas > 1): the tables describe the C tiles of one replica, and each of the G clusters steps every G-th replica.
+struct ResidentShape { unsigned G = 0, C = 0, threads = 0, xThreads = 0, mask = 0, tileCap = 0, nColours = 0, replicas = 1; size_t smem = 0; };
 
 struct ImagePlan {
     int mode = PBD_MODE_GRAPH;                     // what the image runs in: the requested mode, PBD_MODE_AUTO resolved
@@ -76,6 +79,10 @@ struct ImagePlan {
     ResidentShape res;
     std::vector<unsigned> colourStart, tileOff, tileStart, tileSmem, xNbr, xMask;
 };
+
+// Why a batch of `replicas` replicas of n particles cannot run `mode` with these rigid bodies and constraints, or "" (also for one replica
+// within the size limits).  plan_image checks it first; the engine also before it changes the batch size, the mode or the rigid bodies.
+std::string batch_refusal(unsigned replicas, unsigned n, int mode, unsigned nRb, const TypeStore *store);
 
 // Plans the image of `in` into `out`; returns "" or why the model cannot be flattened (for this mode and, resident, this device).
 std::string plan_image(const PlanInput &in, ImagePlan &out);

@@ -178,13 +178,25 @@ __device__ __forceinline__ void project_streamed(float4 *pos, const TypeArrays &
     }
 
 constexpr int kProjectThreads = 256;
+constexpr int kMultiSegments = 4;
 
-template <int T, int VAR>
+// A replica batch (pbd_set_replicas) shares one constraint image; the BATCH instantiations of the projection kernels run replica
+// blockIdx.y, whose particles start at slot y x nPos and whose multipliers of segment k's type start at y x nLambda[k] (k_project: [0]).
+struct ReplicaStrides { unsigned nPos; unsigned nLambda[kMultiSegments]; };
+// the type's arrays with the multipliers of replica `rep`
+__device__ __forceinline__ TypeArrays replica_arrays(const TypeArrays &a, unsigned rep, unsigned nLambda) {
+    TypeArrays r = a;
+    if (r.lambda) r.lambda += (size_t)rep * nLambda;
+    return r;
+}
+
+template <int T, int VAR, bool BATCH>
 __global__ void __launch_bounds__(kProjectThreads) k_project(float4 *pos, TypeArrays a, unsigned first,
-                                                             unsigned count, float dt, int iterZero) {
+                                                             unsigned count, float dt, int iterZero, ReplicaStrides rs) {
     pdl_launch_dependents();
     const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= count) return;  // an exited thread counts as having passed the dependency
+    if (BATCH) { pos += (size_t)blockIdx.y * rs.nPos; a = replica_arrays(a, blockIdx.y, rs.nLambda[0]); }
     const Streamed s = load_streamed<T>(a, first + i);
     pdl_wait_after(s.b.x ^ s.b.y, s.g0.x + s.g1.x + s.s0 + s.s1);
     project_streamed<T, VAR>(pos, a, first + i, s, dt, iterZero != 0);
@@ -229,7 +241,6 @@ __global__ void __launch_bounds__(256) k_jacobi_apply(float4 *__restrict__ pos, 
 // need no ordering among themselves (the reference runs a whole colour group under one `omp parallel for`,
 // TimeStepController.cpp:275-285).  A CTA finds its segment from blockIdx and dispatches on the segment's type.
 // Used when a colour holds more than one constraint type (e.g. FEMTet + Volume in cfg3: 112 buckets but 74 colours).
-constexpr int kMultiSegments = 4;
 struct MultiArgs {
     int nSeg;
     int type[kMultiSegments];
@@ -237,7 +248,8 @@ struct MultiArgs {
     TypeArrays arrays[kMultiSegments];
 };
 
-__global__ void __launch_bounds__(kProjectThreads) k_project_multi(float4 *pos, const __grid_constant__ MultiArgs m, float dt, int iterZero) {
+template <bool BATCH>
+__global__ void __launch_bounds__(kProjectThreads) k_project_multi(float4 *pos, const __grid_constant__ MultiArgs m, float dt, int iterZero, ReplicaStrides rs) {
     pdl_launch_dependents();
     int s = 0;
 #pragma unroll
@@ -245,8 +257,10 @@ __global__ void __launch_bounds__(kProjectThreads) k_project_multi(float4 *pos, 
         if (k < m.nSeg && blockIdx.x >= m.blockStart[k]) s = k;
     const unsigned i = (blockIdx.x - m.blockStart[s]) * blockDim.x + threadIdx.x;
     if (i >= m.count[s]) return;
-    const TypeArrays &a = m.arrays[s];
     const unsigned ci = m.first[s] + i;
+    TypeArrays batchArrays;
+    if (BATCH) { pos += (size_t)blockIdx.y * rs.nPos; batchArrays = replica_arrays(m.arrays[s], blockIdx.y, rs.nLambda[s]); }
+    const TypeArrays &a = BATCH ? batchArrays : m.arrays[s];
     PBD_FOR_TYPE(kMaskAll, m.type[s],
         const Streamed st = load_streamed<T>(a, ci);
         pdl_wait_after(st.b.x ^ st.b.y, st.g0.x + st.g1.x + st.s0 + st.s1);
@@ -364,15 +378,18 @@ __global__ void __launch_bounds__(256) k_velocity(const float4 *__restrict__ pos
 }
 
 // host AoS-3 <-> device float4 conversion (std::vector<Vector3r> layout on the host side); particle i of the host lives
-// in device slot slot[i] (de-interleaved formula of device_image.h, or the tile-major permutation of the tiled mode)
+// in device slot slot[i] (de-interleaved formula of device_image.h, or the tile-major permutation of the tiled mode).  Replica
+// blockIdx.y of a batch: host arrays at y x n particles, device arrays at slot y x n + slot[i].
 __global__ void k_relayout(const float4 *__restrict__ src, float4 *__restrict__ dst, unsigned n, const unsigned *__restrict__ oldSlot,
                            const unsigned *__restrict__ newSlot) {
     const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) dst[newSlot[i]] = src[oldSlot[i]];
+    const size_t r = (size_t)blockIdx.y * n;
+    if (i < n) dst[r + newSlot[i]] = src[r + oldSlot[i]];
 }
 __global__ void k_pack3(const float *__restrict__ src, float4 *__restrict__ dst, unsigned n, int keepW, const unsigned *__restrict__ slot) {
     const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
+    src += (size_t)blockIdx.y * 3 * n; dst += (size_t)blockIdx.y * n;
     const unsigned s = slot[i];
     float4 d = keepW ? dst[s] : make_float4(0.f, 0.f, 0.f, 0.f);
     d.x = src[3 * i]; d.y = src[3 * i + 1]; d.z = src[3 * i + 2];
@@ -381,12 +398,14 @@ __global__ void k_pack3(const float *__restrict__ src, float4 *__restrict__ dst,
 __global__ void k_unpack3(const float4 *__restrict__ src, float *__restrict__ dst, unsigned n, const unsigned *__restrict__ slot) {
     const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
+    src += (size_t)blockIdx.y * n; dst += (size_t)blockIdx.y * 3 * n;
     const float4 s = src[slot[i]];
     dst[3 * i] = s.x; dst[3 * i + 1] = s.y; dst[3 * i + 2] = s.z;
 }
 __global__ void k_set_w(float4 *__restrict__ pos, float4 *__restrict__ vel, const float *__restrict__ mass, unsigned n, const unsigned *__restrict__ slot) {
     const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
+    pos += (size_t)blockIdx.y * n; vel += (size_t)blockIdx.y * n; mass += (size_t)blockIdx.y * n;
     const float m = mass[i];
     const unsigned s = slot[i];
     pos[s].w = (m != 0.0f) ? 1.0f / m : 0.0f;  // ParticleData::setMass (ParticleData.h:239-246)

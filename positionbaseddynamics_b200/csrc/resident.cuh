@@ -22,7 +22,10 @@
 //     fits one cluster (G = 1) has no X items.
 //   Two regimes are used (host/image_plan.cpp:choose_resident_shape): ONE cluster of up to 16 CTAs for scenes whose colour phases are small
 //   (cfg1 / cfg3 / cfg4), and G = #SMs clusters of ONE CTA for big scenes (cfg2 / cfg5: 132 independent CTAs on an H100; the SINGLE
-//   instantiations: plain LDS / STS, __syncthreads).
+//   instantiations: plain LDS / STS, __syncthreads).  A replica batch (pbd_set_replicas, the BATCH instantiations) tiles one replica
+//   into one cluster of C CTAs and launches G such clusters; cluster g steps replicas g, g + G, ... one after the other.  The tables
+//   are tile-local and shared by every cluster; only the particle and multiplier bases move with the replica.  No cluster waits for
+//   another, so nothing beyond one cluster needs to be co-resident.
 //   The order of the items inside a tile's run is chosen at flatten time so that the lanes of a quarter-warp hit distinct 16-byte
 //   bank groups (host/image_plan.cpp:bank_group_fill).
 //
@@ -69,6 +72,10 @@ struct ResidentArgs {
     unsigned long long *trace;    // development aid (PBD_B200_TRACE): globaltimer per (phase, CTA, kTraceSlots)
     unsigned tracePhases;
     TypeArrays types[PBD_NUM_TYPES];
+    // replica batch (BATCH instantiations): cluster g runs replicas g, g + G, ... of `replicas`; replica r's particles start at slot
+    // r x replicaStride, its multipliers of type t at r x lamCount[t]
+    unsigned replicas, replicaStride;
+    unsigned lamCount[PBD_NUM_TYPES];
 };
 
 // ---- cluster primitives --------------------------------------------------------------------------------------------------
@@ -166,10 +173,10 @@ __device__ __forceinline__ void l2_prefetch_bytes(const void *p, size_t bytes) {
         a += chunk;
     }
 }
-// the per-constraint arrays of one type (indices, every geometry array, multipliers): array k of items [first, first + n), one array
-// per calling lane
+// the per-constraint arrays of one type (indices, every geometry array, the multipliers from a.lambda + lamOff): array k of items
+// [first, first + n), one array per calling lane
 template <int T>
-__device__ __forceinline__ void l2_prefetch_run(const TypeArrays &a, unsigned first, unsigned n, unsigned lane) {
+__device__ __forceinline__ void l2_prefetch_run(const TypeArrays &a, unsigned first, unsigned n, unsigned lane, size_t lamOff) {
     constexpr TypeShape sh = type_shape(T);
     if (lane == 0) {
         if (sh.nBodies == 2) l2_prefetch_bytes(a.idx2 + first, (size_t)n * 8u);
@@ -184,7 +191,7 @@ __device__ __forceinline__ void l2_prefetch_run(const TypeArrays &a, unsigned fi
         const unsigned k = lane - 3u - (unsigned)kMaxGeoV;
         if ((int)k < sh.nGeoS && a.gs[k]) l2_prefetch_bytes(a.gs[k] + first, (size_t)n * 4u);
     } else if (lane == 3 + (unsigned)kMaxGeoV + (unsigned)kMaxGeoS) {
-        if (sh.xpbd && a.lambda) l2_prefetch_bytes(a.lambda + first, (size_t)n * 4u);
+        if (sh.xpbd && a.lambda) l2_prefetch_bytes(a.lambda + lamOff + first, (size_t)n * 4u);
     }
 }
 constexpr unsigned kPrefetchLanes = 3u + (unsigned)kMaxGeoV + (unsigned)kMaxGeoS + 1u;
@@ -200,24 +207,30 @@ template <int T> __device__ __forceinline__ constexpr bool is_pipelined() {
 // ... and the ones light enough to keep TWO items ahead in flight (an L2 hit is ~300 cycles, one cloth projection ~60 issue slots)
 template <int T> __device__ __forceinline__ constexpr bool is_pipelined2() { return T == PBD_DISTANCE_XPBD || T == PBD_ISOBENDING_XPBD || T == PBD_DISTANCE || T == PBD_ISOBENDING; }
 
-template <unsigned MASK>
-__device__ __forceinline__ void prefetch_first(const ResidentArgs &A, const RunEntry &r, unsigned bi, bool iterZero, unsigned tid, bool xRun, Prefetched &pre) {
+// the multipliers of type T of replica `rep` of a batch start at A.types[T].lambda + lambda_offset
+template <int T> __device__ __forceinline__ size_t lambda_offset(const ResidentArgs &A, unsigned rep) { return (size_t)rep * A.lamCount[T]; }
+
+template <unsigned MASK, bool BATCH>
+__device__ __forceinline__ void prefetch_first(const ResidentArgs &A, const RunEntry &r, unsigned bi, bool iterZero, unsigned tid, bool xRun, Prefetched &pre,
+                                               unsigned rep) {
     pre.bucket = 0xffffffffu;
     const unsigned first = xRun ? r.firstX : r.firstR, n = xRun ? r.nX : r.nR;
     if (tid >= n) return;
     PBD_FOR_TYPE(MASK, r.type,
         pre.s = load_streamed<T>(A.types[T], first + tid);
-        if (type_shape(T).xpbd && !iterZero) pre.lam = __ldcg(A.types[T].lambda + first + tid);
+        if (type_shape(T).xpbd && !iterZero) pre.lam = __ldcg((BATCH ? A.types[T].lambda + lambda_offset<T>(A, rep) : A.types[T].lambda) + first + tid);
         pre.bucket = bi;)
 }
 
 // items [first, first + n) of a type's arrays: item tid, tid + stride, ... on this thread; with usePre the first one is in `pre`.
 // Software pipelined: the streamed operands (and multiplier) of the next item are in flight while the current one is projected.
-template <unsigned MASK, bool DEEP, class Acc>
+template <unsigned MASK, bool DEEP, bool BATCH, class Acc>
 __device__ __forceinline__ void run_items(const ResidentArgs &A, const Acc &acc, int type, unsigned first, unsigned n, bool iterZero, unsigned tid, unsigned stride,
-                                          bool usePre, const Prefetched &pre) {
+                                          bool usePre, const Prefetched &pre, unsigned rep) {
     PBD_FOR_TYPE(MASK, type,
-        const TypeArrays &ta = A.types[T];
+        TypeArrays batchArrays;  // a batch: the arrays with replica rep's multipliers
+        if (BATCH) batchArrays = replica_arrays(A.types[T], rep, A.lamCount[T]);
+        const TypeArrays &ta = BATCH ? batchArrays : A.types[T];
         unsigned i = tid;
         if (DEEP && is_pipelined2<T>()) {
             if (i < n) {
@@ -295,15 +308,19 @@ __device__ __forceinline__ void x_arrive(unsigned long long *flag, unsigned long
 __device__ __forceinline__ void colour_arrive(bool single) { if (!single) cluster_arrive(); }
 __device__ __forceinline__ void colour_wait(bool single) { if (single) __syncthreads(); else cluster_wait(); }
 
-template <unsigned MASK, int THREADS, bool SINGLE>
+// BATCH: a replica batch (one cluster's tiling of ONE replica, no X items); cluster g steps replicas g, g + G, ... one after the other,
+// each a whole step from the tile load to the tile store, and never waits for another cluster.
+template <unsigned MASK, int THREADS, bool SINGLE, bool BATCH>
 __global__ void __launch_bounds__(THREADS, 1) k_step_resident(const __grid_constant__ ResidentArgs A) {
     extern __shared__ float4 tile[];
     RunEntry *runs = reinterpret_cast<RunEntry *>(tile + A.tileCap);
     unsigned *sMask = reinterpret_cast<unsigned *>(runs + A.nBuckets);  // [1 + nColours]
     unsigned *sColour = sMask + 1 + A.nColours;                         // [nColours + 1]
     unsigned *sNbr = sColour + 1 + A.nColours;                          // [kMaxXNeighbours]
-    const unsigned cta = blockIdx.x;  // tile id = cluster * C + rank (1-D grid, cluster dimension C)
-    const unsigned t0 = __ldg(A.tileStart + cta), nSm = __ldg(A.tileSmem + cta), nAll = __ldg(A.tileStart + cta + 1) - t0;
+    const unsigned cta = BATCH ? blockIdx.x % A.clusterSize : blockIdx.x;  // tile id = cluster * C + rank (1-D grid, cluster dimension C); a batch: the rank
+    const unsigned tile0 = __ldg(A.tileStart + cta), nSm = __ldg(A.tileSmem + cta), nAll = __ldg(A.tileStart + cta + 1) - tile0;
+    unsigned rep = BATCH ? blockIdx.x / A.clusterSize : 0u;  // the replica this cluster steps
+    unsigned t0 = tile0 + (BATCH ? rep * A.replicaStride : 0u);
     const unsigned nGl = nAll - nSm;
     // thread roles: the first RT threads run the shared-memory items; the last XT threads (whole warps) run the X items and the
     // global-homed particles and are the only ones that ever wait for another cluster
@@ -352,91 +369,102 @@ __global__ void __launch_bounds__(THREADS, 1) k_step_resident(const __grid_const
     __syncthreads();
     Prefetched pre;
     pre.bucket = 0xffffffffu; pre.lam = 0.0f;
-    if (!single) { cluster_arrive(); cluster_wait(); }  // every tile of the cluster is loaded (and every CTA has started) before the first DSMEM access
+    for (;;) {  // the replicas of this cluster (one pass outside a batch)
+        if (!single) { cluster_arrive(); cluster_wait(); }  // every tile of the cluster is loaded (and every CTA has started) before the first DSMEM access
 
-    for (unsigned sub = 0; sub < A.subSteps; sub++) {
-        // ---- prologue: lastX = oldX; oldX = x; semi-implicit Euler
-        stamp(0);
-        if (isX) {  // global-homed particles: what other clusters wait for
-            for (unsigned i = xtid; i < nGl; i += XT) {
-                float4 x = __ldcg(A.pos + t0 + nSm + i);
-                if (integrate_particle(A, t0 + nSm + i, x)) __stcg(A.pos + t0 + nSm + i, x);
+        for (unsigned sub = 0; sub < A.subSteps; sub++) {
+            // ---- prologue: lastX = oldX; oldX = x; semi-implicit Euler
+            stamp(0);
+            if (isX) {  // global-homed particles: what other clusters wait for
+                for (unsigned i = xtid; i < nGl; i += XT) {
+                    float4 x = __ldcg(A.pos + t0 + nSm + i);
+                    if (integrate_particle(A, t0 + nSm + i, x)) __stcg(A.pos + t0 + nSm + i, x);
+                }
+                if (nGl) x_publish();
+                stamp(1);
+            } else {
+                for (unsigned i = threadIdx.x; i < nSm; i += RT) {
+                    float4 x = tile[tile_swizzle(i)];
+                    if (integrate_particle(A, t0 + i, x)) tile[tile_swizzle(i)] = x;
+                }
+                if (A.rb.n && cta == 0 && threadIdx.x < A.rb.n) rb_integrate_body(A.rb, threadIdx.x, A.h, A.gx, A.gy, A.gz);
             }
-            if (nGl) x_publish();
-            stamp(1);
-        } else {
-            for (unsigned i = threadIdx.x; i < nSm; i += RT) {
-                float4 x = tile[tile_swizzle(i)];
-                if (integrate_particle(A, t0 + i, x)) tile[tile_swizzle(i)] = x;
-            }
-            if (A.rb.n && cta == 0 && threadIdx.x < A.rb.n) rb_integrate_body(A.rb, threadIdx.x, A.h, A.gx, A.gy, A.gz);
-        }
-        x_count(0);
-        colour_arrive(single);
-        if (A.nColours) prefetch_first<MASK>(A, runs[sColour[0]], sColour[0], true, isX ? xtid : threadIdx.x, isX, pre);
-        stamp(2); colour_wait(single); stamp(3);
-        phase++;
+            x_count(0);
+            colour_arrive(single);
+            if (A.nColours) prefetch_first<MASK, BATCH>(A, runs[sColour[0]], sColour[0], true, isX ? xtid : threadIdx.x, isX, pre, rep);
+            stamp(2); colour_wait(single); stamp(3);
+            phase++;
 
-        // ---- coloured Gauss-Seidel sweeps (TimeStepController.cpp:270-286)
-        for (unsigned it = 0; it < A.maxIter; it++) {
-            const bool iterZero = (it == 0);
-            for (unsigned c = 0; c < A.nColours; c++) {
-                const unsigned b0 = sColour[c], b1 = sColour[c + 1];
-                stamp(0);
-                if (A.l2Prefetch && !isX && (threadIdx.x & 31u) == 0u) {  // the next colour's operand runs of this CTA start travelling DRAM -> L2 now
-                    // one array per R warp (lane 0): the colour barrier waits for the slowest warp, and the arrays issued by the lanes of
-                    // one warp would go one divergent path after the other; the X warps stay free for their cross-tile chain
-                    const unsigned cn = (c + 1 == A.nColours) ? 0u : c + 1u;
-                    for (unsigned k = threadIdx.x >> 5; k < kPrefetchLanes; k += RT >> 5)
-                        for (unsigned bi = sColour[cn]; bi < sColour[cn + 1]; bi++) {
-                            const RunEntry r = runs[bi];
-                            PBD_FOR_TYPE(MASK, r.type, l2_prefetch_run<T>(A.types[T], r.firstX, r.nX + r.nR, k);)
+            // ---- coloured Gauss-Seidel sweeps (TimeStepController.cpp:270-286)
+            for (unsigned it = 0; it < A.maxIter; it++) {
+                const bool iterZero = (it == 0);
+                for (unsigned c = 0; c < A.nColours; c++) {
+                    const unsigned b0 = sColour[c], b1 = sColour[c + 1];
+                    stamp(0);
+                    if (A.l2Prefetch && !isX && (threadIdx.x & 31u) == 0u) {  // the next colour's operand runs of this CTA start travelling DRAM -> L2 now
+                        // one array per R warp (lane 0): the colour barrier waits for the slowest warp, and the arrays issued by the lanes of
+                        // one warp would go one divergent path after the other; the X warps stay free for their cross-tile chain
+                        const unsigned cn = (c + 1 == A.nColours) ? 0u : c + 1u;
+                        for (unsigned k = threadIdx.x >> 5; k < kPrefetchLanes; k += RT >> 5)
+                            for (unsigned bi = sColour[cn]; bi < sColour[cn + 1]; bi++) {
+                                const RunEntry r = runs[bi];
+                                PBD_FOR_TYPE(MASK, r.type, l2_prefetch_run<T>(A.types[T], r.firstX, r.nX + r.nR, k, BATCH ? lambda_offset<T>(A, rep) : 0u);)
+                            }
+                    }
+                    if (isX) {
+                        // X items of every bucket of the colour: they touch global-homed particles and are ordered across CTAs by the flags
+                        bool mine = false;  // CTA-uniform: does this CTA own an X item of this colour?
+                        for (unsigned bi = b0; bi < b1; bi++) mine = mine || (runs[bi].nX != 0u);
+                        if (mine) {
+                            x_sync();
+    #pragma unroll 1
+                            for (unsigned bi = b0; bi < b1; bi++) run_items<MASK, false, BATCH>(A, accX, runs[bi].type, runs[bi].firstX, runs[bi].nX, iterZero, xtid, XT, pre.bucket == bi, pre,
+                                                                                         BATCH ? rep : 0u);
+                            x_publish();
                         }
-                }
-                if (isX) {
-                    // X items of every bucket of the colour: they touch global-homed particles and are ordered across CTAs by the flags
-                    bool mine = false;  // CTA-uniform: does this CTA own an X item of this colour?
-                    for (unsigned bi = b0; bi < b1; bi++) mine = mine || (runs[bi].nX != 0u);
-                    if (mine) {
-                        x_sync();
-#pragma unroll 1
-                        for (unsigned bi = b0; bi < b1; bi++) run_items<MASK, false>(A, accX, runs[bi].type, runs[bi].firstX, runs[bi].nX, iterZero, xtid, XT, pre.bucket == bi, pre);
-                        x_publish();
+                        stamp(1);
+                    } else {
+                        // everything else: shared memory of this cluster only
+    #pragma unroll 1
+                        for (unsigned bi = b0; bi < b1; bi++) {
+                            const unsigned rot = runs[bi].rotR;  // 0 for the first bucket of a colour (the one prefetch_first serves)
+                            run_items<MASK, SINGLE && MASK == kMaskClothXPBD, BATCH>(A, accR, runs[bi].type, runs[bi].firstR, runs[bi].nR, iterZero,
+                                                                               threadIdx.x >= rot ? threadIdx.x - rot : threadIdx.x + RT - rot, RT, pre.bucket == bi, pre,
+                                                                               BATCH ? rep : 0u);
+                        }
                     }
-                    stamp(1);
-                } else {
-                    // everything else: shared memory of this cluster only
-#pragma unroll 1
-                    for (unsigned bi = b0; bi < b1; bi++) {
-                        const unsigned rot = runs[bi].rotR;  // 0 for the first bucket of a colour (the one prefetch_first serves)
-                        run_items<MASK, SINGLE && MASK == kMaskClothXPBD>(A, accR, runs[bi].type, runs[bi].firstR, runs[bi].nR, iterZero,
-                                                                           threadIdx.x >= rot ? threadIdx.x - rot : threadIdx.x + RT - rot, RT, pre.bucket == bi, pre);
+                    x_count(1u + c);
+                    colour_arrive(single);
+                    {   // this thread's first item of the next colour streams in while the CTAs synchronise
+                        const bool lastColour = (c + 1 == A.nColours);
+                        if (!lastColour || it + 1 < A.maxIter) {
+                            const unsigned nb = sColour[lastColour ? 0u : c + 1u];
+                            prefetch_first<MASK, BATCH>(A, runs[nb], nb, false, isX ? xtid : threadIdx.x, isX, pre, rep);
+                        } else pre.bucket = 0xffffffffu;
                     }
+                    stamp(2); colour_wait(single); stamp(3);
+                    phase++;
                 }
-                x_count(1u + c);
-                colour_arrive(single);
-                {   // this thread's first item of the next colour streams in while the CTAs synchronise
-                    const bool lastColour = (c + 1 == A.nColours);
-                    if (!lastColour || it + 1 < A.maxIter) {
-                        const unsigned nb = sColour[lastColour ? 0u : c + 1u];
-                        prefetch_first<MASK>(A, runs[nb], nb, false, isX ? xtid : threadIdx.x, isX, pre);
-                    } else pre.bucket = 0xffffffffu;
-                }
-                stamp(2); colour_wait(single); stamp(3);
-                phase++;
+            }
+
+            // ---- epilogue: velocity update (own particles only; the global-homed ones need the last X items of every neighbour)
+            if (isX) {
+                if (nGl) x_wait(x_peer(), A.xLaunch | xNeed, xLane && xNeed != 0u, XT);
+                for (unsigned i = xtid; i < nGl; i += XT) velocity_particle(A, t0 + nSm + i, __ldcg(A.pos + t0 + nSm + i));
+            } else {
+                for (unsigned i = threadIdx.x; i < nSm; i += RT) velocity_particle(A, t0 + i, tile[tile_swizzle(i)]);
+                if (A.rb.n && cta == 0 && threadIdx.x < A.rb.n) rb_velocity_body(A.rb, threadIdx.x, A.invH, A.twoInvH, A.secondOrder);
             }
         }
-
-        // ---- epilogue: velocity update (own particles only; the global-homed ones need the last X items of every neighbour)
-        if (isX) {
-            if (nGl) x_wait(x_peer(), A.xLaunch | xNeed, xLane && xNeed != 0u, XT);
-            for (unsigned i = xtid; i < nGl; i += XT) velocity_particle(A, t0 + nSm + i, __ldcg(A.pos + t0 + nSm + i));
-        } else {
-            for (unsigned i = threadIdx.x; i < nSm; i += RT) velocity_particle(A, t0 + i, tile[tile_swizzle(i)]);
-            if (A.rb.n && cta == 0 && threadIdx.x < A.rb.n) rb_velocity_body(A.rb, threadIdx.x, A.invH, A.twoInvH, A.secondOrder);
-        }
+        for (unsigned i = threadIdx.x; i < nSm; i += THREADS) __stcg(A.pos + t0 + i, tile[tile_swizzle(i)]);
+        if (!BATCH) break;
+        rep += gridDim.x / A.clusterSize;
+        if (rep >= A.replicas) break;
+        t0 = tile0 + rep * A.replicaStride;
+        __syncthreads();  // the last replica's tile is stored before the next one overwrites it (no other CTA reads it after the last colour barrier)
+        for (unsigned i = threadIdx.x; i < nSm; i += THREADS) tile[tile_swizzle(i)] = __ldcg(A.pos + t0 + i);
+        __syncthreads();
     }
-    for (unsigned i = threadIdx.x; i < nSm; i += THREADS) __stcg(A.pos + t0 + i, tile[tile_swizzle(i)]);
 }
 
 }  // namespace pbdk

@@ -1,0 +1,170 @@
+"""Replica batches on one GPU (pbd_set_replicas): ms per batched step and aggregate projections/s for batches of cfg1-, cfg3-,
+100x100-XPBD-cloth and 100x100-FEMTriangle-cloth replicas over a sweep of K, in graph and resident mode, against the same K replicas
+stepped one after another by a K = 1 engine; the resident cluster size C swept on the cfg1- and cfg3-class batches; the card name and
+power limit read in the same run.  The four scenes run four different resident instantiations (cloth, FEM, cloth-XPBD and light type
+masks).
+
+    python tools/bench_batch.py [--out results.json] [--quick]
+
+Batch times are device times (CUDA events on the engine's stream around `steps` steps, after warm-up steps).  The baseline is measured:
+a K = 1 engine in its faster mode (graph or resident) steps K replicas one after another -- K pbd_step calls, each replica's state
+uploaded before its step and read back after it (pbd_set_attr / pbd_get_attr of x and v), wall clock around the whole sequence.
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+
+import numpy as np  # noqa: E402
+
+import scenes  # noqa: E402
+from positionbaseddynamics_b200 import _capi  # noqa: E402
+from positionbaseddynamics_b200.model import HostModel  # noqa: E402
+
+SCENES = {  # name: (builder, sub_steps, max_iter, K sweep)
+    "cfg1": (lambda m: scenes.cfg1(m), 1, 5, [1, 8, 33, 132, 264, 528, 1056]),
+    "cfg3": (lambda m: scenes.cfg3(m), 10, 5, [1, 4, 8, 16, 33, 66]),
+    "cloth100_xpbd": (lambda m: scenes.cloth(m, 100, 100, cloth_method=4, bending_method=3, dist_k=1.0e5, bend_k=100.0, sub_steps=1, max_iter=20),
+                      1, 20, [1, 8, 33, 66, 132, 264]),
+    "cloth100_femtri": (lambda m: scenes.cloth(m, 100, 100, cloth_method=2, bending_method=1, sub_steps=1, max_iter=5), 1, 5, [1, 8, 33, 66, 132, 264]),
+}
+C_SWEEP = {"cfg1": [8, 132, 528], "cfg3": [8, 33, 66]}  # K at which every cluster size C is measured
+
+
+def card():
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True, timeout=30).stdout
+        return out.strip().splitlines()[0]
+    except Exception as ex:  # the numbers are worth less without it: say so in the output
+        return "unknown (%s)" % ex
+
+
+def model(name):
+    build, sub, it, _ = SCENES[name]
+    hm = HostModel()
+    build(hm)
+    hm.init_groups()
+    types, bodies, params, _ = hm.constraints()
+    off, ids = hm.groups()
+    mass, _ = hm.masses()
+    m = dict(types=types, bodies=bodies, params=params, off=off, ids=ids, x0=hm.get("x0"), mass=mass, sub=sub, it=it)
+    hm.close()
+    return m
+
+
+def engine(m, mode, k, clusters=None):
+    if clusters:
+        os.environ["PBD_B200_CLUSTERS"] = "1x%d" % clusters  # the planner's cluster-size override (read when the image is planned)
+    else:
+        os.environ.pop("PBD_B200_CLUSTERS", None)
+    eng = _capi.Engine(0)
+    eng.set_particles(m["x0"], m["mass"])
+    eng.add_flat(m["types"], m["bodies"], m["params"])
+    eng.set_groups(m["off"], m["ids"])
+    eng.set_params(dt=0.005, sub_steps=m["sub"], max_iter=m["it"])
+    eng.set_mode(mode)
+    if k > 1:
+        eng.set_replicas(k)
+    return eng
+
+
+def timed(eng, warmup=3, min_s=0.4):
+    """ms per step: warm-up steps, a probe to size the window, then a window of at least min_s seconds of device time."""
+    eng.step(warmup); eng.sync()
+    eng.step(2); eng.sync()
+    probe = max(eng.stats().last_step_ms / 2, 1e-3)
+    steps = int(min(2000, max(10, min_s * 1e3 / probe)))
+    eng.step(steps); eng.sync()
+    st = eng.stats()
+    return st.last_step_ms / steps, steps
+
+
+def measure(m, mode, k, clusters=None):
+    t0 = time.time()
+    eng = None
+    try:
+        eng = engine(m, mode, k, clusters)
+        ms, steps = timed(eng)
+        _, active = eng.get_mode()
+    except _capi.PbdError as ex:
+        return {"error": str(ex)}
+    finally:
+        if eng is not None:
+            eng.close()
+    return {"ms": ms, "steps": steps, "active": active, "wall_s": time.time() - t0}
+
+
+def one_after_another(m, mode, k):
+    """ms for K replicas stepped one after another by one K = 1 engine: per replica, its x and v uploaded, one step, x and v read
+    back (the replicas' states are kept on the host between their steps); wall clock around the sequence, after one warm-up pass."""
+    eng = engine(m, mode, 1)
+    try:
+        n = len(m["x0"])
+        xs = np.repeat(np.asarray(m["x0"], np.float32)[None], k, 0)
+        vs = np.zeros_like(xs)
+        for passes in range(2):  # the first pass warms up
+            eng.sync()
+            t0 = time.perf_counter()
+            for r in range(k):
+                eng.set_attr(_capi.ATTR_X, xs[r]); eng.set_attr(_capi.ATTR_V, vs[r])
+                eng.step(1)
+                eng.get_attr(_capi.ATTR_X, xs[r]); eng.get_attr(_capi.ATTR_V, vs[r])
+            eng.sync()
+            ms = (time.perf_counter() - t0) * 1e3
+        assert xs.shape == (k, n, 3)
+        return ms
+    finally:
+        eng.close()
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--out", default=None, help="also write the results as JSON here")
+    ap.add_argument("--quick", action="store_true", help="first two K of every sweep, no C sweep (a rehearsal)")
+    ap.add_argument("--scenes", default=",".join(SCENES))
+    a = ap.parse_args()
+    res = {"card": card(), "rows": [], "c_sweep": []}
+    print("card: %s" % res["card"], flush=True)
+    for name in a.scenes.split(","):
+        m = model(name)
+        ncons = len(m["types"])
+        proj = ncons * m["sub"] * m["it"]
+        solo = {md: measure(m, md, 1) for md in (_capi.MODE_GRAPH, _capi.MODE_RESIDENT)}
+        solo_mode = min((r["ms"], md) for md, r in solo.items() if "ms" in r)[1]
+        ks = SCENES[name][3][:2] if a.quick else SCENES[name][3]
+        print("%s: %d particles, %d constraints, %d x %d; K = 1: graph %.3f ms, resident %s ms" % (
+            name, len(m["x0"]), ncons, m["sub"], m["it"], solo[0]["ms"], "%.3f" % solo[1]["ms"] if "ms" in solo[1] else solo[1]["error"]), flush=True)
+        for k in ks:
+            row = {"scene": name, "K": k, "baseline_ms": one_after_another(m, solo_mode, k)}
+            for label, md in (("graph", _capi.MODE_GRAPH), ("resident", _capi.MODE_RESIDENT), ("auto", _capi.MODE_AUTO)):
+                r = measure(m, md, k)
+                row[label] = r
+                if "ms" in r:
+                    r["proj_per_s"] = k * proj / (r["ms"] * 1e-3)
+            res["rows"].append(row)
+            fmt = lambda r: ("%9.3f ms %8.2e/s" % (r["ms"], r["proj_per_s"])) if "ms" in r else ("refused: " + r["error"][:60])
+            print("  K=%5d  graph %s | resident %s | auto(%s) %s | one after another %9.3f ms" % (
+                k, fmt(row["graph"]), fmt(row["resident"]), row["auto"].get("active"), fmt(row["auto"]), row["baseline_ms"]), flush=True)
+        if a.quick or name not in C_SWEEP:
+            continue
+        for k in C_SWEEP[name]:
+            for c in (1, 2, 4, 8, 16):
+                r = measure(m, _capi.MODE_RESIDENT, k, clusters=c)
+                r.update({"scene": name, "K": k, "C": c})
+                res["c_sweep"].append(r)
+                print("  C sweep K=%5d C=%2d: %s" % (k, c, ("%.3f ms" % r["ms"]) if "ms" in r else r["error"][:80]), flush=True)
+    os.environ.pop("PBD_B200_CLUSTERS", None)
+    if a.out:
+        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
+        with open(a.out, "w") as f:
+            json.dump(res, f, indent=1)
+
+
+if __name__ == "__main__":
+    main()

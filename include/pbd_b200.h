@@ -39,6 +39,10 @@ typedef struct pbd_engine pbd_engine;
  *  PBD_SHAPEMATCHING        4       stiffness, restCm[3], x0[4][3], w[4], numClusters[4]     ShapeMatchingConstraint (4-particle clusters) :1985-2028
  *  PBD_BALLJOINT            2 (rigid body, rigid body)      jointInfo[3x4] column by column  BallJoint                    Constraints.cpp:54-125
  *  PBD_RB_PARTICLE_BALLJOINT 2 (rigid body, particle)       jointInfo[3x2] column by column  RigidBodyParticleBallJoint   Constraints.cpp:925-987
+ *  Material parameters (what pbd_set_replica_materials replaces per replica; everything else is geometry of the rest state):
+ *    Distance(+XPBD), Dihedral, Volume(+XPBD), IsometricBending(+XPBD), ShapeMatching: stiffness;  FEMTriangle: Exx, Eyy, Exy, nu_xy,
+ *    nu_yx;  StrainTriangle: kxx, kyy, kxy, normStretch, normShear;  FEMTet(+XPBD): E, nu;  StrainTet: stretchK, shearK, normStretch,
+ *    normShear;  the two joint types: none.
  *  (joints: only the local connector columns are read, the global ones are recomputed at every solve as
  *   updateConstraint does; rigid bodies must be uploaded with pbd_set_rigid_bodies before joints are added)
  */
@@ -106,6 +110,7 @@ int pbd_add_constraints(pbd_engine *e, int type, unsigned count, const unsigned 
                         const unsigned *ids);
 int pbd_num_bodies(int type);
 int pbd_num_params(int type);
+int pbd_num_materials(int type);  /* how many of the type's parameters are material parameters (table above); 0 for the joints */
 
 /* Colour groups: either import the reference's SimulationModel::m_constraintGroups (offsets[nGroups+1], ids by
  * insertion index) or recompute them with the reference's greedy first-fit (SimulationModel.cpp:1033-1094). */
@@ -186,7 +191,9 @@ int pbd_get_contacts(pbd_engine *e, pbd_contact *out, unsigned capacity, unsigne
  *    pbd_add_constraints, the colour groups, pbd_set_params.
  *  - Calls that MOVE state take the whole batch, replica after replica: pbd_set_attr / pbd_get_attr (K*n*3 floats), pbd_set_masses
  *    (K*n: each replica may pin other particles), pbd_step_host / pbd_step_host_async (K*n*3 per array), pbd_get_lambdas (K*count
- *    multipliers, `ids` count insertion ids).  Constraint parameters are shared.
+ *    multipliers, `ids` count insertion ids).
+ *  - Constraint parameters and gravity are shared unless pbd_set_replica_materials / pbd_set_replica_gravity (below) give every replica
+ *    its own; the geometry of the rest state (rest lengths, Q, inverse rest matrices, areas, volumes) is always shared.
  *  - pbd_get_stats: projections and bytes_per_step count every replica; num_particles and num_constraints are per replica.
  *  - K > 1 is refused with rigid bodies or joints, with colliders and in PBD_MODE_JACOBI.  PBD_MODE_RESIDENT runs one cluster of CTAs
  *    per replica and refuses a replica that does not fit one cluster; PBD_MODE_AUTO then runs the graph mode.
@@ -194,6 +201,17 @@ int pbd_get_contacts(pbd_engine *e, pbd_contact *out, unsigned capacity, unsigne
  * lastX, masses), the XPBD multipliers at zero, and the image is planned again.  At K = 1 every call behaves as for one scene. */
 int pbd_set_replicas(pbd_engine *e, unsigned K);
 int pbd_get_replicas(pbd_engine *e, unsigned *K);
+/* Per-replica parameters of a batch (K > 1; a single-scene engine takes its parameters from pbd_add_constraints / pbd_set_params and
+ * refuses these calls).  Both copy their rows in stream order into device tables that keep their address, so a change between two steps
+ * takes effect at the next step.  pbd_set_replicas drops every override (the rows belong to the old K); nothing else does -- adding
+ * constraints or changing the mode keeps them.
+ * pbd_set_replica_materials: replica r's constraints of `type` all carry the material parameters mat[r*nMat .. r*nMat+nMat), nMat =
+ * pbd_num_materials(type), replacing whatever the constraints were added with (a per-constraint material array of that type is ignored
+ * while the override is set).  mat = NULL: back to the shared parameters.  Replica r then advances bit for bit as a single-scene engine
+ * whose constraints of `type` were added with those values.  Refused for an unknown type and for a type without material parameters.
+ * pbd_set_replica_gravity: replica r integrates with gravity g[3r..3r+3) instead of pbd_set_params' vector.  g = NULL: back to it. */
+int pbd_set_replica_materials(pbd_engine *e, int type, const float *mat /* K * pbd_num_materials(type) */);
+int pbd_set_replica_gravity(pbd_engine *e, const float *g /* K*3 */);
 
 int pbd_get_lambdas(pbd_engine *e, int type, float *dst, unsigned *ids); /* debug: per-type XPBD multipliers + insertion ids */
 int pbd_get_stats(pbd_engine *e, pbd_stats *out);

@@ -25,6 +25,7 @@ SYMBOLS = ["pbd_last_error", "pbd_device_count", "pbd_create", "pbd_destroy", "p
            "pbd_num_params", "pbd_set_groups", "pbd_color_first_fit", "pbd_color_first_fit_device", "pbd_pin_host", "pbd_unpin_host", "pbd_get_num_groups", "pbd_get_groups",
            "pbd_set_params", "pbd_set_mode", "pbd_get_mode", "pbd_step", "pbd_sync", "pbd_step_host", "pbd_step_host_async", "pbd_step_host_wait",
            "pbd_get_lambdas", "pbd_get_stats", "pbd_profile_step", "pbd_set_replicas", "pbd_get_replicas",
+           "pbd_num_materials", "pbd_set_replica_materials", "pbd_set_replica_gravity",
            "pbd_set_colliders", "pbd_set_contact_params", "pbd_record_contacts", "pbd_get_contacts"]
 
 
@@ -102,6 +103,8 @@ def lib():
         _lib.pbd_profile_step.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         _lib.pbd_set_replicas.argtypes = [C.c_void_p, C.c_uint]
         _lib.pbd_get_replicas.argtypes = [C.c_void_p, C.POINTER(C.c_uint)]
+        _lib.pbd_set_replica_materials.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+        _lib.pbd_set_replica_gravity.argtypes = [C.c_void_p, C.c_void_p]
     return _lib
 
 
@@ -132,11 +135,17 @@ def num_params(t):
     return lib().pbd_num_params(t)
 
 
+def num_materials(t):
+    """How many of type t's parameters are material parameters (include/pbd_b200.h); what a row of set_replica_materials holds."""
+    return lib().pbd_num_materials(t)
+
+
 class Engine:
     """One engine <-> one CUDA device + one stream (pbd_create / pbd_destroy).
 
     A replica batch (set_replicas(K), K > 1) steps K independent copies of the model's state at once: the particle state calls then
-    take and return (K, n, 3) / (K, n) arrays and lambdas() (K, count); at K = 1 the shapes are those of one scene."""
+    take and return (K, n, 3) / (K, n) arrays and lambdas() (K, count); at K = 1 the shapes are those of one scene.  The replicas share
+    the model's parameters unless set_replica_materials / set_replica_gravity give each its own."""
 
     def __init__(self, device=0, stream=None):
         self._h = C.c_void_p()
@@ -191,6 +200,23 @@ class Engine:
         k = C.c_uint(0)
         _ck(lib().pbd_get_replicas(self._h, C.byref(k)))
         return k.value
+
+    def set_replica_materials(self, ctype, mat):
+        """Replica r's constraints of `ctype` all carry the material parameters mat[r] ((K, num_materials(ctype)) array); None: the
+        shared parameters again.  K > 1 only."""
+        if mat is not None:
+            mat = _f32(mat)
+            if mat.shape != (self.K, num_materials(ctype)):
+                raise ValueError("set_replica_materials: type %d wants a (%d, %d) array, got %s" % (ctype, self.K, num_materials(ctype), mat.shape))
+        _ck(lib().pbd_set_replica_materials(self._h, int(ctype), _ptr(mat)))
+
+    def set_replica_gravity(self, g):
+        """Replica r integrates with gravity g[r] ((K, 3) array); None: the vector of set_params again.  K > 1 only."""
+        if g is not None:
+            g = _f32(g)
+            if g.shape != (self.K, 3):
+                raise ValueError("set_replica_gravity: wants a (%d, 3) array, got %s" % (self.K, g.shape))
+        _ck(lib().pbd_set_replica_gravity(self._h, _ptr(g)))
 
     # rigid bodies ----------------------------------------------------------------------------------
     def set_rigid_bodies(self, mass, x, q, inertia, v=None, omega=None):

@@ -78,6 +78,18 @@ constexpr TypeShape type_shape(int t) {
     }
 }
 
+// Per-replica material parameters of a batch (pbd_set_replica_materials): one row of kMatRowFloats floats per replica, type t's
+// nMat parameters at mat_offset(t).
+#if defined(__CUDACC__)
+__host__ __device__
+#endif
+constexpr int mat_offset(int t) {
+    int o = 0;
+    for (int u = 0; u < t; u++) o += type_shape(u).nMat;
+    return o;
+}
+constexpr int kMatRowFloats = mat_offset(PBD_NUM_TYPES);
+
 // Algorithmic bytes per projection (SURVEY.md section 8d): indices + particle float4 read + per-constraint constants
 // + particle float4 write (+ lambda read/write for XPBD).  Isometric bending uses the rank-1 figure (4 floats Kp).
 inline double algorithmic_bytes(int t, int isoVariant) {
@@ -134,10 +146,12 @@ __host__ __device__ __forceinline__ unsigned tile_swizzle(unsigned s) { return s
 constexpr int kMaxClusterCtas = 16;   // non-portable cluster size (opt-in attribute), one GPC
 // Dynamic shared memory of a CTA: [tile: tileCap float4][run table: nBuckets x RunEntry][xMask: 1 + nColours][colourStart: nColours + 1]
 // [xNbr: kMaxXNeighbours]
+// A replica batch has no X items: there the xNbr words hold the material row and the gravity of the replica the cluster is stepping.
 // this CTA's two runs of one bucket (absolute indices into the type's arrays); rotR: where the run of shared-memory items starts in the
 // colour's concatenated item sequence, modulo the number of threads that share it (the buckets of one colour go to different threads)
 struct RunEntry { int type; unsigned firstX, nX, firstR, nR, rotR, pad0, pad1; };
 constexpr unsigned kMaxXNeighbours = 32;  // one lane of the first X warp per neighbour
+static_assert(kMatRowFloats + 3 <= (int)kMaxXNeighbours, "a replica's material row and gravity are staged in the xNbr words");
 __host__ __device__ inline size_t resident_smem_bytes(unsigned tileCap, unsigned nBuckets, unsigned nColours) {
     return (size_t)tileCap * sizeof(float4) + (size_t)nBuckets * sizeof(RunEntry) + (size_t)(2u * nColours + 2u + kMaxXNeighbours) * sizeof(unsigned);
 }

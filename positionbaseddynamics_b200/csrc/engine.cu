@@ -83,6 +83,12 @@ struct pbd_engine {
     // particles: K replicas of n (pbd_set_replicas), replica r at device slots [r n, (r + 1) n)
     unsigned n = 0, K = 1;
     DevBuf pos, vel, oldp, lastp, pos0, stage, stage2, massStage, jacobiDelta;
+    // Per-replica parameters of a batch.  repMat [K][kMatRowFloats]: the uniform material parameters of every type, replica by replica --
+    // the shared ones of the image, or a replica's own (pbd_set_replica_materials, the types of repMatMask); repGravity [K][3]
+    // (pbd_set_replica_gravity).  Both keep their address until K changes, so that a captured graph keeps reading the same tables.
+    DevBuf repMat, repGravity;
+    unsigned repMatMask = 0;
+    bool repGravitySet = false;
     // rigid bodies coupled through joints (SURVEY.md 8f-1): float4 arrays X(xyz,invMass) Q(x,y,z,w) V(xyz,mass) W(omega) + history + inertia
     unsigned nRb = 0;
     DevBuf rbX, rbQ, rbV, rbW, rbOldX, rbLastX, rbOldQ, rbLastQ, rbI, rbIinv;
@@ -141,6 +147,7 @@ extern "C" int pbd_device_count(int *count) {
 }
 extern "C" int pbd_num_bodies(int type) { return type_shape(type).nBodies; }
 extern "C" int pbd_num_params(int type) { return type_shape(type).nParams; }
+extern "C" int pbd_num_materials(int type) { return type_shape(type).nMat; }
 
 extern "C" int pbd_create(int device, void *stream, pbd_engine **out) {
     if (!out) return fail("pbd_create: out == NULL");
@@ -324,6 +331,7 @@ extern "C" int pbd_set_replicas(pbd_engine *e, unsigned K) {
             CK(cudaStreamSynchronize(e->stream));  // before `grown` frees the old array
         }
     e->K = K;
+    e->repMat.release(); e->repGravity.release(); e->repMatMask = 0; e->repGravitySet = false;  // rows of the old K
     for (DevBuf *b : {&e->pos, &e->vel, &e->oldp, &e->lastp, &e->pos0}) CKE(broadcast_replica0(e, *b));
     CKE(e->stage.alloc((size_t)K * e->n * 3 * sizeof(float)));
     CKE(e->massStage.alloc((size_t)K * e->n * sizeof(float)));
@@ -332,6 +340,63 @@ extern "C" int pbd_set_replicas(pbd_engine *e, unsigned K) {
     e->autoNoResident = false;  // whether the resident mode takes the model depends on the batch size
     return 0;
 }
+
+static int replica_params_refusal(const pbd_engine *e, const char *what) {
+    if (!e) return fail("%s: null engine", what);
+    if (e->K == 1) return fail("%s: a single-scene engine takes its parameters from pbd_add_constraints / pbd_set_params (pbd_set_replicas first)", what);
+    return 0;
+}
+// type's columns of the K rows of the material table <- rows of nMat floats `pitch` bytes apart (0: the same row for every replica)
+static int write_replica_materials(pbd_engine *e, int type, const float *rows, size_t pitch) {
+    if (!e->repMat.p) {
+        CKE(e->repMat.alloc((size_t)e->K * kMatRowFloats * sizeof(float)));
+        CK(cudaMemsetAsync(e->repMat.p, 0, e->repMat.bytes, e->stream));
+    }
+    const size_t width = type_shape(type).nMat * sizeof(float);
+    std::vector<float> same;
+    if (!pitch) {
+        same.resize((size_t)e->K * type_shape(type).nMat);
+        for (size_t i = 0; i < same.size(); i++) same[i] = rows[i % type_shape(type).nMat];
+        rows = same.data(); pitch = width;
+    }
+    CK(cudaMemcpy2DAsync((float *)e->repMat.p + mat_offset(type), kMatRowFloats * sizeof(float), rows, pitch, width, e->K, cudaMemcpyHostToDevice, e->stream));
+    return 0;
+}
+// The rows are copied in stream order into tables that keep their address: a captured graph reads the new values at its next launch.
+// Only switching an override on or off changes kernel arguments, and so drops the graph.
+extern "C" int pbd_set_replica_materials(pbd_engine *e, int type, const float *mat) {
+    if (type < 0 || type >= PBD_NUM_TYPES) return fail("pbd_set_replica_materials: unknown constraint type %d", type);
+    const int nMat = type_shape(type).nMat;
+    if (nMat == 0) return fail("pbd_set_replica_materials: constraint type %d has no material parameters", type);
+    CKE(replica_params_refusal(e, "pbd_set_replica_materials"));
+    CKE(use(e));
+    const unsigned bit = 1u << type;
+    if (mat) CKE(write_replica_materials(e, type, mat, nMat * sizeof(float)));
+    else if ((e->repMatMask & bit) && !e->imageDirty) CKE(write_replica_materials(e, type, e->dev[type].arrays.matU, 0));  // (a dirty image writes them when it is planned)
+    // (on or off decides whether the per-constraint material arrays of the type count: batch_arrays)
+    if (((e->repMatMask & bit) != 0u) != (mat != nullptr)) { e->repMatMask ^= bit; drop_graph(e); }
+    return 0;
+}
+extern "C" int pbd_set_replica_gravity(pbd_engine *e, const float *g) {
+    CKE(replica_params_refusal(e, "pbd_set_replica_gravity"));
+    CKE(use(e));
+    if (g) {
+        CKE(e->repGravity.alloc((size_t)e->K * 3 * sizeof(float)));
+        CK(cudaMemcpyAsync(e->repGravity.p, g, (size_t)e->K * 3 * sizeof(float), cudaMemcpyHostToDevice, e->stream));
+    }
+    if (e->repGravitySet != (g != nullptr)) { e->repGravitySet = (g != nullptr); drop_graph(e); }
+    return 0;
+}
+// What a batch's per-bucket kernels get for type t: where the replicas have parameters of their own, its place in replica 0's row of the
+// material table (without them the kernel arguments' uniforms do: reading the table for every launch cost the small shared-parameter
+// batches of DESIGN.md section 6 7-17 % in graph mode); and its arrays -- without the per-constraint material arrays in that case.
+static const float *replica_mat(const pbd_engine *e, int t) { return ((e->repMatMask >> t) & 1u) ? (const float *)e->repMat.p + mat_offset(t) : nullptr; }
+static TypeArrays batch_arrays(const pbd_engine *e, int t) {
+    TypeArrays a = e->dev[t].arrays;
+    if ((e->repMatMask >> t) & 1u) for (int k = 0; k < kMaxMat; k++) a.mat[k] = nullptr;
+    return a;
+}
+
 extern "C" int pbd_get_replicas(pbd_engine *e, unsigned *K) {
     if (!e || !K) return fail("pbd_get_replicas: null argument");
     *K = e->K;
@@ -748,6 +813,7 @@ static int upload_type(pbd_engine *e, int t, pbd_b200::TypePlan &p) {
         if (!p.mat[k].empty()) { CKE(upload_vec(d.mat[k], p.mat[k], e->stream)); a.mat[k] = (const float *)d.mat[k].p; }
     }
     a.variant = p.variant;
+    if (e->K > 1 && type_shape(t).nMat && !((e->repMatMask >> t) & 1u)) CKE(write_replica_materials(e, t, a.matU, 0));  // the shared parameters, for every replica
     if (t == PBD_BALLJOINT || t == PBD_RB_PARTICLE_BALLJOINT) {
         a.rbX = (float4 *)e->rbX.p; a.rbQ = (float4 *)e->rbQ.p; a.rbIinv = (const float4 *)e->rbIinv.p;
     }
@@ -852,9 +918,9 @@ template <class F> static int with_project_type(int type, int variant, F &&f) {
 
 // A batch's projection launches run replica blockIdx.y (the BATCH instantiations); their block size follows the whole batch's count.
 static int launch_bucket(pbd_engine *e, const Bucket &b, float h, int iterZero, cudaStream_t s, bool pdl) {
-    const TypeArrays &a = e->dev[b.type].arrays;
+    const TypeArrays a = batch_arrays(e, b.type);
     const unsigned block = project_block(e, b.count * e->K);
-    const ReplicaStrides rs{e->n, {e->dev[b.type].count}};
+    const ReplicaStrides rs{e->n, {e->dev[b.type].count}, {replica_mat(e, b.type)}};
     return with_project_type(b.type, a.variant, [&](auto T, auto V) -> int {
         constexpr int TT = decltype(T)::value, VAR = decltype(V)::value;
         if (e->K > 1) CK(launch_step_kernel(k_project<TT, VAR, true>, dim3(nblk(b.count, block), e->K), block, s, pdl, (float4 *)e->pos.p, a, b.first, b.count, h, iterZero, rs));
@@ -898,7 +964,7 @@ static int launch_colour(pbd_engine *e, size_t b0, size_t b1, float h, int iterZ
     for (size_t c0 = b0; c0 < b1; c0 += kMultiSegments) {
         const size_t c1 = std::min(b1, c0 + (size_t)kMultiSegments);
         MultiArgs m{};
-        ReplicaStrides rs{e->n, {}};
+        ReplicaStrides rs{e->n, {}, {}};
         m.nSeg = (int)(c1 - c0);
         unsigned blocks = 0, total = 0;
         for (size_t i = c0; i < c1; i++) total += e->buckets[i].count;
@@ -907,8 +973,8 @@ static int launch_colour(pbd_engine *e, size_t b0, size_t b1, float h, int iterZ
             const Bucket &b = e->buckets[i];
             const int k = (int)(i - c0);
             m.type[k] = b.type; m.first[k] = b.first; m.count[k] = b.count; m.blockStart[k] = blocks;
-            m.arrays[k] = e->dev[b.type].arrays;
-            rs.nLambda[k] = e->dev[b.type].count;
+            m.arrays[k] = batch_arrays(e, b.type);
+            rs.nLambda[k] = e->dev[b.type].count; rs.mat[k] = replica_mat(e, b.type);
             blocks += nblk(b.count, block);
         }
         for (int k = m.nSeg; k <= kMultiSegments; k++) m.blockStart[k] = blocks;
@@ -937,7 +1003,12 @@ static int enqueue_step_launches(pbd_engine *e, cudaStream_t s, unsigned long lo
     for (unsigned sub = 0; sub < e->subSteps; sub++) {
         if (e->nRb) { CK(launch_step_kernel(k_rb_integrate, nblk(e->nRb, 256), 256, s, pdl, rb, h, e->g[0], e->g[1], e->g[2])); CKE(launched(kLaunchIntegrate)); }
         if (n) {
-            CK(launch_step_kernel(k_integrate, nblk(n, 256), 256, s, pdl, (float4 *)e->pos.p, (float4 *)e->vel.p, (float4 *)e->oldp.p, (float4 *)e->lastp.p, n, h, e->g[0], e->g[1], e->g[2]));
+            if (e->repGravitySet)  // replica blockIdx.y under its own row
+                CK(launch_step_kernel(k_integrate<true>, replica_grid(e, e->K), 256, s, pdl, (float4 *)e->pos.p, (float4 *)e->vel.p, (float4 *)e->oldp.p, (float4 *)e->lastp.p, e->n, h, 0.0f, 0.0f, 0.0f,
+                                      (const float *)e->repGravity.p));
+            else
+                CK(launch_step_kernel(k_integrate<false>, nblk(n, 256), 256, s, pdl, (float4 *)e->pos.p, (float4 *)e->vel.p, (float4 *)e->oldp.p, (float4 *)e->lastp.p, n, h, e->g[0], e->g[1], e->g[2],
+                                      (const float *)nullptr));
             CKE(launched(kLaunchIntegrate));
         }
         for (unsigned it = 0; it < e->maxIter; it++)
@@ -985,8 +1056,9 @@ static int enqueue_step_resident(pbd_engine *e, cudaStream_t s, unsigned long lo
     ra.xFlags = (unsigned long long *)e->dXFlags.p;
     ra.xLaunch = (++e->xLaunch) << 32;  // above every flag value of the earlier launches, whatever subSteps / maxIter they ran with
     ra.rb = rb_state(e);
-    for (int t = 0; t < PBD_NUM_TYPES; t++) { ra.types[t] = e->dev[t].arrays; ra.lamCount[t] = e->dev[t].count; }
+    for (int t = 0; t < PBD_NUM_TYPES; t++) { ra.types[t] = batch_arrays(e, t); ra.lamCount[t] = e->dev[t].count; }
     ra.replicas = e->res.replicas; ra.replicaStride = e->n;
+    ra.repMat = (const float *)e->repMat.p; ra.repGravity = e->repGravitySet ? (const float *)e->repGravity.p : nullptr;
     *launches = 1;
     ra.trace = nullptr; ra.tracePhases = 0;
     static const char *tracePath = getenv("PBD_B200_TRACE");  // development aid: dump per-phase timelines of one step (tools/trace_resident.py)
@@ -1032,7 +1104,7 @@ static int enqueue_step_jacobi(pbd_engine *e, cudaStream_t s, unsigned long long
     const float4 *pos = (const float4 *)e->pos.p; float4 *delta = (float4 *)e->jacobiDelta.p;
     unsigned long long L = 0;
     for (unsigned sub = 0; sub < e->subSteps; sub++) {
-        k_integrate<<<nblk(n, 256), 256, 0, s>>>((float4 *)e->pos.p, (float4 *)e->vel.p, (float4 *)e->oldp.p, (float4 *)e->lastp.p, n, h, e->g[0], e->g[1], e->g[2]); L++;
+        k_integrate<false><<<nblk(n, 256), 256, 0, s>>>((float4 *)e->pos.p, (float4 *)e->vel.p, (float4 *)e->oldp.p, (float4 *)e->lastp.p, n, h, e->g[0], e->g[1], e->g[2], nullptr); L++;
         for (unsigned it = 0; it < e->maxIter; it++) {
             for (int t = 0; t < PBD_BALLJOINT; t++) {
                 const unsigned cnt = e->dev[t].count;

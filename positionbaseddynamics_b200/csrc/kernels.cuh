@@ -34,8 +34,22 @@ __device__ __forceinline__ void pdl_wait_after(unsigned a, float b) {
 __device__ __forceinline__ float4 ldp(const float4 *p) { return *p; }
 __device__ __forceinline__ void stp(float4 *p, const float4 &v) { if (v.w != 0.0f) __stcg(p, v); }  // static particles never move
 
-__device__ __forceinline__ float matv(const TypeArrays &a, int slot, unsigned i) {
-    return a.mat[slot] ? __ldg(a.mat[slot] + i) : a.matU[slot];
+// A replica batch keeps the uniform material parameters of a type in a table row per replica (pbd_set_replica_materials; the shared
+// values where a replica has none of its own).  MatRow: that row in registers, loaded once ahead of a kernel's projections like the
+// other operands that do not depend on the previous colour; `on` false: the uniforms of the kernel arguments.
+struct MatRow { bool on = false; float v[kMaxMat]; };
+template <int T>
+__device__ __forceinline__ MatRow load_mat_row(const float *row) {
+    MatRow r;
+    r.on = row != nullptr;
+    if (r.on) {
+#pragma unroll
+        for (int k = 0; k < type_shape(T).nMat; k++) r.v[k] = row[k];
+    }
+    return r;
+}
+__device__ __forceinline__ float matv(const TypeArrays &a, int slot, unsigned i, const MatRow &row = MatRow{}) {
+    return a.mat[slot] ? __ldg(a.mat[slot] + i) : (row.on ? row.v[slot] : a.matU[slot]);
 }
 __device__ __forceinline__ float xpbd_alpha(float k, float dt) { return (k != 0.0f) ? frcp(k * dt * dt) : 0.0f; }
 
@@ -105,7 +119,7 @@ __device__ __forceinline__ void project_joint(const Acc &acc, const TypeArrays &
 // VAR: compile-time layout variant of the type (IsometricBending: 0 = rank-1 Kp, 1 = full Q), -1 = read a.variant at run time
 template <int T, class Acc, int VAR = -1>
 __device__ __forceinline__ void project_streamed_acc(const Acc &acc, const TypeArrays &a, unsigned i, const Streamed &s, float dt,
-                                                     bool iterZero, bool lambdaGiven = false, float lambdaValue = 0.0f) {
+                                                     bool iterZero, bool lambdaGiven = false, float lambdaValue = 0.0f, const MatRow &matRow = MatRow{}) {
     if (T == PBD_BALLJOINT || T == PBD_RB_PARTICLE_BALLJOINT) { project_joint<T>(acc, a, s); return; }
     constexpr bool XPBD = type_shape(T).xpbd;
     constexpr int NB = type_shape(T).nBodies;
@@ -117,24 +131,24 @@ __device__ __forceinline__ void project_streamed_acc(const Acc &acc, const TypeA
     if (XPBD && !iterZero) lam = lambdaGiven ? lambdaValue : __ldcg(a.lambda + i);  // m_lambda; zero at the first sweep of a substep (Constraints.cpp:1241-1242)
 
     if (T == PBD_DISTANCE) {
-        project_distance(p0, p1, s.s0, matv(a, 0, i));
+        project_distance(p0, p1, s.s0, matv(a, 0, i, matRow));
     } else if (T == PBD_DISTANCE_XPBD) {
-        project_distance_xpbd(p0, p1, s.s0, xpbd_alpha(matv(a, 0, i), dt), lam);
+        project_distance_xpbd(p0, p1, s.s0, xpbd_alpha(matv(a, 0, i, matRow), dt), lam);
     } else if (T == PBD_FEMTRIANGLE) {
-        const FemTriMaterial m = femtri_material(matv(a, 0, i), matv(a, 1, i), matv(a, 2, i), matv(a, 3, i), matv(a, 4, i));
+        const FemTriMaterial m = femtri_material(matv(a, 0, i, matRow), matv(a, 1, i, matRow), matv(a, 2, i, matRow), matv(a, 3, i, matRow), matv(a, 4, i, matRow));
         project_femtriangle(p0, p1, p2, s.s0, s.g0, m);
     } else if (T == PBD_STRAINTRIANGLE) {
-        project_straintriangle(p0, p1, p2, s.g0, matv(a, 0, i), matv(a, 1, i), matv(a, 2, i), matv(a, 3, i) != 0.0f, matv(a, 4, i) != 0.0f);
+        project_straintriangle(p0, p1, p2, s.g0, matv(a, 0, i, matRow), matv(a, 1, i, matRow), matv(a, 2, i, matRow), matv(a, 3, i, matRow) != 0.0f, matv(a, 4, i, matRow) != 0.0f);
     } else if (T == PBD_DIHEDRAL) {
-        project_dihedral(p0, p1, p2, p3, s.s0, matv(a, 0, i));
+        project_dihedral(p0, p1, p2, p3, s.s0, matv(a, 0, i, matRow));
     } else if (T == PBD_VOLUME) {
-        project_volume<false>(p0, p1, p2, p3, s.s0, matv(a, 0, i), 0.0f, lam);
+        project_volume<false>(p0, p1, p2, p3, s.s0, matv(a, 0, i, matRow), 0.0f, lam);
     } else if (T == PBD_VOLUME_XPBD) {
-        const float k = matv(a, 0, i);
+        const float k = matv(a, 0, i, matRow);
         project_volume<true>(p0, p1, p2, p3, s.s0, k, xpbd_alpha(k, dt), lam);
     } else if (T == PBD_ISOBENDING || T == PBD_ISOBENDING_XPBD) {
         constexpr bool X = (T == PBD_ISOBENDING_XPBD);
-        const float k = matv(a, 0, i);
+        const float k = matv(a, 0, i, matRow);
         const float alpha = X ? xpbd_alpha(k, dt) : 0.0f;
         if (VAR == 0 || (VAR < 0 && a.variant == 0)) project_isobending_rank1<X>(p0, p1, p2, p3, s.g0, k, alpha, lam);
         else project_isobending_fullq<X>(p0, p1, p2, p3, s.g0, __ldg(a.gv[1] + i), __ldg(a.gv[2] + i), __ldg(a.gv[3] + i), k, alpha, lam);
@@ -143,11 +157,11 @@ __device__ __forceinline__ void project_streamed_acc(const Acc &acc, const TypeA
         inv.m[0][0] = s.g0.x; inv.m[0][1] = s.g0.y; inv.m[0][2] = s.g0.z; inv.m[1][0] = s.g0.w;
         inv.m[1][1] = s.g1.x; inv.m[1][2] = s.g1.y; inv.m[2][0] = s.g1.z; inv.m[2][1] = s.g1.w;
         inv.m[2][2] = s.s0;
-        if (T == PBD_STRAINTET) project_straintet(p0, p1, p2, p3, inv, matv(a, 0, i), matv(a, 1, i), matv(a, 2, i) != 0.0f, matv(a, 3, i) != 0.0f);
-        else project_femtet<(T == PBD_FEMTET_XPBD)>(p0, p1, p2, p3, s.s1, inv, matv(a, 0, i), matv(a, 1, i), dt, lam);
+        if (T == PBD_STRAINTET) project_straintet(p0, p1, p2, p3, inv, matv(a, 0, i, matRow), matv(a, 1, i, matRow), matv(a, 2, i, matRow) != 0.0f, matv(a, 3, i, matRow) != 0.0f);
+        else project_femtet<(T == PBD_FEMTET_XPBD)>(p0, p1, p2, p3, s.s1, inv, matv(a, 0, i, matRow), matv(a, 1, i, matRow), dt, lam);
     } else if (T == PBD_SHAPEMATCHING) {
         project_shapematching(p0, p1, p2, p3, __ldg(a.gv[0] + i), __ldg(a.gv[1] + i), __ldg(a.gv[2] + i), __ldg(a.gv[3] + i), __ldg(a.gv[4] + i),
-                              __ldg(a.gv[5] + i), matv(a, 0, i));
+                              __ldg(a.gv[5] + i), matv(a, 0, i, matRow));
     }
 
     if (XPBD) __stcg(a.lambda + i, lam);
@@ -157,8 +171,8 @@ __device__ __forceinline__ void project_streamed_acc(const Acc &acc, const TypeA
 }
 
 template <int T, int VAR = -1>
-__device__ __forceinline__ void project_streamed(float4 *pos, const TypeArrays &a, unsigned i, const Streamed &s, float dt, bool iterZero) {
-    project_streamed_acc<T, GlobalAcc, VAR>(GlobalAcc{pos}, a, i, s, dt, iterZero);
+__device__ __forceinline__ void project_streamed(float4 *pos, const TypeArrays &a, unsigned i, const Streamed &s, float dt, bool iterZero, const MatRow &matRow) {
+    project_streamed_acc<T, GlobalAcc, VAR>(GlobalAcc{pos}, a, i, s, dt, iterZero, false, 0.0f, matRow);
 }
 
 // The one list of all constraint types: dispatch a statement on the runtime type, restricted to the types of MASK (T is a
@@ -182,7 +196,12 @@ constexpr int kMultiSegments = 4;
 
 // A replica batch (pbd_set_replicas) shares one constraint image; the BATCH instantiations of the projection kernels run replica
 // blockIdx.y, whose particles start at slot y x nPos and whose multipliers of segment k's type start at y x nLambda[k] (k_project: [0]).
-struct ReplicaStrides { unsigned nPos; unsigned nLambda[kMultiSegments]; };
+// mat[k]: segment k's type in replica 0's row of the batch's material table (rows of kMatRowFloats floats), or null: no replica has
+// material parameters of its own for that type.
+struct ReplicaStrides {
+    unsigned nPos; unsigned nLambda[kMultiSegments]; const float *mat[kMultiSegments];
+    __device__ __forceinline__ const float *mat_row(int k, unsigned rep) const { return mat[k] ? mat[k] + (size_t)rep * kMatRowFloats : nullptr; }
+};
 // the type's arrays with the multipliers of replica `rep`
 __device__ __forceinline__ TypeArrays replica_arrays(const TypeArrays &a, unsigned rep, unsigned nLambda) {
     TypeArrays r = a;
@@ -196,10 +215,11 @@ __global__ void __launch_bounds__(kProjectThreads) k_project(float4 *pos, TypeAr
     pdl_launch_dependents();
     const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= count) return;  // an exited thread counts as having passed the dependency
-    if (BATCH) { pos += (size_t)blockIdx.y * rs.nPos; a = replica_arrays(a, blockIdx.y, rs.nLambda[0]); }
+    MatRow matRow;
+    if (BATCH) { pos += (size_t)blockIdx.y * rs.nPos; a = replica_arrays(a, blockIdx.y, rs.nLambda[0]); matRow = load_mat_row<T>(rs.mat_row(0, blockIdx.y)); }
     const Streamed s = load_streamed<T>(a, first + i);
     pdl_wait_after(s.b.x ^ s.b.y, s.g0.x + s.g1.x + s.s0 + s.s1);
-    project_streamed<T, VAR>(pos, a, first + i, s, dt, iterZero != 0);
+    project_streamed<T, VAR>(pos, a, first + i, s, dt, iterZero != 0, matRow);
 }
 
 // ---- Jacobi comparison path (north_star: "a Jacobi path uses atomicAdd for comparison") -------------------------------------------
@@ -262,9 +282,11 @@ __global__ void __launch_bounds__(kProjectThreads) k_project_multi(float4 *pos, 
     if (BATCH) { pos += (size_t)blockIdx.y * rs.nPos; batchArrays = replica_arrays(m.arrays[s], blockIdx.y, rs.nLambda[s]); }
     const TypeArrays &a = BATCH ? batchArrays : m.arrays[s];
     PBD_FOR_TYPE(kMaskAll, m.type[s],
+        MatRow matRow;
+        if (BATCH) matRow = load_mat_row<T>(rs.mat_row(s, blockIdx.y));
         const Streamed st = load_streamed<T>(a, ci);
         pdl_wait_after(st.b.x ^ st.b.y, st.g0.x + st.g1.x + st.s0 + st.s1);
-        project_streamed<T>(pos, a, ci, st, dt, iterZero != 0);)
+        project_streamed<T>(pos, a, ci, st, dt, iterZero != 0, matRow);)
 }
 
 // The particle updates of a substep, shared by every execution mode and by the linear part of the rigid bodies, so that the modes
@@ -289,12 +311,18 @@ __device__ __forceinline__ void velocity_update(float4 &v, const float4 &x, cons
 }
 
 // lastX = oldX; oldX = x; if (mass != 0) { v += g h; x += v h }
+// BATCH: the n particles of replica blockIdx.y under that replica's row of `replicaG` (pbd_set_replica_gravity)
+template <bool BATCH>
 __global__ void __launch_bounds__(256) k_integrate(float4 *__restrict__ pos, float4 *__restrict__ vel,
                                                    float4 *__restrict__ oldp, float4 *__restrict__ lastp, unsigned n,
-                                                   float h, float gx, float gy, float gz) {
+                                                   float h, float gx, float gy, float gz, const float *__restrict__ replicaG) {
     pdl_launch_dependents();
-    const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
+    unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
+    if (BATCH) {
+        i += blockIdx.y * n;
+        gx = __ldg(replicaG + 3u * blockIdx.y); gy = __ldg(replicaG + 3u * blockIdx.y + 1u); gz = __ldg(replicaG + 3u * blockIdx.y + 2u);
+    }
     pdl_wait();
     float4 x = __ldcg(pos + i);
     __stcs(lastp + i, __ldcs(oldp + i));

@@ -76,6 +76,9 @@ struct ResidentArgs {
     // r x replicaStride, its multipliers of type t at r x lamCount[t]
     unsigned replicas, replicaStride;
     unsigned lamCount[PBD_NUM_TYPES];
+    // per-replica parameters of a batch (pbd_set_replica_materials / pbd_set_replica_gravity): rows of kMatRowFloats floats (the uniform
+    // material parameters of every type) and rows of 3 floats (null: gx, gy, gz for every replica)
+    const float *repMat, *repGravity;
 };
 
 // ---- cluster primitives --------------------------------------------------------------------------------------------------
@@ -224,12 +227,16 @@ __device__ __forceinline__ void prefetch_first(const ResidentArgs &A, const RunE
 
 // items [first, first + n) of a type's arrays: item tid, tid + stride, ... on this thread; with usePre the first one is in `pre`.
 // Software pipelined: the streamed operands (and multiplier) of the next item are in flight while the current one is projected.
+// A batch: `rows` is replica rep's material row, staged in shared memory (a global load at the head of every run would sit on the
+// critical path of the colour phase); a batch's resident kernels take every uniform from it.
 template <unsigned MASK, bool DEEP, bool BATCH, class Acc>
 __device__ __forceinline__ void run_items(const ResidentArgs &A, const Acc &acc, int type, unsigned first, unsigned n, bool iterZero, unsigned tid, unsigned stride,
-                                          bool usePre, const Prefetched &pre, unsigned rep) {
+                                          bool usePre, const Prefetched &pre, unsigned rep, const float *rows) {
     PBD_FOR_TYPE(MASK, type,
         TypeArrays batchArrays;  // a batch: the arrays with replica rep's multipliers
         if (BATCH) batchArrays = replica_arrays(A.types[T], rep, A.lamCount[T]);
+        MatRow matRow;
+        if (BATCH) { matRow = load_mat_row<T>(rows + mat_offset(T)); matRow.on = true; }
         const TypeArrays &ta = BATCH ? batchArrays : A.types[T];
         unsigned i = tid;
         if (DEEP && is_pipelined2<T>()) {
@@ -244,7 +251,7 @@ __device__ __forceinline__ void run_items(const ResidentArgs &A, const Acc &acc,
                     const unsigned j2 = i + 2u * stride;
                     const bool h2 = j2 < n;
                     if (h2) fetch(j2, s2, l2);
-                    project_streamed_acc<T, Acc, 0>(acc, ta, first + i, s0, A.h, iterZero, true, l0);
+                    project_streamed_acc<T, Acc, 0>(acc, ta, first + i, s0, A.h, iterZero, true, l0, matRow);
                     if (!h1) break;
                     s0 = s1; l0 = l1; s1 = s2; l1 = l2; h1 = h2; i += stride;
                 }
@@ -260,7 +267,7 @@ __device__ __forceinline__ void run_items(const ResidentArgs &A, const Acc &acc,
                 const bool more = j < n;
                 Streamed nxt; float lamN = 0.0f;
                 if (is_pipelined<T>() && more) { nxt = load_streamed<T>(ta, first + j); if (type_shape(T).xpbd && !iterZero) lamN = __ldcg(ta.lambda + first + j); }
-                project_streamed_acc<T, Acc, 0>(acc, ta, first + i, cur, A.h, iterZero, true, lam);  // variant 0 only: flatten refuses the full-Q bending layout in this mode
+                project_streamed_acc<T, Acc, 0>(acc, ta, first + i, cur, A.h, iterZero, true, lam, matRow);  // variant 0 only: flatten refuses the full-Q bending layout in this mode
                 if (!more) break;
                 if (!is_pipelined<T>()) { nxt = load_streamed<T>(ta, first + j); if (type_shape(T).xpbd && !iterZero) lamN = __ldcg(ta.lambda + first + j); }
                 cur = nxt; lam = lamN; i = j;
@@ -269,12 +276,12 @@ __device__ __forceinline__ void run_items(const ResidentArgs &A, const Acc &acc,
 }
 
 // semi-implicit Euler of one particle whose position is `x` (TimeStepController.cpp:112-118, TimeIntegration.cpp:7-19)
-__device__ __forceinline__ bool integrate_particle(const ResidentArgs &A, unsigned slot, float4 &x) {
+__device__ __forceinline__ bool integrate_particle(const ResidentArgs &A, unsigned slot, float4 &x, float gx, float gy, float gz) {
     __stcs(A.lastp + slot, __ldcs(A.oldp + slot));
     __stcs(A.oldp + slot, x);
     float4 v = __ldcs(A.vel + slot);
     if (v.w == 0.0f) return false;  // v.w carries the mass
-    semi_implicit_euler(x, v, A.h, A.gx, A.gy, A.gz);
+    semi_implicit_euler(x, v, A.h, gx, gy, gz);
     __stcs(A.vel + slot, v);
     return true;
 }
@@ -317,6 +324,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_step_resident(const __grid_const
     unsigned *sMask = reinterpret_cast<unsigned *>(runs + A.nBuckets);  // [1 + nColours]
     unsigned *sColour = sMask + 1 + A.nColours;                         // [nColours + 1]
     unsigned *sNbr = sColour + 1 + A.nColours;                          // [kMaxXNeighbours]
+    float *const sRep = reinterpret_cast<float *>(sNbr);                // a batch (no X items): the current replica's material row, then its gravity
     const unsigned cta = BATCH ? blockIdx.x % A.clusterSize : blockIdx.x;  // tile id = cluster * C + rank (1-D grid, cluster dimension C); a batch: the rank
     const unsigned tile0 = __ldg(A.tileStart + cta), nSm = __ldg(A.tileSmem + cta), nAll = __ldg(A.tileStart + cta + 1) - tile0;
     unsigned rep = BATCH ? blockIdx.x / A.clusterSize : 0u;  // the replica this cluster steps
@@ -324,8 +332,10 @@ __global__ void __launch_bounds__(THREADS, 1) k_step_resident(const __grid_const
     const unsigned nGl = nAll - nSm;
     // thread roles: the first RT threads run the shared-memory items; the last XT threads (whole warps) run the X items and the
     // global-homed particles and are the only ones that ever wait for another cluster
-    const unsigned XT = A.xThreads, RT = THREADS - XT;
-    const bool isX = threadIdx.x >= RT;
+    // (a batch tiles one replica into one cluster: it has no X items, and its instantiations no X path -- that is where the registers
+    // for the replica's parameters come from)
+    const unsigned XT = BATCH ? 0u : A.xThreads, RT = THREADS - XT;
+    const bool isX = !BATCH && threadIdx.x >= RT;
     const unsigned xtid = threadIdx.x - RT;
     constexpr bool single = SINGLE;  // one CTA per cluster: plain shared-memory accesses, __syncthreads between colours
     typedef typename std::conditional<SINGLE, LocalXAcc, ClusterAcc>::type XAcc;
@@ -358,7 +368,13 @@ __global__ void __launch_bounds__(THREADS, 1) k_step_resident(const __grid_const
         runs[bi] = r;
     }
     for (unsigned i = threadIdx.x; i < 1u + A.nColours; i += THREADS) { sMask[i] = __ldg(A.xMask + (size_t)cta * (1u + A.nColours) + i); sColour[i] = __ldg(A.colourStart + i); }
-    if (threadIdx.x < kMaxXNeighbours) sNbr[threadIdx.x] = __ldg(A.xNbr + (size_t)cta * kMaxXNeighbours + threadIdx.x);
+    if (!BATCH && threadIdx.x < kMaxXNeighbours) sNbr[threadIdx.x] = __ldg(A.xNbr + (size_t)cta * kMaxXNeighbours + threadIdx.x);
+    auto stage_replica = [&]() {  // once per replica, so that no colour phase starts with a load from global memory
+        if (A.repMat && threadIdx.x < (unsigned)kMatRowFloats) sRep[threadIdx.x] = __ldg(A.repMat + (size_t)rep * kMatRowFloats + threadIdx.x);
+        if (threadIdx.x < 3u)
+            sRep[kMatRowFloats + threadIdx.x] = A.repGravity ? __ldg(A.repGravity + 3u * rep + threadIdx.x) : (threadIdx.x == 0u ? A.gx : (threadIdx.x == 1u ? A.gy : A.gz));
+    };
+    if (BATCH) stage_replica();
     __syncthreads();
     for (unsigned c = threadIdx.x; c < A.nColours; c += THREADS) {  // rotations: bucket k of a colour starts where bucket k-1 ended
         unsigned accR = 0;
@@ -375,17 +391,18 @@ __global__ void __launch_bounds__(THREADS, 1) k_step_resident(const __grid_const
         for (unsigned sub = 0; sub < A.subSteps; sub++) {
             // ---- prologue: lastX = oldX; oldX = x; semi-implicit Euler
             stamp(0);
+            const float gx = BATCH ? sRep[kMatRowFloats] : A.gx, gy = BATCH ? sRep[kMatRowFloats + 1] : A.gy, gz = BATCH ? sRep[kMatRowFloats + 2] : A.gz;
             if (isX) {  // global-homed particles: what other clusters wait for
                 for (unsigned i = xtid; i < nGl; i += XT) {
                     float4 x = __ldcg(A.pos + t0 + nSm + i);
-                    if (integrate_particle(A, t0 + nSm + i, x)) __stcg(A.pos + t0 + nSm + i, x);
+                    if (integrate_particle(A, t0 + nSm + i, x, gx, gy, gz)) __stcg(A.pos + t0 + nSm + i, x);
                 }
                 if (nGl) x_publish();
                 stamp(1);
             } else {
                 for (unsigned i = threadIdx.x; i < nSm; i += RT) {
                     float4 x = tile[tile_swizzle(i)];
-                    if (integrate_particle(A, t0 + i, x)) tile[tile_swizzle(i)] = x;
+                    if (integrate_particle(A, t0 + i, x, gx, gy, gz)) tile[tile_swizzle(i)] = x;
                 }
                 if (A.rb.n && cta == 0 && threadIdx.x < A.rb.n) rb_integrate_body(A.rb, threadIdx.x, A.h, A.gx, A.gy, A.gz);
             }
@@ -419,7 +436,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_step_resident(const __grid_const
                             x_sync();
     #pragma unroll 1
                             for (unsigned bi = b0; bi < b1; bi++) run_items<MASK, false, BATCH>(A, accX, runs[bi].type, runs[bi].firstX, runs[bi].nX, iterZero, xtid, XT, pre.bucket == bi, pre,
-                                                                                         BATCH ? rep : 0u);
+                                                                                         BATCH ? rep : 0u, sRep);
                             x_publish();
                         }
                         stamp(1);
@@ -430,7 +447,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_step_resident(const __grid_const
                             const unsigned rot = runs[bi].rotR;  // 0 for the first bucket of a colour (the one prefetch_first serves)
                             run_items<MASK, SINGLE && MASK == kMaskClothXPBD, BATCH>(A, accR, runs[bi].type, runs[bi].firstR, runs[bi].nR, iterZero,
                                                                                threadIdx.x >= rot ? threadIdx.x - rot : threadIdx.x + RT - rot, RT, pre.bucket == bi, pre,
-                                                                               BATCH ? rep : 0u);
+                                                                               BATCH ? rep : 0u, sRep);
                         }
                     }
                     x_count(1u + c);
@@ -462,6 +479,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_step_resident(const __grid_const
         if (rep >= A.replicas) break;
         t0 = tile0 + rep * A.replicaStride;
         __syncthreads();  // the last replica's tile is stored before the next one overwrites it (no other CTA reads it after the last colour barrier)
+        stage_replica();
         for (unsigned i = threadIdx.x; i < nSm; i += THREADS) tile[tile_swizzle(i)] = __ldcg(A.pos + t0 + i);
         __syncthreads();
     }

@@ -4,7 +4,11 @@ stepped one after another by a K = 1 engine; the resident cluster size C swept o
 power limit read in the same run.  The four scenes run four different resident instantiations (cloth, FEM, cloth-XPBD and light type
 masks).
 
-    python tools/bench_batch.py [--out results.json] [--quick]
+    python tools/bench_batch.py [--out results.json] [--quick] [--replica-rows] [--sweep]
+
+--replica-rows measures every batch twice in a row: with the shared parameters, and with per-replica material rows and gravity
+(pbd_set_replica_materials / pbd_set_replica_gravity) equal to the shared values, so that the work is identical and the difference is what
+the tables cost.  --sweep adds one real sweep: 132 cfg1 replicas, each with its own Distance and IsometricBending stiffness.
 
 Batch times are device times (CUDA events on the engine's stream around `steps` steps, after warm-up steps).  The baseline is measured:
 a K = 1 engine in its faster mode (graph or resident) steps K replicas one after another -- K pbd_step calls, each replica's state
@@ -53,12 +57,27 @@ def model(name):
     types, bodies, params, _ = hm.constraints()
     off, ids = hm.groups()
     mass, _ = hm.masses()
-    m = dict(types=types, bodies=bodies, params=params, off=off, ids=ids, x0=hm.get("x0"), mass=mass, sub=sub, it=it)
+    m = dict(types=types, bodies=bodies, params=np.array(params, np.float32), off=off, ids=ids, x0=hm.get("x0"), mass=mass, sub=sub, it=it)
     hm.close()
     return m
 
 
-def engine(m, mode, k, clusters=None):
+def shared_rows(m, k):
+    """Per-replica rows that restate the shared parameters: {type: (k, nMat)} from each type's first constraint, and (k, 3) gravity."""
+    rows = {}
+    for t in range(_capi.NUM_TYPES):
+        sel = np.nonzero(np.asarray(m["types"]) == t)[0]
+        if len(sel) and _capi.num_materials(t):
+            cols = MAT_FIRST_COLUMN[t] + np.arange(_capi.num_materials(t))
+            rows[t] = np.repeat(np.asarray(m["params"], np.float32)[sel[0], cols][None], k, 0)
+    return rows, np.repeat(np.asarray([[0.0, -9.81, 0.0]], np.float32), k, 0)
+
+
+# include/pbd_b200.h: where a type's material parameters start in its parameter layout
+MAT_FIRST_COLUMN = {0: 1, 1: 1, 2: 1, 3: 0, 4: 0, 5: 5, 6: 4, 7: 1, 8: 1, 9: 10, 10: 10, 11: 9, 12: 0}
+
+
+def engine(m, mode, k, clusters=None, rows=None):
     if clusters:
         os.environ["PBD_B200_CLUSTERS"] = "1x%d" % clusters  # the planner's cluster-size override (read when the image is planned)
     else:
@@ -71,6 +90,10 @@ def engine(m, mode, k, clusters=None):
     eng.set_mode(mode)
     if k > 1:
         eng.set_replicas(k)
+    if rows is not None:
+        for t, mat in rows[0].items():
+            eng.set_replica_materials(t, mat)
+        eng.set_replica_gravity(rows[1])
     return eng
 
 
@@ -85,11 +108,11 @@ def timed(eng, warmup=3, min_s=0.4):
     return st.last_step_ms / steps, steps
 
 
-def measure(m, mode, k, clusters=None):
+def measure(m, mode, k, clusters=None, rows=None):
     t0 = time.time()
     eng = None
     try:
-        eng = engine(m, mode, k, clusters)
+        eng = engine(m, mode, k, clusters, rows)
         ms, steps = timed(eng)
         _, active = eng.get_mode()
     except _capi.PbdError as ex:
@@ -128,8 +151,10 @@ def main():
     ap.add_argument("--out", default=None, help="also write the results as JSON here")
     ap.add_argument("--quick", action="store_true", help="first two K of every sweep, no C sweep (a rehearsal)")
     ap.add_argument("--scenes", default=",".join(SCENES))
+    ap.add_argument("--replica-rows", action="store_true", help="every batch also with per-replica rows equal to the shared parameters")
+    ap.add_argument("--sweep", action="store_true", help="132 cfg1 replicas, each with its own stiffnesses")
     a = ap.parse_args()
-    res = {"card": card(), "rows": [], "c_sweep": []}
+    res = {"card": card(), "rows": [], "c_sweep": [], "replica_rows": [], "sweep": []}
     print("card: %s" % res["card"], flush=True)
     for name in a.scenes.split(","):
         m = model(name)
@@ -151,6 +176,25 @@ def main():
             fmt = lambda r: ("%9.3f ms %8.2e/s" % (r["ms"], r["proj_per_s"])) if "ms" in r else ("refused: " + r["error"][:60])
             print("  K=%5d  graph %s | resident %s | auto(%s) %s | one after another %9.3f ms" % (
                 k, fmt(row["graph"]), fmt(row["resident"]), row["auto"].get("active"), fmt(row["auto"]), row["baseline_ms"]), flush=True)
+        for k in (ks if a.replica_rows else []):
+            if k == 1:
+                continue
+            rows = shared_rows(m, k)
+            for label, md in (("graph", _capi.MODE_GRAPH), ("resident", _capi.MODE_RESIDENT)):
+                # shared, rows, shared, rows: the spread of each pair is next to the difference between them
+                ms = [measure(m, md, k, rows=rows if i & 1 else None).get("ms", float("nan")) for i in range(4)]
+                res["replica_rows"].append({"scene": name, "K": k, "mode": label, "shared_ms": ms[0::2], "rows_ms": ms[1::2]})
+                print("  rows K=%5d %-8s shared %.4f %.4f ms | per-replica rows %.4f %.4f ms" % (k, label, ms[0], ms[2], ms[1], ms[3]), flush=True)
+        if a.sweep and name == "cfg1":
+            k = 132
+            rows = shared_rows(m, k)
+            scale = np.linspace(0.1, 1.0, k, dtype=np.float32)[:, None]
+            swept = ({t: mat * scale for t, mat in rows[0].items()}, rows[1])
+            for label, md in (("graph", _capi.MODE_GRAPH), ("resident", _capi.MODE_RESIDENT)):
+                r = measure(m, md, k, rows=swept)
+                r.update({"scene": name, "K": k, "mode": label})
+                res["sweep"].append(r)
+                print("  stiffness sweep K=%5d %-8s %s" % (k, label, ("%.4f ms" % r["ms"]) if "ms" in r else r["error"][:80]), flush=True)
         if a.quick or name not in C_SWEEP:
             continue
         for k in C_SWEEP[name]:

@@ -192,8 +192,9 @@ int pbd_get_contacts(pbd_engine *e, pbd_contact *out, unsigned capacity, unsigne
  *  - Calls that MOVE state take the whole batch, replica after replica: pbd_set_attr / pbd_get_attr (K*n*3 floats), pbd_set_masses
  *    (K*n: each replica may pin other particles), pbd_step_host / pbd_step_host_async (K*n*3 per array), pbd_get_lambdas (K*count
  *    multipliers, `ids` count insertion ids).
- *  - Constraint parameters and gravity are shared unless pbd_set_replica_materials / pbd_set_replica_gravity (below) give every replica
- *    its own; the geometry of the rest state (rest lengths, Q, inverse rest matrices, areas, volumes) is always shared.
+ *  - Constraint parameters, gravity and the geometry of the rest state (rest lengths and angles, Q, inverse rest matrices, areas,
+ *    volumes, shape-matching rest shapes) are shared unless pbd_set_replica_materials / pbd_set_replica_gravity /
+ *    pbd_set_replica_rest_positions (below) give every replica its own.
  *  - pbd_get_stats: projections and bytes_per_step count every replica; num_particles and num_constraints are per replica.
  *  - K > 1 is refused with rigid bodies or joints, with colliders and in PBD_MODE_JACOBI.  PBD_MODE_RESIDENT runs one cluster of CTAs
  *    per replica and refuses a replica that does not fit one cluster; PBD_MODE_AUTO then runs the graph mode.
@@ -212,6 +213,25 @@ int pbd_get_replicas(pbd_engine *e, unsigned *K);
  * pbd_set_replica_gravity: replica r integrates with gravity g[3r..3r+3) instead of pbd_set_params' vector.  g = NULL: back to it. */
 int pbd_set_replica_materials(pbd_engine *e, int type, const float *mat /* K * pbd_num_materials(type) */);
 int pbd_set_replica_gravity(pbd_engine *e, const float *g /* K*3 */);
+/* Per-replica rest shape of a batch (K > 1, refused at K = 1 like the two calls above).  x0: K*n*3 floats, replica after replica.  Sets
+ * PBD_ATTR_X0 of every replica and gives every constraint of replica r the rest geometry that the constraint class's initConstraint derives
+ * from replica r's rest positions (ShapeMatching: and from replica r's inverse masses at the time of the call), computed on the GPU with the
+ * arithmetic of the host mirror's add*Constraint (double precision, rounded to float; Dihedral's acos may differ from the host's by an ulp).
+ * The geometry columns per type: Distance(+XPBD) restLength; Dihedral restAngle; IsometricBending(+XPBD) Q[16]; FEMTriangle area,
+ * invRestMat[4]; StrainTriangle invRestMat[4] (rest triangle in the x-z plane, as the reference takes it); Volume(+XPBD) restVolume;
+ * FEMTet(+XPBD) volume, invRestMat[9]; StrainTet invRestMat[9]; ShapeMatching restCm[3], x0[12], w[4], numClusters[4] (copied).
+ * Refused, with nothing changed, when some replica's rest positions make a constraint degenerate -- where the reference's initConstraint
+ * would return false, or an IsometricBending Q has no rank-one factor; the message names the first such replica and the constraint's
+ * insertion id.  x0 = NULL: back to the shared geometry (PBD_ATTR_X0 is left as it is).
+ * Lifetime: pbd_set_replicas and pbd_set_particles drop the override; adding constraints and changing the mode keep it (the image planned
+ * again derives its geometry from the rest positions this call was given; pbd_add_constraints refuses a constraint that some replica's
+ * kept rest shape makes degenerate, with the same message); a later pbd_set_attr(PBD_ATTR_X0) re-derives nothing, as
+ * editing x0 after initConstraint moves no constraint in the reference.  Calling again with new positions takes effect at the next step. */
+int pbd_set_replica_rest_positions(pbd_engine *e, const float *x0);
+/* The geometry replica r's constraints of `type` are stepped with: K * count * nGeo floats, nGeo = pbd_num_params(type) -
+ * pbd_num_materials(type) (the non-material columns of the type's parameter layout, in layout order), constraints in the order they were
+ * added.  Without an override: the shared geometry, repeated for every replica.  Refused for the joint types. */
+int pbd_get_replica_geometry(pbd_engine *e, int type, float *dst);
 
 int pbd_get_lambdas(pbd_engine *e, int type, float *dst, unsigned *ids); /* debug: per-type XPBD multipliers + insertion ids */
 int pbd_get_stats(pbd_engine *e, pbd_stats *out);

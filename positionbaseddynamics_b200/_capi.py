@@ -26,6 +26,7 @@ SYMBOLS = ["pbd_last_error", "pbd_device_count", "pbd_create", "pbd_destroy", "p
            "pbd_set_params", "pbd_set_mode", "pbd_get_mode", "pbd_step", "pbd_sync", "pbd_step_host", "pbd_step_host_async", "pbd_step_host_wait",
            "pbd_get_lambdas", "pbd_get_stats", "pbd_profile_step", "pbd_set_replicas", "pbd_get_replicas",
            "pbd_num_materials", "pbd_set_replica_materials", "pbd_set_replica_gravity",
+           "pbd_set_replica_rest_positions", "pbd_get_replica_geometry",
            "pbd_set_colliders", "pbd_set_contact_params", "pbd_record_contacts", "pbd_get_contacts"]
 
 
@@ -105,6 +106,8 @@ def lib():
         _lib.pbd_get_replicas.argtypes = [C.c_void_p, C.POINTER(C.c_uint)]
         _lib.pbd_set_replica_materials.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         _lib.pbd_set_replica_gravity.argtypes = [C.c_void_p, C.c_void_p]
+        _lib.pbd_set_replica_rest_positions.argtypes = [C.c_void_p, C.c_void_p]
+        _lib.pbd_get_replica_geometry.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
     return _lib
 
 
@@ -140,12 +143,18 @@ def num_materials(t):
     return lib().pbd_num_materials(t)
 
 
+def num_geometry(t):
+    """How many of type t's parameters are rest geometry (every column that is not a material parameter); a row of replica_geometry."""
+    return lib().pbd_num_params(t) - lib().pbd_num_materials(t)
+
+
 class Engine:
     """One engine <-> one CUDA device + one stream (pbd_create / pbd_destroy).
 
     A replica batch (set_replicas(K), K > 1) steps K independent copies of the model's state at once: the particle state calls then
     take and return (K, n, 3) / (K, n) arrays and lambdas() (K, count); at K = 1 the shapes are those of one scene.  The replicas share
-    the model's parameters unless set_replica_materials / set_replica_gravity give each its own."""
+    the model's parameters, gravity and rest geometry unless set_replica_materials / set_replica_gravity / set_replica_rest_positions
+    give each its own."""
 
     def __init__(self, device=0, stream=None):
         self._h = C.c_void_p()
@@ -217,6 +226,25 @@ class Engine:
             if g.shape != (self.K, 3):
                 raise ValueError("set_replica_gravity: wants a (%d, 3) array, got %s" % (self.K, g.shape))
         _ck(lib().pbd_set_replica_gravity(self._h, _ptr(g)))
+
+    def set_replica_rest_positions(self, x0):
+        """Replica r's constraints get the rest geometry derived from its own rest positions x0[r] ((K, n, 3) array), which also become
+        its x0; None: the shared geometry again.  K > 1 only; refused, with nothing changed, when a replica's rest shape makes a
+        constraint degenerate."""
+        if x0 is not None:
+            x0 = _f32(x0)
+            if x0.shape != (self.K, self.n, 3):
+                raise ValueError("set_replica_rest_positions: wants a (%d, %d, 3) array, got %s" % (self.K, self.n, x0.shape))
+        _ck(lib().pbd_set_replica_rest_positions(self._h, _ptr(x0)))
+
+    def replica_geometry(self, ctype):
+        """(K, count, num_geometry(ctype)): the geometry columns every replica's constraints of `ctype` are stepped with, constraints in
+        the order they were added."""
+        cnt = self.stats().constraints_per_type[ctype]
+        out = np.zeros((self.K, cnt, num_geometry(ctype)), dtype=np.float32)
+        if out.size:
+            _ck(lib().pbd_get_replica_geometry(self._h, int(ctype), _ptr(out)))
+        return out
 
     # rigid bodies ----------------------------------------------------------------------------------
     def set_rigid_bodies(self, mass, x, q, inertia, v=None, omega=None):

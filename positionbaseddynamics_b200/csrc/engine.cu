@@ -69,6 +69,10 @@ struct DevBuf {                   // one device allocation, freed with its owner
 
 struct DevType {
     DevBuf idx[3], gv[kMaxGeoV], gs[kMaxGeoS], mat[kMaxMat], lambda;
+    // replica batch: what its per-replica geometry is derived from (TypePlan::restBodies / restLocal, the insertion ids), the geometry
+    // arrays every replica's projections read while per-replica rest shapes are on (K x count; they keep their address while it stays
+    // on), and the arrays a derivation writes before it is known to be accepted
+    DevBuf restBodies, restLocal, restIds, repGv[kMaxGeoV], repGs[kMaxGeoS], newGv[kMaxGeoV], newGs[kMaxGeoS];
     PodVector<unsigned> order;    // position in the device arrays -> insertion id
     unsigned count = 0;
     TypeArrays arrays{};
@@ -89,6 +93,13 @@ struct pbd_engine {
     DevBuf repMat, repGravity;
     unsigned repMatMask = 0;
     bool repGravitySet = false;
+    // Per-replica rest shapes (pbd_set_replica_rest_positions): the rest positions the call was given, K x n float4 by host index with
+    // .w = the inverse mass at the time of the call; every image planned while repGeo is on derives its geometry from them again.
+    DevBuf restX, restNew, deriveFail, geoRows;
+    bool repGeo = false;
+    // the current image carries what a derivation reads (TypePlan::restBodies / restLocal): planned only while the override is on or
+    // being switched on, so that batches without it do not pay for them
+    bool restTables = false, restWanted = false;
     // rigid bodies coupled through joints (SURVEY.md 8f-1): float4 arrays X(xyz,invMass) Q(x,y,z,w) V(xyz,mass) W(omega) + history + inertia
     unsigned nRb = 0;
     DevBuf rbX, rbQ, rbV, rbW, rbOldX, rbLastX, rbOldQ, rbLastQ, rbI, rbIinv;
@@ -139,6 +150,18 @@ struct pbd_engine {
 };
 
 static int use(pbd_engine *e) { CK(cudaSetDevice(e->device)); return 0; }
+
+// per-replica rest shapes off (the caller drops the graph where the kernel arguments change)
+static void drop_replica_geometry(pbd_engine *e) {
+    e->repGeo = false;
+    e->restX.release(); e->restNew.release(); e->geoRows.release();
+    for (DevType &d : e->dev) {
+        for (DevBuf &b : d.repGv) b.release();
+        for (DevBuf &b : d.repGs) b.release();
+        for (DevBuf &b : d.newGv) b.release();
+        for (DevBuf &b : d.newGs) b.release();
+    }
+}
 
 extern "C" int pbd_device_count(int *count) {
     cudaError_t err = cudaGetDeviceCount(count);
@@ -288,6 +311,7 @@ extern "C" int pbd_set_particles(pbd_engine *e, unsigned n, const float *x, cons
     CKE(e->stage.alloc((size_t)e->K * n * 3 * sizeof(float)));
     CKE(e->massStage.alloc((size_t)e->K * n * sizeof(float)));
     drop_graph(e);  // buffers may have moved
+    drop_replica_geometry(e);  // every replica's state is redefined
     e->slot.resize(n); e->imageDirty = true;
     for (unsigned i = 0; i < n; i++) e->slot[i] = particle_slot(i, n);
     if (n == 0) return 0;
@@ -332,6 +356,7 @@ extern "C" int pbd_set_replicas(pbd_engine *e, unsigned K) {
         }
     e->K = K;
     e->repMat.release(); e->repGravity.release(); e->repMatMask = 0; e->repGravitySet = false;  // rows of the old K
+    drop_replica_geometry(e);
     for (DevBuf *b : {&e->pos, &e->vel, &e->oldp, &e->lastp, &e->pos0}) CKE(broadcast_replica0(e, *b));
     CKE(e->stage.alloc((size_t)K * e->n * 3 * sizeof(float)));
     CKE(e->massStage.alloc((size_t)K * e->n * sizeof(float)));
@@ -390,10 +415,16 @@ extern "C" int pbd_set_replica_gravity(pbd_engine *e, const float *g) {
 // What a batch's per-bucket kernels get for type t: where the replicas have parameters of their own, its place in replica 0's row of the
 // material table (without them the kernel arguments' uniforms do: reading the table for every launch cost the small shared-parameter
 // batches of DESIGN.md section 6 7-17 % in graph mode); and its arrays -- without the per-constraint material arrays in that case.
+// With per-replica rest shapes the geometry arrays are the K x count ones, replica r's at r x replica_geo (0: the shared image's).
 static const float *replica_mat(const pbd_engine *e, int t) { return ((e->repMatMask >> t) & 1u) ? (const float *)e->repMat.p + mat_offset(t) : nullptr; }
+static unsigned replica_geo(const pbd_engine *e, int t) { return e->repGeo ? e->dev[t].count : 0u; }
 static TypeArrays batch_arrays(const pbd_engine *e, int t) {
     TypeArrays a = e->dev[t].arrays;
     if ((e->repMatMask >> t) & 1u) for (int k = 0; k < kMaxMat; k++) a.mat[k] = nullptr;
+    if (e->repGeo) {
+        for (int k = 0; k < kMaxGeoV; k++) if (a.gv[k]) a.gv[k] = (const float4 *)e->dev[t].repGv[k].p;
+        for (int k = 0; k < kMaxGeoS; k++) if (a.gs[k]) a.gs[k] = (const float *)e->dev[t].repGs[k].p;
+    }
     return a;
 }
 
@@ -498,6 +529,30 @@ extern "C" int pbd_clear_constraints(pbd_engine *e) {
     return 0;
 }
 
+// With per-replica rest shapes on, a constraint added later gets its geometry from every replica's kept rest positions when the image is
+// planned again.  Checked here, on the host and with the arithmetic of the device derivation (rest_geometry.cuh), so that a constraint some
+// replica's rest shape makes degenerate is refused by this call instead of failing the next step.
+static int check_added_geometry(pbd_engine *e, int type, unsigned count, const unsigned *bodies, const unsigned *ids) {
+    if (!e->repGeo || !count || !e->n || type >= PBD_BALLJOINT) return 0;
+    CKE(use(e));
+    std::vector<float4> rest((size_t)e->K * e->n);
+    CK(cudaStreamSynchronize(e->stream));
+    CK(cudaMemcpy(rest.data(), e->restX.p, rest.size() * sizeof(float4), cudaMemcpyDeviceToHost));
+    const int nb = type_shape(type).nBodies;
+    for (unsigned r = 0; r < e->K; r++)
+        for (unsigned i = 0; i < count; i++) {
+            float4 x[4];
+            for (int k = 0; k < nb; k++) x[k] = rest[(size_t)r * e->n + bodies[(size_t)i * nb + k]];
+            float geo[kMaxGeoColumns], Kp[4];
+            bool ok = rest_geometry(type, x, geo);
+            if (type == PBD_ISOBENDING || type == PBD_ISOBENDING_XPBD) ok = factor_rank1(geo, Kp) && ok;
+            if (!ok)
+                return fail("pbd_add_constraints: the rest positions of replica %u make constraint %u (type %d) degenerate; the reference's "
+                            "initConstraint would refuse it, and the replicas of a batch share one constraint set", r, ids ? ids[i] : e->numConstraints + i, type);
+        }
+    return 0;
+}
+
 extern "C" int pbd_add_constraints(pbd_engine *e, int type, unsigned count, const unsigned *bodies, const float *params, const unsigned *ids) {
     if (!e) return fail("null engine");
     if (type < 0 || type >= PBD_NUM_TYPES) return fail("pbd_add_constraints: unknown constraint type %d", type);
@@ -508,6 +563,7 @@ extern "C" int pbd_add_constraints(pbd_engine *e, int type, unsigned count, cons
         if (is_rb_body(type, (int)(badAt % s.nBodies))) return fail("pbd_add_constraints: rigid-body index %u out of range (%u bodies; call pbd_set_rigid_bodies first)", bodies[badAt], e->nRb);
         return fail("pbd_add_constraints: particle index %u out of range (n=%u)", bodies[badAt], e->n);
     }
+    CKE(check_added_geometry(e, type, count, bodies, ids));
     TypeStore &h = e->host[type];
     {
         const size_t b0 = h.ids.size();
@@ -813,6 +869,9 @@ static int upload_type(pbd_engine *e, int t, pbd_b200::TypePlan &p) {
         if (!p.mat[k].empty()) { CKE(upload_vec(d.mat[k], p.mat[k], e->stream)); a.mat[k] = (const float *)d.mat[k].p; }
     }
     a.variant = p.variant;
+    if (!p.restBodies.empty()) {
+        CKE(upload_vec(d.restBodies, p.restBodies, e->stream)); CKE(upload_vec(d.restLocal, p.restLocal, e->stream)); CKE(upload_vec(d.restIds, d.order, e->stream));
+    }
     if (e->K > 1 && type_shape(t).nMat && !((e->repMatMask >> t) & 1u)) CKE(write_replica_materials(e, t, a.matU, 0));  // the shared parameters, for every replica
     if (t == PBD_BALLJOINT || t == PBD_RB_PARTICLE_BALLJOINT) {
         a.rbX = (float4 *)e->rbX.p; a.rbQ = (float4 *)e->rbQ.p; a.rbIinv = (const float4 *)e->rbIinv.p;
@@ -822,6 +881,70 @@ static int upload_type(pbd_engine *e, int t, pbd_b200::TypePlan &p) {
         CKE(d.lambda.alloc((size_t)e->K * cnt * sizeof(float) + 16));
         CK(cudaMemsetAsync(d.lambda.p, 0, (size_t)e->K * cnt * sizeof(float), e->stream));
         a.lambda = (float *)d.lambda.p;
+    }
+    return 0;
+}
+
+// ---- per-replica rest shapes of a batch (pbd_set_replica_rest_positions) ------------------------------------------------------
+template <class F> static int with_geometry_type(int type, F &&f) {
+    PBD_FOR_TYPE(kMaskAll & ~(type_bit(PBD_BALLJOINT) | type_bit(PBD_RB_PARTICLE_BALLJOINT)), type, return f(std::integral_constant<int, T>{});)
+    return fail("constraint type %d has no rest geometry of particles", type);
+}
+// Every particle type's geometry of the K replicas derived from `rest` (K x n float4 by host index, k_pack_rest) on the device: packed into
+// the image's layout in newGv / newGs, or with `rows` type rowsType's parameter-layout geometry rows (K x count x num_geo).  *bad: the
+// first constraint refused (replica << 32 | insertion id), ~0 for none.
+static int derive_geometry(pbd_engine *e, const float4 *rest, int rowsType, float *rows, unsigned long long *bad) {
+    CKE(e->deriveFail.alloc(sizeof(unsigned long long)));
+    CK(cudaMemsetAsync(e->deriveFail.p, 0xff, sizeof(unsigned long long), e->stream));
+    for (int t = 0; t < PBD_BALLJOINT; t++) {
+        DevType &d = e->dev[t];
+        if (!d.count || (rows && t != rowsType)) continue;
+        DeriveArgs a{};
+        a.rest = rest; a.n = e->n; a.count = d.count;
+        a.bodies = (const unsigned *)d.restBodies.p; a.ids = (const unsigned *)d.restIds.p; a.local = (const unsigned *)d.restLocal.p;
+        a.clusters = d.arrays.gv[5]; a.variant = d.arrays.variant; a.rows = rows; a.fail = (unsigned long long *)e->deriveFail.p;
+        if (!rows) {
+            const size_t cnt = (size_t)e->K * d.count;  // + 16 like the other streamed arrays: the L2 prefetch of a run rounds its end up
+            for (int k = 0; k < kMaxGeoV; k++) if (d.arrays.gv[k]) { CKE(d.newGv[k].alloc(cnt * sizeof(float4) + 16)); a.gv[k] = (float4 *)d.newGv[k].p; }
+            for (int k = 0; k < kMaxGeoS; k++) if (d.arrays.gs[k]) { CKE(d.newGs[k].alloc(cnt * sizeof(float) + 16)); a.gs[k] = (float *)d.newGs[k].p; }
+        }
+        CKE(with_geometry_type(t, [&](auto T) -> int {
+            k_derive_geometry<decltype(T)::value><<<dim3(nblk(d.count, 128), e->K), 128, 0, e->stream>>>(a);
+            CK(cudaGetLastError());
+            return 0;
+        }));
+    }
+    CK(cudaMemcpyAsync(bad, e->deriveFail.p, sizeof(*bad), cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+    return 0;
+}
+// The geometry derived from `rest` becomes what the projections read -- only when no constraint refuses it: otherwise the error names the
+// first replica and constraint, and nothing has changed.  It is copied into the live arrays in stream order, so that they keep their
+// address and a captured graph reads the new geometry at its next launch.
+static int apply_replica_geometry(pbd_engine *e, const float4 *rest, const char *what) {
+    unsigned long long bad = ~0ull;
+    CKE(derive_geometry(e, rest, -1, nullptr, &bad));
+    if (bad != ~0ull) {
+        const unsigned rep = (unsigned)(bad >> 32), id = (unsigned)bad;
+        int type = -1;
+        for (int t = 0; t < PBD_NUM_TYPES && type < 0; t++)
+            for (unsigned id2 : e->host[t].ids) if (id2 == id) { type = t; break; }
+        return fail("%s: the rest positions of replica %u make constraint %u (type %d) degenerate; the reference's initConstraint would refuse "
+                    "it, and the replicas of a batch share one constraint set", what, rep, id, type);
+    }
+    for (int t = 0; t < PBD_BALLJOINT; t++) {
+        DevType &d = e->dev[t];
+        const size_t cnt = (size_t)e->K * d.count;
+        if (!cnt) continue;
+        for (int k = 0; k < kMaxGeoV; k++)
+            if (d.arrays.gv[k]) { CKE(d.repGv[k].alloc(cnt * sizeof(float4) + 16)); CK(cudaMemcpyAsync(d.repGv[k].p, d.newGv[k].p, cnt * sizeof(float4), cudaMemcpyDeviceToDevice, e->stream)); }
+        for (int k = 0; k < kMaxGeoS; k++)
+            if (d.arrays.gs[k]) { CKE(d.repGs[k].alloc(cnt * sizeof(float) + 16)); CK(cudaMemcpyAsync(d.repGs[k].p, d.newGs[k].p, cnt * sizeof(float), cudaMemcpyDeviceToDevice, e->stream)); }
+    }
+    CK(cudaStreamSynchronize(e->stream));
+    for (DevType &d : e->dev) {  // the scratch arrays are as large as the live ones: not kept between derivations
+        for (DevBuf &b : d.newGv) b.release();
+        for (DevBuf &b : d.newGs) b.release();
     }
     return 0;
 }
@@ -844,6 +967,7 @@ static int flatten(pbd_engine *e) {
     }
     lap("colouring + rest positions");
     pbd_b200::PlanInput in{e->host, e->numConstraints, e->n, e->nRb, &e->groupOff, &e->groupIds, e->mode, x0.data(), 0u, 0u, e->smCount, nullptr, e->autoNoResident, e->K};
+    in.restTables = e->K > 1 && (e->repGeo || e->restWanted);
     if (const char *g = getenv("PBD_B200_CLUSTERS")) {  // development knob "GxC"
         unsigned gg = 0, cc = 0;
         if (sscanf(g, "%ux%u", &gg, &cc) == 2 && gg >= 1 && cc >= 1 && cc <= (unsigned)kMaxClusterCtas && (cc & (cc - 1)) == 0) { in.forcedG = gg; in.forcedC = cc; }
@@ -874,10 +998,68 @@ static int flatten(pbd_engine *e) {
     }
     CK(cudaStreamSynchronize(e->stream));
     lap("relayout + upload");
+    if (e->repGeo) CKE(apply_replica_geometry(e, (const float4 *)e->restX.p, "pbd_set_replica_rest_positions (image planned again)"));  // the new image's geometry, from the rest positions the override was given
+
     e->stats.num_constraints = e->numConstraints;  // per replica, like num_particles
     e->stats.num_groups = (unsigned)e->groupOff.size() - 1;
     e->stats.num_buckets = (unsigned)e->buckets.size();
+    e->restTables = in.restTables;
     e->imageDirty = false;
+    return 0;
+}
+
+// The rest positions go to a buffer of their own (and PBD_ATTR_X0) only after the geometry derived from them has been accepted; the engine
+// keeps them, so that an image planned again (constraints added, another mode) derives its geometry from them too.  Only switching the
+// override on or off changes kernel arguments and so drops the graph.
+extern "C" int pbd_set_replica_rest_positions(pbd_engine *e, const float *x0) {
+    CKE(replica_params_refusal(e, "pbd_set_replica_rest_positions"));
+    CKE(use(e));
+    if (!x0) {
+        if (e->repGeo) { drop_replica_geometry(e); drop_graph(e); }
+        return 0;
+    }
+    if (!e->restTables) e->imageDirty = true;  // planned again with the bodies the derivation reads
+    e->restWanted = true;
+    const int planned = flatten(e);  // the device order of the constraints the geometry is derived for
+    e->restWanted = false;
+    CKE(planned);
+    for (int t = 0; t < PBD_BALLJOINT; t++)  // the resident kernel addresses replica r's geometry as i + r count in 32 bits
+        if ((unsigned long long)e->K * e->dev[t].count >= (1ull << 32))
+            return fail("pbd_set_replica_rest_positions: %u replicas of %u constraints of type %d exceed 2^32 geometry rows", e->K, e->dev[t].count, t);
+    if (e->n) {
+        CKE(e->restNew.alloc((size_t)e->K * e->n * sizeof(float4)));
+        CK(cudaMemcpyAsync(e->stage.p, x0, (size_t)e->K * e->n * 3 * sizeof(float), cudaMemcpyHostToDevice, e->stream));
+        k_pack_rest<<<replica_grid(e, e->K), 256, 0, e->stream>>>((const float *)e->stage.p, (const float4 *)e->pos.p, (float4 *)e->restNew.p, e->n, (const unsigned *)e->dSlot.p);
+        CK(cudaGetLastError());
+        CKE(apply_replica_geometry(e, (const float4 *)e->restNew.p, "pbd_set_replica_rest_positions"));
+        std::swap(e->restX.p, e->restNew.p); std::swap(e->restX.bytes, e->restNew.bytes);
+        CKE(upload3(e, x0, (float4 *)e->pos0.p, 1, e->K));  // PBD_ATTR_X0 of every replica
+        CK(cudaStreamSynchronize(e->stream));
+    }
+    if (!e->repGeo) { e->repGeo = true; drop_graph(e); }
+    return 0;
+}
+
+extern "C" int pbd_get_replica_geometry(pbd_engine *e, int type, float *dst) {
+    if (!e || !dst) return fail("pbd_get_replica_geometry: null argument");
+    if (type < 0 || type >= PBD_BALLJOINT) return fail("pbd_get_replica_geometry: constraint type %d has no rest geometry of particles", type);
+    CKE(use(e)); CKE(flatten(e));
+    const unsigned cnt = e->dev[type].count;
+    const int nGeo = num_geo(type), g0 = geo_first(type), np = type_shape(type).nParams;
+    if (cnt == 0) return 0;
+    const size_t one = (size_t)cnt * nGeo;
+    if (!e->repGeo) {  // the shared geometry, for every replica
+        const TypeStore &h = e->host[type];
+        for (size_t i = 0; i < cnt; i++)
+            for (int j = 0; j < nGeo; j++) dst[i * nGeo + j] = h.params[i * np + g0 + j];
+        for (unsigned r = 1; r < e->K; r++) memcpy(dst + r * one, dst, one * sizeof(float));
+        return 0;
+    }
+    CKE(e->geoRows.alloc((size_t)e->K * one * sizeof(float)));
+    unsigned long long bad = ~0ull;
+    CKE(derive_geometry(e, (const float4 *)e->restX.p, type, (float *)e->geoRows.p, &bad));
+    CK(cudaMemcpy(dst, e->geoRows.p, (size_t)e->K * one * sizeof(float), cudaMemcpyDeviceToHost));
+    e->geoRows.release();
     return 0;
 }
 
@@ -920,7 +1102,7 @@ template <class F> static int with_project_type(int type, int variant, F &&f) {
 static int launch_bucket(pbd_engine *e, const Bucket &b, float h, int iterZero, cudaStream_t s, bool pdl) {
     const TypeArrays a = batch_arrays(e, b.type);
     const unsigned block = project_block(e, b.count * e->K);
-    const ReplicaStrides rs{e->n, {e->dev[b.type].count}, {replica_mat(e, b.type)}};
+    const ReplicaStrides rs{e->n, {e->dev[b.type].count}, {replica_mat(e, b.type)}, {replica_geo(e, b.type)}};
     return with_project_type(b.type, a.variant, [&](auto T, auto V) -> int {
         constexpr int TT = decltype(T)::value, VAR = decltype(V)::value;
         if (e->K > 1) CK(launch_step_kernel(k_project<TT, VAR, true>, dim3(nblk(b.count, block), e->K), block, s, pdl, (float4 *)e->pos.p, a, b.first, b.count, h, iterZero, rs));
@@ -964,7 +1146,7 @@ static int launch_colour(pbd_engine *e, size_t b0, size_t b1, float h, int iterZ
     for (size_t c0 = b0; c0 < b1; c0 += kMultiSegments) {
         const size_t c1 = std::min(b1, c0 + (size_t)kMultiSegments);
         MultiArgs m{};
-        ReplicaStrides rs{e->n, {}, {}};
+        ReplicaStrides rs{e->n, {}, {}, {}};
         m.nSeg = (int)(c1 - c0);
         unsigned blocks = 0, total = 0;
         for (size_t i = c0; i < c1; i++) total += e->buckets[i].count;
@@ -974,7 +1156,7 @@ static int launch_colour(pbd_engine *e, size_t b0, size_t b1, float h, int iterZ
             const int k = (int)(i - c0);
             m.type[k] = b.type; m.first[k] = b.first; m.count[k] = b.count; m.blockStart[k] = blocks;
             m.arrays[k] = batch_arrays(e, b.type);
-            rs.nLambda[k] = e->dev[b.type].count; rs.mat[k] = replica_mat(e, b.type);
+            rs.nLambda[k] = e->dev[b.type].count; rs.mat[k] = replica_mat(e, b.type); rs.nGeo[k] = replica_geo(e, b.type);
             blocks += nblk(b.count, block);
         }
         for (int k = m.nSeg; k <= kMultiSegments; k++) m.blockStart[k] = blocks;
@@ -1056,7 +1238,7 @@ static int enqueue_step_resident(pbd_engine *e, cudaStream_t s, unsigned long lo
     ra.xFlags = (unsigned long long *)e->dXFlags.p;
     ra.xLaunch = (++e->xLaunch) << 32;  // above every flag value of the earlier launches, whatever subSteps / maxIter they ran with
     ra.rb = rb_state(e);
-    for (int t = 0; t < PBD_NUM_TYPES; t++) { ra.types[t] = batch_arrays(e, t); ra.lamCount[t] = e->dev[t].count; }
+    for (int t = 0; t < PBD_NUM_TYPES; t++) { ra.types[t] = batch_arrays(e, t); ra.lamCount[t] = e->dev[t].count; ra.geoCount[t] = replica_geo(e, t); }
     ra.replicas = e->res.replicas; ra.replicaStride = e->n;
     ra.repMat = (const float *)e->repMat.p; ra.repGravity = e->repGravitySet ? (const float *)e->repGravity.p : nullptr;
     *launches = 1;

@@ -3,6 +3,7 @@
 // The image planner (image_plan.h): a constraint list + the reference's colour groups -> (colour,type) buckets of SoA arrays; for the
 // resident mode (resident.cuh) also the tiling of the particles, the per-tile runs and the X-neighbour tables.  No CUDA API call.
 #include "image_plan.h"
+#include "../rest_geometry.cuh"
 #include <algorithm>
 #include <cmath>
 #include <cstdarg>
@@ -78,24 +79,6 @@ static std::string validate_bodies(const PlanInput &in) {
                    isRb ? "rigid body" : "particle", h.bodies[badAt], isRb ? in.nRb : in.n);
     }
     return "";
-}
-
-// Q (row-major 4x4, solver order) = -Kp Kp^T ?  Returns true and Kp when the rank-one negative-semidefinite form of
-// init_IsometricBendingConstraint (PositionBasedDynamics.cpp:169-180) reproduces Q to fp32 accuracy.
-static bool factor_rank1(const float *Q, float Kp[4]) {
-    int piv = 0; float best = 0.0f, maxAbs = 0.0f;
-    for (int j = 0; j < 4; j++) { if (-Q[5 * j] > best) { best = -Q[5 * j]; piv = j; } }
-    for (int i = 0; i < 16; i++) maxAbs = std::max(maxAbs, std::fabs(Q[i]));
-    if (maxAbs == 0.0f) { Kp[0] = Kp[1] = Kp[2] = Kp[3] = 0.0f; return true; }
-    if (!(best > 0.0f)) return false;
-    const double kp = std::sqrt((double)best);
-    double K[4];
-    for (int k = 0; k < 4; k++) K[k] = -(double)Q[4 * piv + k] / kp;
-    for (int j = 0; j < 4; j++)
-        for (int k = 0; k < 4; k++)
-            if (std::fabs((double)Q[4 * j + k] + K[j] * K[k]) > 1e-5 * (double)maxAbs) return false;
-    for (int k = 0; k < 4; k++) Kp[k] = (float)K[k];
-    return true;
 }
 
 // The planner's state: its input, the plan being built, and for the resident mode where every host particle lives.
@@ -452,30 +435,7 @@ static std::string check_colouring(const Ctx &c, const std::vector<unsigned> (&o
     return "";
 }
 
-// Parameter columns (include/pbd_b200.h) of a type's SoA arrays: float4 geometry array k = columns gv[k][0..3], scalar geometry
-// array k = column gs[k], material slot k = column mat[k]; -1 = zero-filled component, or no such array / slot.
-struct PackColumns { signed char gv[kMaxGeoV][4], gs[kMaxGeoS], mat[kMaxMat]; };
-static PackColumns pack_columns(int t) {
-    PackColumns p;
-    memset(&p, -1, sizeof(p));
-    auto gv = [&](int k, int c0, int c1, int c2, int c3) { p.gv[k][0] = c0; p.gv[k][1] = c1; p.gv[k][2] = c2; p.gv[k][3] = c3; };
-    auto mat = [&](int first, int count) { for (int k = 0; k < count; k++) p.mat[k] = first + k; };
-    switch (t) {
-    case PBD_DISTANCE: case PBD_DISTANCE_XPBD: case PBD_DIHEDRAL: case PBD_VOLUME: case PBD_VOLUME_XPBD: p.gs[0] = 0; mat(1, 1); break;
-    case PBD_ISOBENDING: case PBD_ISOBENDING_XPBD: for (int r = 0; r < 4; r++) gv(r, 1 + 4 * r, 2 + 4 * r, 3 + 4 * r, 4 + 4 * r); mat(0, 1); break;  // full Q (see pack_type)
-    case PBD_FEMTRIANGLE: p.gs[0] = 0; gv(0, 1, 2, 3, 4); mat(5, 5); break;
-    case PBD_STRAINTRIANGLE: gv(0, 0, 1, 2, 3); mat(4, 5); break;
-    case PBD_FEMTET: case PBD_FEMTET_XPBD: gv(0, 1, 2, 3, 4); gv(1, 5, 6, 7, 8); p.gs[0] = 9; p.gs[1] = 0; mat(10, 2); break;
-    case PBD_STRAINTET: gv(0, 0, 1, 2, 3); gv(1, 4, 5, 6, 7); p.gs[0] = 8; mat(9, 4); break;
-    // local connectors (jointInfo columns 0 [and 1]); the global columns are recomputed per solve
-    case PBD_BALLJOINT: gv(0, 0, 1, 2, -1); gv(1, 3, 4, 5, -1); break;
-    case PBD_RB_PARTICLE_BALLJOINT: gv(0, 0, 1, 2, -1); break;
-    // restCm | x0[0..3] packed in 3 float4 | w | numClusters ; stiffness is the material slot
-    case PBD_SHAPEMATCHING: gv(0, 1, 2, 3, -1); for (int k = 1; k < 6; k++) gv(k, 4 * k, 4 * k + 1, 4 * k + 2, 4 * k + 3); mat(0, 1); break;
-    }
-    return p;
-}
-
+// (pack_columns and factor_rank1: rest_geometry.cuh, shared with the device derivation of a batch's per-replica geometry)
 // the SoA arrays of type t in device order (order: device position -> local host index)
 static std::string pack_type(Ctx &c, int t, const std::vector<unsigned> &order, Lap &lap) {
     TypePlan &d = c.out.types[t];
@@ -487,6 +447,14 @@ static std::string pack_type(Ctx &c, int t, const std::vector<unsigned> &order, 
     if (cnt == 0) return "";
     #pragma omp parallel for schedule(static) num_threads(host_threads())
     for (long long i = 0; i < (long long)cnt; i++) d.order[i] = h.ids[order[i]];
+    if (c.in.restTables && t < PBD_BALLJOINT) {  // what a batch's per-replica geometry is derived from (k_derive_geometry)
+        d.restBodies.resize((size_t)cnt * s.nBodies); d.restLocal.resize(cnt);
+        #pragma omp parallel for schedule(static) num_threads(host_threads())
+        for (long long i = 0; i < (long long)cnt; i++) {
+            d.restLocal[i] = order[i];
+            for (int k = 0; k < s.nBodies; k++) d.restBodies[(size_t)i * s.nBodies + k] = h.bodies[(size_t)order[i] * s.nBodies + k];
+        }
+    }
     auto P = [&](unsigned i, int k) { return h.params[(size_t)order[i] * s.nParams + k]; };
     auto B = [&](unsigned i, int k) {
         const unsigned raw = h.bodies[(size_t)order[i] * s.nBodies + k];

@@ -53,6 +53,7 @@ struct PlanInput {
     ClusterQuery maxClusters;                      // resident: what the device keeps co-resident
     bool residentRefused = false;                  // PBD_MODE_AUTO: the resident mode refused this model before
     unsigned replicas = 1;                         // replica batch: every replica runs this one image (n, the constraints: one replica)
+    bool restTables = false;                       // replica batch with per-replica rest shapes: also TypePlan::restBodies / restLocal
 };
 
 // One constraint type's arrays in device order (the host side of pbdk::TypeArrays).
@@ -63,6 +64,9 @@ struct TypePlan {
     PodVector<float> gs[pbdk::kMaxGeoS], mat[pbdk::kMaxMat];  // mat[k] empty: every constraint has matU[k]
     float matU[pbdk::kMaxMat] = {};
     int variant = 0;
+    // PlanInput::restTables: device position -> host particle indices of the bodies, and -> position among the type's constraints in the
+    // order they were added (the per-replica geometry of pbd_set_replica_rest_positions is derived from these)
+    PodVector<unsigned> restBodies, restLocal;
 };
 
 // Launch shape of a resident image: G clusters x C CTAs (one tile each), block size and type mask of the instantiation, smem per CTA.

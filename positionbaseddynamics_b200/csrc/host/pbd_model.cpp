@@ -1,5 +1,6 @@
 // positionbaseddynamics_b200/csrc/host/pbd_model.cpp -- see pbd_model.h.
 #include "pbd_model.h"
+#include "../rest_geometry.cuh"
 #include <algorithm>
 #include <cstdlib>
 #include <omp.h>
@@ -9,8 +10,6 @@
 #include <unordered_map>
 
 namespace pbd_b200 {
-
-static const double kEps = 1e-6;  // PositionBasedDynamics.cpp:7 (absolute, not scale aware -- kept literally)
 
 // ============================================================================================================
 // ParticleData
@@ -408,24 +407,16 @@ void SimulationModel::initConstraintGroups() {
 // ------------------------------------------------------------------------------------------------------------
 // constraint factories.  Rest-state data is evaluated in double from the fp32 rest positions and rounded once.
 // ------------------------------------------------------------------------------------------------------------
-struct D3 { double x, y, z; };
-static inline D3 d3(const Vector3r &v) { return {v[0], v[1], v[2]}; }
-static inline D3 operator-(D3 a, D3 b) { return {a.x - b.x, a.y - b.y, a.z - b.z}; }
-static inline D3 operator-(D3 a) { return {-a.x, -a.y, -a.z}; }
-static inline double dotd(D3 a, D3 b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
-static inline D3 crossd(D3 a, D3 b) { return {a.y * b.z - a.z * b.y, a.z * b.x - a.x * b.z, a.x * b.y - a.y * b.x}; }
-static inline double normd(D3 a) { return std::sqrt(dotd(a, a)); }
-static inline D3 normalized(D3 a) { const double z = dotd(a, a); if (z > 0) { const double s = 1.0 / std::sqrt(z); return {a.x * s, a.y * s, a.z * s}; } return a; }
-static inline double cotTheta(D3 v, D3 w) { return dotd(v, w) / normd(crossd(v, w)); }  // MathFunctions.cpp:391-396
-
-static bool invert3(const double m[9], double inv[9]) {
-    const double det = m[0] * (m[4] * m[8] - m[5] * m[7]) - m[1] * (m[3] * m[8] - m[5] * m[6]) + m[2] * (m[3] * m[7] - m[4] * m[6]);
-    if (!(std::fabs(det) > kEps)) return false;
-    const double id = 1.0 / det;
-    inv[0] = (m[4] * m[8] - m[5] * m[7]) * id; inv[1] = (m[2] * m[7] - m[1] * m[8]) * id; inv[2] = (m[1] * m[5] - m[2] * m[4]) * id;
-    inv[3] = (m[5] * m[6] - m[3] * m[8]) * id; inv[4] = (m[0] * m[8] - m[2] * m[6]) * id; inv[5] = (m[2] * m[3] - m[0] * m[5]) * id;
-    inv[6] = (m[3] * m[7] - m[4] * m[6]) * id; inv[7] = (m[1] * m[6] - m[0] * m[7]) * id; inv[8] = (m[0] * m[4] - m[1] * m[3]) * id;
-    return true;
+// The geometry columns of a constraint of `type` on `bodies` from the rest positions (and, ShapeMatching, the inverse masses) into its
+// parameter row, and whether the constraint class's initConstraint accepts them: rest_geometry.cuh, the description the device derivation
+// of a batch's per-replica rest shapes (pbd_set_replica_rest_positions) shares.
+static bool restParams(const ParticleData &pd, int type, const unsigned int *bodies, Real *params) {
+    float4 x[4];
+    for (int k = 0; k < pbdk::type_shape(type).nBodies; k++) {
+        const Vector3r &p = pd.m_x0[bodies[k]];
+        x[k] = make_float4(p[0], p[1], p[2], pd.m_invMasses[bodies[k]]);
+    }
+    return pbdk::rest_geometry(type, x, params + pbdk::geo_first(type));
 }
 
 // the batch builders know how many constraints they are about to add: one allocation instead of repeated vector growth
@@ -476,159 +467,90 @@ static void push_bulk(TypeStore &s, PodVector<ConstraintRef> &order, int type, s
 
 // DistanceConstraint::initConstraint (Constraints.cpp:1166-1181): rest length from x0
 bool SimulationModel::addDistanceConstraint(unsigned int p1, unsigned int p2, Real stiffness) {
-    const ParticleData &pd = m_particles;
     const unsigned int b[2] = {p1, p2};
-    const Real p[2] = {(Real)normd(d3(pd.m_x0[p2]) - d3(pd.m_x0[p1])), stiffness};
-    return pushConstraint(PBD_DISTANCE, b, p, true);
+    Real p[2] = {0, stiffness};
+    return pushConstraint(PBD_DISTANCE, b, p, restParams(m_particles, PBD_DISTANCE, b, p));
 }
 bool SimulationModel::addDistanceConstraint_XPBD(unsigned int p1, unsigned int p2, Real stiffness) {  // Constraints.cpp:1211-1227
-    const ParticleData &pd = m_particles;
     const unsigned int b[2] = {p1, p2};
-    const Real p[2] = {(Real)normd(d3(pd.m_x0[p2]) - d3(pd.m_x0[p1])), stiffness};
-    return pushConstraint(PBD_DISTANCE_XPBD, b, p, true);
+    Real p[2] = {0, stiffness};
+    return pushConstraint(PBD_DISTANCE_XPBD, b, p, restParams(m_particles, PBD_DISTANCE_XPBD, b, p));
 }
 
 // DihedralConstraint::initConstraint (Constraints.cpp:1264-1300)
 bool SimulationModel::addDihedralConstraint(unsigned int i1, unsigned int i2, unsigned int i3, unsigned int i4, Real stiffness) {
-    const ParticleData &pd = m_particles;
-    const D3 p0 = d3(pd.m_x0[i1]), p1 = d3(pd.m_x0[i2]), p2 = d3(pd.m_x0[i3]), p3 = d3(pd.m_x0[i4]);
     const unsigned int b[4] = {i1, i2, i3, i4};
     Real p[2] = {0, stiffness};
-    if (normd(p3 - p2) < 1e-6) return pushConstraint(PBD_DIHEDRAL, b, p, false);
-    const D3 n1 = normalized(crossd(p2 - p0, p3 - p0)), n2 = normalized(crossd(p3 - p1, p2 - p1));
-    double dot = dotd(n1, n2);
-    dot = std::fmin(std::fmax(dot, -1.0), 1.0);
-    p[0] = (Real)std::acos(dot);
-    return pushConstraint(PBD_DIHEDRAL, b, p, true);
+    return pushConstraint(PBD_DIHEDRAL, b, p, restParams(m_particles, PBD_DIHEDRAL, b, p));
 }
 
 // init_IsometricBendingConstraint (PositionBasedDynamics.cpp:145-183): Q = coef K K^T over x = {p2, p3, p0, p1}
-static void isoBendingQ(const ParticleData &pd, unsigned int i1, unsigned int i2, unsigned int i3, unsigned int i4, Real *Q) {
-    const D3 x[4] = {d3(pd.m_x0[i3]), d3(pd.m_x0[i4]), d3(pd.m_x0[i1]), d3(pd.m_x0[i2])};
-    const D3 e0 = x[1] - x[0], e1 = x[2] - x[0], e2 = x[3] - x[0], e3 = x[2] - x[1], e4 = x[3] - x[1];
-    const double c01 = cotTheta(e0, e1), c02 = cotTheta(e0, e2), c03 = cotTheta(-e0, e3), c04 = cotTheta(-e0, e4);
-    const double A0 = 0.5 * normd(crossd(e0, e1)), A1 = 0.5 * normd(crossd(e0, e2));
-    const double coef = -3.0 / (2.0 * (A0 + A1));
-    const double K[4] = {c03 + c04, c01 + c02, -c01 - c03, -c02 - c04};
-    for (int j = 0; j < 4; j++) for (int k = 0; k < 4; k++) Q[4 * j + k] = (Real)(K[j] * coef * K[k]);
-}
 bool SimulationModel::addIsometricBendingConstraint(unsigned int i1, unsigned int i2, unsigned int i3, unsigned int i4, Real stiffness) {
     const unsigned int b[4] = {i1, i2, i3, i4};
     Real p[17]; p[0] = stiffness;
-    isoBendingQ(m_particles, i1, i2, i3, i4, p + 1);
-    return pushConstraint(PBD_ISOBENDING, b, p, true);
+    return pushConstraint(PBD_ISOBENDING, b, p, restParams(m_particles, PBD_ISOBENDING, b, p));
 }
 bool SimulationModel::addIsometricBendingConstraint_XPBD(unsigned int i1, unsigned int i2, unsigned int i3, unsigned int i4, Real stiffness) {
     const unsigned int b[4] = {i1, i2, i3, i4};
     Real p[17]; p[0] = stiffness;
-    isoBendingQ(m_particles, i1, i2, i3, i4, p + 1);
-    return pushConstraint(PBD_ISOBENDING_XPBD, b, p, true);
+    return pushConstraint(PBD_ISOBENDING_XPBD, b, p, restParams(m_particles, PBD_ISOBENDING_XPBD, b, p));
 }
 
 // init_FEMTriangleConstraint (PositionBasedDynamics.cpp:808-841)
 bool SimulationModel::addFEMTriangleConstraint(unsigned int i1, unsigned int i2, unsigned int i3, Real xx, Real yy, Real xy, Real nuxy, Real nuyx) {
-    const ParticleData &pd = m_particles;
-    const D3 p0 = d3(pd.m_x0[i1]), p1 = d3(pd.m_x0[i2]), p2 = d3(pd.m_x0[i3]);
-    const D3 normal0 = crossd(p1 - p0, p2 - p0);
-    const double area = normd(normal0) * 0.5;
-    const D3 axis1 = normalized(p1 - p0), axis2 = normalized(crossd(normal0, axis1));
-    const double q[3][2] = {{dotd(p0, axis2), dotd(p0, axis1)}, {dotd(p1, axis2), dotd(p1, axis1)}, {dotd(p2, axis2), dotd(p2, axis1)}};
-    const double P00 = q[0][0] - q[2][0], P10 = q[0][1] - q[2][1], P01 = q[1][0] - q[2][0], P11 = q[1][1] - q[2][1];
-    const double det = P00 * P11 - P01 * P10;
     const unsigned int b[3] = {i1, i2, i3};
-    Real p[10] = {(Real)area, 0, 0, 0, 0, xx, yy, xy, nuxy, nuyx};
-    if (!(std::fabs(det) > kEps)) return pushConstraint(PBD_FEMTRIANGLE, b, p, false);
-    p[1] = (Real)(P11 / det); p[2] = (Real)(-P01 / det); p[3] = (Real)(-P10 / det); p[4] = (Real)(P00 / det);
-    return pushConstraint(PBD_FEMTRIANGLE, b, p, true);
+    Real p[10] = {0, 0, 0, 0, 0, xx, yy, xy, nuxy, nuyx};
+    return pushConstraint(PBD_FEMTRIANGLE, b, p, restParams(m_particles, PBD_FEMTRIANGLE, b, p));
 }
 
 // StrainTriangleConstraint::initConstraint (Constraints.cpp:1544-1569: the rest triangle is taken in the x-z plane)
 // + init_StrainTriangleConstraint (PositionBasedDynamics.cpp:562-581)
 bool SimulationModel::addStrainTriangleConstraint(unsigned int i1, unsigned int i2, unsigned int i3, Real xx, Real yy, Real xy, bool normalizeStretch, bool normalizeShear) {
-    const ParticleData &pd = m_particles;
-    const Vector3r &x1 = pd.m_x0[i1], &x2 = pd.m_x0[i2], &x3 = pd.m_x0[i3];
-    const double a = (double)x2[0] - x1[0], bb = (double)x3[0] - x1[0], c = (double)x2[2] - x1[2], d = (double)x3[2] - x1[2];
-    const double det = a * d - bb * c;
     const unsigned int b[3] = {i1, i2, i3};
     Real p[9] = {0, 0, 0, 0, xx, yy, xy, normalizeStretch ? 1.0f : 0.0f, normalizeShear ? 1.0f : 0.0f};
-    if (std::fabs(det) < kEps) return pushConstraint(PBD_STRAINTRIANGLE, b, p, false);
-    const double s = 1.0 / det;
-    p[0] = (Real)(d * s); p[1] = (Real)(-bb * s); p[2] = (Real)(-c * s); p[3] = (Real)(a * s);
-    return pushConstraint(PBD_STRAINTRIANGLE, b, p, true);
+    return pushConstraint(PBD_STRAINTRIANGLE, b, p, restParams(m_particles, PBD_STRAINTRIANGLE, b, p));
 }
 
-static double restVolume(const ParticleData &pd, unsigned int i1, unsigned int i2, unsigned int i3, unsigned int i4) {
-    const D3 p0 = d3(pd.m_x0[i1]), p1 = d3(pd.m_x0[i2]), p2 = d3(pd.m_x0[i3]), p3 = d3(pd.m_x0[i4]);
-    return std::fabs((1.0 / 6.0) * dotd(p3 - p0, crossd(p2 - p0, p1 - p0)));
-}
 bool SimulationModel::addVolumeConstraint(unsigned int i1, unsigned int i2, unsigned int i3, unsigned int i4, Real stiffness) {  // Constraints.cpp:1617-1635
     const unsigned int b[4] = {i1, i2, i3, i4};
-    const Real p[2] = {(Real)restVolume(m_particles, i1, i2, i3, i4), stiffness};
-    return pushConstraint(PBD_VOLUME, b, p, true);
+    Real p[2] = {0, stiffness};
+    return pushConstraint(PBD_VOLUME, b, p, restParams(m_particles, PBD_VOLUME, b, p));
 }
 bool SimulationModel::addVolumeConstraint_XPBD(unsigned int i1, unsigned int i2, unsigned int i3, unsigned int i4, Real stiffness) {  // Constraints.cpp:1683-1702
     const unsigned int b[4] = {i1, i2, i3, i4};
-    const Real p[2] = {(Real)restVolume(m_particles, i1, i2, i3, i4), stiffness};
-    return pushConstraint(PBD_VOLUME_XPBD, b, p, true);
+    Real p[2] = {0, stiffness};
+    return pushConstraint(PBD_VOLUME_XPBD, b, p, restParams(m_particles, PBD_VOLUME_XPBD, b, p));
 }
 
 // init_FEMTetraConstraint (PositionBasedDynamics.cpp:933-955): columns p0-p3, p1-p3, p2-p3
-static bool femTetRest(const ParticleData &pd, unsigned int i1, unsigned int i2, unsigned int i3, unsigned int i4, Real *p) {
-    const D3 p0 = d3(pd.m_x0[i1]), p1 = d3(pd.m_x0[i2]), p2 = d3(pd.m_x0[i3]), p3 = d3(pd.m_x0[i4]);
-    p[0] = (Real)std::fabs((1.0 / 6.0) * dotd(p3 - p0, crossd(p2 - p0, p1 - p0)));
-    const D3 a = p0 - p3, b = p1 - p3, c = p2 - p3;
-    const double m[9] = {a.x, b.x, c.x, a.y, b.y, c.y, a.z, b.z, c.z};
-    double inv[9];
-    if (!invert3(m, inv)) { for (int k = 0; k < 9; k++) p[1 + k] = 0; return false; }
-    for (int k = 0; k < 9; k++) p[1 + k] = (Real)inv[k];
-    return true;
-}
 bool SimulationModel::addFEMTetConstraint(unsigned int i1, unsigned int i2, unsigned int i3, unsigned int i4, Real stiffness, Real poissonRatio) {
     const unsigned int b[4] = {i1, i2, i3, i4};
-    Real p[12]; const bool ok = femTetRest(m_particles, i1, i2, i3, i4, p); p[10] = stiffness; p[11] = poissonRatio;
-    return pushConstraint(PBD_FEMTET, b, p, ok);
+    Real p[12]; p[10] = stiffness; p[11] = poissonRatio;
+    return pushConstraint(PBD_FEMTET, b, p, restParams(m_particles, PBD_FEMTET, b, p));
 }
 bool SimulationModel::addFEMTetConstraint_XPBD(unsigned int i1, unsigned int i2, unsigned int i3, unsigned int i4, Real stiffness, Real poissonRatio) {
     const unsigned int b[4] = {i1, i2, i3, i4};
-    Real p[12]; const bool ok = femTetRest(m_particles, i1, i2, i3, i4, p); p[10] = stiffness; p[11] = poissonRatio;
-    return pushConstraint(PBD_FEMTET_XPBD, b, p, ok);
+    Real p[12]; p[10] = stiffness; p[11] = poissonRatio;
+    return pushConstraint(PBD_FEMTET_XPBD, b, p, restParams(m_particles, PBD_FEMTET_XPBD, b, p));
 }
 
 // init_StrainTetraConstraint (PositionBasedDynamics.cpp:691-710): columns p1-p0, p2-p0, p3-p0
 bool SimulationModel::addStrainTetConstraint(unsigned int i1, unsigned int i2, unsigned int i3, unsigned int i4, Real stretchStiffness, Real shearStiffness,
                                              bool normalizeStretch, bool normalizeShear) {
-    const ParticleData &pd = m_particles;
-    const D3 p0 = d3(pd.m_x0[i1]), a = d3(pd.m_x0[i2]) - p0, bb = d3(pd.m_x0[i3]) - p0, c = d3(pd.m_x0[i4]) - p0;
-    const double m[9] = {a.x, bb.x, c.x, a.y, bb.y, c.y, a.z, bb.z, c.z};
-    double inv[9];
-    const bool ok = invert3(m, inv);
     const unsigned int b[4] = {i1, i2, i3, i4};
     Real p[13];
-    for (int k = 0; k < 9; k++) p[k] = ok ? (Real)inv[k] : 0.0f;
     p[9] = stretchStiffness; p[10] = shearStiffness; p[11] = normalizeStretch ? 1.0f : 0.0f; p[12] = normalizeShear ? 1.0f : 0.0f;
-    return pushConstraint(PBD_STRAINTET, b, p, ok);
+    return pushConstraint(PBD_STRAINTET, b, p, restParams(m_particles, PBD_STRAINTET, b, p));
 }
 
 // ShapeMatchingConstraint::initConstraint (Constraints.cpp:1985-2001) + init_ShapeMatchingConstraint
 // (PositionBasedDynamics.cpp:479-497): rest positions and inverse masses are frozen into the constraint.
 bool SimulationModel::addShapeMatchingConstraint(unsigned int numberOfParticles, const unsigned int particleIndices[], const unsigned int numClusters[], Real stiffness) {
     if (numberOfParticles != 4) return false;  // the accelerated path covers the tetrahedral clusters of addSolidConstraints
-    const ParticleData &pd = m_particles;
     Real p[24];
     p[0] = stiffness;
-    double cm[3] = {0, 0, 0}, wsum = 0.0;
-    for (int i = 0; i < 4; i++) {
-        const Vector3r &x0 = pd.m_x0[particleIndices[i]];
-        const Real w = pd.m_invMasses[particleIndices[i]];
-        const double wi = 1.0 / ((double)w + kEps);
-        for (int k = 0; k < 3; k++) { cm[k] += x0[k] * wi; p[4 + 3 * i + k] = x0[k]; }
-        wsum += wi;
-        p[16 + i] = w;
-        p[20 + i] = (Real)numClusters[i];
-    }
-    const bool ok = wsum != 0.0;
-    for (int k = 0; k < 3; k++) p[1 + k] = ok ? (Real)(cm[k] / wsum) : 0.0f;
-    return pushConstraint(PBD_SHAPEMATCHING, particleIndices, p, ok);
+    for (int i = 0; i < 4; i++) p[20 + i] = (Real)numClusters[i];
+    return pushConstraint(PBD_SHAPEMATCHING, particleIndices, p, restParams(m_particles, PBD_SHAPEMATCHING, particleIndices, p));
 }
 
 // SimulationModel::addClothConstraints (SimulationModel.cpp:1125-1184)
@@ -642,7 +564,7 @@ void SimulationModel::addClothConstraints(const TriangleModel *tm, unsigned int 
         const ParticleData &pd = m_particles;
         push_bulk(m_store[type], m_order, type, edges.size(), [](size_t) { return true; }, [&](size_t i, unsigned int *b, Real *p) {
             b[0] = edges[i].m_vert[0] + offset; b[1] = edges[i].m_vert[1] + offset;
-            p[0] = (Real)normd(d3(pd.m_x0[b[1]]) - d3(pd.m_x0[b[0]])); p[1] = distanceStiffness;  // DistanceConstraint::initConstraint
+            restParams(pd, type, b, p); p[1] = distanceStiffness;  // DistanceConstraint::initConstraint
         });
         if (!edges.empty()) { m_groupsInitialized = false; m_generation++; }
     } else if (clothMethod == 2 || clothMethod == 3) {
@@ -684,7 +606,7 @@ void SimulationModel::addBendingConstraints(const TriangleModel *tm, unsigned in
                       opposite(edges[i], point1, point2);
                       b[0] = point1 + offset; b[1] = point2 + offset; b[2] = edges[i].m_vert[0] + offset; b[3] = edges[i].m_vert[1] + offset;
                       p[0] = stiffness;
-                      isoBendingQ(pd, b[0], b[1], b[2], b[3], p + 1);
+                      restParams(pd, type, b, p);
                   });
         if (m_order.size() != before) { m_groupsInitialized = false; m_generation++; }
         return;

@@ -11,6 +11,7 @@
 //   k_step_resident (resident.cuh): the whole step in one launch, positions resident in the shared memory of thread-block clusters
 #pragma once
 #include "device_image.h"
+#include "rest_geometry.cuh"
 #include "solvers.cuh"
 
 namespace pbdk {
@@ -62,9 +63,11 @@ struct Streamed {
     float s0, s1;   // scalar geometry (rest length / angle / volume / area / invRestMat(2,2))
 };
 
-// the indices, the first nStreamV float4 and all nGeoS scalar geometry arrays of type T (type_shape)
+// the indices, the first nStreamV float4 and all nGeoS scalar geometry arrays of type T (type_shape); the geometry of constraint i at
+// i + geoOff (a batch's replica with a rest shape of its own, resident.cuh: an offset costs the register-tight resident kernels less than
+// moved array pointers)
 template <int T>
-__device__ __forceinline__ Streamed load_streamed(const TypeArrays &a, unsigned i) {
+__device__ __forceinline__ Streamed load_streamed(const TypeArrays &a, unsigned i, unsigned geoOff = 0u) {
     constexpr TypeShape sh = type_shape(T);
     static_assert(sh.nStreamV <= 2 && sh.nGeoS <= 2, "Streamed holds two float4 and two scalar geometry values");
     Streamed s;
@@ -77,10 +80,10 @@ __device__ __forceinline__ Streamed load_streamed(const TypeArrays &a, unsigned 
     } else {
         s.b = __ldg(a.idx4 + i);
     }
-    if (sh.nStreamV >= 1) s.g0 = __ldg(a.gv[0] + i);
-    if (sh.nStreamV >= 2) s.g1 = __ldg(a.gv[1] + i);
-    if (sh.nGeoS >= 1) s.s0 = __ldg(a.gs[0] + i);
-    if (sh.nGeoS >= 2) s.s1 = __ldg(a.gs[1] + i);
+    if (sh.nStreamV >= 1) s.g0 = __ldg(a.gv[0] + (i + geoOff));
+    if (sh.nStreamV >= 2) s.g1 = __ldg(a.gv[1] + (i + geoOff));
+    if (sh.nGeoS >= 1) s.s0 = __ldg(a.gs[0] + (i + geoOff));
+    if (sh.nGeoS >= 2) s.s1 = __ldg(a.gs[1] + (i + geoOff));
     return s;
 }
 
@@ -119,7 +122,8 @@ __device__ __forceinline__ void project_joint(const Acc &acc, const TypeArrays &
 // VAR: compile-time layout variant of the type (IsometricBending: 0 = rank-1 Kp, 1 = full Q), -1 = read a.variant at run time
 template <int T, class Acc, int VAR = -1>
 __device__ __forceinline__ void project_streamed_acc(const Acc &acc, const TypeArrays &a, unsigned i, const Streamed &s, float dt,
-                                                     bool iterZero, bool lambdaGiven = false, float lambdaValue = 0.0f, const MatRow &matRow = MatRow{}) {
+                                                     bool iterZero, bool lambdaGiven = false, float lambdaValue = 0.0f, const MatRow &matRow = MatRow{},
+                                                     unsigned geoOff = 0u) {
     if (T == PBD_BALLJOINT || T == PBD_RB_PARTICLE_BALLJOINT) { project_joint<T>(acc, a, s); return; }
     constexpr bool XPBD = type_shape(T).xpbd;
     constexpr int NB = type_shape(T).nBodies;
@@ -151,7 +155,7 @@ __device__ __forceinline__ void project_streamed_acc(const Acc &acc, const TypeA
         const float k = matv(a, 0, i, matRow);
         const float alpha = X ? xpbd_alpha(k, dt) : 0.0f;
         if (VAR == 0 || (VAR < 0 && a.variant == 0)) project_isobending_rank1<X>(p0, p1, p2, p3, s.g0, k, alpha, lam);
-        else project_isobending_fullq<X>(p0, p1, p2, p3, s.g0, __ldg(a.gv[1] + i), __ldg(a.gv[2] + i), __ldg(a.gv[3] + i), k, alpha, lam);
+        else project_isobending_fullq<X>(p0, p1, p2, p3, s.g0, __ldg(a.gv[1] + (i + geoOff)), __ldg(a.gv[2] + (i + geoOff)), __ldg(a.gv[3] + (i + geoOff)), k, alpha, lam);
     } else if (T == PBD_FEMTET || T == PBD_FEMTET_XPBD || T == PBD_STRAINTET) {
         M3 inv;
         inv.m[0][0] = s.g0.x; inv.m[0][1] = s.g0.y; inv.m[0][2] = s.g0.z; inv.m[1][0] = s.g0.w;
@@ -160,8 +164,9 @@ __device__ __forceinline__ void project_streamed_acc(const Acc &acc, const TypeA
         if (T == PBD_STRAINTET) project_straintet(p0, p1, p2, p3, inv, matv(a, 0, i, matRow), matv(a, 1, i, matRow), matv(a, 2, i, matRow) != 0.0f, matv(a, 3, i, matRow) != 0.0f);
         else project_femtet<(T == PBD_FEMTET_XPBD)>(p0, p1, p2, p3, s.s1, inv, matv(a, 0, i, matRow), matv(a, 1, i, matRow), dt, lam);
     } else if (T == PBD_SHAPEMATCHING) {
-        project_shapematching(p0, p1, p2, p3, __ldg(a.gv[0] + i), __ldg(a.gv[1] + i), __ldg(a.gv[2] + i), __ldg(a.gv[3] + i), __ldg(a.gv[4] + i),
-                              __ldg(a.gv[5] + i), matv(a, 0, i, matRow));
+        const unsigned g = i + geoOff;
+        project_shapematching(p0, p1, p2, p3, __ldg(a.gv[0] + g), __ldg(a.gv[1] + g), __ldg(a.gv[2] + g), __ldg(a.gv[3] + g), __ldg(a.gv[4] + g),
+                              __ldg(a.gv[5] + g), matv(a, 0, i, matRow));
     }
 
     if (XPBD) __stcg(a.lambda + i, lam);
@@ -197,18 +202,25 @@ constexpr int kMultiSegments = 4;
 // A replica batch (pbd_set_replicas) shares one constraint image; the BATCH instantiations of the projection kernels run replica
 // blockIdx.y, whose particles start at slot y x nPos and whose multipliers of segment k's type start at y x nLambda[k] (k_project: [0]).
 // mat[k]: segment k's type in replica 0's row of the batch's material table (rows of kMatRowFloats floats), or null: no replica has
-// material parameters of its own for that type.
+// material parameters of its own for that type.  nGeo[k]: with per-replica rest shapes (pbd_set_replica_rest_positions) the geometry
+// arrays hold every replica's, replica y's at y x nGeo[k]; 0: one geometry shared by all.
 struct ReplicaStrides {
-    unsigned nPos; unsigned nLambda[kMultiSegments]; const float *mat[kMultiSegments];
+    unsigned nPos; unsigned nLambda[kMultiSegments]; const float *mat[kMultiSegments]; unsigned nGeo[kMultiSegments];
     __device__ __forceinline__ const float *mat_row(int k, unsigned rep) const { return mat[k] ? mat[k] + (size_t)rep * kMatRowFloats : nullptr; }
 };
-// the type's arrays with the multipliers of replica `rep`
-__device__ __forceinline__ TypeArrays replica_arrays(const TypeArrays &a, unsigned rep, unsigned nLambda) {
+// the type's arrays with the multipliers and the geometry of replica `rep`
+__device__ __forceinline__ TypeArrays replica_arrays(const TypeArrays &a, unsigned rep, unsigned nLambda, unsigned nGeo) {
     TypeArrays r = a;
     if (r.lambda) r.lambda += (size_t)rep * nLambda;
+    if (nGeo) {
+        const size_t o = (size_t)rep * nGeo;
+#pragma unroll
+        for (int k = 0; k < kMaxGeoV; k++) if (r.gv[k]) r.gv[k] += o;
+#pragma unroll
+        for (int k = 0; k < kMaxGeoS; k++) if (r.gs[k]) r.gs[k] += o;
+    }
     return r;
 }
-
 template <int T, int VAR, bool BATCH>
 __global__ void __launch_bounds__(kProjectThreads) k_project(float4 *pos, TypeArrays a, unsigned first,
                                                              unsigned count, float dt, int iterZero, ReplicaStrides rs) {
@@ -216,7 +228,7 @@ __global__ void __launch_bounds__(kProjectThreads) k_project(float4 *pos, TypeAr
     const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= count) return;  // an exited thread counts as having passed the dependency
     MatRow matRow;
-    if (BATCH) { pos += (size_t)blockIdx.y * rs.nPos; a = replica_arrays(a, blockIdx.y, rs.nLambda[0]); matRow = load_mat_row<T>(rs.mat_row(0, blockIdx.y)); }
+    if (BATCH) { pos += (size_t)blockIdx.y * rs.nPos; a = replica_arrays(a, blockIdx.y, rs.nLambda[0], rs.nGeo[0]); matRow = load_mat_row<T>(rs.mat_row(0, blockIdx.y)); }
     const Streamed s = load_streamed<T>(a, first + i);
     pdl_wait_after(s.b.x ^ s.b.y, s.g0.x + s.g1.x + s.s0 + s.s1);
     project_streamed<T, VAR>(pos, a, first + i, s, dt, iterZero != 0, matRow);
@@ -279,7 +291,7 @@ __global__ void __launch_bounds__(kProjectThreads) k_project_multi(float4 *pos, 
     if (i >= m.count[s]) return;
     const unsigned ci = m.first[s] + i;
     TypeArrays batchArrays;
-    if (BATCH) { pos += (size_t)blockIdx.y * rs.nPos; batchArrays = replica_arrays(m.arrays[s], blockIdx.y, rs.nLambda[s]); }
+    if (BATCH) { pos += (size_t)blockIdx.y * rs.nPos; batchArrays = replica_arrays(m.arrays[s], blockIdx.y, rs.nLambda[s], rs.nGeo[s]); }
     const TypeArrays &a = BATCH ? batchArrays : m.arrays[s];
     PBD_FOR_TYPE(kMaskAll, m.type[s],
         MatRow matRow;
@@ -430,6 +442,67 @@ __global__ void k_unpack3(const float4 *__restrict__ src, float *__restrict__ ds
     const float4 s = src[slot[i]];
     dst[3 * i] = s.x; dst[3 * i + 1] = s.y; dst[3 * i + 2] = s.z;
 }
+// the rest positions of pbd_set_replica_rest_positions: host AoS-3 of K replicas -> K x n float4 BY HOST INDEX, .w = the replica's
+// inverse mass now (ShapeMatching freezes it into the constraint)
+__global__ void k_pack_rest(const float *__restrict__ src, const float4 *__restrict__ pos, float4 *__restrict__ dst, unsigned n, const unsigned *__restrict__ slot) {
+    const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    src += (size_t)blockIdx.y * 3 * n; pos += (size_t)blockIdx.y * n; dst += (size_t)blockIdx.y * n;
+    dst[i] = make_float4(src[3 * i], src[3 * i + 1], src[3 * i + 2], pos[slot[i]].w);
+}
+
+// k_derive_geometry: the rest geometry of a batch's replicas (pbd_set_replica_rest_positions), one thread per (constraint i of type T in
+// device order, replica blockIdx.y), with the arithmetic of the host mirror (rest_geometry.cuh).  Replica r's constraint i is packed into
+// the image's layout at r x count + i of the K x count long arrays gv / gs -- or, with `rows`, written as the parameter layout's geometry
+// columns at row r x count + local[i] (pbd_get_replica_geometry).  A constraint the reference's initConstraint would refuse (and an
+// IsometricBending Q that factor_rank1 rejects) lowers *fail to (replica << 32 | insertion id).
+struct DeriveArgs {
+    const float4 *rest;          // K x n rest positions by host index, .w = inverse mass
+    unsigned n, count;
+    const unsigned *bodies;      // [count][nBodies] host particle indices, device order
+    const unsigned *ids;         // [count] insertion ids
+    const unsigned *local;       // [count] position among the type's constraints in the order they were added
+    const float4 *clusters;      // ShapeMatching: numClusters of the shared image (its gv[5]), device order
+    int variant;                 // IsometricBending: 0 = rank-one Kp in gv[0], 1 = full Q in gv[0..3]
+    float4 *gv[kMaxGeoV]; float *gs[kMaxGeoS];
+    float *rows;
+    unsigned long long *fail;
+};
+template <int T>
+__global__ void __launch_bounds__(128) k_derive_geometry(const __grid_constant__ DeriveArgs d) {
+    constexpr TypeShape sh = type_shape(T);
+    constexpr int g0 = geo_first(T), nGeo = num_geo(T);
+    const unsigned i = blockIdx.x * blockDim.x + threadIdx.x, r = blockIdx.y;
+    if (i >= d.count) return;
+    float4 x[4];
+#pragma unroll
+    for (int k = 0; k < sh.nBodies; k++) x[k] = __ldg(d.rest + (size_t)r * d.n + __ldg(d.bodies + (size_t)i * sh.nBodies + k));
+    float p[24];  // the parameter row; its material columns stay zero and are never read
+#pragma unroll
+    for (int k = 0; k < 24; k++) p[k] = 0.0f;
+    bool ok = rest_geometry(T, x, p + g0);
+    if (T == PBD_SHAPEMATCHING) { const float4 c = __ldg(d.clusters + i); p[20] = c.x; p[21] = c.y; p[22] = c.z; p[23] = c.w; }
+    float Kp[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+    if (T == PBD_ISOBENDING || T == PBD_ISOBENDING_XPBD) ok = factor_rank1(p + 1, Kp) && ok;
+    if (!ok) atomicMin(d.fail, ((unsigned long long)r << 32) | __ldg(d.ids + i));
+    if (d.rows) {
+        float *row = d.rows + ((size_t)r * d.count + __ldg(d.local + i)) * nGeo;
+#pragma unroll
+        for (int j = 0; j < nGeo; j++) row[j] = p[g0 + j];
+        return;
+    }
+    const size_t o = (size_t)r * d.count + i;
+    if ((T == PBD_ISOBENDING || T == PBD_ISOBENDING_XPBD) && d.variant == 0) { d.gv[0][o] = make_float4(Kp[0], Kp[1], Kp[2], Kp[3]); return; }
+    const PackColumns pc = pack_columns(T);
+    auto col = [&](int c) { return c < 0 ? 0.0f : p[c]; };
+#pragma unroll
+    for (int k = 0; k < kMaxGeoV; k++)
+        if (d.gv[k]) d.gv[k][o] = make_float4(col(pc.gv[k][0]), col(pc.gv[k][1]), col(pc.gv[k][2]), col(pc.gv[k][3]));
+#pragma unroll
+    for (int k = 0; k < kMaxGeoS; k++)
+        if (d.gs[k]) d.gs[k][o] = col(pc.gs[k]);
+}
+
 __global__ void k_set_w(float4 *__restrict__ pos, float4 *__restrict__ vel, const float *__restrict__ mass, unsigned n, const unsigned *__restrict__ slot) {
     const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;

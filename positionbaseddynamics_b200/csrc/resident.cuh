@@ -79,6 +79,8 @@ struct ResidentArgs {
     // per-replica parameters of a batch (pbd_set_replica_materials / pbd_set_replica_gravity): rows of kMatRowFloats floats (the uniform
     // material parameters of every type) and rows of 3 floats (null: gx, gy, gz for every replica)
     const float *repMat, *repGravity;
+    // per-replica rest shapes (pbd_set_replica_rest_positions): replica r's geometry of type t at r x geoCount[t] (0: shared)
+    unsigned geoCount[PBD_NUM_TYPES];
 };
 
 // ---- cluster primitives --------------------------------------------------------------------------------------------------
@@ -178,8 +180,10 @@ __device__ __forceinline__ void l2_prefetch_bytes(const void *p, size_t bytes) {
 }
 // the per-constraint arrays of one type (indices, every geometry array, the multipliers from a.lambda + lamOff): array k of items
 // [first, first + n), one array per calling lane
+// (geoOff: a batch's replica with geometry of its own starts its geometry arrays there -- an offset rather than a replica_arrays copy,
+// because the arrays are picked by the lane: a copy indexed at run time would live on the stack)
 template <int T>
-__device__ __forceinline__ void l2_prefetch_run(const TypeArrays &a, unsigned first, unsigned n, unsigned lane, size_t lamOff) {
+__device__ __forceinline__ void l2_prefetch_run(const TypeArrays &a, unsigned first, unsigned n, unsigned lane, size_t lamOff, size_t geoOff = 0) {
     constexpr TypeShape sh = type_shape(T);
     if (lane == 0) {
         if (sh.nBodies == 2) l2_prefetch_bytes(a.idx2 + first, (size_t)n * 8u);
@@ -189,10 +193,10 @@ __device__ __forceinline__ void l2_prefetch_run(const TypeArrays &a, unsigned fi
         if (sh.nBodies == 3) l2_prefetch_bytes(a.idx3[lane] + first, (size_t)n * 4u);
     } else if (lane < 3 + (unsigned)kMaxGeoV) {
         const unsigned k = lane - 3u;
-        if ((int)k < sh.nGeoV && a.gv[k]) l2_prefetch_bytes(a.gv[k] + first, (size_t)n * 16u);
+        if ((int)k < sh.nGeoV && a.gv[k]) l2_prefetch_bytes(a.gv[k] + geoOff + first, (size_t)n * 16u);
     } else if (lane < 3 + (unsigned)kMaxGeoV + (unsigned)kMaxGeoS) {
         const unsigned k = lane - 3u - (unsigned)kMaxGeoV;
-        if ((int)k < sh.nGeoS && a.gs[k]) l2_prefetch_bytes(a.gs[k] + first, (size_t)n * 4u);
+        if ((int)k < sh.nGeoS && a.gs[k]) l2_prefetch_bytes(a.gs[k] + geoOff + first, (size_t)n * 4u);
     } else if (lane == 3 + (unsigned)kMaxGeoV + (unsigned)kMaxGeoS) {
         if (sh.xpbd && a.lambda) l2_prefetch_bytes(a.lambda + lamOff + first, (size_t)n * 4u);
     }
@@ -220,7 +224,7 @@ __device__ __forceinline__ void prefetch_first(const ResidentArgs &A, const RunE
     const unsigned first = xRun ? r.firstX : r.firstR, n = xRun ? r.nX : r.nR;
     if (tid >= n) return;
     PBD_FOR_TYPE(MASK, r.type,
-        pre.s = load_streamed<T>(A.types[T], first + tid);
+        pre.s = load_streamed<T>(A.types[T], first + tid, BATCH ? rep * A.geoCount[T] : 0u);
         if (type_shape(T).xpbd && !iterZero) pre.lam = __ldcg((BATCH ? A.types[T].lambda + lambda_offset<T>(A, rep) : A.types[T].lambda) + first + tid);
         pre.bucket = bi;)
 }
@@ -234,14 +238,15 @@ __device__ __forceinline__ void run_items(const ResidentArgs &A, const Acc &acc,
                                           bool usePre, const Prefetched &pre, unsigned rep, const float *rows) {
     PBD_FOR_TYPE(MASK, type,
         TypeArrays batchArrays;  // a batch: the arrays with replica rep's multipliers
-        if (BATCH) batchArrays = replica_arrays(A.types[T], rep, A.lamCount[T]);
+        if (BATCH) batchArrays = replica_arrays(A.types[T], rep, A.lamCount[T], 0u);
+        const unsigned go = BATCH ? rep * A.geoCount[T] : 0u;  // replica rep's geometry (pbd_set_replica_rest_positions; 0: shared)
         MatRow matRow;
         if (BATCH) { matRow = load_mat_row<T>(rows + mat_offset(T)); matRow.on = true; }
         const TypeArrays &ta = BATCH ? batchArrays : A.types[T];
         unsigned i = tid;
         if (DEEP && is_pipelined2<T>()) {
             if (i < n) {
-                auto fetch = [&](unsigned k, Streamed &sx, float &lx) { sx = load_streamed<T>(ta, first + k); if (type_shape(T).xpbd && !iterZero) lx = __ldcg(ta.lambda + first + k); };
+                auto fetch = [&](unsigned k, Streamed &sx, float &lx) { sx = load_streamed<T>(ta, first + k, go); if (type_shape(T).xpbd && !iterZero) lx = __ldcg(ta.lambda + first + k); };
                 Streamed s0, s1, s2; float l0 = 0.0f, l1 = 0.0f, l2 = 0.0f;
                 if (usePre) { s0 = pre.s; l0 = pre.lam; } else fetch(i, s0, l0);
                 bool h1 = i + stride < n;
@@ -251,7 +256,7 @@ __device__ __forceinline__ void run_items(const ResidentArgs &A, const Acc &acc,
                     const unsigned j2 = i + 2u * stride;
                     const bool h2 = j2 < n;
                     if (h2) fetch(j2, s2, l2);
-                    project_streamed_acc<T, Acc, 0>(acc, ta, first + i, s0, A.h, iterZero, true, l0, matRow);
+                    project_streamed_acc<T, Acc, 0>(acc, ta, first + i, s0, A.h, iterZero, true, l0, matRow, go);
                     if (!h1) break;
                     s0 = s1; l0 = l1; s1 = s2; l1 = l2; h1 = h2; i += stride;
                 }
@@ -260,16 +265,16 @@ __device__ __forceinline__ void run_items(const ResidentArgs &A, const Acc &acc,
         if (i < n) {
             Streamed cur; float lam = 0.0f;
             if (usePre) { cur = pre.s; lam = pre.lam; }
-            else { cur = load_streamed<T>(ta, first + i); if (type_shape(T).xpbd && !iterZero) lam = __ldcg(ta.lambda + first + i); }
+            else { cur = load_streamed<T>(ta, first + i, go); if (type_shape(T).xpbd && !iterZero) lam = __ldcg(ta.lambda + first + i); }
             _Pragma("unroll 1")
             for (;;) {
                 const unsigned j = i + stride;
                 const bool more = j < n;
                 Streamed nxt; float lamN = 0.0f;
-                if (is_pipelined<T>() && more) { nxt = load_streamed<T>(ta, first + j); if (type_shape(T).xpbd && !iterZero) lamN = __ldcg(ta.lambda + first + j); }
-                project_streamed_acc<T, Acc, 0>(acc, ta, first + i, cur, A.h, iterZero, true, lam, matRow);  // variant 0 only: flatten refuses the full-Q bending layout in this mode
+                if (is_pipelined<T>() && more) { nxt = load_streamed<T>(ta, first + j, go); if (type_shape(T).xpbd && !iterZero) lamN = __ldcg(ta.lambda + first + j); }
+                project_streamed_acc<T, Acc, 0>(acc, ta, first + i, cur, A.h, iterZero, true, lam, matRow, go);  // variant 0 only: flatten refuses the full-Q bending layout in this mode
                 if (!more) break;
-                if (!is_pipelined<T>()) { nxt = load_streamed<T>(ta, first + j); if (type_shape(T).xpbd && !iterZero) lamN = __ldcg(ta.lambda + first + j); }
+                if (!is_pipelined<T>()) { nxt = load_streamed<T>(ta, first + j, go); if (type_shape(T).xpbd && !iterZero) lamN = __ldcg(ta.lambda + first + j); }
                 cur = nxt; lam = lamN; i = j;
             }
         })
@@ -425,7 +430,8 @@ __global__ void __launch_bounds__(THREADS, 1) k_step_resident(const __grid_const
                         for (unsigned k = threadIdx.x >> 5; k < kPrefetchLanes; k += RT >> 5)
                             for (unsigned bi = sColour[cn]; bi < sColour[cn + 1]; bi++) {
                                 const RunEntry r = runs[bi];
-                                PBD_FOR_TYPE(MASK, r.type, l2_prefetch_run<T>(A.types[T], r.firstX, r.nX + r.nR, k, BATCH ? lambda_offset<T>(A, rep) : 0u);)
+                                PBD_FOR_TYPE(MASK, r.type, l2_prefetch_run<T>(A.types[T], r.firstX, r.nX + r.nR, k, BATCH ? lambda_offset<T>(A, rep) : 0u,
+                                                                              BATCH ? (size_t)rep * A.geoCount[T] : 0u);)
                             }
                     }
                     if (isX) {

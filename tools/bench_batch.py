@@ -4,11 +4,17 @@ stepped one after another by a K = 1 engine; the resident cluster size C swept o
 power limit read in the same run.  The four scenes run four different resident instantiations (cloth, FEM, cloth-XPBD and light type
 masks).
 
-    python tools/bench_batch.py [--out results.json] [--quick] [--replica-rows] [--sweep]
+    python tools/bench_batch.py [--out results.json] [--quick] [--replica-rows] [--sweep] [--rest-shapes] [--ks 8,132] [--no-baseline]
 
 --replica-rows measures every batch twice in a row: with the shared parameters, and with per-replica material rows and gravity
 (pbd_set_replica_materials / pbd_set_replica_gravity) equal to the shared values, so that the work is identical and the difference is what
 the tables cost.  --sweep adds one real sweep: 132 cfg1 replicas, each with its own Distance and IsometricBending stiffness.
+--rest-shapes measures every batch twice in a row with the shared geometry and with per-replica rest shapes
+(pbd_set_replica_rest_positions) equal to the model's own rest positions, so that the work is identical and the difference is what the
+per-replica geometry arrays cost (they are K times the shared ones and leave L2 for large batches).  It also times the device derivation of
+the geometry of K rest shapes against building K host models (the host mirror's add*Constraint) for cfg1 K = 1056 and cfg3 K = 66.
+--ks replaces the K sweep of every scene; --no-baseline skips the one-after-another baseline and the C sweep.  Without --rest-shapes or
+--replica-rows the script also runs against a build without those calls, so that shared-parameter batches can be compared across builds.
 
 Batch times are device times (CUDA events on the engine's stream around `steps` steps, after warm-up steps).  The baseline is measured:
 a K = 1 engine in its faster mode (graph or resident) steps K replicas one after another -- K pbd_step calls, each replica's state
@@ -62,6 +68,63 @@ def model(name):
     return m
 
 
+def topology(name):
+    """The model's triangles or tets, for building a host model on other rest positions."""
+    build, sub, it, _ = SCENES[name]
+    hm = HostModel()
+    build(hm)
+    topo = hm.tri_faces(0) if name.startswith("cfg1") or name.startswith("cloth") else hm.tet_tets(0)
+    hm.close()
+    return topo
+
+
+def host_build(name, x0, mass, topo):
+    """One host model of scene `name` built on rest positions x0 (what a replica's geometry costs without the device derivation)."""
+    hm = HostModel()
+    if name == "cfg3":
+        hm.add_tet_model(x0, topo)
+        for i in np.nonzero(mass == 0)[0]:
+            hm.set_mass(int(i), 0.0)
+        hm.add_solid_constraints(0, 2, k=1.0e6, nu=0.3, vol_k=1.0)
+        for t in topo:
+            hm.add_constraint(scenes.VOLUME, [int(v) for v in t], [1.0])
+    else:
+        hm.add_triangle_model(x0, topo)
+        for i in np.nonzero(mass == 0)[0]:
+            hm.set_mass(int(i), 0.0)
+        hm.add_cloth_constraints(0, 1, dist_k=1.0)
+        hm.add_bending_constraints(0, 2, 0.01)
+    n = hm.num_constraints()
+    hm.close()
+    return n
+
+
+def derive_timing(name, m, k):
+    """Seconds to give K replicas their own rest shapes on the device (pbd_set_replica_rest_positions: upload, derivation, check, copy)
+    against building K host models on those rest positions (three built and timed, scaled to K)."""
+    rng = np.random.default_rng(7)
+    x0 = np.asarray(m["x0"], np.float32)
+    rest = (x0[None] * rng.uniform(0.9, 1.1, (k, 1, 3))).astype(np.float32)
+    eng = engine(m, _capi.MODE_GRAPH, k)
+    try:
+        eng.step(1); eng.sync()
+        t = []
+        for _ in range(3):
+            t0 = time.perf_counter()
+            eng.set_replica_rest_positions(rest)
+            t.append(time.perf_counter() - t0)
+            eng.set_replica_rest_positions(None)
+    finally:
+        eng.close()
+    topo = topology(name)
+    h = []
+    for r in range(3):
+        t0 = time.perf_counter()
+        host_build(name, rest[r], np.asarray(m["mass"]), topo)
+        h.append(time.perf_counter() - t0)
+    return {"scene": name, "K": k, "device_s": min(t), "host_one_s": min(h), "host_K_s": min(h) * k}
+
+
 def shared_rows(m, k):
     """Per-replica rows that restate the shared parameters: {type: (k, nMat)} from each type's first constraint, and (k, 3) gravity."""
     rows = {}
@@ -73,11 +136,14 @@ def shared_rows(m, k):
     return rows, np.repeat(np.asarray([[0.0, -9.81, 0.0]], np.float32), k, 0)
 
 
+# bytes of packed geometry per constraint (the image's float4 and scalar geometry arrays; IsometricBending: the rank-one Kp)
+GEO_BYTES = {0: 4, 1: 4, 2: 4, 3: 16, 4: 16, 5: 20, 6: 16, 7: 4, 8: 4, 9: 40, 10: 40, 11: 36, 12: 96}
+DERIVE_K = {"cfg1": 1056, "cfg3": 66}
 # include/pbd_b200.h: where a type's material parameters start in its parameter layout
 MAT_FIRST_COLUMN = {0: 1, 1: 1, 2: 1, 3: 0, 4: 0, 5: 5, 6: 4, 7: 1, 8: 1, 9: 10, 10: 10, 11: 9, 12: 0}
 
 
-def engine(m, mode, k, clusters=None, rows=None):
+def engine(m, mode, k, clusters=None, rows=None, rest=False):
     if clusters:
         os.environ["PBD_B200_CLUSTERS"] = "1x%d" % clusters  # the planner's cluster-size override (read when the image is planned)
     else:
@@ -94,6 +160,8 @@ def engine(m, mode, k, clusters=None, rows=None):
         for t, mat in rows[0].items():
             eng.set_replica_materials(t, mat)
         eng.set_replica_gravity(rows[1])
+    if rest:  # every replica's rest shape = the model's: the same geometry, from the per-replica arrays
+        eng.set_replica_rest_positions(np.repeat(np.asarray(m["x0"], np.float32)[None], k, 0))
     return eng
 
 
@@ -108,11 +176,11 @@ def timed(eng, warmup=3, min_s=0.4):
     return st.last_step_ms / steps, steps
 
 
-def measure(m, mode, k, clusters=None, rows=None):
+def measure(m, mode, k, clusters=None, rows=None, rest=False):
     t0 = time.time()
     eng = None
     try:
-        eng = engine(m, mode, k, clusters, rows)
+        eng = engine(m, mode, k, clusters, rows, rest)
         ms, steps = timed(eng)
         _, active = eng.get_mode()
     except _capi.PbdError as ex:
@@ -153,8 +221,11 @@ def main():
     ap.add_argument("--scenes", default=",".join(SCENES))
     ap.add_argument("--replica-rows", action="store_true", help="every batch also with per-replica rows equal to the shared parameters")
     ap.add_argument("--sweep", action="store_true", help="132 cfg1 replicas, each with its own stiffnesses")
+    ap.add_argument("--rest-shapes", action="store_true", help="every batch also with per-replica rest shapes; device derivation against host builds")
+    ap.add_argument("--ks", default=None, help="comma-separated K to measure instead of each scene's sweep")
+    ap.add_argument("--no-baseline", action="store_true", help="skip the one-after-another baseline and the C sweep")
     a = ap.parse_args()
-    res = {"card": card(), "rows": [], "c_sweep": [], "replica_rows": [], "sweep": []}
+    res = {"card": card(), "rows": [], "c_sweep": [], "replica_rows": [], "sweep": [], "rest_shapes": [], "derive": []}
     print("card: %s" % res["card"], flush=True)
     for name in a.scenes.split(","):
         m = model(name)
@@ -162,11 +233,11 @@ def main():
         proj = ncons * m["sub"] * m["it"]
         solo = {md: measure(m, md, 1) for md in (_capi.MODE_GRAPH, _capi.MODE_RESIDENT)}
         solo_mode = min((r["ms"], md) for md, r in solo.items() if "ms" in r)[1]
-        ks = SCENES[name][3][:2] if a.quick else SCENES[name][3]
+        ks = [int(v) for v in a.ks.split(",")] if a.ks else (SCENES[name][3][:2] if a.quick else SCENES[name][3])
         print("%s: %d particles, %d constraints, %d x %d; K = 1: graph %.3f ms, resident %s ms" % (
             name, len(m["x0"]), ncons, m["sub"], m["it"], solo[0]["ms"], "%.3f" % solo[1]["ms"] if "ms" in solo[1] else solo[1]["error"]), flush=True)
         for k in ks:
-            row = {"scene": name, "K": k, "baseline_ms": one_after_another(m, solo_mode, k)}
+            row = {"scene": name, "K": k, "baseline_ms": float("nan") if a.no_baseline else one_after_another(m, solo_mode, k)}
             for label, md in (("graph", _capi.MODE_GRAPH), ("resident", _capi.MODE_RESIDENT), ("auto", _capi.MODE_AUTO)):
                 r = measure(m, md, k)
                 row[label] = r
@@ -185,6 +256,19 @@ def main():
                 ms = [measure(m, md, k, rows=rows if i & 1 else None).get("ms", float("nan")) for i in range(4)]
                 res["replica_rows"].append({"scene": name, "K": k, "mode": label, "shared_ms": ms[0::2], "rows_ms": ms[1::2]})
                 print("  rows K=%5d %-8s shared %.4f %.4f ms | per-replica rows %.4f %.4f ms" % (k, label, ms[0], ms[2], ms[1], ms[3]), flush=True)
+        for k in (ks if a.rest_shapes else []):
+            if k == 1:
+                continue
+            for label, md in (("graph", _capi.MODE_GRAPH), ("resident", _capi.MODE_RESIDENT)):
+                # shared, per-replica, shared, per-replica: the spread of each pair is next to the difference between them
+                ms = [measure(m, md, k, rest=bool(i & 1)).get("ms", float("nan")) for i in range(4)]
+                geo_mb = sum(k * int((np.asarray(m["types"]) == t).sum()) * GEO_BYTES.get(t, 0) for t in range(_capi.NUM_TYPES)) * 1e-6
+                res["rest_shapes"].append({"scene": name, "K": k, "mode": label, "shared_ms": ms[0::2], "rest_ms": ms[1::2], "geometry_mb": geo_mb})
+                print("  rest shapes K=%5d %-8s shared %.4f %.4f ms | per-replica %.4f %.4f ms (%.0f MB of geometry)" % (k, label, ms[0], ms[2], ms[1], ms[3], geo_mb), flush=True)
+        if a.rest_shapes and name in DERIVE_K:
+            d = derive_timing(name, m, DERIVE_K[name])
+            res["derive"].append(d)
+            print("  derive K=%5d: device %.3f s, host models %.3f s each -> %.1f s for K" % (d["K"], d["device_s"], d["host_one_s"], d["host_K_s"]), flush=True)
         if a.sweep and name == "cfg1":
             k = 132
             rows = shared_rows(m, k)
@@ -195,7 +279,7 @@ def main():
                 r.update({"scene": name, "K": k, "mode": label})
                 res["sweep"].append(r)
                 print("  stiffness sweep K=%5d %-8s %s" % (k, label, ("%.4f ms" % r["ms"]) if "ms" in r else r["error"][:80]), flush=True)
-        if a.quick or name not in C_SWEEP:
+        if a.quick or a.no_baseline or name not in C_SWEEP:
             continue
         for k in C_SWEEP[name]:
             for c in (1, 2, 4, 8, 16):

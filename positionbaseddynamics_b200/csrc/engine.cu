@@ -69,10 +69,9 @@ struct DevBuf {                   // one device allocation, freed with its owner
 
 struct DevType {
     DevBuf idx[3], gv[kMaxGeoV], gs[kMaxGeoS], mat[kMaxMat], lambda;
-    // replica batch: what its per-replica geometry is derived from (TypePlan::restBodies / restLocal, the insertion ids), the geometry
-    // arrays every replica's projections read while per-replica rest shapes are on (K x count; they keep their address while it stays
-    // on), and the arrays a derivation writes before it is known to be accepted
-    DevBuf restBodies, restLocal, restIds, repGv[kMaxGeoV], repGs[kMaxGeoS], newGv[kMaxGeoV], newGs[kMaxGeoS];
+    // replica batch: what its per-replica geometry is derived from (TypePlan::restBodies / restLocal, the insertion ids), and the geometry
+    // arrays every replica's projections read while per-replica rest shapes are on (K x count; they keep their address while it stays on)
+    DevBuf restBodies, restLocal, restIds, repGv[kMaxGeoV], repGs[kMaxGeoS];
     PodVector<unsigned> order;    // position in the device arrays -> insertion id
     unsigned count = 0;
     TypeArrays arrays{};
@@ -84,22 +83,22 @@ struct pbd_engine {
     bool ownsStream = false;
     int smCount = 132;                    // H100 SXM; read from the device in pbd_create
     size_t l2Bytes = 50u << 20;           // likewise
-    // particles: K replicas of n (pbd_set_replicas), replica r at device slots [r n, (r + 1) n)
-    unsigned n = 0, K = 1;
+    // particles: batch.K replicas of n (pbd_set_replicas), replica r at device slots [r n, (r + 1) n)
+    unsigned n = 0;
     DevBuf pos, vel, oldp, lastp, pos0, stage, stage2, massStage, jacobiDelta;
-    // Per-replica parameters of a batch.  repMat [K][kMatRowFloats]: the uniform material parameters of every type, replica by replica --
-    // the shared ones of the image, or a replica's own (pbd_set_replica_materials, the types of repMatMask); repGravity [K][3]
-    // (pbd_set_replica_gravity).  Both keep their address until K changes, so that a captured graph keeps reading the same tables.
-    DevBuf repMat, repGravity;
-    unsigned repMatMask = 0;
-    bool repGravitySet = false;
-    // Per-replica rest shapes (pbd_set_replica_rest_positions): the rest positions the call was given, K x n float4 by host index with
-    // .w = the inverse mass at the time of the call; every image planned while repGeo is on derives its geometry from them again.
-    DevBuf restX, restNew, deriveFail, geoRows;
-    bool repGeo = false;
-    // the current image carries what a derivation reads (TypePlan::restBodies / restLocal): planned only while the override is on or
-    // being switched on, so that batches without it do not pay for them
-    bool restTables = false, restWanted = false;
+    // A replica batch and what its replicas have of their own (batch_arrays, replica_mat and replica_geo turn it into what the kernels see).
+    // mat [K][kMatRowFloats]: the uniform material parameters of every type, replica by replica -- the shared ones of the image, or a
+    // replica's own (pbd_set_replica_materials, the types of matMask); gravity [K][3] (pbd_set_replica_gravity).  Both keep their address
+    // until K changes, so that a captured graph keeps reading the same tables.
+    // restX: per-replica rest shapes (pbd_set_replica_rest_positions), the rest positions the call was given, K x n float4 by host index
+    // with .w = the inverse mass at the time of the call; every image planned while restShapes is on derives its geometry from them.
+    // restTables: the current image carries what a derivation reads (TypePlan::restBodies / restLocal), planned only while the override
+    // is on or being switched on, so that batches without it do not pay for them.
+    struct Batch {
+        unsigned K = 1, matMask = 0;
+        DevBuf mat, gravity, restX;
+        bool gravitySet = false, restShapes = false, restTables = false;
+    } batch;
     // rigid bodies coupled through joints (SURVEY.md 8f-1): float4 arrays X(xyz,invMass) Q(x,y,z,w) V(xyz,mass) W(omega) + history + inertia
     unsigned nRb = 0;
     DevBuf rbX, rbQ, rbV, rbW, rbOldX, rbLastX, rbOldQ, rbLastQ, rbI, rbIinv;
@@ -153,13 +152,11 @@ static int use(pbd_engine *e) { CK(cudaSetDevice(e->device)); return 0; }
 
 // per-replica rest shapes off (the caller drops the graph where the kernel arguments change)
 static void drop_replica_geometry(pbd_engine *e) {
-    e->repGeo = false;
-    e->restX.release(); e->restNew.release(); e->geoRows.release();
+    e->batch.restShapes = false;
+    e->batch.restX.release();
     for (DevType &d : e->dev) {
         for (DevBuf &b : d.repGv) b.release();
         for (DevBuf &b : d.repGs) b.release();
-        for (DevBuf &b : d.newGv) b.release();
-        for (DevBuf &b : d.newGs) b.release();
     }
 }
 
@@ -252,9 +249,9 @@ static int relayout(pbd_engine *e, const std::vector<unsigned> &newSlot) {
     CK(cudaMemcpy(e->dSlotOld.p, e->slot.data(), nb, cudaMemcpyHostToDevice));
     e->slot = newSlot;
     CKE(upload_slot_map(e));
-    CKE(e->relayoutTmp.alloc((size_t)e->K * e->n * sizeof(float4)));
+    CKE(e->relayoutTmp.alloc((size_t)e->batch.K * e->n * sizeof(float4)));
     for (DevBuf *b : {&e->pos, &e->vel, &e->oldp, &e->lastp, &e->pos0}) {
-        k_relayout<<<dim3((e->n + 255) / 256, e->K), 256, 0, e->stream>>>((const float4 *)b->p, (float4 *)e->relayoutTmp.p, e->n, (const unsigned *)e->dSlotOld.p, (const unsigned *)e->dSlot.p);
+        k_relayout<<<dim3((e->n + 255) / 256, e->batch.K), 256, 0, e->stream>>>((const float4 *)b->p, (float4 *)e->relayoutTmp.p, e->n, (const unsigned *)e->dSlotOld.p, (const unsigned *)e->dSlot.p);
         CK(cudaGetLastError());
         CK(cudaStreamSynchronize(e->stream));
         std::swap(b->p, e->relayoutTmp.p); std::swap(b->bytes, e->relayoutTmp.bytes);
@@ -287,29 +284,29 @@ extern "C" int pbd_set_masses(pbd_engine *e, const float *mass) {
     if (!e || !mass) return fail("pbd_set_masses: null argument");
     CKE(use(e));
     if (e->n == 0) return 0;
-    return set_w(e, mass, e->K);
+    return set_w(e, mass, e->batch.K);
 }
 
 // replica 0 of a particle array copied to replicas 1 .. K-1 (doubling copies)
 static int broadcast_replica0(pbd_engine *e, DevBuf &b) {
     const size_t one = (size_t)e->n * sizeof(float4);
-    for (size_t have = 1; have < e->K; have *= 2)
-        CK(cudaMemcpyAsync((char *)b.p + have * one, b.p, std::min(have, (size_t)e->K - have) * one, cudaMemcpyDeviceToDevice, e->stream));
+    for (size_t have = 1; have < e->batch.K; have *= 2)
+        CK(cudaMemcpyAsync((char *)b.p + have * one, b.p, std::min(have, (size_t)e->batch.K - have) * one, cudaMemcpyDeviceToDevice, e->stream));
     return 0;
 }
 
 extern "C" int pbd_set_particles(pbd_engine *e, unsigned n, const float *x, const float *x0, const float *v, const float *mass) {
     if (!e || (n && (!x || !mass))) return fail("pbd_set_particles: null argument");
-    const std::string why = pbd_b200::batch_refusal(e->K, n, e->mode, e->nRb, e->host);
+    const std::string why = pbd_b200::batch_refusal(e->batch.K, n, e->mode, e->nRb, e->host);
     if (!why.empty()) return fail("pbd_set_particles: %s", why.c_str());
     CKE(use(e));
     CK(cudaStreamSynchronize(e->stream));
     if (n != e->n) { e->imageDirty = true; drop_graph(e); }
     e->n = n;
     const size_t b4 = (size_t)n * sizeof(float4);
-    for (auto *b : {&e->pos, &e->vel, &e->oldp, &e->lastp, &e->pos0}) CKE(b->alloc(b4 * e->K));
-    CKE(e->stage.alloc((size_t)e->K * n * 3 * sizeof(float)));
-    CKE(e->massStage.alloc((size_t)e->K * n * sizeof(float)));
+    for (auto *b : {&e->pos, &e->vel, &e->oldp, &e->lastp, &e->pos0}) CKE(b->alloc(b4 * e->batch.K));
+    CKE(e->stage.alloc((size_t)e->batch.K * n * 3 * sizeof(float)));
+    CKE(e->massStage.alloc((size_t)e->batch.K * n * sizeof(float)));
     drop_graph(e);  // buffers may have moved
     drop_replica_geometry(e);  // every replica's state is redefined
     e->slot.resize(n); e->imageDirty = true;
@@ -354,8 +351,8 @@ extern "C" int pbd_set_replicas(pbd_engine *e, unsigned K) {
             std::swap(b->p, grown.p); std::swap(b->bytes, grown.bytes);
             CK(cudaStreamSynchronize(e->stream));  // before `grown` frees the old array
         }
-    e->K = K;
-    e->repMat.release(); e->repGravity.release(); e->repMatMask = 0; e->repGravitySet = false;  // rows of the old K
+    e->batch.K = K;
+    e->batch.mat.release(); e->batch.gravity.release(); e->batch.matMask = 0; e->batch.gravitySet = false;  // rows of the old K
     drop_replica_geometry(e);
     for (DevBuf *b : {&e->pos, &e->vel, &e->oldp, &e->lastp, &e->pos0}) CKE(broadcast_replica0(e, *b));
     CKE(e->stage.alloc((size_t)K * e->n * 3 * sizeof(float)));
@@ -368,23 +365,23 @@ extern "C" int pbd_set_replicas(pbd_engine *e, unsigned K) {
 
 static int replica_params_refusal(const pbd_engine *e, const char *what) {
     if (!e) return fail("%s: null engine", what);
-    if (e->K == 1) return fail("%s: a single-scene engine takes its parameters from pbd_add_constraints / pbd_set_params (pbd_set_replicas first)", what);
+    if (e->batch.K == 1) return fail("%s: a single-scene engine takes its parameters from pbd_add_constraints / pbd_set_params (pbd_set_replicas first)", what);
     return 0;
 }
 // type's columns of the K rows of the material table <- rows of nMat floats `pitch` bytes apart (0: the same row for every replica)
 static int write_replica_materials(pbd_engine *e, int type, const float *rows, size_t pitch) {
-    if (!e->repMat.p) {
-        CKE(e->repMat.alloc((size_t)e->K * kMatRowFloats * sizeof(float)));
-        CK(cudaMemsetAsync(e->repMat.p, 0, e->repMat.bytes, e->stream));
+    if (!e->batch.mat.p) {
+        CKE(e->batch.mat.alloc((size_t)e->batch.K * kMatRowFloats * sizeof(float)));
+        CK(cudaMemsetAsync(e->batch.mat.p, 0, e->batch.mat.bytes, e->stream));
     }
     const size_t width = type_shape(type).nMat * sizeof(float);
     std::vector<float> same;
     if (!pitch) {
-        same.resize((size_t)e->K * type_shape(type).nMat);
+        same.resize((size_t)e->batch.K * type_shape(type).nMat);
         for (size_t i = 0; i < same.size(); i++) same[i] = rows[i % type_shape(type).nMat];
         rows = same.data(); pitch = width;
     }
-    CK(cudaMemcpy2DAsync((float *)e->repMat.p + mat_offset(type), kMatRowFloats * sizeof(float), rows, pitch, width, e->K, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemcpy2DAsync((float *)e->batch.mat.p + mat_offset(type), kMatRowFloats * sizeof(float), rows, pitch, width, e->batch.K, cudaMemcpyHostToDevice, e->stream));
     return 0;
 }
 // The rows are copied in stream order into tables that keep their address: a captured graph reads the new values at its next launch.
@@ -397,31 +394,31 @@ extern "C" int pbd_set_replica_materials(pbd_engine *e, int type, const float *m
     CKE(use(e));
     const unsigned bit = 1u << type;
     if (mat) CKE(write_replica_materials(e, type, mat, nMat * sizeof(float)));
-    else if ((e->repMatMask & bit) && !e->imageDirty) CKE(write_replica_materials(e, type, e->dev[type].arrays.matU, 0));  // (a dirty image writes them when it is planned)
+    else if ((e->batch.matMask & bit) && !e->imageDirty) CKE(write_replica_materials(e, type, e->dev[type].arrays.matU, 0));  // (a dirty image writes them when it is planned)
     // (on or off decides whether the per-constraint material arrays of the type count: batch_arrays)
-    if (((e->repMatMask & bit) != 0u) != (mat != nullptr)) { e->repMatMask ^= bit; drop_graph(e); }
+    if (((e->batch.matMask & bit) != 0u) != (mat != nullptr)) { e->batch.matMask ^= bit; drop_graph(e); }
     return 0;
 }
 extern "C" int pbd_set_replica_gravity(pbd_engine *e, const float *g) {
     CKE(replica_params_refusal(e, "pbd_set_replica_gravity"));
     CKE(use(e));
     if (g) {
-        CKE(e->repGravity.alloc((size_t)e->K * 3 * sizeof(float)));
-        CK(cudaMemcpyAsync(e->repGravity.p, g, (size_t)e->K * 3 * sizeof(float), cudaMemcpyHostToDevice, e->stream));
+        CKE(e->batch.gravity.alloc((size_t)e->batch.K * 3 * sizeof(float)));
+        CK(cudaMemcpyAsync(e->batch.gravity.p, g, (size_t)e->batch.K * 3 * sizeof(float), cudaMemcpyHostToDevice, e->stream));
     }
-    if (e->repGravitySet != (g != nullptr)) { e->repGravitySet = (g != nullptr); drop_graph(e); }
+    if (e->batch.gravitySet != (g != nullptr)) { e->batch.gravitySet = (g != nullptr); drop_graph(e); }
     return 0;
 }
 // What a batch's per-bucket kernels get for type t: where the replicas have parameters of their own, its place in replica 0's row of the
 // material table (without them the kernel arguments' uniforms do: reading the table for every launch cost the small shared-parameter
 // batches of DESIGN.md section 6 7-17 % in graph mode); and its arrays -- without the per-constraint material arrays in that case.
 // With per-replica rest shapes the geometry arrays are the K x count ones, replica r's at r x replica_geo (0: the shared image's).
-static const float *replica_mat(const pbd_engine *e, int t) { return ((e->repMatMask >> t) & 1u) ? (const float *)e->repMat.p + mat_offset(t) : nullptr; }
-static unsigned replica_geo(const pbd_engine *e, int t) { return e->repGeo ? e->dev[t].count : 0u; }
+static const float *replica_mat(const pbd_engine *e, int t) { return ((e->batch.matMask >> t) & 1u) ? (const float *)e->batch.mat.p + mat_offset(t) : nullptr; }
+static unsigned replica_geo(const pbd_engine *e, int t) { return e->batch.restShapes ? e->dev[t].count : 0u; }
 static TypeArrays batch_arrays(const pbd_engine *e, int t) {
     TypeArrays a = e->dev[t].arrays;
-    if ((e->repMatMask >> t) & 1u) for (int k = 0; k < kMaxMat; k++) a.mat[k] = nullptr;
-    if (e->repGeo) {
+    if ((e->batch.matMask >> t) & 1u) for (int k = 0; k < kMaxMat; k++) a.mat[k] = nullptr;
+    if (e->batch.restShapes) {
         for (int k = 0; k < kMaxGeoV; k++) if (a.gv[k]) a.gv[k] = (const float4 *)e->dev[t].repGv[k].p;
         for (int k = 0; k < kMaxGeoS; k++) if (a.gs[k]) a.gs[k] = (const float *)e->dev[t].repGs[k].p;
     }
@@ -430,7 +427,7 @@ static TypeArrays batch_arrays(const pbd_engine *e, int t) {
 
 extern "C" int pbd_get_replicas(pbd_engine *e, unsigned *K) {
     if (!e || !K) return fail("pbd_get_replicas: null argument");
-    *K = e->K;
+    *K = e->batch.K;
     return 0;
 }
 
@@ -440,7 +437,7 @@ extern "C" int pbd_set_attr(pbd_engine *e, int attr, const float *src) {
     float4 *dst = attr_buf(e, attr);
     if (!dst) return fail("pbd_set_attr: bad attribute %d", attr);
     if (e->n == 0) return 0;
-    CKE(upload3(e, src, dst, 1, e->K));
+    CKE(upload3(e, src, dst, 1, e->batch.K));
     CK(cudaStreamSynchronize(e->stream));
     return 0;
 }
@@ -451,9 +448,9 @@ extern "C" int pbd_get_attr(pbd_engine *e, int attr, float *dst) {
     const float4 *src = attr_buf(e, attr);
     if (!src) return fail("pbd_get_attr: bad attribute %d", attr);
     if (e->n == 0) return 0;
-    k_unpack3<<<replica_grid(e, e->K), 256, 0, e->stream>>>(src, (float *)e->stage.p, e->n, (const unsigned *)e->dSlot.p);
+    k_unpack3<<<replica_grid(e, e->batch.K), 256, 0, e->stream>>>(src, (float *)e->stage.p, e->n, (const unsigned *)e->dSlot.p);
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(dst, e->stage.p, (size_t)e->K * e->n * 3 * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaMemcpyAsync(dst, e->stage.p, (size_t)e->batch.K * e->n * 3 * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
     CK(cudaStreamSynchronize(e->stream));
     return 0;
 }
@@ -464,7 +461,7 @@ extern "C" int pbd_get_attr(pbd_engine *e, int attr, float *dst) {
 extern "C" int pbd_set_rigid_bodies(pbd_engine *e, unsigned n, const float *mass, const float *x, const float *q, const float *inertia,
                                     const float *v, const float *omega) {
     if (!e || (n && (!mass || !x || !q || !inertia))) return fail("pbd_set_rigid_bodies: null argument");
-    const std::string why = pbd_b200::batch_refusal(e->K, e->n, e->mode, n, e->host);
+    const std::string why = pbd_b200::batch_refusal(e->batch.K, e->n, e->mode, n, e->host);
     if (!why.empty()) return fail("pbd_set_rigid_bodies: %s", why.c_str());
     CKE(use(e));
     CK(cudaStreamSynchronize(e->stream));
@@ -533,13 +530,13 @@ extern "C" int pbd_clear_constraints(pbd_engine *e) {
 // planned again.  Checked here, on the host and with the arithmetic of the device derivation (rest_geometry.cuh), so that a constraint some
 // replica's rest shape makes degenerate is refused by this call instead of failing the next step.
 static int check_added_geometry(pbd_engine *e, int type, unsigned count, const unsigned *bodies, const unsigned *ids) {
-    if (!e->repGeo || !count || !e->n || type >= PBD_BALLJOINT) return 0;
+    if (!e->batch.restShapes || !count || !e->n || type >= PBD_BALLJOINT) return 0;
     CKE(use(e));
-    std::vector<float4> rest((size_t)e->K * e->n);
+    std::vector<float4> rest((size_t)e->batch.K * e->n);
     CK(cudaStreamSynchronize(e->stream));
-    CK(cudaMemcpy(rest.data(), e->restX.p, rest.size() * sizeof(float4), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(rest.data(), e->batch.restX.p, rest.size() * sizeof(float4), cudaMemcpyDeviceToHost));
     const int nb = type_shape(type).nBodies;
-    for (unsigned r = 0; r < e->K; r++)
+    for (unsigned r = 0; r < e->batch.K; r++)
         for (unsigned i = 0; i < count; i++) {
             float4 x[4];
             for (int k = 0; k < nb; k++) x[k] = rest[(size_t)r * e->n + bodies[(size_t)i * nb + k]];
@@ -783,10 +780,10 @@ extern "C" int pbd_set_mode(pbd_engine *e, int mode) {
     if (!e) return fail("null engine");
     if (mode != PBD_MODE_GRAPH && mode != PBD_MODE_RESIDENT && mode != PBD_MODE_LAUNCH && mode != PBD_MODE_JACOBI && mode != PBD_MODE_AUTO) return fail("unknown solver mode %d", mode);
     if (mode == e->mode) return 0;
-    const std::string why = pbd_b200::batch_refusal(e->K, e->n, mode, e->nRb, e->host);
+    const std::string why = pbd_b200::batch_refusal(e->batch.K, e->n, mode, e->nRb, e->host);
     if (!why.empty()) return fail("pbd_set_mode: %s", why.c_str());
     // only the resident image is laid out differently: the others run the image they share
-    const int active = pbd_b200::preferred_mode(mode, e->host, e->n, e->numConstraints, false, e->K);
+    const int active = pbd_b200::preferred_mode(mode, e->host, e->n, e->numConstraints, false, e->batch.K);
     if ((active == PBD_MODE_RESIDENT) != (e->active == PBD_MODE_RESIDENT)) e->imageDirty = true;
     e->mode = mode; e->active = active; e->autoNoResident = false;
     drop_graph(e);
@@ -831,11 +828,11 @@ static void resident_launch_config(unsigned mask, unsigned C, bool batch, unsign
 
 // how many clusters of C CTAs (one CTA per SM, `smem` bytes each) of the instantiation for `mask` the device keeps resident at the same time
 static int resident_max_clusters(const pbd_engine *e, unsigned mask, unsigned C, size_t smem, int *out) {
-    return with_resident_kernel(mask, C, e->K > 1, [&](auto kernel) -> int {
+    return with_resident_kernel(mask, C, e->batch.K > 1, [&](auto kernel) -> int {
         CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynamicSmem));
         CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
         cudaLaunchConfig_t cfg; cudaLaunchAttribute attr[1];
-        resident_launch_config(mask, C, e->K > 1, C, smem, e->stream, cfg, attr);
+        resident_launch_config(mask, C, e->batch.K > 1, C, smem, e->stream, cfg, attr);
         cudaError_t err = cudaOccupancyMaxActiveClusters(out, kernel, &cfg);
         if (err != cudaSuccess) { cudaGetLastError(); *out = 0; }
         return 0;
@@ -872,14 +869,14 @@ static int upload_type(pbd_engine *e, int t, pbd_b200::TypePlan &p) {
     if (!p.restBodies.empty()) {
         CKE(upload_vec(d.restBodies, p.restBodies, e->stream)); CKE(upload_vec(d.restLocal, p.restLocal, e->stream)); CKE(upload_vec(d.restIds, d.order, e->stream));
     }
-    if (e->K > 1 && type_shape(t).nMat && !((e->repMatMask >> t) & 1u)) CKE(write_replica_materials(e, t, a.matU, 0));  // the shared parameters, for every replica
+    if (e->batch.K > 1 && type_shape(t).nMat && !((e->batch.matMask >> t) & 1u)) CKE(write_replica_materials(e, t, a.matU, 0));  // the shared parameters, for every replica
     if (t == PBD_BALLJOINT || t == PBD_RB_PARTICLE_BALLJOINT) {
         a.rbX = (float4 *)e->rbX.p; a.rbQ = (float4 *)e->rbQ.p; a.rbIinv = (const float4 *)e->rbIinv.p;
     }
     if (type_shape(t).xpbd) {
         // replica r's multipliers at [r cnt, (r + 1) cnt); + 16 like the other streamed arrays: the L2 prefetch of a run rounds its end up to 16 bytes
-        CKE(d.lambda.alloc((size_t)e->K * cnt * sizeof(float) + 16));
-        CK(cudaMemsetAsync(d.lambda.p, 0, (size_t)e->K * cnt * sizeof(float), e->stream));
+        CKE(d.lambda.alloc((size_t)e->batch.K * cnt * sizeof(float) + 16));
+        CK(cudaMemsetAsync(d.lambda.p, 0, (size_t)e->batch.K * cnt * sizeof(float), e->stream));
         a.lambda = (float *)d.lambda.p;
     }
     return 0;
@@ -890,40 +887,44 @@ template <class F> static int with_geometry_type(int type, F &&f) {
     PBD_FOR_TYPE(kMaskAll & ~(type_bit(PBD_BALLJOINT) | type_bit(PBD_RB_PARTICLE_BALLJOINT)), type, return f(std::integral_constant<int, T>{});)
     return fail("constraint type %d has no rest geometry of particles", type);
 }
+struct GeoBufs { DevBuf gv[kMaxGeoV], gs[kMaxGeoS]; };  // one type's geometry arrays in the image's layout
 // Every particle type's geometry of the K replicas derived from `rest` (K x n float4 by host index, k_pack_rest) on the device: packed into
-// the image's layout in newGv / newGs, or with `rows` type rowsType's parameter-layout geometry rows (K x count x num_geo).  *bad: the
+// the image's layout in fresh[type], or with `rows` type rowsType's parameter-layout geometry rows (K x count x num_geo).  *bad: the
 // first constraint refused (replica << 32 | insertion id), ~0 for none.
-static int derive_geometry(pbd_engine *e, const float4 *rest, int rowsType, float *rows, unsigned long long *bad) {
-    CKE(e->deriveFail.alloc(sizeof(unsigned long long)));
-    CK(cudaMemsetAsync(e->deriveFail.p, 0xff, sizeof(unsigned long long), e->stream));
+static int derive_geometry(pbd_engine *e, const float4 *rest, GeoBufs *fresh, int rowsType, float *rows, unsigned long long *bad) {
+    DevBuf failed;
+    CKE(failed.alloc(sizeof(unsigned long long)));
+    CK(cudaMemsetAsync(failed.p, 0xff, sizeof(unsigned long long), e->stream));
     for (int t = 0; t < PBD_BALLJOINT; t++) {
         DevType &d = e->dev[t];
         if (!d.count || (rows && t != rowsType)) continue;
         DeriveArgs a{};
         a.rest = rest; a.n = e->n; a.count = d.count;
         a.bodies = (const unsigned *)d.restBodies.p; a.ids = (const unsigned *)d.restIds.p; a.local = (const unsigned *)d.restLocal.p;
-        a.clusters = d.arrays.gv[5]; a.variant = d.arrays.variant; a.rows = rows; a.fail = (unsigned long long *)e->deriveFail.p;
+        a.clusters = d.arrays.gv[5]; a.variant = d.arrays.variant; a.rows = rows; a.fail = (unsigned long long *)failed.p;
         if (!rows) {
-            const size_t cnt = (size_t)e->K * d.count;  // + 16 like the other streamed arrays: the L2 prefetch of a run rounds its end up
-            for (int k = 0; k < kMaxGeoV; k++) if (d.arrays.gv[k]) { CKE(d.newGv[k].alloc(cnt * sizeof(float4) + 16)); a.gv[k] = (float4 *)d.newGv[k].p; }
-            for (int k = 0; k < kMaxGeoS; k++) if (d.arrays.gs[k]) { CKE(d.newGs[k].alloc(cnt * sizeof(float) + 16)); a.gs[k] = (float *)d.newGs[k].p; }
+            const size_t cnt = (size_t)e->batch.K * d.count;  // + 16 like the other streamed arrays: the L2 prefetch of a run rounds its end up
+            for (int k = 0; k < kMaxGeoV; k++) if (d.arrays.gv[k]) { CKE(fresh[t].gv[k].alloc(cnt * sizeof(float4) + 16)); a.gv[k] = (float4 *)fresh[t].gv[k].p; }
+            for (int k = 0; k < kMaxGeoS; k++) if (d.arrays.gs[k]) { CKE(fresh[t].gs[k].alloc(cnt * sizeof(float) + 16)); a.gs[k] = (float *)fresh[t].gs[k].p; }
         }
         CKE(with_geometry_type(t, [&](auto T) -> int {
-            k_derive_geometry<decltype(T)::value><<<dim3(nblk(d.count, 128), e->K), 128, 0, e->stream>>>(a);
+            k_derive_geometry<decltype(T)::value><<<dim3(nblk(d.count, 128), e->batch.K), 128, 0, e->stream>>>(a);
             CK(cudaGetLastError());
             return 0;
         }));
     }
-    CK(cudaMemcpyAsync(bad, e->deriveFail.p, sizeof(*bad), cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaMemcpyAsync(bad, failed.p, sizeof(*bad), cudaMemcpyDeviceToHost, e->stream));
     CK(cudaStreamSynchronize(e->stream));
     return 0;
 }
 // The geometry derived from `rest` becomes what the projections read -- only when no constraint refuses it: otherwise the error names the
 // first replica and constraint, and nothing has changed.  It is copied into the live arrays in stream order, so that they keep their
-// address and a captured graph reads the new geometry at its next launch.
+// address and a captured graph reads the new geometry at its next launch.  The scratch arrays are as large as the live ones: they are
+// freed on return.
 static int apply_replica_geometry(pbd_engine *e, const float4 *rest, const char *what) {
     unsigned long long bad = ~0ull;
-    CKE(derive_geometry(e, rest, -1, nullptr, &bad));
+    GeoBufs fresh[PBD_BALLJOINT];
+    CKE(derive_geometry(e, rest, fresh, -1, nullptr, &bad));
     if (bad != ~0ull) {
         const unsigned rep = (unsigned)(bad >> 32), id = (unsigned)bad;
         int type = -1;
@@ -934,31 +935,27 @@ static int apply_replica_geometry(pbd_engine *e, const float4 *rest, const char 
     }
     for (int t = 0; t < PBD_BALLJOINT; t++) {
         DevType &d = e->dev[t];
-        const size_t cnt = (size_t)e->K * d.count;
+        const size_t cnt = (size_t)e->batch.K * d.count;
         if (!cnt) continue;
         for (int k = 0; k < kMaxGeoV; k++)
-            if (d.arrays.gv[k]) { CKE(d.repGv[k].alloc(cnt * sizeof(float4) + 16)); CK(cudaMemcpyAsync(d.repGv[k].p, d.newGv[k].p, cnt * sizeof(float4), cudaMemcpyDeviceToDevice, e->stream)); }
+            if (d.arrays.gv[k]) { CKE(d.repGv[k].alloc(cnt * sizeof(float4) + 16)); CK(cudaMemcpyAsync(d.repGv[k].p, fresh[t].gv[k].p, cnt * sizeof(float4), cudaMemcpyDeviceToDevice, e->stream)); }
         for (int k = 0; k < kMaxGeoS; k++)
-            if (d.arrays.gs[k]) { CKE(d.repGs[k].alloc(cnt * sizeof(float) + 16)); CK(cudaMemcpyAsync(d.repGs[k].p, d.newGs[k].p, cnt * sizeof(float), cudaMemcpyDeviceToDevice, e->stream)); }
+            if (d.arrays.gs[k]) { CKE(d.repGs[k].alloc(cnt * sizeof(float) + 16)); CK(cudaMemcpyAsync(d.repGs[k].p, fresh[t].gs[k].p, cnt * sizeof(float), cudaMemcpyDeviceToDevice, e->stream)); }
     }
     CK(cudaStreamSynchronize(e->stream));
-    for (DevType &d : e->dev) {  // the scratch arrays are as large as the live ones: not kept between derivations
-        for (DevBuf &b : d.newGv) b.release();
-        for (DevBuf &b : d.newGs) b.release();
-    }
     return 0;
 }
 
 // constraints + colour groups -> the device image of the requested mode (the planner resolves PBD_MODE_AUTO): the planner's inputs
-// gathered, the plan uploaded
-static int flatten(pbd_engine *e) {
+// gathered, the plan uploaded.  restTables: plan what a derivation reads even while per-replica rest shapes are off (being switched on).
+static int flatten(pbd_engine *e, bool restTables = false) {
     if (!e->imageDirty) return 0;
     CKE(use(e));
     pbd_b200::Lap lap;
     CKE(colour_if_needed(e));
     drop_graph(e);
     std::vector<float4> x0;  // resident: rest positions by host index
-    if (pbd_b200::preferred_mode(e->mode, e->host, e->n, e->numConstraints, e->autoNoResident, e->K) == PBD_MODE_RESIDENT && e->n) {
+    if (pbd_b200::preferred_mode(e->mode, e->host, e->n, e->numConstraints, e->autoNoResident, e->batch.K) == PBD_MODE_RESIDENT && e->n) {
         std::vector<float4> raw(e->n);
         CK(cudaStreamSynchronize(e->stream));
         CK(cudaMemcpy(raw.data(), e->pos0.p, (size_t)e->n * sizeof(float4), cudaMemcpyDeviceToHost));
@@ -966,8 +963,8 @@ static int flatten(pbd_engine *e) {
         for (unsigned i = 0; i < e->n; i++) x0[i] = raw[e->slot[i]];
     }
     lap("colouring + rest positions");
-    pbd_b200::PlanInput in{e->host, e->numConstraints, e->n, e->nRb, &e->groupOff, &e->groupIds, e->mode, x0.data(), 0u, 0u, e->smCount, nullptr, e->autoNoResident, e->K};
-    in.restTables = e->K > 1 && (e->repGeo || e->restWanted);
+    pbd_b200::PlanInput in{e->host, e->numConstraints, e->n, e->nRb, &e->groupOff, &e->groupIds, e->mode, x0.data(), 0u, 0u, e->smCount, nullptr, e->autoNoResident, e->batch.K};
+    in.restTables = e->batch.K > 1 && (e->batch.restShapes || restTables);
     if (const char *g = getenv("PBD_B200_CLUSTERS")) {  // development knob "GxC"
         unsigned gg = 0, cc = 0;
         if (sscanf(g, "%ux%u", &gg, &cc) == 2 && gg >= 1 && cc >= 1 && cc <= (unsigned)kMaxClusterCtas && (cc & (cc - 1)) == 0) { in.forcedG = gg; in.forcedC = cc; }
@@ -998,12 +995,12 @@ static int flatten(pbd_engine *e) {
     }
     CK(cudaStreamSynchronize(e->stream));
     lap("relayout + upload");
-    if (e->repGeo) CKE(apply_replica_geometry(e, (const float4 *)e->restX.p, "pbd_set_replica_rest_positions (image planned again)"));  // the new image's geometry, from the rest positions the override was given
+    if (e->batch.restShapes) CKE(apply_replica_geometry(e, (const float4 *)e->batch.restX.p, "pbd_set_replica_rest_positions (image planned again)"));  // the new image's geometry, from the rest positions the override was given
 
     e->stats.num_constraints = e->numConstraints;  // per replica, like num_particles
     e->stats.num_groups = (unsigned)e->groupOff.size() - 1;
     e->stats.num_buckets = (unsigned)e->buckets.size();
-    e->restTables = in.restTables;
+    e->batch.restTables = in.restTables;
     e->imageDirty = false;
     return 0;
 }
@@ -1015,28 +1012,26 @@ extern "C" int pbd_set_replica_rest_positions(pbd_engine *e, const float *x0) {
     CKE(replica_params_refusal(e, "pbd_set_replica_rest_positions"));
     CKE(use(e));
     if (!x0) {
-        if (e->repGeo) { drop_replica_geometry(e); drop_graph(e); }
+        if (e->batch.restShapes) { drop_replica_geometry(e); drop_graph(e); }
         return 0;
     }
-    if (!e->restTables) e->imageDirty = true;  // planned again with the bodies the derivation reads
-    e->restWanted = true;
-    const int planned = flatten(e);  // the device order of the constraints the geometry is derived for
-    e->restWanted = false;
-    CKE(planned);
+    if (!e->batch.restTables) e->imageDirty = true;  // planned again with the bodies the derivation reads
+    CKE(flatten(e, true));  // the device order of the constraints the geometry is derived for
     for (int t = 0; t < PBD_BALLJOINT; t++)  // the resident kernel addresses replica r's geometry as i + r count in 32 bits
-        if ((unsigned long long)e->K * e->dev[t].count >= (1ull << 32))
-            return fail("pbd_set_replica_rest_positions: %u replicas of %u constraints of type %d exceed 2^32 geometry rows", e->K, e->dev[t].count, t);
+        if ((unsigned long long)e->batch.K * e->dev[t].count >= (1ull << 32))
+            return fail("pbd_set_replica_rest_positions: %u replicas of %u constraints of type %d exceed 2^32 geometry rows", e->batch.K, e->dev[t].count, t);
     if (e->n) {
-        CKE(e->restNew.alloc((size_t)e->K * e->n * sizeof(float4)));
-        CK(cudaMemcpyAsync(e->stage.p, x0, (size_t)e->K * e->n * 3 * sizeof(float), cudaMemcpyHostToDevice, e->stream));
-        k_pack_rest<<<replica_grid(e, e->K), 256, 0, e->stream>>>((const float *)e->stage.p, (const float4 *)e->pos.p, (float4 *)e->restNew.p, e->n, (const unsigned *)e->dSlot.p);
+        DevBuf rest;
+        CKE(rest.alloc((size_t)e->batch.K * e->n * sizeof(float4)));
+        CK(cudaMemcpyAsync(e->stage.p, x0, (size_t)e->batch.K * e->n * 3 * sizeof(float), cudaMemcpyHostToDevice, e->stream));
+        k_pack_rest<<<replica_grid(e, e->batch.K), 256, 0, e->stream>>>((const float *)e->stage.p, (const float4 *)e->pos.p, (float4 *)rest.p, e->n, (const unsigned *)e->dSlot.p);
         CK(cudaGetLastError());
-        CKE(apply_replica_geometry(e, (const float4 *)e->restNew.p, "pbd_set_replica_rest_positions"));
-        std::swap(e->restX.p, e->restNew.p); std::swap(e->restX.bytes, e->restNew.bytes);
-        CKE(upload3(e, x0, (float4 *)e->pos0.p, 1, e->K));  // PBD_ATTR_X0 of every replica
+        CKE(apply_replica_geometry(e, (const float4 *)rest.p, "pbd_set_replica_rest_positions"));
+        std::swap(e->batch.restX.p, rest.p); std::swap(e->batch.restX.bytes, rest.bytes);
+        CKE(upload3(e, x0, (float4 *)e->pos0.p, 1, e->batch.K));  // PBD_ATTR_X0 of every replica
         CK(cudaStreamSynchronize(e->stream));
     }
-    if (!e->repGeo) { e->repGeo = true; drop_graph(e); }
+    if (!e->batch.restShapes) { e->batch.restShapes = true; drop_graph(e); }
     return 0;
 }
 
@@ -1048,18 +1043,18 @@ extern "C" int pbd_get_replica_geometry(pbd_engine *e, int type, float *dst) {
     const int nGeo = num_geo(type), g0 = geo_first(type), np = type_shape(type).nParams;
     if (cnt == 0) return 0;
     const size_t one = (size_t)cnt * nGeo;
-    if (!e->repGeo) {  // the shared geometry, for every replica
+    if (!e->batch.restShapes) {  // the shared geometry, for every replica
         const TypeStore &h = e->host[type];
         for (size_t i = 0; i < cnt; i++)
             for (int j = 0; j < nGeo; j++) dst[i * nGeo + j] = h.params[i * np + g0 + j];
-        for (unsigned r = 1; r < e->K; r++) memcpy(dst + r * one, dst, one * sizeof(float));
+        for (unsigned r = 1; r < e->batch.K; r++) memcpy(dst + r * one, dst, one * sizeof(float));
         return 0;
     }
-    CKE(e->geoRows.alloc((size_t)e->K * one * sizeof(float)));
+    DevBuf rows;
+    CKE(rows.alloc((size_t)e->batch.K * one * sizeof(float)));
     unsigned long long bad = ~0ull;
-    CKE(derive_geometry(e, (const float4 *)e->restX.p, type, (float *)e->geoRows.p, &bad));
-    CK(cudaMemcpy(dst, e->geoRows.p, (size_t)e->K * one * sizeof(float), cudaMemcpyDeviceToHost));
-    e->geoRows.release();
+    CKE(derive_geometry(e, (const float4 *)e->batch.restX.p, nullptr, type, (float *)rows.p, &bad));
+    CK(cudaMemcpy(dst, rows.p, (size_t)e->batch.K * one * sizeof(float), cudaMemcpyDeviceToHost));
     return 0;
 }
 
@@ -1101,11 +1096,11 @@ template <class F> static int with_project_type(int type, int variant, F &&f) {
 // A batch's projection launches run replica blockIdx.y (the BATCH instantiations); their block size follows the whole batch's count.
 static int launch_bucket(pbd_engine *e, const Bucket &b, float h, int iterZero, cudaStream_t s, bool pdl) {
     const TypeArrays a = batch_arrays(e, b.type);
-    const unsigned block = project_block(e, b.count * e->K);
+    const unsigned block = project_block(e, b.count * e->batch.K);
     const ReplicaStrides rs{e->n, {e->dev[b.type].count}, {replica_mat(e, b.type)}, {replica_geo(e, b.type)}};
     return with_project_type(b.type, a.variant, [&](auto T, auto V) -> int {
         constexpr int TT = decltype(T)::value, VAR = decltype(V)::value;
-        if (e->K > 1) CK(launch_step_kernel(k_project<TT, VAR, true>, dim3(nblk(b.count, block), e->K), block, s, pdl, (float4 *)e->pos.p, a, b.first, b.count, h, iterZero, rs));
+        if (e->batch.K > 1) CK(launch_step_kernel(k_project<TT, VAR, true>, dim3(nblk(b.count, block), e->batch.K), block, s, pdl, (float4 *)e->pos.p, a, b.first, b.count, h, iterZero, rs));
         else CK(launch_step_kernel(k_project<TT, VAR, false>, nblk(b.count, block), block, s, pdl, (float4 *)e->pos.p, a, b.first, b.count, h, iterZero, rs));
         return 0;
     });
@@ -1134,7 +1129,7 @@ static int launch_colour(pbd_engine *e, size_t b0, size_t b1, float h, int iterZ
     constexpr unsigned kMergeMaxConstraints = 65536;
     unsigned colourTotal = 0;
     for (size_t i = b0; i < b1; i++) colourTotal += e->buckets[i].count;
-    colourTotal *= e->K;
+    colourTotal *= e->batch.K;
     if (b1 - b0 == 1 || log || colourTotal > kMergeMaxConstraints) {
         for (size_t i = b0; i < b1; i++) {
             CKE(launch_bucket(e, e->buckets[i], h, iterZero, s, !log));
@@ -1150,7 +1145,7 @@ static int launch_colour(pbd_engine *e, size_t b0, size_t b1, float h, int iterZ
         m.nSeg = (int)(c1 - c0);
         unsigned blocks = 0, total = 0;
         for (size_t i = c0; i < c1; i++) total += e->buckets[i].count;
-        const unsigned block = project_block(e, total * e->K);
+        const unsigned block = project_block(e, total * e->batch.K);
         for (size_t i = c0; i < c1; i++) {
             const Bucket &b = e->buckets[i];
             const int k = (int)(i - c0);
@@ -1160,7 +1155,7 @@ static int launch_colour(pbd_engine *e, size_t b0, size_t b1, float h, int iterZ
             blocks += nblk(b.count, block);
         }
         for (int k = m.nSeg; k <= kMultiSegments; k++) m.blockStart[k] = blocks;
-        if (e->K > 1) CK(launch_step_kernel(k_project_multi<true>, dim3(blocks, e->K), block, s, true, (float4 *)e->pos.p, m, h, iterZero, rs));
+        if (e->batch.K > 1) CK(launch_step_kernel(k_project_multi<true>, dim3(blocks, e->batch.K), block, s, true, (float4 *)e->pos.p, m, h, iterZero, rs));
         else CK(launch_step_kernel(k_project_multi<false>, blocks, block, s, true, (float4 *)e->pos.p, m, h, iterZero, rs));
         (*launches)++;
     }
@@ -1177,7 +1172,7 @@ static RbState rb_state(const pbd_engine *e) {
 static int enqueue_step_launches(pbd_engine *e, cudaStream_t s, unsigned long long *launches, LaunchLog *log = nullptr) {
     const float h = e->dt / (float)e->subSteps;  // TimeStepController.cpp:91
     const float invH = (float)(1.0 / (double)h);
-    const unsigned n = e->n * e->K;  // the particle updates run over every replica's slots at once
+    const unsigned n = e->n * e->batch.K;  // the particle updates run over every replica's slots at once
     const bool pdl = !log;
     const RbState rb = rb_state(e);
     unsigned long long L = 0;
@@ -1185,9 +1180,9 @@ static int enqueue_step_launches(pbd_engine *e, cudaStream_t s, unsigned long lo
     for (unsigned sub = 0; sub < e->subSteps; sub++) {
         if (e->nRb) { CK(launch_step_kernel(k_rb_integrate, nblk(e->nRb, 256), 256, s, pdl, rb, h, e->g[0], e->g[1], e->g[2])); CKE(launched(kLaunchIntegrate)); }
         if (n) {
-            if (e->repGravitySet)  // replica blockIdx.y under its own row
-                CK(launch_step_kernel(k_integrate<true>, replica_grid(e, e->K), 256, s, pdl, (float4 *)e->pos.p, (float4 *)e->vel.p, (float4 *)e->oldp.p, (float4 *)e->lastp.p, e->n, h, 0.0f, 0.0f, 0.0f,
-                                      (const float *)e->repGravity.p));
+            if (e->batch.gravitySet)  // replica blockIdx.y under its own row
+                CK(launch_step_kernel(k_integrate<true>, replica_grid(e, e->batch.K), 256, s, pdl, (float4 *)e->pos.p, (float4 *)e->vel.p, (float4 *)e->oldp.p, (float4 *)e->lastp.p, e->n, h, 0.0f, 0.0f, 0.0f,
+                                      (const float *)e->batch.gravity.p));
             else
                 CK(launch_step_kernel(k_integrate<false>, nblk(n, 256), 256, s, pdl, (float4 *)e->pos.p, (float4 *)e->vel.p, (float4 *)e->oldp.p, (float4 *)e->lastp.p, n, h, e->g[0], e->g[1], e->g[2],
                                       (const float *)nullptr));
@@ -1240,7 +1235,7 @@ static int enqueue_step_resident(pbd_engine *e, cudaStream_t s, unsigned long lo
     ra.rb = rb_state(e);
     for (int t = 0; t < PBD_NUM_TYPES; t++) { ra.types[t] = batch_arrays(e, t); ra.lamCount[t] = e->dev[t].count; ra.geoCount[t] = replica_geo(e, t); }
     ra.replicas = e->res.replicas; ra.replicaStride = e->n;
-    ra.repMat = (const float *)e->repMat.p; ra.repGravity = e->repGravitySet ? (const float *)e->repGravity.p : nullptr;
+    ra.repMat = (const float *)e->batch.mat.p; ra.repGravity = e->batch.gravitySet ? (const float *)e->batch.gravity.p : nullptr;
     *launches = 1;
     ra.trace = nullptr; ra.tracePhases = 0;
     static const char *tracePath = getenv("PBD_B200_TRACE");  // development aid: dump per-phase timelines of one step (tools/trace_resident.py)
@@ -1314,7 +1309,7 @@ static int enqueue_step_jacobi(pbd_engine *e, cudaStream_t s, unsigned long long
 // ------------------------------------------------------------------------------------------------------------
 extern "C" int pbd_set_colliders(pbd_engine *e, unsigned nP, const pbd_particle_collider *pc, unsigned nR, const pbd_rigid_collider *rc) {
     if (!e || (nP && !pc) || (nR && !rc)) return fail("pbd_set_colliders: null argument");
-    CKE(collider_refusal(e, e->K, (size_t)nP + nR));
+    CKE(collider_refusal(e, e->batch.K, (size_t)nP + nR));
     CKE(use(e));
     if (nR > (unsigned)kMaxRigidColliders) return fail("pbd_set_colliders: %u rigid colliders (the contact kernel keeps up to %d contacts per particle)", nR, kMaxRigidColliders);
     std::vector<ParticleCollider> P(nP);
@@ -1431,7 +1426,7 @@ extern "C" int pbd_step(pbd_engine *e, unsigned nSteps) {
         CKE(enqueue_contacts(e, e->stream, &L));
         e->stats.kernel_launches += L;
         e->stats.steps++;
-        e->stats.projections += (unsigned long long)e->numConstraints * e->subSteps * e->maxIter * e->K;
+        e->stats.projections += (unsigned long long)e->numConstraints * e->subSteps * e->maxIter * e->batch.K;
     }
     CK(cudaEventRecord(e->evStop, e->stream));
     e->timingPending = true;
@@ -1467,8 +1462,8 @@ extern "C" int pbd_step_host(pbd_engine *e, unsigned nSteps, const float *x_in, 
     if (!e) return fail("null engine");
     CKE(use(e));
     if (e->n == 0) return pbd_step(e, nSteps);
-    const size_t bytes = (size_t)e->K * e->n * 3 * sizeof(float);
-    const dim3 grid = replica_grid(e, e->K);
+    const size_t bytes = (size_t)e->batch.K * e->n * 3 * sizeof(float);
+    const dim3 grid = replica_grid(e, e->batch.K);
     // two staging areas so that x and v uploads do not serialise on a host sync
     CKE(e->stage.alloc(bytes));
     DevBuf &stage2 = e->stage2;
@@ -1502,8 +1497,8 @@ extern "C" int pbd_step_host_async(pbd_engine *e, unsigned nSteps, const float *
     if (!e) return fail("null engine");
     CKE(use(e));
     if (e->n == 0) return pbd_step(e, nSteps);
-    const size_t bytes = (size_t)e->K * e->n * 3 * sizeof(float);
-    const dim3 grid = replica_grid(e, e->K);
+    const size_t bytes = (size_t)e->batch.K * e->n * 3 * sizeof(float);
+    const dim3 grid = replica_grid(e, e->batch.K);
     auto &P = e->pipe;
     if (!P.ready) {
         CK(cudaStreamCreateWithFlags(&P.up, cudaStreamNonBlocking));
@@ -1565,7 +1560,7 @@ extern "C" int pbd_get_lambdas(pbd_engine *e, int type, float *dst, unsigned *id
     DevType &d = e->dev[type];
     if (d.count == 0) return 0;
     CK(cudaStreamSynchronize(e->stream));
-    CK(cudaMemcpy(dst, d.lambda.p, (size_t)e->K * d.count * sizeof(float), cudaMemcpyDeviceToHost));  // replica after replica
+    CK(cudaMemcpy(dst, d.lambda.p, (size_t)e->batch.K * d.count * sizeof(float), cudaMemcpyDeviceToHost));  // replica after replica
     if (ids) memcpy(ids, d.order.data(), (size_t)d.count * sizeof(unsigned));
     return 0;
 }
@@ -1577,7 +1572,7 @@ extern "C" int pbd_get_stats(pbd_engine *e, pbd_stats *out) {
     for (int t = 0; t < PBD_NUM_TYPES; t++) sweep += (double)e->dev[t].count * algorithmic_bytes(t, e->dev[t].arrays.variant);
     // per particle per substep: integrate 48 read + 64 write = 112, velocity update 32 read + 16 write = 48 (SURVEY.md 8d)
     const double perParticle = 112.0 + 48.0 + (e->velMethod ? 16.0 : 0.0);
-    e->stats.bytes_per_step = (sweep * e->maxIter + (double)e->n * perParticle) * e->subSteps * e->K;
+    e->stats.bytes_per_step = (sweep * e->maxIter + (double)e->n * perParticle) * e->subSteps * e->batch.K;
     *out = e->stats;
     return 0;
 }
@@ -1611,6 +1606,6 @@ extern "C" int pbd_profile_step(pbd_engine *e, float *msPerType, float *msIntegr
     if (msIntegrate) *msIntegrate = mi;
     if (msVelocity) *msVelocity = mv;
     e->stats.steps++;
-    e->stats.projections += (unsigned long long)e->numConstraints * e->subSteps * e->maxIter * e->K;
+    e->stats.projections += (unsigned long long)e->numConstraints * e->subSteps * e->maxIter * e->batch.K;
     return 0;
 }

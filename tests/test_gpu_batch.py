@@ -1,87 +1,14 @@
 """Replica batches on the GPU (pbd_set_replicas): replica r of a batch must advance bit for bit as an engine of its own started from
-replica r's state, in every mode, including the XPBD multipliers.  Each scene is built by tests/scenes.py on a HostModel and handed to
-_capi.Engine through add_flat / set_groups / set_particles, the batch and the single-scene engines alike."""
+replica r's state, in every mode, including the XPBD multipliers."""
 import numpy as np
 import pytest
 
 import scenes
+from batch_util import AUTO, GRAPH, JACOBI, MODES, RESIDENT, SCENES, engine, model, replica_state, run, set_state
 
 pytestmark = pytest.mark.gpu
 
-GRAPH, RESIDENT, LAUNCH, JACOBI, AUTO = 0, 1, 2, 3, 4
-XPBD_TYPES = (1, 4, 8, 10)
-
-SCENES = {  # name: (builder, dt, sub_steps, max_iter)
-    "cfg1": (lambda m: scenes.cfg1(m), 0.005, 1, 5),
-    "xpbd_cloth64": (lambda m: scenes.cloth(m, 64, 64, cloth_method=4, bending_method=3, dist_k=1.0e5, bend_k=100.0, sub_steps=1, max_iter=5), 0.005, 1, 5),
-    "fem_volume_bar": (lambda m: scenes.bar(m, 9, 4, 4, solid_method=2, k=1.0e5, extra_volume=True, sub_steps=2, max_iter=3), 0.005, 2, 3),
-    "mixed": (lambda m: scenes.mixed(m), 0.005, 5, 1),
-    # the light-mask resident kernels (FEMTriangle + Dihedral + IsometricBending_XPBD) and the all-types ones (StrainTriangle)
-    "femtri_dihedral_cloth": (lambda m: (scenes.cloth(m, 40, 40, cloth_method=2, bending_method=1, sub_steps=2, max_iter=3),
-                                         m.add_bending_constraints(0, 3, 100.0)), 0.005, 2, 3),
-    "strain_cloth": (lambda m: scenes.cloth(m, 40, 40, cloth_method=3, bending_method=3, bend_k=100.0, sub_steps=2, max_iter=3), 0.005, 2, 3),
-}
-_models = {}
 _solo = {}
-
-
-def model(name):
-    if name not in _models:
-        from positionbaseddynamics_b200.model import HostModel
-        build, dt, sub, it = SCENES[name]
-        hm = HostModel()
-        build(hm)
-        hm.init_groups()
-        types, bodies, params, _ = hm.constraints()
-        off, ids = hm.groups()
-        mass, _ = hm.masses()
-        _models[name] = dict(types=types, bodies=bodies, params=params, off=off, ids=ids, x=np.asarray(hm.get("x"), np.float32).copy(),
-                             x0=np.asarray(hm.get("x0"), np.float32).copy(), mass=np.asarray(mass, np.float32).copy(), dt=dt, sub=sub, it=it)
-        hm.close()
-    return _models[name]
-
-
-def replica_state(m, r):
-    """Replica r's own seeded perturbation of x and v; replica 1 also pins every 7th particle through its masses."""
-    rng = np.random.default_rng(1000 + r)
-    scale = float(np.ptp(m["x"], axis=0).max())
-    x = (m["x"] + rng.normal(0.0, 0.01 * scale, m["x"].shape)).astype(np.float32)
-    v = rng.normal(0.0, 0.1, m["x"].shape).astype(np.float32)
-    mass = m["mass"].copy()
-    if r == 1:
-        mass[::7] = 0.0
-    return x, v, mass
-
-
-def engine(m, mode, replicas=None):
-    from positionbaseddynamics_b200 import _capi
-    eng = _capi.Engine(0)
-    eng.set_particles(m["x"], m["mass"], x0=m["x0"])
-    eng.add_flat(m["types"], m["bodies"], m["params"])
-    eng.set_groups(m["off"], m["ids"])
-    eng.set_params(dt=m["dt"], sub_steps=m["sub"], max_iter=m["it"])
-    eng.set_mode(mode)
-    if replicas is not None:
-        eng.set_replicas(replicas)
-    return eng
-
-
-def run(eng, m):
-    """The step sequence every engine of these tests runs: steps, then other subSteps / maxIter / velocity method, then an edit of the
-    velocities with set_attr, then a last step.  Returns x, v and the multipliers of every XPBD type present."""
-    from positionbaseddynamics_b200 import _capi
-    eng.step(2)
-    eng.set_params(dt=m["dt"], sub_steps=m["sub"] + 1, max_iter=m["it"] + 1, vel_method=1)
-    eng.step(2)
-    eng.set_attr(_capi.ATTR_V, eng.get_attr(_capi.ATTR_V) * np.float32(0.5))
-    eng.step(1)
-    eng.sync()
-    lam = {}
-    for t in XPBD_TYPES:
-        if (m["types"] == t).any():
-            l, ids = eng.lambdas(t)
-            lam[t] = l[..., np.argsort(ids)].copy()  # by insertion id: the resident image orders a colour's constraints by tile
-    return eng.get_attr(_capi.ATTR_X).copy(), eng.get_attr(_capi.ATTR_V).copy(), lam
 
 
 def solo(name, r):
@@ -97,7 +24,7 @@ def solo(name, r):
     return _solo[(name, r)]
 
 
-@pytest.mark.parametrize("mode", [GRAPH, LAUNCH, RESIDENT, AUTO], ids=["graph", "launch", "resident", "auto"])
+@MODES
 @pytest.mark.parametrize("k", [1, 3, 300])
 @pytest.mark.parametrize("name", sorted(SCENES))
 def test_batch_equals_solo_runs(name, k, mode):
@@ -108,9 +35,7 @@ def test_batch_equals_solo_runs(name, k, mode):
     states = [replica_state(m, r) for r in range(k)]
     eng = engine(m, mode, replicas=k)
     assert eng.replicas() == k
-    eng.set_attr(_capi.ATTR_X, np.stack([s[0] for s in states]))
-    eng.set_attr(_capi.ATTR_V, np.stack([s[1] for s in states]))
-    eng.set_masses(np.stack([s[2] for s in states]))
+    set_state(eng, states)
     x, v, lam = run(eng, m)
     st = eng.stats()
     eng.close()

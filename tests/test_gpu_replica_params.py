@@ -1,67 +1,24 @@
 """Per-replica material parameters and gravity of a batch (pbd_set_replica_materials / pbd_set_replica_gravity): replica r must advance
 bit for bit as a single-scene engine whose constraints were added with replica r's row and whose gravity is replica r's vector, in every
-mode.  The scenes are those of test_gpu_batch.py: between them they run all six resident type masks and every type with more than one
+mode.  The scenes are the batch scenes of batch_util.py: between them they run all six resident type masks and every type with more than one
 material parameter."""
 import numpy as np
 import pytest
 
-import scenes
+from batch_util import DEFAULT_G, GRAPH, MODES, RESIDENT, SCENES, engine, model, replica_state, results, run, set_state
 
 pytestmark = pytest.mark.gpu
 
-GRAPH, RESIDENT, LAUNCH, JACOBI, AUTO = 0, 1, 2, 3, 4
-MODES = pytest.mark.parametrize("mode", [GRAPH, LAUNCH, RESIDENT, AUTO], ids=["graph", "launch", "resident", "auto"])
-XPBD_TYPES = (1, 4, 8, 10)
-DEFAULT_G = (0.0, -9.81, 0.0)
 # include/pbd_b200.h: the material columns of every type's parameter layout, and what each is: s = stiffness / modulus, n = Poisson
 # ratio, f = flag
 MAT = {0: ([1], "s"), 1: ([1], "s"), 2: ([1], "s"), 3: ([0], "s"), 4: ([0], "s"), 5: ([5, 6, 7, 8, 9], "sssnn"), 6: ([4, 5, 6, 7, 8], "sssff"),
        7: ([1], "s"), 8: ([1], "s"), 9: ([10, 11], "sn"), 10: ([10, 11], "sn"), 11: ([9, 10, 11, 12], "ssff"), 12: ([0], "s")}
 
-SCENES = {  # name: (builder, dt, sub_steps, max_iter)
-    "cfg1": (lambda m: scenes.cfg1(m), 0.005, 1, 5),
-    "xpbd_cloth64": (lambda m: scenes.cloth(m, 64, 64, cloth_method=4, bending_method=3, dist_k=1.0e5, bend_k=100.0, sub_steps=1, max_iter=5), 0.005, 1, 5),
-    "fem_volume_bar": (lambda m: scenes.bar(m, 9, 4, 4, solid_method=2, k=1.0e5, extra_volume=True, sub_steps=2, max_iter=3), 0.005, 2, 3),
-    "mixed": (lambda m: scenes.mixed(m), 0.005, 5, 1),
-    "femtri_dihedral_cloth": (lambda m: (scenes.cloth(m, 40, 40, cloth_method=2, bending_method=1, sub_steps=2, max_iter=3),
-                                         m.add_bending_constraints(0, 3, 100.0)), 0.005, 2, 3),
-    "strain_cloth": (lambda m: scenes.cloth(m, 40, 40, cloth_method=3, bending_method=3, bend_k=100.0, sub_steps=2, max_iter=3), 0.005, 2, 3),
-}
-_models = {}
 _solo = {}
-
-
-def model(name):
-    if name not in _models:
-        from positionbaseddynamics_b200.model import HostModel
-        build, dt, sub, it = SCENES[name]
-        hm = HostModel()
-        build(hm)
-        hm.init_groups()
-        types, bodies, params, _ = hm.constraints()
-        off, ids = hm.groups()
-        mass, _ = hm.masses()
-        _models[name] = dict(types=np.asarray(types).copy(), bodies=np.asarray(bodies).copy(), params=np.asarray(params, np.float32).copy(), off=off, ids=ids,
-                             x=np.asarray(hm.get("x"), np.float32).copy(), x0=np.asarray(hm.get("x0"), np.float32).copy(),
-                             mass=np.asarray(mass, np.float32).copy(), dt=dt, sub=sub, it=it)
-        hm.close()
-    return _models[name]
 
 
 def present(m):
     return [t for t in sorted(MAT) if (m["types"] == t).any()]
-
-
-def replica_state(m, r):
-    """Replica r's own seeded perturbation of x and v; replica 1 also pins every 7th particle through its masses."""
-    rng = np.random.default_rng(1000 + r)
-    scale = float(np.ptp(m["x"], axis=0).max())
-    x = (m["x"] + rng.normal(0.0, 0.01 * scale, m["x"].shape)).astype(np.float32)
-    v = rng.normal(0.0, 0.1, m["x"].shape).astype(np.float32)
-    mass = m["mass"].copy()
-    if r == 1:
-        mass[::7] = 0.0
-    return x, v, mass
 
 
 def material_row(m, t, r, zero=False):
@@ -91,49 +48,6 @@ def with_materials(m, rows):
         sel = np.nonzero(m["types"] == t)[0]
         params[np.ix_(sel, MAT[t][0])] = row
     return dict(m, params=params)
-
-
-def engine(m, mode, replicas=None, gravity=DEFAULT_G):
-    from positionbaseddynamics_b200 import _capi
-    eng = _capi.Engine(0)
-    eng.set_particles(m["x"], m["mass"], x0=m["x0"])
-    eng.add_flat(m["types"], m["bodies"], m["params"])
-    eng.set_groups(m["off"], m["ids"])
-    eng.set_params(dt=m["dt"], sub_steps=m["sub"], max_iter=m["it"], gravity=gravity)
-    eng.set_mode(mode)
-    if replicas is not None:
-        eng.set_replicas(replicas)
-    return eng
-
-
-def results(eng, m):
-    from positionbaseddynamics_b200 import _capi
-    eng.sync()
-    lam = {}
-    for t in XPBD_TYPES:
-        if (m["types"] == t).any():
-            l, ids = eng.lambdas(t)
-            lam[t] = l[..., np.argsort(ids)].copy()  # by insertion id: the resident image orders a colour's constraints by tile
-    return eng.get_attr(_capi.ATTR_X).copy(), eng.get_attr(_capi.ATTR_V).copy(), lam
-
-
-def run(eng, m, gravity=DEFAULT_G):
-    """The step sequence of test_gpu_batch.py: steps, then other subSteps / maxIter / velocity method, then an edit of the velocities
-    with set_attr, then a last step.  `gravity` is what set_params carries: a batch's per-replica rows must outlive that call."""
-    from positionbaseddynamics_b200 import _capi
-    eng.step(2)
-    eng.set_params(dt=m["dt"], sub_steps=m["sub"] + 1, max_iter=m["it"] + 1, vel_method=1, gravity=gravity)
-    eng.step(2)
-    eng.set_attr(_capi.ATTR_V, eng.get_attr(_capi.ATTR_V) * np.float32(0.5))
-    eng.step(1)
-    return results(eng, m)
-
-
-def set_state(eng, states):
-    from positionbaseddynamics_b200 import _capi
-    eng.set_attr(_capi.ATTR_X, np.stack([s[0] for s in states]))
-    eng.set_attr(_capi.ATTR_V, np.stack([s[1] for s in states]))
-    eng.set_masses(np.stack([s[2] for s in states]))
 
 
 def solo(name, r, zero, own_gravity):

@@ -1,37 +1,27 @@
 """Per-replica rest shapes of a batch (pbd_set_replica_rest_positions / pbd_get_replica_geometry): the geometry every replica's constraints
 are stepped with is derived on the GPU from that replica's own rest positions, as the host mirror's add*Constraint derives it, and replica r
-then advances bit for bit as a single-scene engine whose constraints carry that geometry.  The scenes are the six of
-test_gpu_replica_params.py (all six resident type masks) and small tet bars with the solid methods those lack (FEMTet_XPBD, StrainTet,
+then advances bit for bit as a single-scene engine whose constraints carry that geometry.  The scenes are the six batch
+scenes of batch_util.py (all six resident type masks) and small tet bars with the solid methods those lack (FEMTet_XPBD, StrainTet,
 ShapeMatching, Distance_XPBD + Volume_XPBD), so that every particle constraint type is derived."""
 import numpy as np
 import pytest
 
+import batch_util
 import scenes
+from batch_util import GRAPH, LAUNCH, MODES, RESIDENT, engine, replica_state, results, run, set_state
 
 pytestmark = pytest.mark.gpu
 
-GRAPH, RESIDENT, LAUNCH, JACOBI, AUTO = 0, 1, 2, 3, 4
-MODES = pytest.mark.parametrize("mode", [GRAPH, LAUNCH, RESIDENT, AUTO], ids=["graph", "launch", "resident", "auto"])
-XPBD_TYPES = (1, 4, 8, 10)
-DEFAULT_G = (0.0, -9.81, 0.0)
 PARTICLE_TYPES = range(13)
 DIHEDRAL = 2
 GEO_FIRST = {3: 1, 4: 1, 12: 1}  # the geometry columns start behind the stiffness for these types, at column 0 for the others
 
-SCENES = {  # name: (builder, dt, sub_steps, max_iter)
-    "cfg1": (lambda m: scenes.cfg1(m), 0.005, 1, 5),
-    "xpbd_cloth64": (lambda m: scenes.cloth(m, 64, 64, cloth_method=4, bending_method=3, dist_k=1.0e5, bend_k=100.0, sub_steps=1, max_iter=5), 0.005, 1, 5),
-    "fem_volume_bar": (lambda m: scenes.bar(m, 9, 4, 4, solid_method=2, k=1.0e5, extra_volume=True, sub_steps=2, max_iter=3), 0.005, 2, 3),
-    "mixed": (lambda m: scenes.mixed(m), 0.005, 5, 1),
-    "femtri_dihedral_cloth": (lambda m: (scenes.cloth(m, 40, 40, cloth_method=2, bending_method=1, sub_steps=2, max_iter=3),
-                                         m.add_bending_constraints(0, 3, 100.0)), 0.005, 2, 3),
-    "strain_cloth": (lambda m: scenes.cloth(m, 40, 40, cloth_method=3, bending_method=3, bend_k=100.0, sub_steps=2, max_iter=3), 0.005, 2, 3),
+SCENES = {**batch_util.SCENES,  # name: (builder, dt, sub_steps, max_iter)
     "femtet_xpbd_bar": (lambda m: scenes.bar(m, 8, 3, 3, solid_method=3, k=1.0e5, sub_steps=2, max_iter=3), 0.005, 2, 3),
     "straintet_bar": (lambda m: scenes.bar(m, 8, 3, 3, solid_method=4, k=1.0, sub_steps=2, max_iter=3), 0.005, 2, 3),
     "shapematching_bar": (lambda m: scenes.bar(m, 8, 3, 3, solid_method=5, k=1.0, sub_steps=2, max_iter=3), 0.005, 2, 3),
     "xpbd_distance_volume_bar": (lambda m: scenes.bar(m, 8, 3, 3, solid_method=6, k=1.0e4, vol_k=1.0e4, sub_steps=2, max_iter=3), 0.005, 2, 3),
 }
-_models = {}
 
 
 class _Shaped:
@@ -60,20 +50,7 @@ class _Shaped:
 
 
 def model(name):
-    if name not in _models:
-        from positionbaseddynamics_b200.model import HostModel
-        build, dt, sub, it = SCENES[name]
-        hm = HostModel()
-        build(hm)
-        hm.init_groups()
-        types, bodies, params, _ = hm.constraints()
-        off, ids = hm.groups()
-        mass, _ = hm.masses()
-        _models[name] = dict(types=np.asarray(types).copy(), bodies=np.asarray(bodies).copy(), params=np.asarray(params, np.float32).copy(), off=off, ids=ids,
-                             x=np.asarray(hm.get("x"), np.float32).copy(), x0=np.asarray(hm.get("x0"), np.float32).copy(),
-                             mass=np.asarray(mass, np.float32).copy(), dt=dt, sub=sub, it=it, name=name)
-        hm.close()
-    return _models[name]
+    return batch_util.model(name, SCENES)
 
 
 def present(m):
@@ -106,18 +83,6 @@ def rest_shape(m, r, scale=None):
     return (c + ((x0 - c) * s) @ R.T + rng.normal(0.0, 0.01 * edge, x0.shape)).astype(np.float32)
 
 
-def replica_state(m, r):
-    """Replica r's own perturbed x and v; replica 1 also pins every 7th particle through its masses."""
-    rng = np.random.default_rng(1000 + r)
-    scale = float(np.ptp(m["x"], axis=0).max())
-    x = (m["x"] + rng.normal(0.0, 0.01 * scale, m["x"].shape)).astype(np.float32)
-    v = rng.normal(0.0, 0.1, m["x"].shape).astype(np.float32)
-    mass = m["mass"].copy()
-    if r == 1:
-        mass[::7] = 0.0
-    return x, v, mass
-
-
 def host_geometry(m, x0, mass):
     """{type: (count, nGeo)} the host mirror's geometry of the model built on these rest positions and masses."""
     from positionbaseddynamics_b200.model import HostModel
@@ -136,47 +101,6 @@ def with_geometry(m, geo):
         sel = np.nonzero(m["types"] == t)[0]
         params[np.ix_(sel, geo_cols(t))] = rows
     return dict(m, params=params)
-
-
-def engine(m, mode, replicas=None, gravity=DEFAULT_G):
-    from positionbaseddynamics_b200 import _capi
-    eng = _capi.Engine(0)
-    eng.set_particles(m["x"], m["mass"], x0=m["x0"])
-    eng.add_flat(m["types"], m["bodies"], m["params"])
-    eng.set_groups(m["off"], m["ids"])
-    eng.set_params(dt=m["dt"], sub_steps=m["sub"], max_iter=m["it"], gravity=gravity)
-    eng.set_mode(mode)
-    if replicas is not None:
-        eng.set_replicas(replicas)
-    return eng
-
-
-def results(eng, m):
-    from positionbaseddynamics_b200 import _capi
-    eng.sync()
-    lam = {}
-    for t in XPBD_TYPES:
-        if (m["types"] == t).any():
-            l, ids = eng.lambdas(t)
-            lam[t] = l[..., np.argsort(ids)].copy()
-    return eng.get_attr(_capi.ATTR_X).copy(), eng.get_attr(_capi.ATTR_V).copy(), lam
-
-
-def run(eng, m):
-    from positionbaseddynamics_b200 import _capi
-    eng.step(2)
-    eng.set_params(dt=m["dt"], sub_steps=m["sub"] + 1, max_iter=m["it"] + 1, vel_method=1)
-    eng.step(2)
-    eng.set_attr(_capi.ATTR_V, eng.get_attr(_capi.ATTR_V) * np.float32(0.5))
-    eng.step(1)
-    return results(eng, m)
-
-
-def set_state(eng, states):
-    from positionbaseddynamics_b200 import _capi
-    eng.set_attr(_capi.ATTR_X, np.stack([s[0] for s in states]))
-    eng.set_attr(_capi.ATTR_V, np.stack([s[1] for s in states]))
-    eng.set_masses(np.stack([s[2] for s in states]))
 
 
 def ulps(a, b):

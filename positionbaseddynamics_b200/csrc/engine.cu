@@ -88,8 +88,7 @@ struct pbd_engine {
     DevBuf pos, vel, oldp, lastp, pos0, stage, stage2, massStage, jacobiDelta;
     // A replica batch and what its replicas have of their own (batch_arrays, replica_mat and replica_geo turn it into what the kernels see).
     // mat [K][kMatRowFloats]: the uniform material parameters of every type, replica by replica -- the shared ones of the image, or a
-    // replica's own (pbd_set_replica_materials, the types of matMask); gravity [K][3] (pbd_set_replica_gravity).  Both keep their address
-    // until K changes, so that a captured graph keeps reading the same tables.
+    // replica's own (pbd_set_replica_materials, the types of matMask); gravity [K][3] (pbd_set_replica_gravity).
     // restX: per-replica rest shapes (pbd_set_replica_rest_positions), the rest positions the call was given, K x n float4 by host index
     // with .w = the inverse mass at the time of the call; every image planned while restShapes is on derives its geometry from them.
     // restTables: the current image carries what a derivation reads (TypePlan::restBodies / restLocal), planned only while the override
@@ -111,15 +110,15 @@ struct pbd_engine {
     DevType dev[PBD_NUM_TYPES];
     std::vector<Bucket> buckets;
     DevBuf dBuckets, dTrace;
-    bool imageDirty = true;
+    bool imageDirty = true; unsigned long long imageGen = 0;  // imageGen: images planned so far
     // parameters
     float dt = 0.005f; unsigned subSteps = 5, maxIter = 1; int velMethod = 0; float g[3] = {0.f, -9.81f, 0.f};
     int mode = PBD_MODE_AUTO;             // requested (pbd_set_mode)
     int active = PBD_MODE_GRAPH;          // what the current image runs in: == mode, or the resolution of PBD_MODE_AUTO (image_plan.h)
     bool autoNoResident = false;          // PBD_MODE_AUTO: the resident mode was tried for this model and refused
-    // graph cache
+    // graph cache: the captured step and the graph_key it was captured under
     cudaGraphExec_t graphExec = nullptr;
-    bool graphValid = false;
+    std::vector<unsigned char> graphKey;
     unsigned long long graphLaunches = 0;  // kernel nodes of the captured step
     // stats
     pbd_stats stats{};
@@ -150,7 +149,6 @@ struct pbd_engine {
 
 static int use(pbd_engine *e) { CK(cudaSetDevice(e->device)); return 0; }
 
-// per-replica rest shapes off (the caller drops the graph where the kernel arguments change)
 static void drop_replica_geometry(pbd_engine *e) {
     e->batch.restShapes = false;
     e->batch.restX.release();
@@ -196,16 +194,11 @@ extern "C" int pbd_create(int device, void *stream, pbd_engine **out) {
     return 0;
 }
 
-static void drop_graph(pbd_engine *e) {
-    if (e->graphExec) { cudaGraphExecDestroy(e->graphExec); e->graphExec = nullptr; }
-    e->graphValid = false;
-}
-
 extern "C" int pbd_destroy(pbd_engine *e) {
     if (!e) return 0;
     cudaSetDevice(e->device);
     cudaStreamSynchronize(e->stream);
-    drop_graph(e);
+    if (e->graphExec) cudaGraphExecDestroy(e->graphExec);
     if (e->evStart) cudaEventDestroy(e->evStart);
     if (e->evStop) cudaEventDestroy(e->evStop);
     if (e->pipe.ready) {
@@ -301,15 +294,13 @@ extern "C" int pbd_set_particles(pbd_engine *e, unsigned n, const float *x, cons
     if (!why.empty()) return fail("pbd_set_particles: %s", why.c_str());
     CKE(use(e));
     CK(cudaStreamSynchronize(e->stream));
-    if (n != e->n) { e->imageDirty = true; drop_graph(e); }
-    e->n = n;
+    e->n = n; e->imageDirty = true;
     const size_t b4 = (size_t)n * sizeof(float4);
     for (auto *b : {&e->pos, &e->vel, &e->oldp, &e->lastp, &e->pos0}) CKE(b->alloc(b4 * e->batch.K));
     CKE(e->stage.alloc((size_t)e->batch.K * n * 3 * sizeof(float)));
     CKE(e->massStage.alloc((size_t)e->batch.K * n * sizeof(float)));
-    drop_graph(e);  // buffers may have moved
     drop_replica_geometry(e);  // every replica's state is redefined
-    e->slot.resize(n); e->imageDirty = true;
+    e->slot.resize(n);
     for (unsigned i = 0; i < n; i++) e->slot[i] = particle_slot(i, n);
     if (n == 0) return 0;
     CKE(upload_slot_map(e));
@@ -341,7 +332,6 @@ extern "C" int pbd_set_replicas(pbd_engine *e, unsigned K) {
     CKE(collider_refusal(e, K, e->pColliders.size() + e->rColliders.size()));
     CKE(use(e));
     CK(cudaStreamSynchronize(e->stream));
-    drop_graph(e);
     const size_t one = (size_t)e->n * sizeof(float4);
     if (e->n)
         for (DevBuf *b : {&e->pos, &e->vel, &e->oldp, &e->lastp, &e->pos0}) {  // replica 0 kept, the others copies of it
@@ -384,8 +374,6 @@ static int write_replica_materials(pbd_engine *e, int type, const float *rows, s
     CK(cudaMemcpy2DAsync((float *)e->batch.mat.p + mat_offset(type), kMatRowFloats * sizeof(float), rows, pitch, width, e->batch.K, cudaMemcpyHostToDevice, e->stream));
     return 0;
 }
-// The rows are copied in stream order into tables that keep their address: a captured graph reads the new values at its next launch.
-// Only switching an override on or off changes kernel arguments, and so drops the graph.
 extern "C" int pbd_set_replica_materials(pbd_engine *e, int type, const float *mat) {
     if (type < 0 || type >= PBD_NUM_TYPES) return fail("pbd_set_replica_materials: unknown constraint type %d", type);
     const int nMat = type_shape(type).nMat;
@@ -395,8 +383,7 @@ extern "C" int pbd_set_replica_materials(pbd_engine *e, int type, const float *m
     const unsigned bit = 1u << type;
     if (mat) CKE(write_replica_materials(e, type, mat, nMat * sizeof(float)));
     else if ((e->batch.matMask & bit) && !e->imageDirty) CKE(write_replica_materials(e, type, e->dev[type].arrays.matU, 0));  // (a dirty image writes them when it is planned)
-    // (on or off decides whether the per-constraint material arrays of the type count: batch_arrays)
-    if (((e->batch.matMask & bit) != 0u) != (mat != nullptr)) { e->batch.matMask ^= bit; drop_graph(e); }
+    if (mat) e->batch.matMask |= bit; else e->batch.matMask &= ~bit;
     return 0;
 }
 extern "C" int pbd_set_replica_gravity(pbd_engine *e, const float *g) {
@@ -406,7 +393,7 @@ extern "C" int pbd_set_replica_gravity(pbd_engine *e, const float *g) {
         CKE(e->batch.gravity.alloc((size_t)e->batch.K * 3 * sizeof(float)));
         CK(cudaMemcpyAsync(e->batch.gravity.p, g, (size_t)e->batch.K * 3 * sizeof(float), cudaMemcpyHostToDevice, e->stream));
     }
-    if (e->batch.gravitySet != (g != nullptr)) { e->batch.gravitySet = (g != nullptr); drop_graph(e); }
+    e->batch.gravitySet = (g != nullptr);
     return 0;
 }
 // What a batch's per-bucket kernels get for type t: where the replicas have parameters of their own, its place in replica 0's row of the
@@ -466,7 +453,6 @@ extern "C" int pbd_set_rigid_bodies(pbd_engine *e, unsigned n, const float *mass
     CKE(use(e));
     CK(cudaStreamSynchronize(e->stream));
     if (n != e->nRb) { e->imageDirty = true; e->groupsSet = e->groupsSet && n == e->nRb; }
-    drop_graph(e);
     e->nRb = n;
     e->rbMass.assign(mass, mass + n);
     if (n == 0) return 0;
@@ -768,12 +754,8 @@ extern "C" int pbd_set_params(pbd_engine *e, float dt, unsigned subSteps, unsign
     if (maxIter < 1) return fail("maxIterations must be >= 1 (TimeStepController.cpp:55)");
     if (velMethod != 0 && velMethod != 1) return fail("velocityUpdateMethod must be 0 or 1");
     if (!(dt > 0.0f)) return fail("time step size must be positive");
-    const bool same = e->dt == dt && e->subSteps == subSteps && e->maxIter == maxIter && e->velMethod == velMethod &&
-                      (!gravity || (e->g[0] == gravity[0] && e->g[1] == gravity[1] && e->g[2] == gravity[2]));
-    if (same) return 0;  // callers such as a TimeStep adapter set the parameters before every step: keep the captured graph
     e->dt = dt; e->subSteps = subSteps; e->maxIter = maxIter; e->velMethod = velMethod;
     if (gravity) { e->g[0] = gravity[0]; e->g[1] = gravity[1]; e->g[2] = gravity[2]; }
-    drop_graph(e);
     return 0;
 }
 extern "C" int pbd_set_mode(pbd_engine *e, int mode) {
@@ -786,7 +768,6 @@ extern "C" int pbd_set_mode(pbd_engine *e, int mode) {
     const int active = pbd_b200::preferred_mode(mode, e->host, e->n, e->numConstraints, false, e->batch.K);
     if ((active == PBD_MODE_RESIDENT) != (e->active == PBD_MODE_RESIDENT)) e->imageDirty = true;
     e->mode = mode; e->active = active; e->autoNoResident = false;
-    drop_graph(e);
     return 0;
 }
 extern "C" int pbd_get_mode(pbd_engine *e, int *requested, int *active) {
@@ -919,8 +900,7 @@ static int derive_geometry(pbd_engine *e, const float4 *rest, GeoBufs *fresh, in
 }
 // The geometry derived from `rest` becomes what the projections read -- only when no constraint refuses it: otherwise the error names the
 // first replica and constraint, and nothing has changed.  It is copied into the live arrays in stream order, so that they keep their
-// address and a captured graph reads the new geometry at its next launch.  The scratch arrays are as large as the live ones: they are
-// freed on return.
+// address and the captured graph stays valid.  The scratch arrays are as large as the live ones: they are freed on return.
 static int apply_replica_geometry(pbd_engine *e, const float4 *rest, const char *what) {
     unsigned long long bad = ~0ull;
     GeoBufs fresh[PBD_BALLJOINT];
@@ -953,7 +933,7 @@ static int flatten(pbd_engine *e, bool restTables = false) {
     CKE(use(e));
     pbd_b200::Lap lap;
     CKE(colour_if_needed(e));
-    drop_graph(e);
+    e->imageGen++;
     std::vector<float4> x0;  // resident: rest positions by host index
     if (pbd_b200::preferred_mode(e->mode, e->host, e->n, e->numConstraints, e->autoNoResident, e->batch.K) == PBD_MODE_RESIDENT && e->n) {
         std::vector<float4> raw(e->n);
@@ -1006,15 +986,11 @@ static int flatten(pbd_engine *e, bool restTables = false) {
 }
 
 // The rest positions go to a buffer of their own (and PBD_ATTR_X0) only after the geometry derived from them has been accepted; the engine
-// keeps them, so that an image planned again (constraints added, another mode) derives its geometry from them too.  Only switching the
-// override on or off changes kernel arguments and so drops the graph.
+// keeps them, so that an image planned again (constraints added, another mode) derives its geometry from them too.
 extern "C" int pbd_set_replica_rest_positions(pbd_engine *e, const float *x0) {
     CKE(replica_params_refusal(e, "pbd_set_replica_rest_positions"));
     CKE(use(e));
-    if (!x0) {
-        if (e->batch.restShapes) { drop_replica_geometry(e); drop_graph(e); }
-        return 0;
-    }
+    if (!x0) { drop_replica_geometry(e); return 0; }
     if (!e->batch.restTables) e->imageDirty = true;  // planned again with the bodies the derivation reads
     CKE(flatten(e, true));  // the device order of the constraints the geometry is derived for
     for (int t = 0; t < PBD_BALLJOINT; t++)  // the resident kernel addresses replica r's geometry as i + r count in 32 bits
@@ -1031,7 +1007,7 @@ extern "C" int pbd_set_replica_rest_positions(pbd_engine *e, const float *x0) {
         CKE(upload3(e, x0, (float4 *)e->pos0.p, 1, e->batch.K));  // PBD_ATTR_X0 of every replica
         CK(cudaStreamSynchronize(e->stream));
     }
-    if (!e->batch.restShapes) { e->batch.restShapes = true; drop_graph(e); }
+    e->batch.restShapes = true;
     return 0;
 }
 
@@ -1395,8 +1371,31 @@ static int enqueue_contacts(pbd_engine *e, cudaStream_t s, unsigned long long *l
     return 0;
 }
 
+template <class... V> static void append_bytes(std::vector<unsigned char> &key, const V &...v) {
+    static_assert((std::is_scalar_v<std::remove_all_extents_t<V>> && ...), "padding bytes would make equal states compare unequal");
+    size_t at = key.size();
+    key.resize(at + (sizeof(V) + ...));
+    ((std::memcpy(&key[at], &v, sizeof(V)), at += sizeof(V)), ...);
+}
+// Everything enqueue_step_launches reads, which a captured step bakes in, as the bytes of scalars and arrays of them (no padding).
+// imageGen stands for the bucket table.  The structured bindings do not compile once RbState or TypeArrays gains a member not listed here.
+static std::vector<unsigned char> graph_key(const pbd_engine *e) {
+    std::vector<unsigned char> key;
+    key.reserve(4096);
+    const auto [X, Q, V, W, oldX, lastX, oldQ, lastQ, I, Iinv, nRb] = rb_state(e);
+    append_bytes(key, e->imageGen, e->n, e->batch.K, e->dt, e->subSteps, e->maxIter, e->velMethod, e->g, e->pos.p, e->vel.p, e->oldp.p, e->lastp.p,
+                 e->batch.gravitySet ? e->batch.gravity.p : nullptr, X, Q, V, W, oldX, lastX, oldQ, lastQ, I, Iinv, nRb);
+    for (int t = 0; t < PBD_NUM_TYPES; t++) {
+        const auto [idx2, idx4, idx3, gv, gs, mat, matU, lambda, rbX, rbQ, rbIinv, variant] = batch_arrays(e, t);
+        append_bytes(key, idx2, idx4, idx3, gv, gs, mat, matU, lambda, rbX, rbQ, rbIinv, variant, replica_mat(e, t), replica_geo(e, t), e->dev[t].count);
+    }
+    return key;
+}
+
 static int ensure_graph(pbd_engine *e) {
-    if (e->graphValid) return 0;
+    std::vector<unsigned char> key = graph_key(e);
+    if (e->graphExec && key == e->graphKey) return 0;
+    if (e->graphExec) { cudaGraphExecDestroy(e->graphExec); e->graphExec = nullptr; }
     cudaGraph_t graph = nullptr;
     CK(cudaStreamBeginCapture(e->stream, cudaStreamCaptureModeThreadLocal));
     unsigned long long L = 0;
@@ -1406,8 +1405,8 @@ static int ensure_graph(pbd_engine *e) {
     if (err != cudaSuccess) return fail("cudaStreamEndCapture -> %s", cudaGetErrorString(err));
     err = cudaGraphInstantiate(&e->graphExec, graph, 0);
     cudaGraphDestroy(graph);
-    if (err != cudaSuccess) return fail("cudaGraphInstantiate -> %s", cudaGetErrorString(err));
-    e->graphValid = true;
+    if (err != cudaSuccess) { e->graphExec = nullptr; return fail("cudaGraphInstantiate -> %s", cudaGetErrorString(err)); }
+    e->graphKey.swap(key);
     e->graphLaunches = L;
     return 0;
 }
@@ -1422,7 +1421,7 @@ extern "C" int pbd_step(pbd_engine *e, unsigned nSteps) {
         if (e->active == PBD_MODE_LAUNCH) CKE(enqueue_step_launches(e, e->stream, &L));
         else if (e->active == PBD_MODE_RESIDENT) CKE(enqueue_step_resident(e, e->stream, &L));
         else if (e->active == PBD_MODE_JACOBI) CKE(enqueue_step_jacobi(e, e->stream, &L));
-        else { CKE(ensure_graph(e)); CK(cudaGraphLaunch(e->graphExec, e->stream)); L = e->graphLaunches; }
+        else { if (s == 0) CKE(ensure_graph(e)); CK(cudaGraphLaunch(e->graphExec, e->stream)); L = e->graphLaunches; }
         CKE(enqueue_contacts(e, e->stream, &L));
         e->stats.kernel_launches += L;
         e->stats.steps++;

@@ -929,11 +929,7 @@ bool TimeStepController::step(SimulationModel &model) {
     if ((m_collisionDetection || !m_collidersSent.empty()) && !uploadColliders(model)) return false;
     const float g[3] = {m_gravitation[0], m_gravitation[1], m_gravitation[2]};
     if (m_mode != m_modeSent) { if (pbd_set_mode(m_engine, m_mode)) return fail("pbd_set_mode"); m_modeSent = m_mode; }
-    SentParams now = {m_tm.getTimeStepSize(), m_subSteps, m_maxIterations, m_velocityUpdateMethod, {g[0], g[1], g[2]}};
-    if (!m_sentValid || std::memcmp(&now, &m_sent, sizeof(now)) != 0) {  // pbd_set_params invalidates the captured graph
-        if (pbd_set_params(m_engine, now.dt, now.subSteps, now.maxIter, now.velMethod, g)) return fail("pbd_set_params");
-        m_sent = now; m_sentValid = true;
-    }
+    if (pbd_set_params(m_engine, m_tm.getTimeStepSize(), m_subSteps, m_maxIterations, m_velocityUpdateMethod, g)) return fail("pbd_set_params");
     if (pbd_step(m_engine, 1)) return fail("pbd_step");
     if (!model.getRigidBodies().empty()) {  // a handful of bodies: mirror their state right away
         SimulationModel::RigidBodyVector &rbs = model.getRigidBodies();

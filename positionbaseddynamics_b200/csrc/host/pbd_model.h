@@ -419,8 +419,6 @@ private:
     int m_velocityUpdateMethod = 0;
     Vector3r m_gravitation = Vector3r(0, static_cast<Real>(-9.81), 0);  // Simulation.cpp:16
     int m_mode = PBD_MODE_AUTO, m_modeSent = -1;
-    struct SentParams { float dt; unsigned int subSteps, maxIter; int velMethod; float g[3]; } m_sent{};
-    bool m_sentValid = false;
     const SimulationModel *m_boundModel = nullptr;
     uint64_t m_boundGeneration = 0;
     unsigned int m_boundParticles = 0, m_boundRigidBodies = 0;

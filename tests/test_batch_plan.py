@@ -8,7 +8,8 @@ import numpy as np
 import pytest
 
 import scenes
-from test_image_plan import AUTO, GRAPH, JACOBI, LAUNCH, RESIDENT, Scene, check_plan, cloth, mixed, mode_of, rig, same_image, u32
+from plan_util import AUTO, GRAPH, JACOBI, LAUNCH, RESIDENT, Scene, check_plan, mode_of, same_image, u32
+from test_image_plan import cloth, mixed, rig
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PKG = os.path.join(ROOT, "positionbaseddynamics_b200")

@@ -127,7 +127,7 @@ int pbd_get_groups(pbd_engine *e, unsigned *offsets, unsigned *ids);
 int pbd_set_params(pbd_engine *e, float dt, unsigned subSteps, unsigned maxIter, int velocityUpdateMethod,
                    const float gravity[3]);
 int pbd_set_mode(pbd_engine *e, int mode);
-int pbd_get_mode(pbd_engine *e, int *requested, int *active);  /* active = the mode the current image runs in (resolved at the first step) */
+int pbd_get_mode(pbd_engine *e, int *requested, int *active);  /* active = the mode the next step runs in (the image is brought up to date first) */
 
 /* nSteps x TimeStepController::step, asynchronous on the engine's stream. */
 int pbd_step(pbd_engine *e, unsigned nSteps);

@@ -316,7 +316,7 @@ class Engine:
         _ck(lib().pbd_set_mode(self._h, int(mode)))
 
     def get_mode(self):
-        """(requested, active): active is what the current image runs in (the resolution of MODE_AUTO after the first step)."""
+        """(requested, active): active is what the next step runs in (the resolution of MODE_AUTO for the current model)."""
         r, a = C.c_int(0), C.c_int(0)
         _ck(lib().pbd_get_mode(self._h, C.byref(r), C.byref(a)))
         return r.value, a.value

@@ -91,8 +91,8 @@ struct pbd_engine {
     // replica's own (pbd_set_replica_materials, the types of matMask); gravity [K][3] (pbd_set_replica_gravity).
     // restX: per-replica rest shapes (pbd_set_replica_rest_positions), the rest positions the call was given, K x n float4 by host index
     // with .w = the inverse mass at the time of the call; every image planned while restShapes is on derives its geometry from them.
-    // restTables: the current image carries what a derivation reads (TypePlan::restBodies / restLocal), planned only while the override
-    // is on or being switched on, so that batches without it do not pay for them.
+    // restTables: images carry what a derivation reads (TypePlan::restBodies / restLocal), from the first pbd_set_replica_rest_positions
+    // until the override is dropped, so that batches without it do not pay for them.
     struct Batch {
         unsigned K = 1, matMask = 0;
         DevBuf mat, gravity, restX;
@@ -105,17 +105,15 @@ struct pbd_engine {
     TypeStore host[PBD_NUM_TYPES];
     unsigned numConstraints = 0;
     std::vector<unsigned> groupOff, groupIds;
-    bool groupsSet = false;
-    // device image
+    bool groupsSet = false; unsigned long long modelGen = 0;  // modelGen: counts model_changed (particles, constraints or groups replaced)
+    // device image, and the image_key it was planned under
     DevType dev[PBD_NUM_TYPES];
     std::vector<Bucket> buckets;
     DevBuf dBuckets, dTrace;
-    bool imageDirty = true; unsigned long long imageGen = 0;  // imageGen: images planned so far
+    std::vector<unsigned char> imageKey; unsigned long long imageGen = 0;  // imageGen: images planned so far
     // parameters
     float dt = 0.005f; unsigned subSteps = 5, maxIter = 1; int velMethod = 0; float g[3] = {0.f, -9.81f, 0.f};
-    int mode = PBD_MODE_AUTO;             // requested (pbd_set_mode)
-    int active = PBD_MODE_GRAPH;          // what the current image runs in: == mode, or the resolution of PBD_MODE_AUTO (image_plan.h)
-    bool autoNoResident = false;          // PBD_MODE_AUTO: the resident mode was tried for this model and refused
+    int mode = PBD_MODE_AUTO;             // requested (pbd_set_mode); what the image runs in: active_mode
     // graph cache: the captured step and the graph_key it was captured under
     cudaGraphExec_t graphExec = nullptr;
     std::vector<unsigned char> graphKey;
@@ -141,7 +139,7 @@ struct pbd_engine {
     bool timingPending = false;
     std::vector<unsigned> slot;          // host particle index -> device slot (formula layouts or the tile-major permutation)
     DevBuf dSlot, dSlotOld, relayoutTmp;
-    // resident mode (resident.cuh): the launch shape of the current image
+    // resident mode (resident.cuh): the launch shape of the current image (res.G == 0: the image is not tiled)
     pbd_b200::ResidentShape res;
     DevBuf dColourStart, dTileOff, dTileStart, dTileSmem, dXNbr, dXMask, dXFlags;
     unsigned long long xLaunch = 0;       // resident launches so far: the high word of the X arrival flags
@@ -149,8 +147,9 @@ struct pbd_engine {
 
 static int use(pbd_engine *e) { CK(cudaSetDevice(e->device)); return 0; }
 
+static void model_changed(pbd_engine *e) { e->modelGen++; }  // what the device image is planned from (image_key) replaced
 static void drop_replica_geometry(pbd_engine *e) {
-    e->batch.restShapes = false;
+    e->batch.restShapes = e->batch.restTables = false;
     e->batch.restX.release();
     for (DevType &d : e->dev) {
         for (DevBuf &b : d.repGv) b.release();
@@ -294,7 +293,7 @@ extern "C" int pbd_set_particles(pbd_engine *e, unsigned n, const float *x, cons
     if (!why.empty()) return fail("pbd_set_particles: %s", why.c_str());
     CKE(use(e));
     CK(cudaStreamSynchronize(e->stream));
-    e->n = n; e->imageDirty = true;
+    e->n = n; model_changed(e);  // and the formula slot map below
     const size_t b4 = (size_t)n * sizeof(float4);
     for (auto *b : {&e->pos, &e->vel, &e->oldp, &e->lastp, &e->pos0}) CKE(b->alloc(b4 * e->batch.K));
     CKE(e->stage.alloc((size_t)e->batch.K * n * 3 * sizeof(float)));
@@ -348,8 +347,7 @@ extern "C" int pbd_set_replicas(pbd_engine *e, unsigned K) {
     CKE(e->stage.alloc((size_t)K * e->n * 3 * sizeof(float)));
     CKE(e->massStage.alloc((size_t)K * e->n * sizeof(float)));
     CK(cudaStreamSynchronize(e->stream));
-    e->imageDirty = true;  // re-planned for the batch; the multipliers of every replica start at zero
-    e->autoNoResident = false;  // whether the resident mode takes the model depends on the batch size
+    model_changed(e);  // every replica is redefined: planned again, with the shared material rows and zero multipliers
     return 0;
 }
 
@@ -382,7 +380,7 @@ extern "C" int pbd_set_replica_materials(pbd_engine *e, int type, const float *m
     CKE(use(e));
     const unsigned bit = 1u << type;
     if (mat) CKE(write_replica_materials(e, type, mat, nMat * sizeof(float)));
-    else if ((e->batch.matMask & bit) && !e->imageDirty) CKE(write_replica_materials(e, type, e->dev[type].arrays.matU, 0));  // (a dirty image writes them when it is planned)
+    else if (e->batch.matMask & bit) CKE(write_replica_materials(e, type, e->dev[type].arrays.matU, 0));  // (an image planned again writes them too)
     if (mat) e->batch.matMask |= bit; else e->batch.matMask &= ~bit;
     return 0;
 }
@@ -452,7 +450,7 @@ extern "C" int pbd_set_rigid_bodies(pbd_engine *e, unsigned n, const float *mass
     if (!why.empty()) return fail("pbd_set_rigid_bodies: %s", why.c_str());
     CKE(use(e));
     CK(cudaStreamSynchronize(e->stream));
-    if (n != e->nRb) { e->imageDirty = true; e->groupsSet = e->groupsSet && n == e->nRb; }
+    if (n != e->nRb) e->groupsSet = false;  // the colouring covers the bodies
     e->nRb = n;
     e->rbMass.assign(mass, mass + n);
     if (n == 0) return 0;
@@ -470,7 +468,6 @@ extern "C" int pbd_set_rigid_bodies(pbd_engine *e, unsigned n, const float *mass
     struct { DevBuf *d; const std::vector<float4> *h; } up[] = {{&e->rbX, &X}, {&e->rbQ, &Q}, {&e->rbV, &V}, {&e->rbW, &W}, {&e->rbOldX, &X}, {&e->rbLastX, &X},
                                                               {&e->rbOldQ, &Q}, {&e->rbLastQ, &Q}, {&e->rbI, &I}, {&e->rbIinv, &Ii}};
     for (auto &u : up) { CKE(u.d->alloc(b)); CK(cudaMemcpy(u.d->p, u.h->data(), b, cudaMemcpyHostToDevice)); }
-    e->imageDirty = true;  // joint type arrays hold the rigid-body pointers
     return 0;
 }
 
@@ -508,7 +505,7 @@ extern "C" int pbd_clear_constraints(pbd_engine *e) {
     for (auto &h : e->host) { h.ids.clear(); h.bodies.clear(); h.params.clear(); }
     e->numConstraints = 0;
     e->groupOff.clear(); e->groupIds.clear(); e->groupsSet = false;
-    e->imageDirty = true; e->autoNoResident = false;
+    model_changed(e);
     return 0;
 }
 
@@ -562,7 +559,7 @@ extern "C" int pbd_add_constraints(pbd_engine *e, int type, unsigned count, cons
     }
     e->numConstraints += count;
     e->groupsSet = false;  // any add invalidates the groups (SimulationModel: m_groupsInitialized = false)
-    e->imageDirty = true; e->autoNoResident = false;
+    model_changed(e);
     return 0;
 }
 
@@ -583,7 +580,7 @@ extern "C" int pbd_set_groups(pbd_engine *e, unsigned nGroups, const unsigned *o
     e->groupIds.assign(ids, ids + N);
     if (nGroups == 0) e->groupOff.assign(1, 0u);
     e->groupsSet = true;
-    e->imageDirty = true;
+    model_changed(e);
     return 0;
 }
 
@@ -647,7 +644,7 @@ static void groups_from_colours(pbd_engine *e, const std::vector<unsigned> &colo
         for (size_t id = lo; id < hi; id++) e->groupIds[h[colour[id]]++] = (unsigned)id;
     }
     e->groupOff = goff;
-    e->groupsSet = true; e->imageDirty = true;
+    e->groupsSet = true; model_changed(e);
 }
 
 // Greedy first fit in insertion order == SimulationModel::initConstraintGroups (Simulation/SimulationModel.cpp:1033-1094);
@@ -669,7 +666,7 @@ extern "C" int pbd_color_first_fit_device(pbd_engine *e, float *ms, unsigned *wa
     const unsigned N = e->numConstraints, V = e->n + e->nRb;
     if (ms) *ms = 0.0f;
     if (wavefronts) *wavefronts = 0;
-    if (N == 0) { e->groupOff.assign(1, 0u); e->groupIds.clear(); e->groupsSet = true; e->imageDirty = true; return 0; }
+    if (N == 0) { e->groupOff.assign(1, 0u); e->groupIds.clear(); e->groupsSet = true; model_changed(e); return 0; }
     std::vector<unsigned> off, bodies;
     CKE(build_id_csr(e, off, bodies));
     const unsigned M = (unsigned)bodies.size();
@@ -761,19 +758,9 @@ extern "C" int pbd_set_params(pbd_engine *e, float dt, unsigned subSteps, unsign
 extern "C" int pbd_set_mode(pbd_engine *e, int mode) {
     if (!e) return fail("null engine");
     if (mode != PBD_MODE_GRAPH && mode != PBD_MODE_RESIDENT && mode != PBD_MODE_LAUNCH && mode != PBD_MODE_JACOBI && mode != PBD_MODE_AUTO) return fail("unknown solver mode %d", mode);
-    if (mode == e->mode) return 0;
     const std::string why = pbd_b200::batch_refusal(e->batch.K, e->n, mode, e->nRb, e->host);
     if (!why.empty()) return fail("pbd_set_mode: %s", why.c_str());
-    // only the resident image is laid out differently: the others run the image they share
-    const int active = pbd_b200::preferred_mode(mode, e->host, e->n, e->numConstraints, false, e->batch.K);
-    if ((active == PBD_MODE_RESIDENT) != (e->active == PBD_MODE_RESIDENT)) e->imageDirty = true;
-    e->mode = mode; e->active = active; e->autoNoResident = false;
-    return 0;
-}
-extern "C" int pbd_get_mode(pbd_engine *e, int *requested, int *active) {
-    if (!e) return fail("null engine");
-    if (requested) *requested = e->mode;
-    if (active) *active = e->active;
+    e->mode = mode;
     return 0;
 }
 
@@ -822,7 +809,6 @@ static int resident_max_clusters(const pbd_engine *e, unsigned mask, unsigned C,
 // colour groups when none were given: the reference-order-preserving first fit on the GPU (colouring.cuh), the host version as the fallback
 static int colour_if_needed(pbd_engine *e) {
     if (e->groupsSet) return 0;
-    if (e->numConstraints == 0) { e->groupOff.assign(1, 0u); e->groupIds.clear(); e->groupsSet = true; return 0; }
     if (pbd_color_first_fit_device(e, nullptr, nullptr)) CKE(pbd_color_first_fit(e));
     return 0;
 }
@@ -926,16 +912,33 @@ static int apply_replica_geometry(pbd_engine *e, const float4 *rest, const char 
     return 0;
 }
 
-// constraints + colour groups -> the device image of the requested mode (the planner resolves PBD_MODE_AUTO): the planner's inputs
-// gathered, the plan uploaded.  restTables: plan what a derivation reads even while per-replica rest shapes are off (being switched on).
-static int flatten(pbd_engine *e, bool restTables = false) {
-    if (!e->imageDirty) return 0;
-    CKE(use(e));
+template <class... V> static void append_bytes(std::vector<unsigned char> &key, const V &...v) {
+    static_assert((std::is_scalar_v<std::remove_all_extents_t<V>> && ...), "padding bytes would make equal states compare unequal");
+    size_t at = key.size();
+    key.resize(at + (sizeof(V) + ...));
+    ((std::memcpy(&key[at], &v, sizeof(V)), at += sizeof(V)), ...);
+}
+// Everything the image is planned and uploaded from; the joint arrays hold the rigid-body pointers.  The mode counts where it asks for a
+// tiled image: AUTO then falls back to graph where the resident mode refuses the model, RESIDENT fails.  Left out: the rest positions the
+// tiling bisects (they decide how fast a tiled image runs, not what it computes) and PBD_B200_CLUSTERS (a knob read at planning time).
+static std::vector<unsigned char> image_key(const pbd_engine *e) {
+    std::vector<unsigned char> key;
+    const bool tiled = pbd_b200::preferred_mode(e->mode, e->host, e->n, e->numConstraints, e->batch.K) == PBD_MODE_RESIDENT;
+    append_bytes(key, e->modelGen, e->n, e->nRb, e->rbX.p, e->rbQ.p, e->rbIinv.p, e->batch.K, tiled ? e->mode : -1, e->batch.restTables);
+    return key;
+}
+
+// The device image of the requested mode (the planner resolves PBD_MODE_AUTO), planned again whenever image_key changes: colour groups
+// made where none were given, the planner's inputs gathered, the plan uploaded.
+static int flatten(pbd_engine *e) {
     pbd_b200::Lap lap;
-    CKE(colour_if_needed(e));
+    CKE(colour_if_needed(e));  // before the key: the groups it makes are the model's from now on
+    std::vector<unsigned char> key = image_key(e);
+    if (key == e->imageKey) return 0;
+    CKE(use(e));
     e->imageGen++;
     std::vector<float4> x0;  // resident: rest positions by host index
-    if (pbd_b200::preferred_mode(e->mode, e->host, e->n, e->numConstraints, e->autoNoResident, e->batch.K) == PBD_MODE_RESIDENT && e->n) {
+    if (pbd_b200::preferred_mode(e->mode, e->host, e->n, e->numConstraints, e->batch.K) == PBD_MODE_RESIDENT && e->n) {
         std::vector<float4> raw(e->n);
         CK(cudaStreamSynchronize(e->stream));
         CK(cudaMemcpy(raw.data(), e->pos0.p, (size_t)e->n * sizeof(float4), cudaMemcpyDeviceToHost));
@@ -943,8 +946,8 @@ static int flatten(pbd_engine *e, bool restTables = false) {
         for (unsigned i = 0; i < e->n; i++) x0[i] = raw[e->slot[i]];
     }
     lap("colouring + rest positions");
-    pbd_b200::PlanInput in{e->host, e->numConstraints, e->n, e->nRb, &e->groupOff, &e->groupIds, e->mode, x0.data(), 0u, 0u, e->smCount, nullptr, e->autoNoResident, e->batch.K};
-    in.restTables = e->batch.K > 1 && (e->batch.restShapes || restTables);
+    pbd_b200::PlanInput in{e->host, e->numConstraints, e->n, e->nRb, &e->groupOff, &e->groupIds, e->mode, x0.data(), 0u, 0u, e->smCount, nullptr,
+                           e->batch.restTables, e->batch.K};
     if (const char *g = getenv("PBD_B200_CLUSTERS")) {  // development knob "GxC"
         unsigned gg = 0, cc = 0;
         if (sscanf(g, "%ux%u", &gg, &cc) == 2 && gg >= 1 && cc >= 1 && cc <= (unsigned)kMaxClusterCtas && (cc & (cc - 1)) == 0) { in.forcedG = gg; in.forcedC = cc; }
@@ -952,18 +955,14 @@ static int flatten(pbd_engine *e, bool restTables = false) {
     in.maxClusters = [&](unsigned mask, unsigned C, size_t smem) { int mc = 0; return resident_max_clusters(e, mask, C, smem, &mc) ? 0 : mc; };
     pbd_b200::ImagePlan plan;
     const std::string err = pbd_b200::plan_image(in, plan);
-    if (!plan.residentRefusal.empty()) {
-        if (verbose()) fprintf(stderr, "[pbd_b200] auto mode: resident refused (%s), using the graph mode\n", plan.residentRefusal.c_str());
-        e->autoNoResident = true;
-    }
+    if (!plan.residentRefusal.empty() && verbose()) fprintf(stderr, "[pbd_b200] auto mode: resident refused (%s), using the graph mode\n", plan.residentRefusal.c_str());
     if (!err.empty()) return fail("%s", err.c_str());
-    e->active = plan.mode;
     CKE(relayout(e, plan.slot));
     for (int t = 0; t < PBD_NUM_TYPES; t++) CKE(upload_type(e, t, plan.types[t]));
     e->buckets.swap(plan.buckets);
     CKE(upload_vec(e->dBuckets, e->buckets, e->stream));
+    e->res = plan.res;
     if (plan.mode == PBD_MODE_RESIDENT) {
-        e->res = plan.res;
         CKE(upload_vec(e->dTileStart, plan.tileStart, e->stream));
         CKE(upload_vec(e->dTileSmem, plan.tileSmem, e->stream));
         CKE(upload_vec(e->dColourStart, plan.colourStart, e->stream));
@@ -980,8 +979,17 @@ static int flatten(pbd_engine *e, bool restTables = false) {
     e->stats.num_constraints = e->numConstraints;  // per replica, like num_particles
     e->stats.num_groups = (unsigned)e->groupOff.size() - 1;
     e->stats.num_buckets = (unsigned)e->buckets.size();
-    e->batch.restTables = in.restTables;
-    e->imageDirty = false;
+    e->imageKey.swap(key);
+    return 0;
+}
+// What the current image runs in: a tiled image the resident mode, any other the requested mode, PBD_MODE_AUTO resolved to graph.
+static int active_mode(const pbd_engine *e) { return e->res.G ? PBD_MODE_RESIDENT : e->mode == PBD_MODE_AUTO ? PBD_MODE_GRAPH : e->mode; }
+
+extern "C" int pbd_get_mode(pbd_engine *e, int *requested, int *active) {
+    if (!e) return fail("null engine");
+    CKE(flatten(e));
+    if (requested) *requested = e->mode;
+    if (active) *active = active_mode(e);
     return 0;
 }
 
@@ -991,8 +999,8 @@ extern "C" int pbd_set_replica_rest_positions(pbd_engine *e, const float *x0) {
     CKE(replica_params_refusal(e, "pbd_set_replica_rest_positions"));
     CKE(use(e));
     if (!x0) { drop_replica_geometry(e); return 0; }
-    if (!e->batch.restTables) e->imageDirty = true;  // planned again with the bodies the derivation reads
-    CKE(flatten(e, true));  // the device order of the constraints the geometry is derived for
+    e->batch.restTables = true;  // planned again, if need be, with the bodies the derivation reads
+    CKE(flatten(e));  // the device order of the constraints the geometry is derived for
     for (int t = 0; t < PBD_BALLJOINT; t++)  // the resident kernel addresses replica r's geometry as i + r count in 32 bits
         if ((unsigned long long)e->batch.K * e->dev[t].count >= (1ull << 32))
             return fail("pbd_set_replica_rest_positions: %u replicas of %u constraints of type %d exceed 2^32 geometry rows", e->batch.K, e->dev[t].count, t);
@@ -1371,12 +1379,6 @@ static int enqueue_contacts(pbd_engine *e, cudaStream_t s, unsigned long long *l
     return 0;
 }
 
-template <class... V> static void append_bytes(std::vector<unsigned char> &key, const V &...v) {
-    static_assert((std::is_scalar_v<std::remove_all_extents_t<V>> && ...), "padding bytes would make equal states compare unequal");
-    size_t at = key.size();
-    key.resize(at + (sizeof(V) + ...));
-    ((std::memcpy(&key[at], &v, sizeof(V)), at += sizeof(V)), ...);
-}
 // Everything enqueue_step_launches reads, which a captured step bakes in, as the bytes of scalars and arrays of them (no padding).
 // imageGen stands for the bucket table.  The structured bindings do not compile once RbState or TypeArrays gains a member not listed here.
 static std::vector<unsigned char> graph_key(const pbd_engine *e) {
@@ -1415,12 +1417,13 @@ extern "C" int pbd_step(pbd_engine *e, unsigned nSteps) {
     if (!e) return fail("null engine");
     CKE(use(e));
     CKE(flatten(e));
+    const int active = active_mode(e);
     CK(cudaEventRecord(e->evStart, e->stream));
     for (unsigned s = 0; s < nSteps; s++) {
         unsigned long long L = 0;
-        if (e->active == PBD_MODE_LAUNCH) CKE(enqueue_step_launches(e, e->stream, &L));
-        else if (e->active == PBD_MODE_RESIDENT) CKE(enqueue_step_resident(e, e->stream, &L));
-        else if (e->active == PBD_MODE_JACOBI) CKE(enqueue_step_jacobi(e, e->stream, &L));
+        if (active == PBD_MODE_LAUNCH) CKE(enqueue_step_launches(e, e->stream, &L));
+        else if (active == PBD_MODE_RESIDENT) CKE(enqueue_step_resident(e, e->stream, &L));
+        else if (active == PBD_MODE_JACOBI) CKE(enqueue_step_jacobi(e, e->stream, &L));
         else { if (s == 0) CKE(ensure_graph(e)); CK(cudaGraphLaunch(e->graphExec, e->stream)); L = e->graphLaunches; }
         CKE(enqueue_contacts(e, e->stream, &L));
         e->stats.kernel_launches += L;
@@ -1578,8 +1581,8 @@ extern "C" int pbd_get_stats(pbd_engine *e, pbd_stats *out) {
 
 extern "C" int pbd_profile_step(pbd_engine *e, float *msPerType, float *msIntegrate, float *msVelocity, unsigned *launchesPerType) {
     if (!e) return fail("null engine");
-    if (e->active == PBD_MODE_RESIDENT || e->active == PBD_MODE_JACOBI || e->mode == PBD_MODE_AUTO) return fail("pbd_profile_step: per-bucket launches do not exist in this mode (select PBD_MODE_GRAPH or PBD_MODE_LAUNCH first)");
     CKE(use(e)); CKE(flatten(e));
+    if (e->mode != PBD_MODE_GRAPH && e->mode != PBD_MODE_LAUNCH) return fail("pbd_profile_step: per-bucket launches do not exist in this mode (select PBD_MODE_GRAPH or PBD_MODE_LAUNCH first)");
     CK(cudaStreamSynchronize(e->stream));
     // One event after every launch, all recorded in stream order without host synchronisation (a host sync per launch would time
     // the idle-launch latency, not the kernel); read back after one final sync.

@@ -648,7 +648,7 @@ static std::string build_phase_tables(Ctx &c, const std::vector<unsigned> (&orde
 
 // PBD_MODE_AUTO: the resident mode where it is the faster exact mode -- models made of cloth and FEM / volume constraints with at
 // least kAutoResidentMinParticles particles (cfg2, cfg3, cfg5); small models (cfg1), mixed models with rigid coupling and the heavy
-// solver families (cfg4) stay in graph mode, and so does a model the resident mode has refused.
+// solver families (cfg4) stay in graph mode, and so does a model the resident mode refuses (plan_image).
 // Measured on an H100 80GB HBM3 (SXM, 400 W, 1980 MHz), XPBD cloth 1 x 20, ms per step graph / resident: 100x100 0.66 / 0.79,
 // 200x200 0.93 / 0.92, 300x300 1.20 / 1.02; cfg1 (50x50) 0.129 / 0.183; cfg3 (44,541 particles) 8.03 / 7.69.
 // Replica batches take the resident mode from kAutoResidentMinReplicas replicas on whatever the size of a replica, from twice as many
@@ -658,9 +658,9 @@ static std::string build_phase_tables(Ctx &c, const std::vector<unsigned> (&orde
 // cfg3 K = 4 13.42 / 7.88, K = 66 127.9 / 44.1; 100x100 FEMTriangle + Dihedral cloth 1 x 5 (light) K = 33 0.531 / 0.692, K = 66
 // 0.838 / 0.717, K = 132 1.412 / 0.745.
 constexpr unsigned kAutoResidentMinParticles = 40000, kAutoResidentMinReplicas = 32;
-int preferred_mode(int requested, const TypeStore *store, unsigned n, unsigned numConstraints, bool residentRefused, unsigned replicas) {
+int preferred_mode(int requested, const TypeStore *store, unsigned n, unsigned numConstraints, unsigned replicas) {
     if (requested != PBD_MODE_AUTO) return requested;
-    if (residentRefused || numConstraints == 0) return PBD_MODE_GRAPH;
+    if (numConstraints == 0) return PBD_MODE_GRAPH;
     unsigned present = 0;
     for (int t = 0; t < PBD_NUM_TYPES; t++) if (!store[t].ids.empty()) present |= 1u << t;
     const bool clothFem = (present & ~(kMaskCloth | kMaskFem)) == 0, light = (present & ~kMaskLight) == 0;
@@ -725,7 +725,7 @@ std::string batch_refusal(unsigned replicas, unsigned n, int mode, unsigned nRb,
 std::string plan_image(const PlanInput &in, ImagePlan &out) {
     const std::string refusal = batch_refusal(in.replicas, in.n, in.mode, in.nRb, in.store);
     if (!refusal.empty()) return refusal;
-    out.mode = preferred_mode(in.mode, in.store, in.n, in.numConstraints, in.residentRefused, in.replicas);
+    out.mode = preferred_mode(in.mode, in.store, in.n, in.numConstraints, in.replicas);
     const std::string err = plan_mode(in, out.mode == PBD_MODE_RESIDENT, out);
     if (err.empty() || in.mode != PBD_MODE_AUTO || out.mode != PBD_MODE_RESIDENT) return err;
     // AUTO, and the resident mode refused the model (does not fit, user-modified bending Q, ...): the graph image, planned from scratch

@@ -31,9 +31,9 @@ long long bad_body_index(int type, const unsigned *bodies, size_t count, unsigne
 // insertion id -> (type, local index) of the N constraints in store[PBD_NUM_TYPES]; "" or why the ids are not a permutation of 0..N-1
 std::string build_id_map(const TypeStore *store, unsigned N, std::vector<std::pair<int, unsigned>> &map);
 
-// The mode an image is planned for: `requested`, or for PBD_MODE_AUTO the resident mode where it is faster and not refused yet, else graph.
-// `replicas`: the size of the replica batch the image serves (pbd_set_replicas).
-int preferred_mode(int requested, const TypeStore *store, unsigned n, unsigned numConstraints, bool residentRefused, unsigned replicas = 1);
+// The mode an image is planned for: `requested`, or for PBD_MODE_AUTO the resident mode where it is faster, else graph (plan_image falls
+// back to graph where the resident mode refuses the model).  `replicas`: the size of the replica batch the image serves (pbd_set_replicas).
+int preferred_mode(int requested, const TypeStore *store, unsigned n, unsigned numConstraints, unsigned replicas = 1);
 
 // Clusters of C CTAs with `smem` bytes each the device keeps co-resident; a query of the type mask alone answers for every cluster shape.
 struct ClusterQuery : std::function<int(unsigned mask, unsigned C, size_t smem)> {
@@ -51,9 +51,8 @@ struct PlanInput {
     unsigned forcedG, forcedC;                     // resident: G x C clusters x CTAs (PBD_B200_CLUSTERS), 0 = chosen from the model
     int smCount;
     ClusterQuery maxClusters;                      // resident: what the device keeps co-resident
-    bool residentRefused = false;                  // PBD_MODE_AUTO: the resident mode refused this model before
-    unsigned replicas = 1;                         // replica batch: every replica runs this one image (n, the constraints: one replica)
     bool restTables = false;                       // replica batch with per-replica rest shapes: also TypePlan::restBodies / restLocal
+    unsigned replicas = 1;                         // replica batch: every replica runs this one image (n, the constraints: one replica)
 };
 
 // One constraint type's arrays in device order (the host side of pbdk::TypeArrays).

@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE: runs the image planner of libpbd_b200.so (csrc/host/image_plan.h) on a model read from a file and writes every
 // array of the plan to another, for tests/test_image_plan.py.  Needs no GPU: the co-residency query answers a constant from the input.
 //   plan_image <input> <output>
-// input : u32 n, nRb, numConstraints, mode, residentRefused, forcedG, forcedC, smCount, maxClusters, nGroups; u32 groupOff[nGroups + 1];
+// input : u32 n, nRb, numConstraints, mode, restTables, forcedG, forcedC, smCount, maxClusters, nGroups; u32 groupOff[nGroups + 1];
 //         u32 groupIds[numConstraints]; float4 x0[n]; per type: u32 count, u32 ids[count], u32 bodies[count nBodies], f32 params[count nParams]
 // output: records of (char name[32], u64 bytes, bytes of data); "error" and "residentRefusal" first, the plan's mode and arrays after
 //         them when the error is empty
@@ -28,7 +28,7 @@ template <class V> static void put(const char *name, int t, int k, const V &v) {
 
 int main(int argc, char **argv) {
     if (argc != 3 || !(fin = fopen(argv[1], "rb")) || !(fout = fopen(argv[2], "wb"))) { fprintf(stderr, "usage: plan_image <input> <output>\n"); return 2; }
-    const unsigned n = get1(), nRb = get1(), N = get1(), mode = get1(), refused = get1(), G = get1(), C = get1(), smCount = get1(), maxClusters = get1(),
+    const unsigned n = get1(), nRb = get1(), N = get1(), mode = get1(), restTables = get1(), G = get1(), C = get1(), smCount = get1(), maxClusters = get1(),
                    nGroups = get1();
     std::vector<unsigned> groupOff(nGroups + 1), groupIds(N);
     get(groupOff.data(), groupOff.size()); get(groupIds.data(), N);
@@ -43,7 +43,7 @@ int main(int argc, char **argv) {
         get(h.ids.data(), h.ids.size()); get(h.bodies.data(), h.bodies.size()); get(h.params.data(), h.params.size());
     }
     const PlanInput in{store, N, n, nRb, &groupOff, &groupIds, (int)mode, x0.data(), G, C, (int)smCount, [=](unsigned) { return (int)maxClusters; },
-                       refused != 0};
+                       restTables != 0};
     ImagePlan p;
     const std::string err = plan_image(in, p);
     put("error", err);

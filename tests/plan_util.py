@@ -72,10 +72,10 @@ class Scene:
         return col
 
 
-def plan(driver, tmp_path, sc, mode, shape=(0, 0), threads=None, tag="p", refused=False, max_clusters=132):
+def plan(driver, tmp_path, sc, mode, shape=(0, 0), threads=None, tag="p", max_clusters=132):
     """The plan of `sc` in `mode` on a device of 132 SMs that keeps `max_clusters` clusters of any shape co-resident."""
     x0 = np.zeros((sc.n, 4), np.float32); x0[:, :3] = sc.x0
-    head = [sc.n, sc.nrb, sc.N, mode, int(refused), shape[0], shape[1], 132, max_clusters, len(sc.off) - 1]
+    head = [sc.n, sc.nrb, sc.N, mode, 0, shape[0], shape[1], 132, max_clusters, len(sc.off) - 1]
     parts = [np.asarray(head, np.uint32), sc.off, sc.ids, x0]
     for ids, b, p in sc.store:
         parts += [np.asarray([len(ids)], np.uint32), ids, b, p]

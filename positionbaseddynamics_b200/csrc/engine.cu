@@ -67,6 +67,8 @@ struct DevBuf {                   // one device allocation, freed with its owner
     void release() { if (p) cudaFree(p); p = nullptr; bytes = 0; }
 };
 
+constexpr int kNumAttrs = PBD_ATTR_LASTX + 1;  // x, v, x0, oldX, lastX
+
 struct DevType {
     DevBuf idx[3], gv[kMaxGeoV], gs[kMaxGeoS], mat[kMaxMat], lambda;
     // replica batch: what its per-replica geometry is derived from (TypePlan::restBodies / restLocal, the insertion ids), and the geometry
@@ -83,9 +85,11 @@ struct pbd_engine {
     bool ownsStream = false;
     int smCount = 132;                    // H100 SXM; read from the device in pbd_create
     size_t l2Bytes = 50u << 20;           // likewise
-    // particles: batch.K replicas of n (pbd_set_replicas), replica r at device slots [r n, (r + 1) n)
+    // particles: batch.K replicas of n (pbd_set_replicas), replica r at device slots [r n, (r + 1) n); one float4 array per attribute,
+    // indexed by pbd_attr (attr_ptr).  stage: the host copies' staging areas, K n 3 floats each (upload_attr / download_attr; set_w's
+    // masses in stage[0]); stage[1] only for pbd_step_host, so that its x and v uploads do not wait on each other.
     unsigned n = 0;
-    DevBuf pos, vel, oldp, lastp, pos0, stage, stage2, massStage, jacobiDelta;
+    DevBuf attr[kNumAttrs], stage[2], jacobiDelta;
     // A replica batch and what its replicas have of their own (batch_arrays, replica_mat and replica_geo turn it into what the kernels see).
     // mat [K][kMatRowFloats]: the uniform material parameters of every type, replica by replica -- the shared ones of the image, or a
     // replica's own (pbd_set_replica_materials, the types of matMask); gravity [K][3] (pbd_set_replica_gravity).
@@ -216,16 +220,7 @@ extern "C" int pbd_destroy(pbd_engine *e) {
 // ------------------------------------------------------------------------------------------------------------
 static inline unsigned nblk(unsigned n, unsigned t) { return (n + t - 1) / t; }
 
-static float4 *attr_buf(pbd_engine *e, int attr) {
-    switch (attr) {
-    case PBD_ATTR_X: return (float4 *)e->pos.p;
-    case PBD_ATTR_V: return (float4 *)e->vel.p;
-    case PBD_ATTR_X0: return (float4 *)e->pos0.p;
-    case PBD_ATTR_OLDX: return (float4 *)e->oldp.p;
-    case PBD_ATTR_LASTX: return (float4 *)e->lastp.p;
-    default: return nullptr;
-    }
-}
+static float4 *attr_ptr(const pbd_engine *e, int a) { return (float4 *)e->attr[a].p; }
 
 static int upload_slot_map(pbd_engine *e) {
     if (e->n == 0) return 0;
@@ -242,11 +237,11 @@ static int relayout(pbd_engine *e, const std::vector<unsigned> &newSlot) {
     e->slot = newSlot;
     CKE(upload_slot_map(e));
     CKE(e->relayoutTmp.alloc((size_t)e->batch.K * e->n * sizeof(float4)));
-    for (DevBuf *b : {&e->pos, &e->vel, &e->oldp, &e->lastp, &e->pos0}) {
-        k_relayout<<<dim3((e->n + 255) / 256, e->batch.K), 256, 0, e->stream>>>((const float4 *)b->p, (float4 *)e->relayoutTmp.p, e->n, (const unsigned *)e->dSlotOld.p, (const unsigned *)e->dSlot.p);
+    for (DevBuf &b : e->attr) {
+        k_relayout<<<dim3((e->n + 255) / 256, e->batch.K), 256, 0, e->stream>>>((const float4 *)b.p, (float4 *)e->relayoutTmp.p, e->n, (const unsigned *)e->dSlotOld.p, (const unsigned *)e->dSlot.p);
         CK(cudaGetLastError());
         CK(cudaStreamSynchronize(e->stream));
-        std::swap(b->p, e->relayoutTmp.p); std::swap(b->bytes, e->relayoutTmp.bytes);
+        std::swap(b.p, e->relayoutTmp.p); std::swap(b.bytes, e->relayoutTmp.bytes);
     }
     return 0;
 }
@@ -254,19 +249,31 @@ static int relayout(pbd_engine *e, const std::vector<unsigned> &newSlot) {
 // grid of a per-particle kernel over `replicas` replicas: blockIdx.y = replica (kernels.cuh: k_pack3 ...)
 static dim3 replica_grid(const pbd_engine *e, unsigned replicas) { return dim3(nblk(e->n, 256), replicas); }
 
-// host AoS-3 of the first `replicas` replicas -> staging -> float4 (keeps .w)
-static int upload3(pbd_engine *e, const float *src, float4 *dst, int keepW, unsigned replicas) {
-    const size_t bytes = (size_t)replicas * e->n * 3 * sizeof(float);
-    CK(cudaMemcpyAsync(e->stage.p, src, bytes, cudaMemcpyHostToDevice, e->stream));
-    k_pack3<<<replica_grid(e, replicas), 256, 0, e->stream>>>((const float *)e->stage.p, dst, e->n, keepW, (const unsigned *)e->dSlot.p);
+// Host AoS-3 of the first `replicas` replicas -> `staging` on stream `copy` -> attribute `a` by k_pack3 on the engine stream (.w kept
+// with keepW).  host == nullptr: `staging` holds the copy already.  A copy stream other than the engine's comes with `copied`, through
+// which the pack waits for the copy.
+static int upload_attr(pbd_engine *e, int a, const float *host, int keepW, unsigned replicas, const DevBuf &staging, cudaStream_t copy,
+                       cudaEvent_t copied = nullptr) {
+    if (host) CK(cudaMemcpyAsync(staging.p, host, (size_t)replicas * e->n * 3 * sizeof(float), cudaMemcpyHostToDevice, copy));
+    if (copied) { CK(cudaEventRecord(copied, copy)); CK(cudaStreamWaitEvent(e->stream, copied, 0)); }
+    k_pack3<<<replica_grid(e, replicas), 256, 0, e->stream>>>((const float *)staging.p, attr_ptr(e, a), e->n, keepW, (const unsigned *)e->dSlot.p);
     CK(cudaGetLastError());
     return 0;
 }
+// Attribute `a` of every replica -> `staging` by k_unpack3 on the engine stream -> host AoS-3 on stream `copy`.  A copy stream other
+// than the engine's comes with `unpacked`, through which the copy waits for the unpack.
+static int download_attr(pbd_engine *e, int a, float *host, const DevBuf &staging, cudaStream_t copy, cudaEvent_t unpacked = nullptr) {
+    k_unpack3<<<replica_grid(e, e->batch.K), 256, 0, e->stream>>>(attr_ptr(e, a), (float *)staging.p, e->n, (const unsigned *)e->dSlot.p);
+    CK(cudaGetLastError());
+    if (unpacked) { CK(cudaEventRecord(unpacked, e->stream)); CK(cudaStreamWaitEvent(copy, unpacked, 0)); }
+    CK(cudaMemcpyAsync(host, staging.p, (size_t)e->batch.K * e->n * 3 * sizeof(float), cudaMemcpyDeviceToHost, copy));
+    return 0;
+}
 
-// masses of the first `replicas` replicas (n floats each)
+// masses of the first `replicas` replicas (n floats each), staged in stage[0]
 static int set_w(pbd_engine *e, const float *mass, unsigned replicas) {
-    CK(cudaMemcpyAsync(e->massStage.p, mass, (size_t)replicas * e->n * sizeof(float), cudaMemcpyHostToDevice, e->stream));
-    k_set_w<<<replica_grid(e, replicas), 256, 0, e->stream>>>((float4 *)e->pos.p, (float4 *)e->vel.p, (const float *)e->massStage.p, e->n, (const unsigned *)e->dSlot.p);
+    CK(cudaMemcpyAsync(e->stage[0].p, mass, (size_t)replicas * e->n * sizeof(float), cudaMemcpyHostToDevice, e->stream));
+    k_set_w<<<replica_grid(e, replicas), 256, 0, e->stream>>>(attr_ptr(e, PBD_ATTR_X), attr_ptr(e, PBD_ATTR_V), (const float *)e->stage[0].p, e->n, (const unsigned *)e->dSlot.p);
     CK(cudaGetLastError());
     CK(cudaStreamSynchronize(e->stream));  // staging buffers are reused by the next call
     return 0;
@@ -279,12 +286,29 @@ extern "C" int pbd_set_masses(pbd_engine *e, const float *mass) {
     return set_w(e, mass, e->batch.K);
 }
 
-// replica 0 of a particle array copied to replicas 1 .. K-1 (doubling copies)
-static int broadcast_replica0(pbd_engine *e, DevBuf &b) {
+// replica 0 of every particle array copied to replicas 1 .. K-1 (doubling copies)
+static int broadcast_replica0(pbd_engine *e, unsigned K) {
     const size_t one = (size_t)e->n * sizeof(float4);
-    for (size_t have = 1; have < e->batch.K; have *= 2)
-        CK(cudaMemcpyAsync((char *)b.p + have * one, b.p, std::min(have, (size_t)e->batch.K - have) * one, cudaMemcpyDeviceToDevice, e->stream));
+    for (DevBuf &b : e->attr)
+        for (size_t have = 1; have < K; have *= 2)
+            CK(cudaMemcpyAsync((char *)b.p + have * one, b.p, std::min(have, (size_t)K - have) * one, cudaMemcpyDeviceToDevice, e->stream));
     return 0;
+}
+// The particle arrays sized for K replicas of n, and stage[0] for their host copies.  keepReplica0: replica 0 moves into fresh arrays
+// (the old ones are freed) and replicas 1 .. K-1 become copies of it; otherwise what the arrays hold is the caller's to write.
+static int size_particles(pbd_engine *e, unsigned K, bool keepReplica0) {
+    const size_t one = (size_t)e->n * sizeof(float4);
+    const bool keep = keepReplica0 && one;
+    for (DevBuf &b : e->attr) {
+        if (!keep) { CKE(b.alloc(one * K)); continue; }
+        DevBuf grown;
+        CKE(grown.alloc(one * K));
+        CK(cudaMemcpyAsync(grown.p, b.p, one, cudaMemcpyDeviceToDevice, e->stream));
+        std::swap(b.p, grown.p); std::swap(b.bytes, grown.bytes);
+        CK(cudaStreamSynchronize(e->stream));  // before `grown` frees the old array
+    }
+    CKE(e->stage[0].alloc((size_t)K * e->n * 3 * sizeof(float)));
+    return keep ? broadcast_replica0(e, K) : 0;
 }
 
 extern "C" int pbd_set_particles(pbd_engine *e, unsigned n, const float *x, const float *x0, const float *v, const float *mass) {
@@ -294,25 +318,21 @@ extern "C" int pbd_set_particles(pbd_engine *e, unsigned n, const float *x, cons
     CKE(use(e));
     CK(cudaStreamSynchronize(e->stream));
     e->n = n; model_changed(e);  // and the formula slot map below
-    const size_t b4 = (size_t)n * sizeof(float4);
-    for (auto *b : {&e->pos, &e->vel, &e->oldp, &e->lastp, &e->pos0}) CKE(b->alloc(b4 * e->batch.K));
-    CKE(e->stage.alloc((size_t)e->batch.K * n * 3 * sizeof(float)));
-    CKE(e->massStage.alloc((size_t)e->batch.K * n * sizeof(float)));
+    CKE(size_particles(e, e->batch.K, false));
     drop_replica_geometry(e);  // every replica's state is redefined
     e->slot.resize(n);
     for (unsigned i = 0; i < n; i++) e->slot[i] = particle_slot(i, n);
     if (n == 0) return 0;
     CKE(upload_slot_map(e));
-    CK(cudaMemsetAsync(e->vel.p, 0, b4, e->stream));
-    CKE(upload3(e, x, (float4 *)e->pos.p, 0, 1)); CK(cudaStreamSynchronize(e->stream));
-    if (v) { CKE(upload3(e, v, (float4 *)e->vel.p, 0, 1)); CK(cudaStreamSynchronize(e->stream)); }
+    const size_t b4 = (size_t)n * sizeof(float4);
+    CK(cudaMemsetAsync(attr_ptr(e, PBD_ATTR_V), 0, b4, e->stream));
+    CKE(upload_attr(e, PBD_ATTR_X, x, 0, 1, e->stage[0], e->stream)); CK(cudaStreamSynchronize(e->stream));
+    if (v) { CKE(upload_attr(e, PBD_ATTR_V, v, 0, 1, e->stage[0], e->stream)); CK(cudaStreamSynchronize(e->stream)); }
     CKE(set_w(e, mass, 1));
     // oldX = lastX = x, x0 = x unless given (ParticleData::addVertex, ParticleData.h:127-137)
-    CK(cudaMemcpyAsync(e->oldp.p, e->pos.p, b4, cudaMemcpyDeviceToDevice, e->stream));
-    CK(cudaMemcpyAsync(e->lastp.p, e->pos.p, b4, cudaMemcpyDeviceToDevice, e->stream));
-    CK(cudaMemcpyAsync(e->pos0.p, e->pos.p, b4, cudaMemcpyDeviceToDevice, e->stream));
-    if (x0) { CKE(upload3(e, x0, (float4 *)e->pos0.p, 1, 1)); }
-    for (DevBuf *b : {&e->pos, &e->vel, &e->oldp, &e->lastp, &e->pos0}) CKE(broadcast_replica0(e, *b));  // every replica of a batch starts here
+    for (int a : {PBD_ATTR_OLDX, PBD_ATTR_LASTX, PBD_ATTR_X0}) CK(cudaMemcpyAsync(attr_ptr(e, a), attr_ptr(e, PBD_ATTR_X), b4, cudaMemcpyDeviceToDevice, e->stream));
+    if (x0) CKE(upload_attr(e, PBD_ATTR_X0, x0, 1, 1, e->stage[0], e->stream));
+    CKE(broadcast_replica0(e, e->batch.K));  // every replica of a batch starts here
     CK(cudaStreamSynchronize(e->stream));
     e->stats.num_particles = n;
     return 0;
@@ -331,21 +351,10 @@ extern "C" int pbd_set_replicas(pbd_engine *e, unsigned K) {
     CKE(collider_refusal(e, K, e->pColliders.size() + e->rColliders.size()));
     CKE(use(e));
     CK(cudaStreamSynchronize(e->stream));
-    const size_t one = (size_t)e->n * sizeof(float4);
-    if (e->n)
-        for (DevBuf *b : {&e->pos, &e->vel, &e->oldp, &e->lastp, &e->pos0}) {  // replica 0 kept, the others copies of it
-            DevBuf grown;
-            CKE(grown.alloc(one * K));
-            CK(cudaMemcpyAsync(grown.p, b->p, one, cudaMemcpyDeviceToDevice, e->stream));
-            std::swap(b->p, grown.p); std::swap(b->bytes, grown.bytes);
-            CK(cudaStreamSynchronize(e->stream));  // before `grown` frees the old array
-        }
+    CKE(size_particles(e, K, true));  // replica 0 kept, the others copies of it
     e->batch.K = K;
     e->batch.mat.release(); e->batch.gravity.release(); e->batch.matMask = 0; e->batch.gravitySet = false;  // rows of the old K
     drop_replica_geometry(e);
-    for (DevBuf *b : {&e->pos, &e->vel, &e->oldp, &e->lastp, &e->pos0}) CKE(broadcast_replica0(e, *b));
-    CKE(e->stage.alloc((size_t)K * e->n * 3 * sizeof(float)));
-    CKE(e->massStage.alloc((size_t)K * e->n * sizeof(float)));
     CK(cudaStreamSynchronize(e->stream));
     model_changed(e);  // every replica is redefined: planned again, with the shared material rows and zero multipliers
     return 0;
@@ -419,10 +428,9 @@ extern "C" int pbd_get_replicas(pbd_engine *e, unsigned *K) {
 extern "C" int pbd_set_attr(pbd_engine *e, int attr, const float *src) {
     if (!e || !src) return fail("pbd_set_attr: null argument");
     CKE(use(e));
-    float4 *dst = attr_buf(e, attr);
-    if (!dst) return fail("pbd_set_attr: bad attribute %d", attr);
+    if (attr < 0 || attr >= kNumAttrs) return fail("pbd_set_attr: bad attribute %d", attr);
     if (e->n == 0) return 0;
-    CKE(upload3(e, src, dst, 1, e->batch.K));
+    CKE(upload_attr(e, attr, src, 1, e->batch.K, e->stage[0], e->stream));
     CK(cudaStreamSynchronize(e->stream));
     return 0;
 }
@@ -430,12 +438,9 @@ extern "C" int pbd_set_attr(pbd_engine *e, int attr, const float *src) {
 extern "C" int pbd_get_attr(pbd_engine *e, int attr, float *dst) {
     if (!e || !dst) return fail("pbd_get_attr: null argument");
     CKE(use(e));
-    const float4 *src = attr_buf(e, attr);
-    if (!src) return fail("pbd_get_attr: bad attribute %d", attr);
+    if (attr < 0 || attr >= kNumAttrs) return fail("pbd_get_attr: bad attribute %d", attr);
     if (e->n == 0) return 0;
-    k_unpack3<<<replica_grid(e, e->batch.K), 256, 0, e->stream>>>(src, (float *)e->stage.p, e->n, (const unsigned *)e->dSlot.p);
-    CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(dst, e->stage.p, (size_t)e->batch.K * e->n * 3 * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
+    CKE(download_attr(e, attr, dst, e->stage[0], e->stream));
     CK(cudaStreamSynchronize(e->stream));
     return 0;
 }
@@ -941,7 +946,7 @@ static int flatten(pbd_engine *e) {
     if (pbd_b200::preferred_mode(e->mode, e->host, e->n, e->numConstraints, e->batch.K) == PBD_MODE_RESIDENT && e->n) {
         std::vector<float4> raw(e->n);
         CK(cudaStreamSynchronize(e->stream));
-        CK(cudaMemcpy(raw.data(), e->pos0.p, (size_t)e->n * sizeof(float4), cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(raw.data(), attr_ptr(e, PBD_ATTR_X0), (size_t)e->n * sizeof(float4), cudaMemcpyDeviceToHost));
         x0.resize(e->n);
         for (unsigned i = 0; i < e->n; i++) x0[i] = raw[e->slot[i]];
     }
@@ -1007,12 +1012,12 @@ extern "C" int pbd_set_replica_rest_positions(pbd_engine *e, const float *x0) {
     if (e->n) {
         DevBuf rest;
         CKE(rest.alloc((size_t)e->batch.K * e->n * sizeof(float4)));
-        CK(cudaMemcpyAsync(e->stage.p, x0, (size_t)e->batch.K * e->n * 3 * sizeof(float), cudaMemcpyHostToDevice, e->stream));
-        k_pack_rest<<<replica_grid(e, e->batch.K), 256, 0, e->stream>>>((const float *)e->stage.p, (const float4 *)e->pos.p, (float4 *)rest.p, e->n, (const unsigned *)e->dSlot.p);
+        CK(cudaMemcpyAsync(e->stage[0].p, x0, (size_t)e->batch.K * e->n * 3 * sizeof(float), cudaMemcpyHostToDevice, e->stream));
+        k_pack_rest<<<replica_grid(e, e->batch.K), 256, 0, e->stream>>>((const float *)e->stage[0].p, attr_ptr(e, PBD_ATTR_X), (float4 *)rest.p, e->n, (const unsigned *)e->dSlot.p);
         CK(cudaGetLastError());
         CKE(apply_replica_geometry(e, (const float4 *)rest.p, "pbd_set_replica_rest_positions"));
         std::swap(e->batch.restX.p, rest.p); std::swap(e->batch.restX.bytes, rest.bytes);
-        CKE(upload3(e, x0, (float4 *)e->pos0.p, 1, e->batch.K));  // PBD_ATTR_X0 of every replica
+        CKE(upload_attr(e, PBD_ATTR_X0, nullptr, 1, e->batch.K, e->stage[0], e->stream));  // PBD_ATTR_X0 of every replica, from x0 still in stage[0]
         CK(cudaStreamSynchronize(e->stream));
     }
     e->batch.restShapes = true;
@@ -1084,8 +1089,8 @@ static int launch_bucket(pbd_engine *e, const Bucket &b, float h, int iterZero, 
     const ReplicaStrides rs{e->n, {e->dev[b.type].count}, {replica_mat(e, b.type)}, {replica_geo(e, b.type)}};
     return with_project_type(b.type, a.variant, [&](auto T, auto V) -> int {
         constexpr int TT = decltype(T)::value, VAR = decltype(V)::value;
-        if (e->batch.K > 1) CK(launch_step_kernel(k_project<TT, VAR, true>, dim3(nblk(b.count, block), e->batch.K), block, s, pdl, (float4 *)e->pos.p, a, b.first, b.count, h, iterZero, rs));
-        else CK(launch_step_kernel(k_project<TT, VAR, false>, nblk(b.count, block), block, s, pdl, (float4 *)e->pos.p, a, b.first, b.count, h, iterZero, rs));
+        if (e->batch.K > 1) CK(launch_step_kernel(k_project<TT, VAR, true>, dim3(nblk(b.count, block), e->batch.K), block, s, pdl, attr_ptr(e, PBD_ATTR_X), a, b.first, b.count, h, iterZero, rs));
+        else CK(launch_step_kernel(k_project<TT, VAR, false>, nblk(b.count, block), block, s, pdl, attr_ptr(e, PBD_ATTR_X), a, b.first, b.count, h, iterZero, rs));
         return 0;
     });
 }
@@ -1139,8 +1144,8 @@ static int launch_colour(pbd_engine *e, size_t b0, size_t b1, float h, int iterZ
             blocks += nblk(b.count, block);
         }
         for (int k = m.nSeg; k <= kMultiSegments; k++) m.blockStart[k] = blocks;
-        if (e->batch.K > 1) CK(launch_step_kernel(k_project_multi<true>, dim3(blocks, e->batch.K), block, s, true, (float4 *)e->pos.p, m, h, iterZero, rs));
-        else CK(launch_step_kernel(k_project_multi<false>, blocks, block, s, true, (float4 *)e->pos.p, m, h, iterZero, rs));
+        if (e->batch.K > 1) CK(launch_step_kernel(k_project_multi<true>, dim3(blocks, e->batch.K), block, s, true, attr_ptr(e, PBD_ATTR_X), m, h, iterZero, rs));
+        else CK(launch_step_kernel(k_project_multi<false>, blocks, block, s, true, attr_ptr(e, PBD_ATTR_X), m, h, iterZero, rs));
         (*launches)++;
     }
     return 0;
@@ -1159,16 +1164,17 @@ static int enqueue_step_launches(pbd_engine *e, cudaStream_t s, unsigned long lo
     const unsigned n = e->n * e->batch.K;  // the particle updates run over every replica's slots at once
     const bool pdl = !log;
     const RbState rb = rb_state(e);
+    float4 *x = attr_ptr(e, PBD_ATTR_X), *v = attr_ptr(e, PBD_ATTR_V), *oldX = attr_ptr(e, PBD_ATTR_OLDX), *lastX = attr_ptr(e, PBD_ATTR_LASTX);
     unsigned long long L = 0;
     auto launched = [&](int kind) { L++; return log ? log->mark(s, kind) : 0; };
     for (unsigned sub = 0; sub < e->subSteps; sub++) {
         if (e->nRb) { CK(launch_step_kernel(k_rb_integrate, nblk(e->nRb, 256), 256, s, pdl, rb, h, e->g[0], e->g[1], e->g[2])); CKE(launched(kLaunchIntegrate)); }
         if (n) {
             if (e->batch.gravitySet)  // replica blockIdx.y under its own row
-                CK(launch_step_kernel(k_integrate<true>, replica_grid(e, e->batch.K), 256, s, pdl, (float4 *)e->pos.p, (float4 *)e->vel.p, (float4 *)e->oldp.p, (float4 *)e->lastp.p, e->n, h, 0.0f, 0.0f, 0.0f,
+                CK(launch_step_kernel(k_integrate<true>, replica_grid(e, e->batch.K), 256, s, pdl, x, v, oldX, lastX, e->n, h, 0.0f, 0.0f, 0.0f,
                                       (const float *)e->batch.gravity.p));
             else
-                CK(launch_step_kernel(k_integrate<false>, nblk(n, 256), 256, s, pdl, (float4 *)e->pos.p, (float4 *)e->vel.p, (float4 *)e->oldp.p, (float4 *)e->lastp.p, n, h, e->g[0], e->g[1], e->g[2],
+                CK(launch_step_kernel(k_integrate<false>, nblk(n, 256), 256, s, pdl, x, v, oldX, lastX, n, h, e->g[0], e->g[1], e->g[2],
                                       (const float *)nullptr));
             CKE(launched(kLaunchIntegrate));
         }
@@ -1180,7 +1186,7 @@ static int enqueue_step_launches(pbd_engine *e, cudaStream_t s, unsigned long lo
                 b0 = b1;
             }
         if (n) {
-            CK(launch_step_kernel(k_velocity, nblk(n, 256), 256, s, pdl, (const float4 *)e->pos.p, (float4 *)e->vel.p, (const float4 *)e->oldp.p, (const float4 *)e->lastp.p, n, invH, e->velMethod));
+            CK(launch_step_kernel(k_velocity, nblk(n, 256), 256, s, pdl, x, v, oldX, lastX, n, invH, e->velMethod));
             CKE(launched(kLaunchVelocity));
         }
         if (e->nRb) { CK(launch_step_kernel(k_rb_velocity, nblk(e->nRb, 256), 256, s, pdl, rb, invH, (float)(2.0 / (double)h), e->velMethod)); CKE(launched(kLaunchVelocity)); }
@@ -1194,7 +1200,7 @@ static int enqueue_step_launches(pbd_engine *e, cudaStream_t s, unsigned long lo
 static int enqueue_step_resident(pbd_engine *e, cudaStream_t s, unsigned long long *launches) {
     const float h = e->dt / (float)e->subSteps;
     ResidentArgs ra;
-    ra.pos = (float4 *)e->pos.p; ra.vel = (float4 *)e->vel.p; ra.oldp = (float4 *)e->oldp.p; ra.lastp = (float4 *)e->lastp.p;
+    ra.pos = attr_ptr(e, PBD_ATTR_X); ra.vel = attr_ptr(e, PBD_ATTR_V); ra.oldp = attr_ptr(e, PBD_ATTR_OLDX); ra.lastp = attr_ptr(e, PBD_ATTR_LASTX);
     ra.buckets = (const Bucket *)e->dBuckets.p;
     ra.colourStart = (const unsigned *)e->dColourStart.p; ra.tileOff = (const unsigned *)e->dTileOff.p;
     ra.tileStart = (const unsigned *)e->dTileStart.p; ra.tileSmem = (const unsigned *)e->dTileSmem.p;
@@ -1262,10 +1268,11 @@ static int enqueue_step_jacobi(pbd_engine *e, cudaStream_t s, unsigned long long
         CKE(e->jacobiDelta.alloc((size_t)n * sizeof(float4)));
         CK(cudaMemsetAsync(e->jacobiDelta.p, 0, (size_t)n * sizeof(float4), s));
     }
-    const float4 *pos = (const float4 *)e->pos.p; float4 *delta = (float4 *)e->jacobiDelta.p;
+    float4 *x = attr_ptr(e, PBD_ATTR_X), *v = attr_ptr(e, PBD_ATTR_V), *oldX = attr_ptr(e, PBD_ATTR_OLDX), *lastX = attr_ptr(e, PBD_ATTR_LASTX);
+    float4 *delta = (float4 *)e->jacobiDelta.p;
     unsigned long long L = 0;
     for (unsigned sub = 0; sub < e->subSteps; sub++) {
-        k_integrate<false><<<nblk(n, 256), 256, 0, s>>>((float4 *)e->pos.p, (float4 *)e->vel.p, (float4 *)e->oldp.p, (float4 *)e->lastp.p, n, h, e->g[0], e->g[1], e->g[2], nullptr); L++;
+        k_integrate<false><<<nblk(n, 256), 256, 0, s>>>(x, v, oldX, lastX, n, h, e->g[0], e->g[1], e->g[2], nullptr); L++;
         for (unsigned it = 0; it < e->maxIter; it++) {
             for (int t = 0; t < PBD_BALLJOINT; t++) {
                 const unsigned cnt = e->dev[t].count;
@@ -1274,14 +1281,14 @@ static int enqueue_step_jacobi(pbd_engine *e, cudaStream_t s, unsigned long long
                 CKE(with_project_type(t, a.variant, [&](auto T, auto V) -> int {
                     constexpr int TT = decltype(T)::value, VAR = decltype(V)::value;
                     if constexpr (TT < PBD_BALLJOINT)  // the joints are refused above
-                        k_project_jacobi<TT, VAR><<<nblk(cnt, 128), 128, 0, s>>>(pos, delta, a, cnt, h, it == 0);
+                        k_project_jacobi<TT, VAR><<<nblk(cnt, 128), 128, 0, s>>>(x, delta, a, cnt, h, it == 0);
                     return 0;
                 }));
                 L++;
             }
-            k_jacobi_apply<<<nblk(n, 256), 256, 0, s>>>((float4 *)e->pos.p, delta, n); L++;
+            k_jacobi_apply<<<nblk(n, 256), 256, 0, s>>>(x, delta, n); L++;
         }
-        k_velocity<<<nblk(n, 256), 256, 0, s>>>((const float4 *)e->pos.p, (float4 *)e->vel.p, (const float4 *)e->oldp.p, (const float4 *)e->lastp.p, n, invH, e->velMethod); L++;
+        k_velocity<<<nblk(n, 256), 256, 0, s>>>(x, v, oldX, lastX, n, invH, e->velMethod); L++;
     }
     CK(cudaGetLastError());
     *launches = L;
@@ -1365,7 +1372,7 @@ static int enqueue_contacts(pbd_engine *e, cudaStream_t s, unsigned long long *l
     for (const ParticleCollider &c : e->pColliders)
         if ((unsigned long long)c.offset + c.count > e->n) return fail("contact path: a particle collider covers particles beyond the %u the engine holds", e->n);
     ContactArgs a;
-    a.pos = (float4 *)e->pos.p; a.vel = (float4 *)e->vel.p; a.slot = (const unsigned *)e->dSlot.p;
+    a.pos = attr_ptr(e, PBD_ATTR_X); a.vel = attr_ptr(e, PBD_ATTR_V); a.slot = (const unsigned *)e->dSlot.p;
     a.rbX = (const float4 *)e->rbX.p; a.rbV = (const float4 *)e->rbV.p; a.rbW = (const float4 *)e->rbW.p;
     a.rigid = (const RigidCollider *)e->dRColliders.p; a.nRigid = (unsigned)e->rColliders.size();
     a.ranges = (const ParticleCollider *)e->dPColliders.p; a.nRanges = (unsigned)e->pColliders.size();
@@ -1385,7 +1392,8 @@ static std::vector<unsigned char> graph_key(const pbd_engine *e) {
     std::vector<unsigned char> key;
     key.reserve(4096);
     const auto [X, Q, V, W, oldX, lastX, oldQ, lastQ, I, Iinv, nRb] = rb_state(e);
-    append_bytes(key, e->imageGen, e->n, e->batch.K, e->dt, e->subSteps, e->maxIter, e->velMethod, e->g, e->pos.p, e->vel.p, e->oldp.p, e->lastp.p,
+    append_bytes(key, e->imageGen, e->n, e->batch.K, e->dt, e->subSteps, e->maxIter, e->velMethod, e->g,
+                 attr_ptr(e, PBD_ATTR_X), attr_ptr(e, PBD_ATTR_V), attr_ptr(e, PBD_ATTR_OLDX), attr_ptr(e, PBD_ATTR_LASTX),
                  e->batch.gravitySet ? e->batch.gravity.p : nullptr, X, Q, V, W, oldX, lastX, oldQ, lastQ, I, Iinv, nRb);
     for (int t = 0; t < PBD_NUM_TYPES; t++) {
         const auto [idx2, idx4, idx3, gv, gs, mat, matU, lambda, rbX, rbQ, rbIinv, variant] = batch_arrays(e, t);
@@ -1464,31 +1472,13 @@ extern "C" int pbd_step_host(pbd_engine *e, unsigned nSteps, const float *x_in, 
     if (!e) return fail("null engine");
     CKE(use(e));
     if (e->n == 0) return pbd_step(e, nSteps);
-    const size_t bytes = (size_t)e->batch.K * e->n * 3 * sizeof(float);
-    const dim3 grid = replica_grid(e, e->batch.K);
     // two staging areas so that x and v uploads do not serialise on a host sync
-    CKE(e->stage.alloc(bytes));
-    DevBuf &stage2 = e->stage2;
-    CKE(stage2.alloc(bytes));
-    if (x_in) {
-        CK(cudaMemcpyAsync(e->stage.p, x_in, bytes, cudaMemcpyHostToDevice, e->stream));
-        k_pack3<<<grid, 256, 0, e->stream>>>((const float *)e->stage.p, (float4 *)e->pos.p, e->n, 1, (const unsigned *)e->dSlot.p);
-    }
-    if (v_in) {
-        CK(cudaMemcpyAsync(stage2.p, v_in, bytes, cudaMemcpyHostToDevice, e->stream));
-        k_pack3<<<grid, 256, 0, e->stream>>>((const float *)stage2.p, (float4 *)e->vel.p, e->n, 1, (const unsigned *)e->dSlot.p);
-    }
-    CK(cudaGetLastError());
+    for (DevBuf &b : e->stage) CKE(b.alloc((size_t)e->batch.K * e->n * 3 * sizeof(float)));
+    if (x_in) CKE(upload_attr(e, PBD_ATTR_X, x_in, 1, e->batch.K, e->stage[0], e->stream));
+    if (v_in) CKE(upload_attr(e, PBD_ATTR_V, v_in, 1, e->batch.K, e->stage[1], e->stream));
     CKE(pbd_step(e, nSteps));
-    if (x_out) {
-        k_unpack3<<<grid, 256, 0, e->stream>>>((const float4 *)e->pos.p, (float *)e->stage.p, e->n, (const unsigned *)e->dSlot.p);
-        CK(cudaMemcpyAsync(x_out, e->stage.p, bytes, cudaMemcpyDeviceToHost, e->stream));
-    }
-    if (v_out) {
-        k_unpack3<<<grid, 256, 0, e->stream>>>((const float4 *)e->vel.p, (float *)stage2.p, e->n, (const unsigned *)e->dSlot.p);
-        CK(cudaMemcpyAsync(v_out, stage2.p, bytes, cudaMemcpyDeviceToHost, e->stream));
-    }
-    CK(cudaGetLastError());
+    if (x_out) CKE(download_attr(e, PBD_ATTR_X, x_out, e->stage[0], e->stream));
+    if (v_out) CKE(download_attr(e, PBD_ATTR_V, v_out, e->stage[1], e->stream));
     CK(cudaStreamSynchronize(e->stream));
     return 0;
 }
@@ -1500,7 +1490,6 @@ extern "C" int pbd_step_host_async(pbd_engine *e, unsigned nSteps, const float *
     CKE(use(e));
     if (e->n == 0) return pbd_step(e, nSteps);
     const size_t bytes = (size_t)e->batch.K * e->n * 3 * sizeof(float);
-    const dim3 grid = replica_grid(e, e->batch.K);
     auto &P = e->pipe;
     if (!P.ready) {
         CK(cudaStreamCreateWithFlags(&P.up, cudaStreamNonBlocking));
@@ -1511,29 +1500,14 @@ extern "C" int pbd_step_host_async(pbd_engine *e, unsigned nSteps, const float *
     }
     const int s = (int)(P.issued & 1);
     const bool reuse = P.issued >= 2;  // the slot was used by call k-2: its consumers are ordered before us by events
-    const unsigned *slot = (const unsigned *)e->dSlot.p;
-    if (x_in || v_in) {
-        if (reuse) CK(cudaStreamWaitEvent(P.up, P.consumed[s], 0));
-        if (x_in) { CKE(P.inX[s].alloc(bytes)); CK(cudaMemcpyAsync(P.inX[s].p, x_in, bytes, cudaMemcpyHostToDevice, P.up)); }
-        if (v_in) { CKE(P.inV[s].alloc(bytes)); CK(cudaMemcpyAsync(P.inV[s].p, v_in, bytes, cudaMemcpyHostToDevice, P.up)); }
-        CK(cudaEventRecord(P.uploaded[s], P.up));
-        CK(cudaStreamWaitEvent(e->stream, P.uploaded[s], 0));
-        if (x_in) k_pack3<<<grid, 256, 0, e->stream>>>((const float *)P.inX[s].p, (float4 *)e->pos.p, e->n, 1, slot);
-        if (v_in) k_pack3<<<grid, 256, 0, e->stream>>>((const float *)P.inV[s].p, (float4 *)e->vel.p, e->n, 1, slot);
-        CK(cudaGetLastError());
-    }
+    if (reuse && (x_in || v_in)) CK(cudaStreamWaitEvent(P.up, P.consumed[s], 0));
+    if (x_in) { CKE(P.inX[s].alloc(bytes)); CKE(upload_attr(e, PBD_ATTR_X, x_in, 1, e->batch.K, P.inX[s], P.up, P.uploaded[s])); }
+    if (v_in) { CKE(P.inV[s].alloc(bytes)); CKE(upload_attr(e, PBD_ATTR_V, v_in, 1, e->batch.K, P.inV[s], P.up, P.uploaded[s])); }
     CK(cudaEventRecord(P.consumed[s], e->stream));
     CKE(pbd_step(e, nSteps));
-    if (x_out || v_out) {
-        if (reuse) CK(cudaStreamWaitEvent(e->stream, P.downloaded[s], 0));
-        if (x_out) { CKE(P.outX[s].alloc(bytes)); k_unpack3<<<grid, 256, 0, e->stream>>>((const float4 *)e->pos.p, (float *)P.outX[s].p, e->n, slot); }
-        if (v_out) { CKE(P.outV[s].alloc(bytes)); k_unpack3<<<grid, 256, 0, e->stream>>>((const float4 *)e->vel.p, (float *)P.outV[s].p, e->n, slot); }
-        CK(cudaGetLastError());
-        CK(cudaEventRecord(P.produced[s], e->stream));
-        CK(cudaStreamWaitEvent(P.down, P.produced[s], 0));
-        if (x_out) CK(cudaMemcpyAsync(x_out, P.outX[s].p, bytes, cudaMemcpyDeviceToHost, P.down));
-        if (v_out) CK(cudaMemcpyAsync(v_out, P.outV[s].p, bytes, cudaMemcpyDeviceToHost, P.down));
-    }
+    if (reuse && (x_out || v_out)) CK(cudaStreamWaitEvent(e->stream, P.downloaded[s], 0));
+    if (x_out) { CKE(P.outX[s].alloc(bytes)); CKE(download_attr(e, PBD_ATTR_X, x_out, P.outX[s], P.down, P.produced[s])); }
+    if (v_out) { CKE(P.outV[s].alloc(bytes)); CKE(download_attr(e, PBD_ATTR_V, v_out, P.outV[s], P.down, P.produced[s])); }
     CK(cudaEventRecord(P.downloaded[s], P.down));
     P.issued++;
     return 0;

@@ -72,6 +72,14 @@ def test_replicas_start_as_copies_of_replica_zero():
     lam, _ = eng.lambdas(_capi.DISTANCE_XPBD)
     assert lam.shape[0] == 4 and all(np.array_equal(lam[r], lam[0]) for r in range(4))
     eng.close()
+    # a batch size set while the engine holds no particles: the particles set afterwards start every replica
+    empty = _capi.Engine(0)
+    empty.set_replicas(3)
+    empty.set_particles(x, mass, v=v)
+    assert empty.replicas() == 3
+    for a, w in ((_capi.ATTR_X, x), (_capi.ATTR_V, v), (_capi.ATTR_X0, x)):
+        assert all(np.array_equal(g, w) for g in empty.get_attr(a)), a
+    empty.close()
 
 
 @pytest.mark.parametrize("mode", [GRAPH, RESIDENT], ids=["graph", "resident"])

@@ -1171,6 +1171,12 @@ void orc_get_rigid_bodies(double *out) {
     }
 }
 
+void orc_set_rigid_body_velocity(unsigned i, const double *v, const double *omega) {
+    RigidBody *b = &G->rbs[i];
+    b->v = V((real)v[0], (real)v[1], (real)v[2]);
+    b->omega = V((real)omega[0], (real)omega[1], (real)omega[2]);
+}
+
 /* PositionBasedRigidBodyDynamics::computeMatrixK, PositionBasedRigidBodyDynamics.cpp:11-45 */
 static void compute_matrix_k(vec3 connector, real invMass, vec3 x, const mat3 *J, mat3 *K) {
     if (invMass != R(0.0)) {

@@ -68,6 +68,7 @@ int orc_add_constraint(int type, const unsigned *bodies, const double *p);
 unsigned orc_add_rigid_body(double mass, const double *x, const double *inertia, const double *q);
 unsigned orc_num_rigid_bodies(void);
 void orc_get_rigid_bodies(double *out); /* per body: x(3) q(w,x,y,z) v(3) omega(3) = 13 doubles */
+void orc_set_rigid_body_velocity(unsigned i, const double *v, const double *omega); /* RigidBody::setVelocity / setAngularVelocity */
 
 void orc_set_params(double dt, unsigned subSteps, unsigned maxIter, int velMethod, const double *g);
 void orc_init_groups(void);

@@ -136,6 +136,10 @@ class CpuPbd:
         self.f("add_rigid_body").restype = C.c_uint
         return self.f("add_rigid_body")(_D(mass), _dp(_f64(x)), _dp(_f64(inertia)), _dp(_f64(q)))
 
+    def set_rigid_body_velocity(self, i, v, omega):
+        """RigidBody::setVelocity / setAngularVelocity of body i."""
+        self.f("set_rigid_body_velocity")(int(i), _dp(_f64(v)), _dp(_f64(omega)))
+
     def add_rigid_body_mesh(self, density, verts, faces, x=(0, 0, 0), R=np.eye(3), scale=(1, 1, 1)):
         """ref only: RigidBody::initBody(density, x, rotation, vertices, mesh, scale); returns (index, [mass, inertia(3), x(3), q(w,x,y,z)])."""
         assert self.kind != "oracle"

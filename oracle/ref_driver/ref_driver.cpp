@@ -156,6 +156,11 @@ void ref_get_rigid_body_props(unsigned i, double *out) {
     const Quaternionr &q = rb->getRotation();
     out[7] = q.w(); out[8] = q.x(); out[9] = q.y(); out[10] = q.z();
 }
+void ref_set_rigid_body_velocity(unsigned i, const double *v, const double *omega) {
+    RigidBody *rb = g_model->getRigidBodies()[i];
+    rb->setVelocity(v3(v));
+    rb->setAngularVelocity(v3(omega));
+}
 unsigned ref_num_rigid_bodies() { return (unsigned)g_model->getRigidBodies().size(); }
 void ref_get_rigid_bodies(double *out) {
     auto &rbs = g_model->getRigidBodies();

@@ -409,7 +409,8 @@ __global__ void __launch_bounds__(THREADS, 1) k_step_resident(const __grid_const
                     float4 x = tile[tile_swizzle(i)];
                     if (integrate_particle(A, t0 + i, x, gx, gy, gz)) tile[tile_swizzle(i)] = x;
                 }
-                if (A.rb.n && cta == 0 && threadIdx.x < A.rb.n) rb_integrate_body(A.rb, threadIdx.x, A.h, A.gx, A.gy, A.gz);
+                if (!BATCH && cta == 0)  // every body, in CTA 0: with G > 1 no joint reads them, in one cluster the cluster barrier orders them
+                    for (unsigned i = threadIdx.x; i < A.rb.n; i += RT) rb_integrate_body(A.rb, i, A.h, A.gx, A.gy, A.gz);
             }
             x_count(0);
             colour_arrive(single);
@@ -476,7 +477,8 @@ __global__ void __launch_bounds__(THREADS, 1) k_step_resident(const __grid_const
                 for (unsigned i = xtid; i < nGl; i += XT) velocity_particle(A, t0 + nSm + i, __ldcg(A.pos + t0 + nSm + i));
             } else {
                 for (unsigned i = threadIdx.x; i < nSm; i += RT) velocity_particle(A, t0 + i, tile[tile_swizzle(i)]);
-                if (A.rb.n && cta == 0 && threadIdx.x < A.rb.n) rb_velocity_body(A.rb, threadIdx.x, A.invH, A.twoInvH, A.secondOrder);
+                if (!BATCH && cta == 0)  // (replica batches hold no rigid bodies)
+                    for (unsigned i = threadIdx.x; i < A.rb.n; i += RT) rb_velocity_body(A.rb, i, A.invH, A.twoInvH, A.secondOrder);
             }
         }
         for (unsigned i = threadIdx.x; i < nSm; i += THREADS) __stcg(A.pos + t0 + i, tile[tile_swizzle(i)]);

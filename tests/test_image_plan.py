@@ -133,3 +133,55 @@ def test_plan_is_deterministic(driver, tmp_path):
     one = plan(driver, tmp_path, sc, RESIDENT, (37, 1), threads=1, tag="t1")
     four = plan(driver, tmp_path, sc, RESIDENT, (37, 1), threads=4, tag="t4")
     assert one["error"] == b"" and one["raw"] == four["raw"]
+
+
+def test_joints_in_one_cluster_only(driver, tmp_path):
+    """The rigid-body cases of tests/rigid_cases.py on rest positions in a random order.  Independent CTAs (a forced G > 1) are refused:
+    a joint's bodies are stepped by CTA 0 alone.  One cluster of four is admitted: every BallJoint runs in tile 0, every particle joint in
+    the tile of its particle, so the joints of one body run in several CTAs, ordered by the cluster barrier."""
+    import rigid_cases as rc
+    from plan_util import u32
+    m = rc.make_model(3, 8)
+    sc = Scene(m.n, m.nb, m.types, m.bodies, m.params, m.off, m.ids, rc.tile_x0(m, np.random.default_rng(5)))
+    p = plan(driver, tmp_path, sc, RESIDENT, (4, 1), tag="g4")
+    assert p["error"] == b"resident mode: rigid-body coupling is supported for scenes that fit one cluster (use PBD_MODE_GRAPH)"
+    p = plan(driver, tmp_path, sc, RESIDENT, (1, 4), tag="c4")
+    assert check_plan(sc, p, True) == (1, 4)
+    buckets = np.frombuffer(p["buckets"], np.int32).reshape(-1, 4)
+    tile_off = u32(p, "tileOff").astype(np.int64).reshape(len(buckets), 9)
+    tstart = u32(p, "tileStart").astype(np.int64)
+    ptile = np.searchsorted(tstart, u32(p, "slot"), "right") - 1
+    for t in (rc.BJ, rc.RBP):
+        ids, b, _ = sc.store[t]
+        b = b[np.searchsorted(ids, u32(p, "order%d" % t))]  # device order
+        ex = np.full(len(ids), -1)
+        for bi in np.nonzero(buckets[:, 0] == t)[0]:
+            lab = np.repeat(np.arange(8), np.diff(tile_off[bi]))
+            assert (lab % 2 == 1).all()  # shared-memory items only
+            ex[buckets[bi, 1]:buckets[bi, 1] + buckets[bi, 2]] = lab // 2
+        if t == rc.BJ:
+            assert (ex == 0).all()
+        else:
+            assert np.array_equal(ex, ptile[b[:, 1]]) and set(ex) == {0, 1, 2, 3}
+
+
+def test_free_bodies_beyond_the_block_are_planned_as_intended(driver, tmp_path):
+    """The 210 x 210 cloth and 700 free bodies of tests/test_gpu_rigid_answers.py: MODE_AUTO plans one resident cluster whose CTAs have
+    fewer threads than there are bodies, and the forced independent CTAs give part of every CTA to X threads, so fewer still step bodies
+    in CTA 0.  Both shapes the GPU tests run are admitted as intended."""
+    from plan_util import u32
+    from test_gpu_rigid_answers import INDEPENDENT_CTAS, cloth_and_free_bodies
+    m, (x, _, (types, bodies, params, off, ids)) = cloth_and_free_bodies()
+    sc = Scene(len(x), m.nb, types, bodies, params, off, ids, x)
+    shapes = {"auto": (0, 0), "forced": tuple(int(v) for v in INDEPENDENT_CTAS.split("x"))}
+    res = {}
+    for name, shape in shapes.items():
+        p = plan(driver, tmp_path, sc, AUTO if name == "auto" else RESIDENT, shape, tag=name)
+        assert mode_of(p) == RESIDENT and p["residentRefusal"] == b""
+        G, C = check_plan(sc, p, True)
+        threads, xthreads = (int(v) for v in u32(p, "res")[2:4])
+        res[name] = (G, C, threads, xthreads)
+        print("%s: %d x %d, %d threads, %d for X items; %d bodies" % (name, G, C, threads, xthreads, m.nb))
+        assert threads - xthreads < m.nb
+    assert res["auto"][0] == 1 and res["auto"][3] == 0
+    assert res["forced"][:2] == shapes["forced"] and res["forced"][3] > 0

@@ -132,3 +132,30 @@ def test_contact_path_restatement_is_pinned_to_the_reference(precision, cpu_libs
         worst_dv = max(worst_dv, float(dv.max()))
     print("contact restatement, %s: %d contact events, %d grazing, worst |dx| %.2e, worst |dv| %.2e" % (precision, events, grazing, worst_x, worst_dv))
     assert events > 2000 and grazing <= 4 and worst_dv <= tol_v
+
+
+@needs_ref
+@pytest.mark.parametrize("config", [(1, 1, 0), (2, 3, 1)], ids=["1x1_v0", "2x3_v1"])
+def test_rigid_cases_in_lockstep(cpu_libs, config):
+    """The rigid-body cases of tests/rigid_cases.py (both ball joints, chains, free spinning bodies; initial v and omega through
+    set_rigid_body_velocity) in the reference and the C restatement, both fp64, in lockstep: bodies and particles equal to 1e-9 of each
+    quantity's scale after every step."""
+    import rigid_cases as rc
+    ref = cpu_libs.CpuPbd("ref", "f64")
+    if not hasattr(ref.lib, "ref_set_rigid_body_velocity"):
+        pytest.skip("the prebuilt oracle/_ref predates set_rigid_body_velocity")
+    m = rc.make_model(4, 31)
+    orc = cpu_libs.CpuPbd("oracle", "f64")
+    for ck in (ref, orc):
+        rc.load(m, ck)
+        ck.set_params(dt=rc.DT, sub_steps=config[0], max_iter=config[1], vel_method=config[2], gravity=rc.GRAVITY)
+    (tr, br, pr, _), (to, bo, po_, _) = ref.constraints(), orc.constraints()
+    assert np.array_equal(tr, to) and np.array_equal(br, bo) and np.abs(pr - po_).max() <= 1e-12 * np.abs(pr).max()
+    assert all(np.array_equal(a, b) for a, b in zip(ref.groups(), orc.groups()))
+    for _ in range(3):
+        ref.step(1); orc.step(1)
+        rr, ro = ref.rigid_bodies(), orc.rigid_bodies()
+        for k in (slice(0, 3), slice(3, 7), slice(7, 10), slice(10, 13)):
+            assert np.abs(rr[:, k] - ro[:, k]).max() <= 1e-9 * max(np.abs(rr[:, k]).max(), 1.0), k
+        for name in ("x", "v"):
+            assert np.abs(ref.get(name) - orc.get(name)).max() <= 1e-9 * max(np.abs(ref.get(name)).max(), 1.0), name

@@ -151,6 +151,7 @@ constexpr int kMaxClusterCtas = 16;   // non-portable cluster size (opt-in attri
 // colour's concatenated item sequence, modulo the number of threads that share it (the buckets of one colour go to different threads)
 struct RunEntry { int type; unsigned firstX, nX, firstR, nR, rotR, pad0, pad1; };
 constexpr unsigned kMaxXNeighbours = 32;  // one lane of the first X warp per neighbour
+constexpr unsigned kXFlagStride = 16;     // unsigned long longs: every CTA's arrival flag on its own 128-byte line
 static_assert(kMatRowFloats + 3 <= (int)kMaxXNeighbours, "a replica's material row and gravity are staged in the xNbr words");
 __host__ __device__ inline size_t resident_smem_bytes(unsigned tileCap, unsigned nBuckets, unsigned nColours) {
     return (size_t)tileCap * sizeof(float4) + (size_t)nBuckets * sizeof(RunEntry) + (size_t)(2u * nColours + 2u + kMaxXNeighbours) * sizeof(unsigned);

@@ -70,13 +70,14 @@ struct DevBuf {                   // one device allocation, freed with its owner
 constexpr int kNumAttrs = PBD_ATTR_LASTX + 1;  // x, v, x0, oldX, lastX
 
 struct DevType {
-    DevBuf idx[3], gv[kMaxGeoV], gs[kMaxGeoS], mat[kMaxMat], lambda;
-    // replica batch: what its per-replica geometry is derived from (TypePlan::restBodies / restLocal, the insertion ids), and the geometry
-    // arrays every replica's projections read while per-replica rest shapes are on (K x count; they keep their address while it stays on)
-    DevBuf restBodies, restLocal, restIds, repGv[kMaxGeoV], repGs[kMaxGeoS];
+    // replica batch: the geometry arrays every replica's projections read while per-replica rest shapes are on (K x count; they keep
+    // their address while it stays on)
+    DevBuf repGv[kMaxGeoV], repGs[kMaxGeoS];
     PodVector<unsigned> order;    // position in the device arrays -> insertion id
     unsigned count = 0;
+    // pointers into the image (upload_image): the arrays the kernels read, and what a batch's per-replica geometry is derived from
     TypeArrays arrays{};
+    pbd_b200::RestTables rest{};
 };
 
 struct pbd_engine {
@@ -110,10 +111,11 @@ struct pbd_engine {
     unsigned numConstraints = 0;
     std::vector<unsigned> groupOff, groupIds;
     bool groupsSet = false; unsigned long long modelGen = 0;  // modelGen: counts model_changed (particles, constraints or groups replaced)
-    // device image, and the image_key it was planned under
+    // device image: one allocation (upload_image), and the image_key it was planned under
     DevType dev[PBD_NUM_TYPES];
     std::vector<Bucket> buckets;
-    DevBuf dBuckets, dTrace;
+    DevBuf image, dTrace;
+    pbd_b200::ImageTables tables{};
     std::vector<unsigned char> imageKey; unsigned long long imageGen = 0;  // imageGen: images planned so far
     // parameters
     float dt = 0.005f; unsigned subSteps = 5, maxIter = 1; int velMethod = 0; float g[3] = {0.f, -9.81f, 0.f};
@@ -145,7 +147,6 @@ struct pbd_engine {
     DevBuf dSlot, dSlotOld, relayoutTmp;
     // resident mode (resident.cuh): the launch shape of the current image (res.G == 0: the image is not tiled)
     pbd_b200::ResidentShape res;
-    DevBuf dColourStart, dTileOff, dTileStart, dTileSmem, dXNbr, dXMask, dXFlags;
     unsigned long long xLaunch = 0;       // resident launches so far: the high word of the X arrival flags
 };
 
@@ -494,7 +495,7 @@ extern "C" int pbd_get_rigid_bodies(pbd_engine *e, float *x, float *q, float *v,
 template <class V> static int upload_vec(DevBuf &buf, const V &v, cudaStream_t s) {  // V: std::vector / PodVector of PODs
     typedef typename V::value_type T;
     if (v.empty()) return 0;
-    if (buf.alloc(v.size() * sizeof(T) + 16)) return 1;
+    if (buf.alloc(v.size() * sizeof(T))) return 1;
     cudaError_t e = cudaMemcpyAsync(buf.p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice, s);
     if (e != cudaSuccess) return fail("upload -> %s", cudaGetErrorString(e));
     e = cudaStreamSynchronize(s);  // the host vector dies with the caller's scope
@@ -818,38 +819,39 @@ static int colour_if_needed(pbd_engine *e) {
     return 0;
 }
 
-// one type's planned arrays to the device, and its TypeArrays pointed at them
-static int upload_type(pbd_engine *e, int t, pbd_b200::TypePlan &p) {
+// The planned image in its one allocation (pbd_b200::image_layout): `ptr` pointed at every array (nullptr: the arrays without bytes), each
+// copied to its place, the zeroed regions -- the layout puts them last -- cleared by one memset.  Returns once the copies have read the plan.
+static int upload_image(pbd_engine *e, const pbd_b200::ImagePlan &plan, pbd_b200::ImagePointers &ptr) {
+    const pbd_b200::ImageLayout l = pbd_b200::image_layout(plan, e->batch.K);
+    CKE(e->image.alloc(l.bytes));
+    ptr = pbd_b200::ImagePointers{};
+    size_t zeroed = l.bytes;
+    for (const pbd_b200::ImageArray &a : l.arrays) {
+        if (!a.bytes) continue;
+        char *at = (char *)e->image.p + a.offset;
+        std::memcpy((char *)&ptr + a.slot, &at, sizeof(at));
+        if (a.zeroed) zeroed = std::min(zeroed, a.offset);
+        else CK(cudaMemcpyAsync(at, a.src, a.bytes, cudaMemcpyHostToDevice, e->stream));
+    }
+    if (zeroed < l.bytes) CK(cudaMemsetAsync((char *)e->image.p + zeroed, 0, l.bytes - zeroed, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+    return 0;
+}
+// one type of the uploaded image: its TypeArrays and rest tables, what of them is not an array, and a batch's shared material rows
+static int upload_type(pbd_engine *e, int t, pbd_b200::TypePlan &p, const pbd_b200::ImagePointers &ptr) {
     DevType &d = e->dev[t];
     const unsigned cnt = (unsigned)p.order.size();
     d.count = cnt;
     e->stats.constraints_per_type[t] = cnt;
-    d.arrays = TypeArrays{};
+    d.arrays = ptr.types[t]; d.rest = ptr.rest[t];
     d.order.swap(p.order);
     if (cnt == 0) return 0;
     TypeArrays &a = d.arrays;
-    if (!p.idx2.empty()) { CKE(upload_vec(d.idx[0], p.idx2, e->stream)); a.idx2 = (const uint2 *)d.idx[0].p; }
-    if (!p.idx4.empty()) { CKE(upload_vec(d.idx[0], p.idx4, e->stream)); a.idx4 = (const uint4 *)d.idx[0].p; }
-    for (int k = 0; k < 3; k++) if (!p.idx3[k].empty()) { CKE(upload_vec(d.idx[k], p.idx3[k], e->stream)); a.idx3[k] = (const unsigned *)d.idx[k].p; }
-    for (int k = 0; k < kMaxGeoV; k++) if (!p.gv[k].empty()) { CKE(upload_vec(d.gv[k], p.gv[k], e->stream)); a.gv[k] = (const float4 *)d.gv[k].p; }
-    for (int k = 0; k < kMaxGeoS; k++) if (!p.gs[k].empty()) { CKE(upload_vec(d.gs[k], p.gs[k], e->stream)); a.gs[k] = (const float *)d.gs[k].p; }
-    for (int k = 0; k < kMaxMat; k++) {
-        a.matU[k] = p.matU[k];
-        if (!p.mat[k].empty()) { CKE(upload_vec(d.mat[k], p.mat[k], e->stream)); a.mat[k] = (const float *)d.mat[k].p; }
-    }
+    for (int k = 0; k < kMaxMat; k++) a.matU[k] = p.matU[k];
     a.variant = p.variant;
-    if (!p.restBodies.empty()) {
-        CKE(upload_vec(d.restBodies, p.restBodies, e->stream)); CKE(upload_vec(d.restLocal, p.restLocal, e->stream)); CKE(upload_vec(d.restIds, d.order, e->stream));
-    }
     if (e->batch.K > 1 && type_shape(t).nMat && !((e->batch.matMask >> t) & 1u)) CKE(write_replica_materials(e, t, a.matU, 0));  // the shared parameters, for every replica
     if (t == PBD_BALLJOINT || t == PBD_RB_PARTICLE_BALLJOINT) {
         a.rbX = (float4 *)e->rbX.p; a.rbQ = (float4 *)e->rbQ.p; a.rbIinv = (const float4 *)e->rbIinv.p;
-    }
-    if (type_shape(t).xpbd) {
-        // replica r's multipliers at [r cnt, (r + 1) cnt); + 16 like the other streamed arrays: the L2 prefetch of a run rounds its end up to 16 bytes
-        CKE(d.lambda.alloc((size_t)e->batch.K * cnt * sizeof(float) + 16));
-        CK(cudaMemsetAsync(d.lambda.p, 0, (size_t)e->batch.K * cnt * sizeof(float), e->stream));
-        a.lambda = (float *)d.lambda.p;
     }
     return 0;
 }
@@ -872,12 +874,12 @@ static int derive_geometry(pbd_engine *e, const float4 *rest, GeoBufs *fresh, in
         if (!d.count || (rows && t != rowsType)) continue;
         DeriveArgs a{};
         a.rest = rest; a.n = e->n; a.count = d.count;
-        a.bodies = (const unsigned *)d.restBodies.p; a.ids = (const unsigned *)d.restIds.p; a.local = (const unsigned *)d.restLocal.p;
+        a.bodies = d.rest.bodies; a.ids = d.rest.ids; a.local = d.rest.local;
         a.clusters = d.arrays.gv[5]; a.variant = d.arrays.variant; a.rows = rows; a.fail = (unsigned long long *)failed.p;
         if (!rows) {
-            const size_t cnt = (size_t)e->batch.K * d.count;  // + 16 like the other streamed arrays: the L2 prefetch of a run rounds its end up
-            for (int k = 0; k < kMaxGeoV; k++) if (d.arrays.gv[k]) { CKE(fresh[t].gv[k].alloc(cnt * sizeof(float4) + 16)); a.gv[k] = (float4 *)fresh[t].gv[k].p; }
-            for (int k = 0; k < kMaxGeoS; k++) if (d.arrays.gs[k]) { CKE(fresh[t].gs[k].alloc(cnt * sizeof(float) + 16)); a.gs[k] = (float *)fresh[t].gs[k].p; }
+            const size_t cnt = (size_t)e->batch.K * d.count;
+            for (int k = 0; k < kMaxGeoV; k++) if (d.arrays.gv[k]) { CKE(fresh[t].gv[k].alloc(pbd_b200::padded_bytes(cnt * sizeof(float4)))); a.gv[k] = (float4 *)fresh[t].gv[k].p; }
+            for (int k = 0; k < kMaxGeoS; k++) if (d.arrays.gs[k]) { CKE(fresh[t].gs[k].alloc(pbd_b200::padded_bytes(cnt * sizeof(float)))); a.gs[k] = (float *)fresh[t].gs[k].p; }
         }
         CKE(with_geometry_type(t, [&](auto T) -> int {
             k_derive_geometry<decltype(T)::value><<<dim3(nblk(d.count, 128), e->batch.K), 128, 0, e->stream>>>(a);
@@ -909,9 +911,9 @@ static int apply_replica_geometry(pbd_engine *e, const float4 *rest, const char 
         const size_t cnt = (size_t)e->batch.K * d.count;
         if (!cnt) continue;
         for (int k = 0; k < kMaxGeoV; k++)
-            if (d.arrays.gv[k]) { CKE(d.repGv[k].alloc(cnt * sizeof(float4) + 16)); CK(cudaMemcpyAsync(d.repGv[k].p, fresh[t].gv[k].p, cnt * sizeof(float4), cudaMemcpyDeviceToDevice, e->stream)); }
+            if (d.arrays.gv[k]) { CKE(d.repGv[k].alloc(pbd_b200::padded_bytes(cnt * sizeof(float4)))); CK(cudaMemcpyAsync(d.repGv[k].p, fresh[t].gv[k].p, cnt * sizeof(float4), cudaMemcpyDeviceToDevice, e->stream)); }
         for (int k = 0; k < kMaxGeoS; k++)
-            if (d.arrays.gs[k]) { CKE(d.repGs[k].alloc(cnt * sizeof(float) + 16)); CK(cudaMemcpyAsync(d.repGs[k].p, fresh[t].gs[k].p, cnt * sizeof(float), cudaMemcpyDeviceToDevice, e->stream)); }
+            if (d.arrays.gs[k]) { CKE(d.repGs[k].alloc(pbd_b200::padded_bytes(cnt * sizeof(float)))); CK(cudaMemcpyAsync(d.repGs[k].p, fresh[t].gs[k].p, cnt * sizeof(float), cudaMemcpyDeviceToDevice, e->stream)); }
     }
     CK(cudaStreamSynchronize(e->stream));
     return 0;
@@ -963,20 +965,12 @@ static int flatten(pbd_engine *e) {
     if (!plan.residentRefusal.empty() && verbose()) fprintf(stderr, "[pbd_b200] auto mode: resident refused (%s), using the graph mode\n", plan.residentRefusal.c_str());
     if (!err.empty()) return fail("%s", err.c_str());
     CKE(relayout(e, plan.slot));
-    for (int t = 0; t < PBD_NUM_TYPES; t++) CKE(upload_type(e, t, plan.types[t]));
+    pbd_b200::ImagePointers ptr;
+    CKE(upload_image(e, plan, ptr));
+    for (int t = 0; t < PBD_NUM_TYPES; t++) CKE(upload_type(e, t, plan.types[t], ptr));
     e->buckets.swap(plan.buckets);
-    CKE(upload_vec(e->dBuckets, e->buckets, e->stream));
+    e->tables = ptr.tables;
     e->res = plan.res;
-    if (plan.mode == PBD_MODE_RESIDENT) {
-        CKE(upload_vec(e->dTileStart, plan.tileStart, e->stream));
-        CKE(upload_vec(e->dTileSmem, plan.tileSmem, e->stream));
-        CKE(upload_vec(e->dColourStart, plan.colourStart, e->stream));
-        CKE(upload_vec(e->dTileOff, plan.tileOff, e->stream));
-        CKE(upload_vec(e->dXNbr, plan.xNbr, e->stream));
-        CKE(upload_vec(e->dXMask, plan.xMask, e->stream));
-        CKE(e->dXFlags.alloc((size_t)e->res.G * e->res.C * kXFlagStride * sizeof(unsigned long long)));
-        CK(cudaMemsetAsync(e->dXFlags.p, 0, e->dXFlags.bytes, e->stream));
-    }
     CK(cudaStreamSynchronize(e->stream));
     lap("relayout + upload");
     if (e->batch.restShapes) CKE(apply_replica_geometry(e, (const float4 *)e->batch.restX.p, "pbd_set_replica_rest_positions (image planned again)"));  // the new image's geometry, from the rest positions the override was given
@@ -1201,10 +1195,9 @@ static int enqueue_step_resident(pbd_engine *e, cudaStream_t s, unsigned long lo
     const float h = e->dt / (float)e->subSteps;
     ResidentArgs ra;
     ra.pos = attr_ptr(e, PBD_ATTR_X); ra.vel = attr_ptr(e, PBD_ATTR_V); ra.oldp = attr_ptr(e, PBD_ATTR_OLDX); ra.lastp = attr_ptr(e, PBD_ATTR_LASTX);
-    ra.buckets = (const Bucket *)e->dBuckets.p;
-    ra.colourStart = (const unsigned *)e->dColourStart.p; ra.tileOff = (const unsigned *)e->dTileOff.p;
-    ra.tileStart = (const unsigned *)e->dTileStart.p; ra.tileSmem = (const unsigned *)e->dTileSmem.p;
-    ra.xNbr = (const unsigned *)e->dXNbr.p; ra.xMask = (const unsigned *)e->dXMask.p;
+    const pbd_b200::ImageTables &tb = e->tables;
+    ra.buckets = tb.buckets; ra.colourStart = tb.colourStart; ra.tileOff = tb.tileOff; ra.tileStart = tb.tileStart; ra.tileSmem = tb.tileSmem;
+    ra.xNbr = tb.xNbr; ra.xMask = tb.xMask; ra.xFlags = tb.xFlags;
     const bool batch = e->res.replicas > 1;  // the tables hold the C tiles of one replica
     ra.nBuckets = (unsigned)e->buckets.size(); ra.nColours = e->res.nColours; ra.nTiles = batch ? e->res.C : e->res.G * e->res.C; ra.subSteps = e->subSteps; ra.maxIter = e->maxIter;
     ra.tileCap = e->res.tileCap; ra.xThreads = e->res.xThreads; ra.clusterSize = e->res.C;
@@ -1220,7 +1213,6 @@ static int enqueue_step_resident(pbd_engine *e, cudaStream_t s, unsigned long lo
     }
     ra.h = h; ra.invH = (float)(1.0 / (double)h); ra.twoInvH = (float)(2.0 / (double)h); ra.gx = e->g[0]; ra.gy = e->g[1]; ra.gz = e->g[2];
     ra.secondOrder = e->velMethod;
-    ra.xFlags = (unsigned long long *)e->dXFlags.p;
     ra.xLaunch = (++e->xLaunch) << 32;  // above every flag value of the earlier launches, whatever subSteps / maxIter they ran with
     ra.rb = rb_state(e);
     for (int t = 0; t < PBD_NUM_TYPES; t++) { ra.types[t] = batch_arrays(e, t); ra.lamCount[t] = e->dev[t].count; ra.geoCount[t] = replica_geo(e, t); }
@@ -1536,7 +1528,7 @@ extern "C" int pbd_get_lambdas(pbd_engine *e, int type, float *dst, unsigned *id
     DevType &d = e->dev[type];
     if (d.count == 0) return 0;
     CK(cudaStreamSynchronize(e->stream));
-    CK(cudaMemcpy(dst, d.lambda.p, (size_t)e->batch.K * d.count * sizeof(float), cudaMemcpyDeviceToHost));  // replica after replica
+    CK(cudaMemcpy(dst, d.arrays.lambda, (size_t)e->batch.K * d.count * sizeof(float), cudaMemcpyDeviceToHost));  // replica after replica
     if (ids) memcpy(ids, d.order.data(), (size_t)d.count * sizeof(unsigned));
     return 0;
 }

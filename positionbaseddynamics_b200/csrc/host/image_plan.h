@@ -90,4 +90,23 @@ std::string batch_refusal(unsigned replicas, unsigned n, int mode, unsigned nRb,
 // Plans the image of `in` into `out`; returns "" or why the model cannot be flattened (for this mode and, resident, this device).
 std::string plan_image(const PlanInput &in, ImagePlan &out);
 
+// Device bytes an array of `bytes` takes: the L2 prefetch of a run (resident.cuh: l2_prefetch_bytes) rounds its end up to 16 bytes, so
+// every streamed array is followed by 16 bytes of its own allocation.
+inline size_t padded_bytes(size_t bytes) { return bytes + 16; }
+
+// What the device addresses of an image's arrays become: every type's TypeArrays, the tables a batch's per-replica geometry is derived
+// from (pbdk::DeriveArgs: TypePlan::restBodies / restLocal, and the insertion ids in device order), and the image-wide tables.  Every
+// pointer in it has the representation of a char *.
+struct RestTables { const unsigned *bodies, *local, *ids; };
+struct ImageTables { const pbdk::Bucket *buckets; const unsigned *colourStart, *tileOff, *tileStart, *tileSmem, *xNbr, *xMask; unsigned long long *xFlags; };
+struct ImagePointers { pbdk::TypeArrays types[PBD_NUM_TYPES]; RestTables rest[PBD_NUM_TYPES]; ImageTables tables; };
+
+// One device array of an image: its name (the record of the CPU planner drivers), its host source or `zeroed` (the region starts zeroed),
+// its place in the image's allocation, and the pointer of ImagePointers it becomes (`slot`: its byte offset there).
+struct ImageArray { std::string name; const void *src; size_t bytes; bool zeroed; size_t slot, offset; };
+struct ImageLayout { std::vector<ImageArray> arrays; size_t bytes = 0; };
+// Every array the image `p` of a batch of `replicas` may hold, laid out in one allocation of `bytes` (arrays without bytes take no room):
+// the plan's arrays, then the zeroed regions -- the XPBD multipliers and the resident mode's X arrival flags.  The sources point into `p`.
+ImageLayout image_layout(const ImagePlan &p, unsigned replicas);
+
 }  // namespace pbd_b200

@@ -45,7 +45,6 @@
 namespace pbdk {
 
 // (the index encoding, tile swizzle, run table and shared-memory layout of the image are defined in device_image.h)
-constexpr unsigned kXFlagStride = 16;     // unsigned long longs: every CTA's arrival flag on its own 128-byte line
 // PBD_B200_TRACE record per (phase, CTA): [0] phase start, [1] X items done, [2] other items done + colour arrive issued,
 // [3] colour wait returned, [4] X wait returned (0 where the CTA has no X items in the phase); tools/trace_resident.py
 constexpr unsigned kTraceSlots = 5;

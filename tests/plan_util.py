@@ -72,10 +72,10 @@ class Scene:
         return col
 
 
-def plan(driver, tmp_path, sc, mode, shape=(0, 0), threads=None, tag="p", max_clusters=132):
-    """The plan of `sc` in `mode` on a device of 132 SMs that keeps `max_clusters` clusters of any shape co-resident."""
+def plan(driver, tmp_path, sc, mode, shape=(0, 0), threads=None, tag="p", max_clusters=132, replicas=1, rest_tables=False):
+    """The plan of `replicas` replicas of `sc` in `mode` on a device of 132 SMs that keeps `max_clusters` clusters of any shape co-resident."""
     x0 = np.zeros((sc.n, 4), np.float32); x0[:, :3] = sc.x0
-    head = [sc.n, sc.nrb, sc.N, mode, 0, shape[0], shape[1], 132, max_clusters, len(sc.off) - 1]
+    head = [replicas, sc.n, sc.nrb, sc.N, mode, int(rest_tables), shape[0], shape[1], 132, max_clusters, len(sc.off) - 1]
     parts = [np.asarray(head, np.uint32), sc.off, sc.ids, x0]
     for ids, b, p in sc.store:
         parts += [np.asarray([len(ids)], np.uint32), ids, b, p]
@@ -106,8 +106,9 @@ def mode_of(p):
 
 
 def same_image(a, b, *skip):
-    """The plans `a` and `b` are byte-identical, apart from the refusal and the records in `skip`."""
-    drop = {"raw", "residentRefusal"} | set(skip)
+    """The plans `a` and `b` are byte-identical, apart from the refusal, the layout (its multipliers and X flags are sized by the batch and
+    the clusters launched, not by the image) and the records in `skip`."""
+    drop = {"raw", "residentRefusal", "layout"} | set(skip)
     return {k: v for k, v in a.items() if k not in drop} == {k: v for k, v in b.items() if k not in drop}
 
 

@@ -182,6 +182,26 @@ int pbd_set_contact_params(pbd_engine *e, float tolerance, float stiffness, unsi
  * (particle, body) and the number found (which may exceed what was kept) */
 int pbd_record_contacts(pbd_engine *e, unsigned capacity);
 int pbd_get_contacts(pbd_engine *e, pbd_contact *out, unsigned capacity, unsigned *count);
+/* Contacts of a replica batch (K > 1).  pc: nParticleColliders particle ranges of ONE replica's particles, shared by every replica
+ * (as pbd_set_colliders).  rc: K*nRigidColliders rigid colliders, replica after replica; replica r's list may differ from the
+ * others in everything: shape, dims, thickness, invert_sdf, coefficients, R, v1, v2, aabb.  body_x / body_v / body_omega:
+ * K*nRigidColliders*3 floats each.  They are the centre of mass, velocity and angular velocity of the static body carrying each
+ * collider.  body_v and body_omega may be NULL (= 0).  rc[i].body is only the id reported in pbd_contact.body.
+ * Replica r then advances bit for bit as a single-scene engine given
+ *   pbd_set_rigid_bodies(nR, masses 0, body_x of replica r, ..., body_v / body_omega of replica r)
+ *   and pbd_set_colliders(nP, pc, nR, rc + r*nR) with rc[i].body = i.
+ * nRigidColliders = 0 or rc = NULL: no contacts.  A replica that needs fewer colliders gives the others an empty box
+ * (aabb_min > aabb_max), which no particle passes.
+ * Refused, with the colliders of the previous call left in force: at K = 1, more than 8 rigid colliders per replica, an unknown shape,
+ * a particle range beyond n, body_x = NULL with nRigidColliders > 0.  Calling again with the same nParticleColliders and
+ * nRigidColliders copies the new rows in stream order into device tables that keep their address, without a host synchronisation: the
+ * next step enqueued (pbd_step, pbd_step_host_async, ...) reads them, so obstacles may move per replica between any two steps.  A call
+ * that changes either count, or switches the contacts on or off, may synchronise.  pbd_set_replicas drops them; nothing else does.
+ * pbd_set_contact_params is shared by all replicas.  pbd_get_contacts reports particle = r*n + i (the index in the K*n state arrays)
+ * and body = rc.body, sorted by (particle, body), i.e. replica after replica; the recording capacity is shared by all replicas. */
+int pbd_set_replica_colliders(pbd_engine *e, unsigned nParticleColliders, const pbd_particle_collider *pc,
+                              unsigned nRigidColliders, const pbd_rigid_collider *rc,
+                              const float *body_x, const float *body_v, const float *body_omega);
 
 /* ---- Replica batch: K independent copies of one model's state stepped together on one device ---------------------------------
  * One engine holds one model (particles, constraints, groups, parameters) and K copies of its state; one pbd_step advances all K,
@@ -195,8 +215,10 @@ int pbd_get_contacts(pbd_engine *e, pbd_contact *out, unsigned capacity, unsigne
  *  - Constraint parameters, gravity and the geometry of the rest state (rest lengths and angles, Q, inverse rest matrices, areas,
  *    volumes, shape-matching rest shapes) are shared unless pbd_set_replica_materials / pbd_set_replica_gravity /
  *    pbd_set_replica_rest_positions (below) give every replica its own.
+ *  - Contacts: every replica against its own static colliders through pbd_set_replica_colliders (contact section above); the
+ *    colliders of pbd_set_colliders belong to one scene.
  *  - pbd_get_stats: projections and bytes_per_step count every replica; num_particles and num_constraints are per replica.
- *  - K > 1 is refused with rigid bodies or joints, with colliders and in PBD_MODE_JACOBI.  PBD_MODE_RESIDENT runs one cluster of CTAs
+ *  - K > 1 is refused with rigid bodies or joints, with pbd_set_colliders' colliders and in PBD_MODE_JACOBI.  PBD_MODE_RESIDENT runs one cluster of CTAs
  *    per replica and refuses a replica that does not fit one cluster; PBD_MODE_AUTO then runs the graph mode.
  * pbd_set_replicas: 1 <= K <= 65535 and K*n < 2^31.  Every replica starts as a copy of replica 0's current state (x, v, x0, oldX,
  * lastX, masses), the XPBD multipliers at zero, and the image is planned again.  At K = 1 every call behaves as for one scene. */

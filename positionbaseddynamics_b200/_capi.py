@@ -27,7 +27,7 @@ SYMBOLS = ["pbd_last_error", "pbd_device_count", "pbd_create", "pbd_destroy", "p
            "pbd_get_lambdas", "pbd_get_stats", "pbd_profile_step", "pbd_set_replicas", "pbd_get_replicas",
            "pbd_num_materials", "pbd_set_replica_materials", "pbd_set_replica_gravity",
            "pbd_set_replica_rest_positions", "pbd_get_replica_geometry",
-           "pbd_set_colliders", "pbd_set_contact_params", "pbd_record_contacts", "pbd_get_contacts"]
+           "pbd_set_colliders", "pbd_set_contact_params", "pbd_record_contacts", "pbd_get_contacts", "pbd_set_replica_colliders"]
 
 
 SHAPE_BOX, SHAPE_SPHERE, SHAPE_TORUS, SHAPE_CYLINDER, SHAPE_HOLLOW_SPHERE, SHAPE_HOLLOW_BOX = range(6)
@@ -96,6 +96,7 @@ def lib():
         _lib.pbd_step_host_async.argtypes = [C.c_void_p, C.c_uint, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         _lib.pbd_step_host_wait.argtypes = [C.c_void_p, C.c_uint]
         _lib.pbd_set_colliders.argtypes = [C.c_void_p, C.c_uint, C.c_void_p, C.c_uint, C.c_void_p]
+        _lib.pbd_set_replica_colliders.argtypes = [C.c_void_p, C.c_uint, C.c_void_p, C.c_uint, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         _lib.pbd_set_contact_params.argtypes = [C.c_void_p, C.c_float, C.c_float, C.c_uint]
         _lib.pbd_record_contacts.argtypes = [C.c_void_p, C.c_uint]
         _lib.pbd_get_contacts.argtypes = [C.c_void_p, C.c_void_p, C.c_uint, C.POINTER(C.c_uint)]
@@ -154,7 +155,7 @@ class Engine:
     A replica batch (set_replicas(K), K > 1) steps K independent copies of the model's state at once: the particle state calls then
     take and return (K, n, 3) / (K, n) arrays and lambdas() (K, count); at K = 1 the shapes are those of one scene.  The replicas share
     the model's parameters, gravity and rest geometry unless set_replica_materials / set_replica_gravity / set_replica_rest_positions
-    give each its own."""
+    give each its own; set_replica_colliders gives each replica its own static colliders."""
 
     def __init__(self, device=0, stream=None):
         self._h = C.c_void_p()
@@ -343,6 +344,29 @@ class Engine:
         pa = (ParticleCollider * max(len(particle_colliders), 1))(*particle_colliders)
         ra = (RigidCollider * max(len(rigid_colliders), 1))(*rigid_colliders)
         _ck(lib().pbd_set_colliders(self._h, len(particle_colliders), C.cast(pa, C.c_void_p), len(rigid_colliders), C.cast(ra, C.c_void_p)))
+
+    def set_replica_colliders(self, particle_colliders, rigid_colliders, body_x=None, body_v=None, body_omega=None):
+        """pbd_set_replica_colliders: every replica against its own static colliders.  particle_colliders: ParticleCollider ranges of
+        one replica's particles, shared by all; rigid_colliders: K lists of nR RigidCollider, one per replica; body_x / body_v / body_omega:
+        (K, nR, 3) centre of mass, velocity and angular velocity of the static body carrying each collider (v, omega: None = 0).
+        rigid_colliders None: no contacts.  K > 1 only."""
+        if rigid_colliders is None:
+            _ck(lib().pbd_set_replica_colliders(self._h, 0, None, 0, None, None, None, None))
+            return
+        if len(rigid_colliders) != self.K or len(set(len(r) for r in rigid_colliders)) > 1:
+            raise ValueError("set_replica_colliders: wants %d lists of the same number of rigid colliders, got %s" % (self.K, [len(r) for r in rigid_colliders]))
+        nr = len(rigid_colliders[0]) if len(rigid_colliders) else 0
+        flat = [c for r in rigid_colliders for c in r]
+        arrays = []
+        for name, a in (("body_x", body_x), ("body_v", body_v), ("body_omega", body_omega)):
+            if a is not None:
+                a = _f32(a)
+                if a.shape != (self.K, nr, 3):
+                    raise ValueError("set_replica_colliders: %s wants a (%d, %d, 3) array, got %s" % (name, self.K, nr, a.shape))
+            arrays.append(a)
+        pa = (ParticleCollider * max(len(particle_colliders), 1))(*particle_colliders)
+        ra = (RigidCollider * max(len(flat), 1))(*flat)
+        _ck(lib().pbd_set_replica_colliders(self._h, len(particle_colliders), C.cast(pa, C.c_void_p), nr, C.cast(ra, C.c_void_p), *[_ptr(a) for a in arrays]))
 
     def set_contact_params(self, tolerance=0.01, stiffness=100.0, max_iter_v=5):
         _ck(lib().pbd_set_contact_params(self._h, float(tolerance), float(stiffness), int(max_iter_v)))

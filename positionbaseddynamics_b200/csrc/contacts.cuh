@@ -15,6 +15,9 @@
 // bounding-sphere hierarchy; with exact (1-Lipschitz) distance functions the set of points that pass collisionTest is the same as
 // testing every point, which is what one thread per particle does.  Dynamic bodies in contact, rigid-rigid and particle-tet contacts
 // stay on the reference's CPU time step (the engine and the adapter refuse them).
+//
+// A replica batch runs the same per-particle body as k_contacts_batch: replica r's particles against replica r's own colliders and
+// static bodies, one grid row per replica, each replica computing what k_contacts computes for it alone.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -47,6 +50,9 @@ struct ContactArgs {
     unsigned total;
     float tolerance, stiffness; unsigned maxIterV;
     ContactRecord *record; unsigned *recordCount; unsigned recordCap;
+    // replica batch (k_contacts_batch): particles per replica.  Replica r's particles sit at slots r n + slot[i], its colliders at
+    // rigid[r nRigid ..] and the bodies carrying them at rbX / rbV / rbW[r nRigid ..], one body per collider
+    unsigned n = 0;
 };
 
 // ---- distance functions (double precision, as the reference evaluates them) ------------------------------------------------------
@@ -118,20 +124,23 @@ __device__ __forceinline__ bool collision_test(const RigidCollider &c, const flo
 struct LiveContact {  // ParticleRigidBodyContactConstraint: m_constraintInfo (3x5), m_sum_impulses, m_frictionCoeff
     float cp0[3], cp1[3], n[3], t[3];
     float nKnInv, pMax, goal, sum, friction;
-    unsigned body;
+    unsigned body;  // where the carrying body's state sits in rbX / rbV / rbW
 };
 
 // One thread per particle of the registered triangle / tet models: collision test against every rigid collider in list order (the
 // order of the reference's contact list for this particle), contact initialisation with the velocities before any contact impulse,
-// then maxIterV sweeps over the particle's contacts.
-__global__ void __launch_bounds__(128) k_contacts(const ContactArgs A) {
-    const unsigned gid = blockIdx.x * blockDim.x + threadIdx.x;
+// then maxIterV sweeps over the particle's contacts.  BATCH: the particle, colliders and bodies of replica `replica` (ContactArgs::n);
+// one scene: the body of a collider is its `body`, which indexes rbX / rbV / rbW.
+template <bool BATCH>
+__device__ __forceinline__ void contacts_particle(const ContactArgs &A, const unsigned gid, const unsigned replica) {
     if (gid >= A.total) return;
     unsigned r = 0;
     while (r + 1 < A.nRanges && gid >= A.rangeStart[r + 1]) r++;
     const ParticleCollider pc = A.ranges[r];
     const unsigned particle = pc.offset + (gid - A.rangeStart[r]);
-    const unsigned slot = A.slot[particle];
+    const unsigned first = BATCH ? replica * A.nRigid : 0u;      // the replica's first collider and body
+    const unsigned shift = BATCH ? replica * A.n : 0u;           // the replica's first particle
+    const unsigned slot = shift + A.slot[particle];
     const float4 X = A.pos[slot];
     float4 V; bool haveV = false;  // the velocity is fetched for candidates only: most particles leave after the bounding-box tests
     const float invMass0 = X.w;
@@ -139,11 +148,12 @@ __global__ void __launch_bounds__(128) k_contacts(const ContactArgs A) {
     LiveContact live[kMaxRigidColliders];
     unsigned nLive = 0;
     for (unsigned k = 0; k < A.nRigid; k++) {
-        const RigidCollider &c = A.rigid[k];
+        const RigidCollider &c = A.rigid[first + k];
+        const unsigned body = BATCH ? first + k : c.body;
         // candidates outside the collider's (tolerance-extended) bounding box never reach collisionTest in the reference either
         if (X.x < c.aabbMin[0] || X.y < c.aabbMin[1] || X.z < c.aabbMin[2] || X.x > c.aabbMax[0] || X.y > c.aabbMax[1] || X.z > c.aabbMax[2]) continue;
         if (!haveV) { V = A.vel[slot]; haveV = true; }
-        const float4 com = A.rbX[c.body];
+        const float4 com = A.rbX[body];
         const float d[3] = {X.x - com.x, X.y - com.y, X.z - com.z};
         float xl[3], cp[3], nl[3], dist;
         for (int i = 0; i < 3; i++) xl[i] = c.R[3 * i] * d[0] + c.R[3 * i + 1] * d[1] + c.R[3 * i + 2] * d[2] + c.v1[i];
@@ -154,10 +164,10 @@ __global__ void __launch_bounds__(128) k_contacts(const ContactArgs A) {
             L.n[i] = c.R[i] * nl[0] + c.R[3 + i] * nl[1] + c.R[6 + i] * nl[2];
         }
         L.cp0[0] = X.x; L.cp0[1] = X.y; L.cp0[2] = X.z;
-        L.body = c.body; L.friction = pc.friction + c.friction; L.sum = 0.0f;
+        L.body = body; L.friction = pc.friction + c.friction; L.sum = 0.0f;
         const float restitution = pc.restitution * c.restitution;
         // init_ParticleRigidBodyContactConstraint (body 1 static: K = invMass0 * I)
-        const float4 v1 = A.rbV[c.body], w1 = A.rbW[c.body];
+        const float4 v1 = A.rbV[body], w1 = A.rbW[body];
         const float r1[3] = {L.cp1[0] - com.x, L.cp1[1] - com.y, L.cp1[2] - com.z};
         const float u1[3] = {v1.x + (w1.y * r1[2] - w1.z * r1[1]), v1.y + (w1.z * r1[0] - w1.x * r1[2]), v1.z + (w1.x * r1[1] - w1.y * r1[0])};
         const float ur[3] = {V.x - u1[0], V.y - u1[1], V.z - u1[2]};
@@ -172,7 +182,7 @@ __global__ void __launch_bounds__(128) k_contacts(const ContactArgs A) {
         if (A.record) {
             const unsigned at = atomicAdd(A.recordCount, 1u);
             if (at < A.recordCap) {
-                ContactRecord rec; rec.particle = particle; rec.body = c.body; rec.dist = dist;
+                ContactRecord rec; rec.particle = shift + particle; rec.body = c.body; rec.dist = dist;
                 for (int i = 0; i < 3; i++) { rec.cp0[i] = L.cp0[i]; rec.cp1[i] = L.cp1[i]; rec.n[i] = L.n[i]; }
                 A.record[at] = rec;
             }
@@ -207,5 +217,9 @@ __global__ void __launch_bounds__(128) k_contacts(const ContactArgs A) {
     }
     A.vel[slot] = V;
 }
+
+__global__ void __launch_bounds__(128) k_contacts(const ContactArgs A) { contacts_particle<false>(A, blockIdx.x * blockDim.x + threadIdx.x, 0u); }
+// grid (ceil(total / 128), K): replica = blockIdx.y, so that every collider and body load of a block is uniform
+__global__ void __launch_bounds__(128) k_contacts_batch(const ContactArgs A) { contacts_particle<true>(A, blockIdx.x * blockDim.x + threadIdx.x, blockIdx.y); }
 
 }  // namespace pbdk

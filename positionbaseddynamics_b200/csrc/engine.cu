@@ -142,6 +142,14 @@ struct pbd_engine {
     DevBuf dPColliders, dRColliders, dRangeStart, dContacts, dContactCount;
     unsigned contactTotal = 0, contactCap = 0;
     float contactTolerance = 0.01f, contactStiffness = 100.0f; unsigned maxIterV = 5;  // CollisionDetection.cpp:25, SimulationModel.cpp:34, TimeStepController.cpp:23
+    // contacts of a replica batch (pbd_set_replica_colliders): one replica's particle ranges, K x nRigid colliders and the bodies carrying
+    // them, replica after replica (rbX / rbV / rbW as float4, one body per collider).  The device tables keep their address while nP and
+    // nRigid stay, so that new rows are copied in stream order between steps.  nRigid == 0: off.
+    struct ReplicaColliders {
+        std::vector<ParticleCollider> ranges;
+        unsigned nRigid = 0, total = 0;
+        DevBuf dRanges, dStart, dRigid, dX, dV, dW;
+    } repColliders;
     bool timingPending = false;
     std::vector<unsigned> slot;          // host particle index -> device slot (formula layouts or the tile-major permutation)
     DevBuf dSlot, dSlotOld, relayoutTmp;
@@ -339,10 +347,16 @@ extern "C" int pbd_set_particles(pbd_engine *e, unsigned n, const float *x, cons
     return 0;
 }
 
-// collider-based contacts run one scene per engine: the contact kernel indexes particles of one replica
+// pbd_set_colliders' colliders belong to one scene; a batch takes its own per replica (pbd_set_replica_colliders)
 static int collider_refusal(const pbd_engine *e, unsigned K, size_t nColliders) {
-    if (K > 1 && nColliders) return fail("replica batch: colliders (pbd_set_colliders) are stepped one scene per engine (pbd_set_replicas 1)");
+    if (K > 1 && nColliders)
+        return fail("replica batch: colliders of pbd_set_colliders are stepped one scene per engine (pbd_set_replicas 1); a batch takes per-replica colliders from pbd_set_replica_colliders");
     return 0;
+}
+static void drop_replica_colliders(pbd_engine *e) {
+    pbd_engine::ReplicaColliders &c = e->repColliders;
+    c.ranges.clear(); c.nRigid = c.total = 0;
+    for (DevBuf *b : {&c.dRanges, &c.dStart, &c.dRigid, &c.dX, &c.dV, &c.dW}) b->release();
 }
 
 extern "C" int pbd_set_replicas(pbd_engine *e, unsigned K) {
@@ -356,6 +370,7 @@ extern "C" int pbd_set_replicas(pbd_engine *e, unsigned K) {
     e->batch.K = K;
     e->batch.mat.release(); e->batch.gravity.release(); e->batch.matMask = 0; e->batch.gravitySet = false;  // rows of the old K
     drop_replica_geometry(e);
+    drop_replica_colliders(e);
     CK(cudaStreamSynchronize(e->stream));
     model_changed(e);  // every replica is redefined: planned again, with the shared material rows and zero multipliers
     return 0;
@@ -1290,29 +1305,41 @@ static int enqueue_step_jacobi(pbd_engine *e, cudaStream_t s, unsigned long long
 // ------------------------------------------------------------------------------------------------------------
 // contact path (contacts.cuh)
 // ------------------------------------------------------------------------------------------------------------
+// the kernel's form of a pbd_rigid_collider; refused: an unknown shape
+static int convert_collider(const char *what, unsigned i, const pbd_rigid_collider &c, RigidCollider &d) {
+    if (c.shape < 0 || c.shape >= kNumShapes) return fail("%s: rigid collider %u has unknown shape %d", what, i, c.shape);
+    d.shape = c.shape; d.body = c.body; d.thickness = c.thickness; d.invert = c.invert_sdf ? -1.0f : 1.0f; d.restitution = c.restitution; d.friction = c.friction;
+    for (int k = 0; k < 3; k++) { d.dim[k] = c.dim[k]; d.v1[k] = c.v1[k]; d.v2[k] = c.v2[k]; d.aabbMin[k] = c.aabb_min[k]; d.aabbMax[k] = c.aabb_max[k]; }
+    for (int k = 0; k < 9; k++) d.R[k] = c.R[k];
+    return 0;
+}
+// one replica's particle ranges and the prefix sums of their counts; refused: a range beyond the engine's n particles
+static int convert_ranges(const pbd_engine *e, const char *what, unsigned nP, const pbd_particle_collider *pc, std::vector<ParticleCollider> &P,
+                          std::vector<unsigned> &start) {
+    P.resize(nP); start.assign(nP + 1, 0u);
+    for (unsigned i = 0; i < nP; i++) {
+        if ((unsigned long long)pc[i].offset + pc[i].count > e->n) return fail("%s: particle collider %u covers [%u, %u), the engine holds %u particles", what, i, pc[i].offset, pc[i].offset + pc[i].count, e->n);
+        P[i].offset = pc[i].offset; P[i].count = pc[i].count; P[i].restitution = pc[i].restitution; P[i].friction = pc[i].friction;
+        start[i + 1] = start[i] + pc[i].count;
+    }
+    return 0;
+}
+
 extern "C" int pbd_set_colliders(pbd_engine *e, unsigned nP, const pbd_particle_collider *pc, unsigned nR, const pbd_rigid_collider *rc) {
     if (!e || (nP && !pc) || (nR && !rc)) return fail("pbd_set_colliders: null argument");
     CKE(collider_refusal(e, e->batch.K, (size_t)nP + nR));
     CKE(use(e));
     if (nR > (unsigned)kMaxRigidColliders) return fail("pbd_set_colliders: %u rigid colliders (the contact kernel keeps up to %d contacts per particle)", nR, kMaxRigidColliders);
-    std::vector<ParticleCollider> P(nP);
+    std::vector<ParticleCollider> P;
     std::vector<RigidCollider> R(nR);
-    std::vector<unsigned> start(nP + 1, 0u);
-    for (unsigned i = 0; i < nP; i++) {
-        if ((unsigned long long)pc[i].offset + pc[i].count > e->n) return fail("pbd_set_colliders: particle collider %u covers [%u, %u), the engine holds %u particles", i, pc[i].offset, pc[i].offset + pc[i].count, e->n);
-        P[i].offset = pc[i].offset; P[i].count = pc[i].count; P[i].restitution = pc[i].restitution; P[i].friction = pc[i].friction;
-        start[i + 1] = start[i] + pc[i].count;
-    }
+    std::vector<unsigned> start;
+    CKE(convert_ranges(e, "pbd_set_colliders", nP, pc, P, start));
     for (unsigned i = 0; i < nR; i++) {
         const pbd_rigid_collider &c = rc[i];
-        if (c.shape < 0 || c.shape >= kNumShapes) return fail("pbd_set_colliders: rigid collider %u has unknown shape %d", i, c.shape);
+        CKE(convert_collider("pbd_set_colliders", i, c, R[i]));
         if (c.body >= e->nRb) return fail("pbd_set_colliders: rigid collider %u refers to rigid body %u, the engine holds %u (pbd_set_rigid_bodies first)", i, c.body, e->nRb);
         if (e->rbMass[c.body] != 0.0f)
             return fail("pbd_set_colliders: rigid body %u has mass %g; contacts with dynamic bodies couple through the body and stay on the CPU time step (static colliders only)", c.body, e->rbMass[c.body]);
-        RigidCollider &d = R[i];
-        d.shape = c.shape; d.body = c.body; d.thickness = c.thickness; d.invert = c.invert_sdf ? -1.0f : 1.0f; d.restitution = c.restitution; d.friction = c.friction;
-        for (int k = 0; k < 3; k++) { d.dim[k] = c.dim[k]; d.v1[k] = c.v1[k]; d.v2[k] = c.v2[k]; d.aabbMin[k] = c.aabb_min[k]; d.aabbMax[k] = c.aabb_max[k]; }
-        for (int k = 0; k < 9; k++) d.R[k] = c.R[k];
     }
     CK(cudaStreamSynchronize(e->stream));
     e->pColliders.swap(P); e->rColliders.swap(R);
@@ -1320,6 +1347,48 @@ extern "C" int pbd_set_colliders(pbd_engine *e, unsigned nP, const pbd_particle_
     if (nP) { CKE(upload_vec(e->dPColliders, e->pColliders, e->stream)); CKE(upload_vec(e->dRangeStart, start, e->stream)); }
     if (nR) CKE(upload_vec(e->dRColliders, e->rColliders, e->stream));
     CK(cudaStreamSynchronize(e->stream));
+    return 0;
+}
+extern "C" int pbd_set_replica_colliders(pbd_engine *e, unsigned nP, const pbd_particle_collider *pc, unsigned nR, const pbd_rigid_collider *rc,
+                                         const float *body_x, const float *body_v, const float *body_omega) {
+    CKE(replica_params_refusal(e, "pbd_set_replica_colliders"));
+    if (!rc) nR = 0;
+    if (nP && !pc) return fail("pbd_set_replica_colliders: null argument");
+    if (nR && !body_x) return fail("pbd_set_replica_colliders: body_x == NULL with %u rigid colliders per replica", nR);
+    if (nR > (unsigned)kMaxRigidColliders) return fail("pbd_set_replica_colliders: %u rigid colliders per replica (the contact kernel keeps up to %d contacts per particle)", nR, kMaxRigidColliders);
+    CKE(use(e));
+    const unsigned K = e->batch.K;
+    const size_t rows = (size_t)K * nR;
+    std::vector<ParticleCollider> P;
+    std::vector<unsigned> start;
+    CKE(convert_ranges(e, "pbd_set_replica_colliders", nP, pc, P, start));
+    std::vector<RigidCollider> R(rows);
+    for (size_t i = 0; i < rows; i++) CKE(convert_collider("pbd_set_replica_colliders", (unsigned)i, rc[i], R[i]));
+    std::vector<float4> X(rows), V(rows), W(rows);  // the static bodies: w = inverse mass / mass / unused, all 0
+    for (size_t i = 0; i < rows; i++) {
+        X[i] = make_float4(body_x[3 * i], body_x[3 * i + 1], body_x[3 * i + 2], 0.f);
+        V[i] = body_v ? make_float4(body_v[3 * i], body_v[3 * i + 1], body_v[3 * i + 2], 0.f) : make_float4(0.f, 0.f, 0.f, 0.f);
+        W[i] = body_omega ? make_float4(body_omega[3 * i], body_omega[3 * i + 1], body_omega[3 * i + 2], 0.f) : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    pbd_engine::ReplicaColliders &c = e->repColliders;
+    if (nR == 0) {  // off
+        CK(cudaStreamSynchronize(e->stream));
+        drop_replica_colliders(e);
+        return 0;
+    }
+    const struct { DevBuf *d; const void *h; size_t bytes; } up[] = {
+        {&c.dRanges, P.data(), nP * sizeof(ParticleCollider)}, {&c.dStart, start.data(), (nP + 1) * sizeof(unsigned)},
+        {&c.dRigid, R.data(), rows * sizeof(RigidCollider)}, {&c.dX, X.data(), rows * sizeof(float4)}, {&c.dV, V.data(), rows * sizeof(float4)},
+        {&c.dW, W.data(), rows * sizeof(float4)}};
+    if (nP != c.ranges.size() || nR != c.nRigid) {  // new table sizes: allocated again once the steps in flight are done
+        CK(cudaStreamSynchronize(e->stream));
+        drop_replica_colliders(e);
+        for (const auto &u : up) CKE(u.d->alloc(u.bytes));
+    }
+    // Stream-ordered copies into tables that keep their address: the next step enqueued reads the new rows, the steps before it the old
+    // ones.  The sources are pageable, so the driver has staged them when the call returns and the vectors may go.
+    for (const auto &u : up) if (u.bytes) CK(cudaMemcpyAsync(u.d->p, u.h, u.bytes, cudaMemcpyHostToDevice, e->stream));
+    c.ranges.swap(P); c.nRigid = nR; c.total = start[nP];
     return 0;
 }
 extern "C" int pbd_set_contact_params(pbd_engine *e, float tolerance, float stiffness, unsigned maxIterationsV) {
@@ -1357,22 +1426,34 @@ extern "C" int pbd_get_contacts(pbd_engine *e, pbd_contact *out, unsigned capaci
     return 0;
 }
 // after the substeps of a step: collision detection + velocity-level contact solve (TimeStepController.cpp:189-196)
+// A batch's replica colliders (pbd_set_replica_colliders) run k_contacts_batch, one grid row per replica; pbd_set_colliders' k_contacts.
 static int enqueue_contacts(pbd_engine *e, cudaStream_t s, unsigned long long *launches) {
-    if (e->rColliders.empty() || e->contactTotal == 0) return 0;
-    for (const RigidCollider &c : e->rColliders)  // the bodies may have been replaced since pbd_set_colliders
-        if (c.body >= e->nRb || e->rbMass[c.body] != 0.0f) return fail("contact path: collider on rigid body %u, which is missing or not static any more (pbd_set_colliders again)", c.body);
-    for (const ParticleCollider &c : e->pColliders)
+    const pbd_engine::ReplicaColliders &rep = e->repColliders;
+    const bool batch = rep.nRigid != 0;
+    if (batch ? rep.total == 0 : (e->rColliders.empty() || e->contactTotal == 0)) return 0;
+    if (!batch)
+        for (const RigidCollider &c : e->rColliders)  // the bodies may have been replaced since pbd_set_colliders
+            if (c.body >= e->nRb || e->rbMass[c.body] != 0.0f) return fail("contact path: collider on rigid body %u, which is missing or not static any more (pbd_set_colliders again)", c.body);
+    for (const ParticleCollider &c : batch ? rep.ranges : e->pColliders)
         if ((unsigned long long)c.offset + c.count > e->n) return fail("contact path: a particle collider covers particles beyond the %u the engine holds", e->n);
     ContactArgs a;
     a.pos = attr_ptr(e, PBD_ATTR_X); a.vel = attr_ptr(e, PBD_ATTR_V); a.slot = (const unsigned *)e->dSlot.p;
-    a.rbX = (const float4 *)e->rbX.p; a.rbV = (const float4 *)e->rbV.p; a.rbW = (const float4 *)e->rbW.p;
-    a.rigid = (const RigidCollider *)e->dRColliders.p; a.nRigid = (unsigned)e->rColliders.size();
-    a.ranges = (const ParticleCollider *)e->dPColliders.p; a.nRanges = (unsigned)e->pColliders.size();
-    a.rangeStart = (const unsigned *)e->dRangeStart.p; a.total = e->contactTotal;
+    if (batch) {
+        a.rbX = (const float4 *)rep.dX.p; a.rbV = (const float4 *)rep.dV.p; a.rbW = (const float4 *)rep.dW.p;
+        a.rigid = (const RigidCollider *)rep.dRigid.p; a.nRigid = rep.nRigid;
+        a.ranges = (const ParticleCollider *)rep.dRanges.p; a.nRanges = (unsigned)rep.ranges.size();
+        a.rangeStart = (const unsigned *)rep.dStart.p; a.total = rep.total; a.n = e->n;
+    } else {
+        a.rbX = (const float4 *)e->rbX.p; a.rbV = (const float4 *)e->rbV.p; a.rbW = (const float4 *)e->rbW.p;
+        a.rigid = (const RigidCollider *)e->dRColliders.p; a.nRigid = (unsigned)e->rColliders.size();
+        a.ranges = (const ParticleCollider *)e->dPColliders.p; a.nRanges = (unsigned)e->pColliders.size();
+        a.rangeStart = (const unsigned *)e->dRangeStart.p; a.total = e->contactTotal;
+    }
     a.tolerance = e->contactTolerance; a.stiffness = e->contactStiffness; a.maxIterV = e->maxIterV;
     a.record = e->contactCap ? (ContactRecord *)e->dContacts.p : nullptr; a.recordCount = (unsigned *)e->dContactCount.p; a.recordCap = e->contactCap;
     if (e->contactCap) CK(cudaMemsetAsync(e->dContactCount.p, 0, sizeof(unsigned), s));
-    k_contacts<<<(a.total + 127u) / 128u, 128, 0, s>>>(a);
+    if (batch) k_contacts_batch<<<dim3((a.total + 127u) / 128u, e->batch.K), 128, 0, s>>>(a);
+    else k_contacts<<<(a.total + 127u) / 128u, 128, 0, s>>>(a);
     CK(cudaGetLastError());
     *launches += 1;
     return 0;

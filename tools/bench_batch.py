@@ -4,7 +4,7 @@ stepped one after another by a K = 1 engine; the resident cluster size C swept o
 power limit read in the same run.  The four scenes run four different resident instantiations (cloth, FEM, cloth-XPBD and light type
 masks).
 
-    python tools/bench_batch.py [--out results.json] [--quick] [--replica-rows] [--sweep] [--rest-shapes] [--ks 8,132] [--no-baseline]
+    python tools/bench_batch.py [--out results.json] [--quick] [--replica-rows] [--sweep] [--rest-shapes] [--colliders] [--ks 8,132] [--no-baseline]
 
 --replica-rows measures every batch twice in a row: with the shared parameters, and with per-replica material rows and gravity
 (pbd_set_replica_materials / pbd_set_replica_gravity) equal to the shared values, so that the work is identical and the difference is what
@@ -13,6 +13,9 @@ the tables cost.  --sweep adds one real sweep: 132 cfg1 replicas, each with its 
 (pbd_set_replica_rest_positions) equal to the model's own rest positions, so that the work is identical and the difference is what the
 per-replica geometry arrays cost (they are K times the shared ones and leave L2 for large batches).  It also times the device derivation of
 the geometry of K rest shapes against building K host models (the host mirror's add*Constraint) for cfg1 K = 1056 and cfg3 K = 66.
+--colliders measures only the contact path of batches: cfg1 at K = 8, 132, 1056 and the 100x100 XPBD cloth at K = 33, 264, each in graph
+and resident mode, without and with three per-replica colliders (pbd_set_replica_colliders: a sphere, a rotated box and a torus cutting
+through the cloth's plane at random places, every replica its own), alternating.  The difference is the cost of the contact launch.
 --ks replaces the K sweep of every scene; --no-baseline skips the one-after-another baseline and the C sweep.  Without --rest-shapes or
 --replica-rows the script also runs against a build without those calls, so that shared-parameter batches can be compared across builds.
 
@@ -143,7 +146,36 @@ DERIVE_K = {"cfg1": 1056, "cfg3": 66}
 MAT_FIRST_COLUMN = {0: 1, 1: 1, 2: 1, 3: 0, 4: 0, 5: 5, 6: 4, 7: 1, 8: 1, 9: 10, 10: 10, 11: 9, 12: 0}
 
 
-def engine(m, mode, k, clusters=None, rows=None, rest=False):
+COLLIDER_KS = {"cfg1": [8, 132, 1056], "cloth100_xpbd": [33, 264]}
+
+
+def replica_colliders(m, k):
+    """Three static colliders per replica across the cloth's plane, each replica's at its own random places: (rigid lists, body_x)."""
+    x0 = np.asarray(m["x0"], np.float64)
+    lo, hi = x0.min(axis=0), x0.max(axis=0)
+    c, h = (lo + hi) / 2.0, (hi - lo) / 2.0
+    size = float(min(h[0], h[2]))
+    rng = np.random.default_rng(3)
+    rigid, body_x = [], np.zeros((k, 3, 3), np.float32)
+    for r in range(k):
+        cols = []
+        for j, shape in enumerate((_capi.SHAPE_SPHERE, _capi.SHAPE_BOX, _capi.SHAPE_TORUS)):
+            centre = c + np.array([rng.uniform(-0.6, 0.6) * h[0], -0.1 * size, rng.uniform(-0.6, 0.6) * h[2]])
+            a = rng.normal(size=3); a /= np.linalg.norm(a); t = rng.uniform(0.0, 1.0)
+            kx = np.array([[0.0, -a[2], a[1]], [a[2], 0.0, -a[0]], [-a[1], a[0], 0.0]])
+            rot = np.eye(3) + np.sin(t) * kx + (1.0 - np.cos(t)) * (kx @ kx)
+            s = 0.2 * size
+            dim = {_capi.SHAPE_SPHERE: (s, 0.0, 0.0), _capi.SHAPE_BOX: (s, 0.5 * s, s), _capi.SHAPE_TORUS: (s, 0.4 * s, 0.0)}[shape]
+            half = {_capi.SHAPE_SPHERE: np.full(3, s), _capi.SHAPE_BOX: np.array(dim), _capi.SHAPE_TORUS: np.array([1.4 * s, 0.4 * s, 1.4 * s])}[shape]
+            half = np.abs(rot) @ half + 0.05
+            rc = _capi.RigidCollider(); rc.shape = shape; rc.body = j; rc.dim[:] = list(dim); rc.restitution = 0.6; rc.friction = 0.2
+            rc.R[:] = rot.T.reshape(-1).tolist(); rc.v2[:] = centre.tolist(); rc.aabb_min[:] = (centre - half).tolist(); rc.aabb_max[:] = (centre + half).tolist()
+            cols.append(rc); body_x[r, j] = centre
+        rigid.append(cols)
+    return rigid, body_x
+
+
+def engine(m, mode, k, clusters=None, rows=None, rest=False, colliders=False):
     if clusters:
         os.environ["PBD_B200_CLUSTERS"] = "1x%d" % clusters  # the planner's cluster-size override (read when the image is planned)
     else:
@@ -162,6 +194,10 @@ def engine(m, mode, k, clusters=None, rows=None, rest=False):
         eng.set_replica_gravity(rows[1])
     if rest:  # every replica's rest shape = the model's: the same geometry, from the per-replica arrays
         eng.set_replica_rest_positions(np.repeat(np.asarray(m["x0"], np.float32)[None], k, 0))
+    if colliders:
+        rigid, body_x = replica_colliders(m, k)
+        eng.set_replica_colliders([_capi.ParticleCollider(0, len(m["x0"]), 0.5, 0.1)], rigid, body_x)
+        eng.set_contact_params(0.05, 100.0, 5)
     return eng
 
 
@@ -176,11 +212,11 @@ def timed(eng, warmup=3, min_s=0.4):
     return st.last_step_ms / steps, steps
 
 
-def measure(m, mode, k, clusters=None, rows=None, rest=False):
+def measure(m, mode, k, clusters=None, rows=None, rest=False, colliders=False):
     t0 = time.time()
     eng = None
     try:
-        eng = engine(m, mode, k, clusters, rows, rest)
+        eng = engine(m, mode, k, clusters, rows, rest, colliders)
         ms, steps = timed(eng)
         _, active = eng.get_mode()
     except _capi.PbdError as ex:
@@ -222,11 +258,28 @@ def main():
     ap.add_argument("--replica-rows", action="store_true", help="every batch also with per-replica rows equal to the shared parameters")
     ap.add_argument("--sweep", action="store_true", help="132 cfg1 replicas, each with its own stiffnesses")
     ap.add_argument("--rest-shapes", action="store_true", help="every batch also with per-replica rest shapes; device derivation against host builds")
+    ap.add_argument("--colliders", action="store_true", help="only the contact path: batches without and with three per-replica colliders")
     ap.add_argument("--ks", default=None, help="comma-separated K to measure instead of each scene's sweep")
     ap.add_argument("--no-baseline", action="store_true", help="skip the one-after-another baseline and the C sweep")
     a = ap.parse_args()
-    res = {"card": card(), "rows": [], "c_sweep": [], "replica_rows": [], "sweep": [], "rest_shapes": [], "derive": []}
+    res = {"card": card(), "rows": [], "c_sweep": [], "replica_rows": [], "sweep": [], "rest_shapes": [], "derive": [], "colliders": []}
     print("card: %s" % res["card"], flush=True)
+    if a.colliders:
+        for name, ks in COLLIDER_KS.items():
+            m = model(name)
+            for k in ([int(v) for v in a.ks.split(",")] if a.ks else ks):
+                for label, md in (("graph", _capi.MODE_GRAPH), ("resident", _capi.MODE_RESIDENT)):
+                    # without, with, without, with: the spread of each pair is next to the difference between them
+                    ms = [measure(m, md, k, colliders=bool(i & 1)).get("ms", float("nan")) for i in range(4)]
+                    launch = min(ms[1::2]) - min(ms[0::2])
+                    res["colliders"].append({"scene": name, "K": k, "mode": label, "without_ms": ms[0::2], "with_ms": ms[1::2], "contact_launch_ms": launch})
+                    print("  colliders %-13s K=%5d %-8s without %.4f %.4f ms | with 3 per replica %.4f %.4f ms | contact launch %.4f ms (%.1f %% of the step)"
+                          % (name, k, label, ms[0], ms[2], ms[1], ms[3], launch, 100.0 * launch / min(ms[0::2])), flush=True)
+        if a.out:
+            os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
+            with open(a.out, "w") as f:
+                json.dump(res, f, indent=1)
+        return
     for name in a.scenes.split(","):
         m = model(name)
         ncons = len(m["types"])

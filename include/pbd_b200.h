@@ -150,6 +150,24 @@ int pbd_step_host(pbd_engine *e, unsigned nSteps, const float *x_in, const float
 int pbd_step_host_async(pbd_engine *e, unsigned nSteps, const float *x_in, const float *v_in, float *x_out, float *v_out);
 int pbd_step_host_wait(pbd_engine *e, unsigned lag);
 
+/* Particle state in device memory (PyTorch / CuPy buffers).  Same layouts as pbd_set_attr / pbd_get_attr / pbd_set_masses: K*n*3 floats
+ * (K*n masses), replica after replica, host particle order -- the slot map and tile permutation stay invisible.  Pointers must be device
+ * memory of the engine's device (or managed memory); host memory, pinned included, is refused (use the host calls).
+ * stream: the caller's stream (e.g. torch.cuda.current_stream().cuda_stream; the legacy default stream is cudaStreamLegacy) or NULL = the
+ * engine's stream.  The copy runs after the work already enqueued on `stream` and on the engine's stream (earlier steps included).  Later
+ * work on `stream`, and every later engine call, runs after the copy, so `src` may be freed or reused on `stream` as soon as the call
+ * returns.  No call blocks the host.  A stream being captured into a graph is refused.
+ * replicas (set calls only): NULL = every replica; else K bytes in device memory.  Replica r is written iff replicas[r] != 0; the other
+ * replicas are left bit for bit as they were and their rows of src/mass are not read.  At K = 1 `replicas` has one byte.
+ * Refused, with nothing enqueued and the state unchanged: a null pointer, an attribute out of range, host memory, memory of another
+ * device, a capturing stream.  K*n = 0 is a no-op.
+ * Restarting replicas (episodes that ended, Monte-Carlo restarts): write X, V, OLDX = X and LASTX = X for the chosen replicas (masses too
+ * if they change), all with the same `replicas` mask.  Each restarted replica then advances bit for bit as a single-scene engine that
+ * pbd_set_particles started from that state; the XPBD multipliers need no reset (they are zeroed at the first sweep of every substep). */
+int pbd_set_attr_device(pbd_engine *e, int attr, const float *src, const unsigned char *replicas, void *stream);
+int pbd_get_attr_device(pbd_engine *e, int attr, float *dst, void *stream);
+int pbd_set_masses_device(pbd_engine *e, const float *mass, const unsigned char *replicas, void *stream);
+
 /* ---- Contact path (SURVEY.md section 8 row f-4, its data-parallel part) ----------------------------------------------------
  * Particles of triangle / tet models against analytic distance fields carried by STATIC rigid bodies, and the velocity-level
  * contact solve: DistanceFieldCollisionDetection::collisionDetection + collisionDetectionRBSolid
@@ -210,8 +228,8 @@ int pbd_set_replica_colliders(pbd_engine *e, unsigned nParticleColliders, const 
  *  - Calls that DEFINE the model describe one replica: pbd_set_particles (n, and it sets EVERY replica to the given state),
  *    pbd_add_constraints, the colour groups, pbd_set_params.
  *  - Calls that MOVE state take the whole batch, replica after replica: pbd_set_attr / pbd_get_attr (K*n*3 floats), pbd_set_masses
- *    (K*n: each replica may pin other particles), pbd_step_host / pbd_step_host_async (K*n*3 per array), pbd_get_lambdas (K*count
- *    multipliers, `ids` count insertion ids).
+ *    (K*n: each replica may pin other particles), their device-memory forms (whose set calls may write chosen replicas only),
+ *    pbd_step_host / pbd_step_host_async (K*n*3 per array), pbd_get_lambdas (K*count multipliers, `ids` count insertion ids).
  *  - Constraint parameters, gravity and the geometry of the rest state (rest lengths and angles, Q, inverse rest matrices, areas,
  *    volumes, shape-matching rest shapes) are shared unless pbd_set_replica_materials / pbd_set_replica_gravity /
  *    pbd_set_replica_rest_positions (below) give every replica its own.

@@ -27,7 +27,8 @@ SYMBOLS = ["pbd_last_error", "pbd_device_count", "pbd_create", "pbd_destroy", "p
            "pbd_get_lambdas", "pbd_get_stats", "pbd_profile_step", "pbd_set_replicas", "pbd_get_replicas",
            "pbd_num_materials", "pbd_set_replica_materials", "pbd_set_replica_gravity",
            "pbd_set_replica_rest_positions", "pbd_get_replica_geometry",
-           "pbd_set_colliders", "pbd_set_contact_params", "pbd_record_contacts", "pbd_get_contacts", "pbd_set_replica_colliders"]
+           "pbd_set_colliders", "pbd_set_contact_params", "pbd_record_contacts", "pbd_get_contacts", "pbd_set_replica_colliders",
+           "pbd_set_attr_device", "pbd_get_attr_device", "pbd_set_masses_device"]
 
 
 SHAPE_BOX, SHAPE_SPHERE, SHAPE_TORUS, SHAPE_CYLINDER, SHAPE_HOLLOW_SPHERE, SHAPE_HOLLOW_BOX = range(6)
@@ -109,6 +110,9 @@ def lib():
         _lib.pbd_set_replica_gravity.argtypes = [C.c_void_p, C.c_void_p]
         _lib.pbd_set_replica_rest_positions.argtypes = [C.c_void_p, C.c_void_p]
         _lib.pbd_get_replica_geometry.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+        _lib.pbd_set_attr_device.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+        _lib.pbd_get_attr_device.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
+        _lib.pbd_set_masses_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     return _lib
 
 
@@ -123,6 +127,39 @@ def _f32(a):
 
 def _ptr(a):
     return a.ctypes.data_as(C.c_void_p) if a is not None else None
+
+
+def _device_ptr(what, a, typestrs, count, writable=False):
+    """The device pointer of `a`, an object with __cuda_array_interface__ (a torch CUDA tensor, a CuPy array), after the checks the C
+    calls cannot make: element type one of `typestrs`, C-contiguous, `count` elements, and not read-only where it is written."""
+    iface = getattr(a, "__cuda_array_interface__", None)
+    if iface is None:
+        raise TypeError("%s: wants device memory, an object with __cuda_array_interface__ (a torch CUDA tensor, a CuPy array), got %s; "
+                        "host arrays go through the host calls" % (what, type(a).__name__))
+    if iface["typestr"] not in typestrs:
+        raise ValueError("%s: element type %s, wants %s" % (what, iface["typestr"], " or ".join(typestrs)))
+    shape, strides = tuple(iface["shape"]), iface.get("strides")
+    if strides is not None:
+        step = int(iface["typestr"][2:])
+        for extent, stride in reversed(list(zip(shape, strides))):
+            if extent != 1 and stride != step:
+                raise ValueError("%s: not C-contiguous (shape %s, strides %s)" % (what, shape, tuple(strides)))
+            step *= extent
+    size = int(np.prod(shape, dtype=np.int64))
+    if size != count:
+        raise ValueError("%s: %d elements (shape %s), wants %d" % (what, size, shape, count))
+    ptr, readonly = iface["data"]
+    if writable and readonly:
+        raise ValueError("%s: read-only" % what)
+    return ptr
+
+
+def _stream(stream):
+    """A stream handle for the device calls: None = the engine's stream; 0, what torch reports for the legacy default stream, becomes
+    cudaStreamLegacy (a NULL handle would mean the engine's stream)."""
+    if stream is None:
+        return None
+    return C.c_void_p(int(stream) or 1)
 
 
 def device_count():
@@ -199,6 +236,36 @@ class Engine:
     def set_masses(self, mass):
         mass = _f32(mass).reshape(-1); assert len(mass) == self.K * self.n
         _ck(lib().pbd_set_masses(self._h, _ptr(mass)))
+
+    # particle state in device memory ----------------------------------------------------------------
+    # The arrays are objects with __cuda_array_interface__ on the engine's device (torch CUDA tensors, CuPy arrays), float32,
+    # C-contiguous, laid out as the host calls' arrays: K*n*3 elements (K*n masses), replica after replica.  stream: an integer stream
+    # handle (torch.cuda.current_stream().cuda_stream; 0 = the legacy default stream) or None for the engine's stream.  The copy is
+    # ordered after the work enqueued so far on `stream` and before the work enqueued on it later; nothing blocks the host.
+    # replicas: None for every replica, or K bools / uint8 in device memory, nonzero where the replica is written.
+    def _mask(self, what, replicas):
+        return None if replicas is None else C.c_void_p(_device_ptr(what + ": replicas", replicas, ("|b1", "|u1"), self.K))
+
+    def set_attr_device(self, attr, src, replicas=None, stream=None):
+        """pbd_set_attr_device: attribute `attr` of the replicas in `replicas` from src (K*n*3 floats)."""
+        p = _device_ptr("set_attr_device: src", src, ("<f4",), self.K * self.n * 3)
+        mask = self._mask("set_attr_device", replicas)
+        if self.K * self.n:
+            _ck(lib().pbd_set_attr_device(self._h, int(attr), C.c_void_p(p), mask, _stream(stream)))
+
+    def get_attr_device(self, attr, out, stream=None):
+        """pbd_get_attr_device: attribute `attr` of every replica into out (K*n*3 floats); returns out."""
+        p = _device_ptr("get_attr_device: out", out, ("<f4",), self.K * self.n * 3, writable=True)
+        if self.K * self.n:
+            _ck(lib().pbd_get_attr_device(self._h, int(attr), C.c_void_p(p), _stream(stream)))
+        return out
+
+    def set_masses_device(self, mass, replicas=None, stream=None):
+        """pbd_set_masses_device: the masses of the replicas in `replicas` from mass (K*n floats)."""
+        p = _device_ptr("set_masses_device: mass", mass, ("<f4",), self.K * self.n)
+        mask = self._mask("set_masses_device", replicas)
+        if self.K * self.n:
+            _ck(lib().pbd_set_masses_device(self._h, C.c_void_p(p), mask, _stream(stream)))
 
     # replica batch ---------------------------------------------------------------------------------
     def set_replicas(self, k):

@@ -127,6 +127,9 @@ struct pbd_engine {
     // stats
     pbd_stats stats{};
     cudaEvent_t evStart = nullptr, evStop = nullptr;
+    // the device-memory state calls (pbd_set_attr_device ...) on a caller's stream: the engine stream waits for evCaller, recorded on the
+    // caller's stream, before the copy; the caller's stream waits for evEngine, recorded on the engine stream, after it
+    cudaEvent_t evCaller = nullptr, evEngine = nullptr;
     // pbd_step_host_async: two staging slots, one upload and one download stream next to the compute stream
     struct HostPipe {
         cudaStream_t up = nullptr, down = nullptr;
@@ -202,6 +205,7 @@ extern "C" int pbd_create(int device, void *stream, pbd_engine **out) {
         e->ownsStream = true;
     }
     cudaEventCreate(&e->evStart); cudaEventCreate(&e->evStop);
+    cudaEventCreateWithFlags(&e->evCaller, cudaEventDisableTiming); cudaEventCreateWithFlags(&e->evEngine, cudaEventDisableTiming);
     *out = e;
     return 0;
 }
@@ -213,6 +217,8 @@ extern "C" int pbd_destroy(pbd_engine *e) {
     if (e->graphExec) cudaGraphExecDestroy(e->graphExec);
     if (e->evStart) cudaEventDestroy(e->evStart);
     if (e->evStop) cudaEventDestroy(e->evStop);
+    if (e->evCaller) cudaEventDestroy(e->evCaller);
+    if (e->evEngine) cudaEventDestroy(e->evEngine);
     if (e->pipe.ready) {
         cudaStreamSynchronize(e->pipe.up); cudaStreamSynchronize(e->pipe.down);
         for (int s = 0; s < 2; s++)
@@ -258,6 +264,24 @@ static int relayout(pbd_engine *e, const std::vector<unsigned> &newSlot) {
 // grid of a per-particle kernel over `replicas` replicas: blockIdx.y = replica (kernels.cuh: k_pack3 ...)
 static dim3 replica_grid(const pbd_engine *e, unsigned replicas) { return dim3(nblk(e->n, 256), replicas); }
 
+// The per-particle copies between AoS-3 device buffers (K n 3 floats, host particle order) and the particle arrays, on the engine stream.
+// mask: the replicas written (k_pack3 / k_set_w), nullptr for all of them.
+static int pack_attr(pbd_engine *e, int a, const float *src, int keepW, unsigned replicas, const unsigned char *mask) {
+    k_pack3<<<replica_grid(e, replicas), 256, 0, e->stream>>>(src, attr_ptr(e, a), e->n, keepW, (const unsigned *)e->dSlot.p, mask);
+    CK(cudaGetLastError());
+    return 0;
+}
+static int unpack_attr(pbd_engine *e, int a, float *dst) {
+    k_unpack3<<<replica_grid(e, e->batch.K), 256, 0, e->stream>>>(attr_ptr(e, a), dst, e->n, (const unsigned *)e->dSlot.p);
+    CK(cudaGetLastError());
+    return 0;
+}
+static int pack_w(pbd_engine *e, const float *mass, unsigned replicas, const unsigned char *mask) {
+    k_set_w<<<replica_grid(e, replicas), 256, 0, e->stream>>>(attr_ptr(e, PBD_ATTR_X), attr_ptr(e, PBD_ATTR_V), mass, e->n, (const unsigned *)e->dSlot.p, mask);
+    CK(cudaGetLastError());
+    return 0;
+}
+
 // Host AoS-3 of the first `replicas` replicas -> `staging` on stream `copy` -> attribute `a` by k_pack3 on the engine stream (.w kept
 // with keepW).  host == nullptr: `staging` holds the copy already.  A copy stream other than the engine's comes with `copied`, through
 // which the pack waits for the copy.
@@ -265,15 +289,12 @@ static int upload_attr(pbd_engine *e, int a, const float *host, int keepW, unsig
                        cudaEvent_t copied = nullptr) {
     if (host) CK(cudaMemcpyAsync(staging.p, host, (size_t)replicas * e->n * 3 * sizeof(float), cudaMemcpyHostToDevice, copy));
     if (copied) { CK(cudaEventRecord(copied, copy)); CK(cudaStreamWaitEvent(e->stream, copied, 0)); }
-    k_pack3<<<replica_grid(e, replicas), 256, 0, e->stream>>>((const float *)staging.p, attr_ptr(e, a), e->n, keepW, (const unsigned *)e->dSlot.p);
-    CK(cudaGetLastError());
-    return 0;
+    return pack_attr(e, a, (const float *)staging.p, keepW, replicas, nullptr);
 }
 // Attribute `a` of every replica -> `staging` by k_unpack3 on the engine stream -> host AoS-3 on stream `copy`.  A copy stream other
 // than the engine's comes with `unpacked`, through which the copy waits for the unpack.
 static int download_attr(pbd_engine *e, int a, float *host, const DevBuf &staging, cudaStream_t copy, cudaEvent_t unpacked = nullptr) {
-    k_unpack3<<<replica_grid(e, e->batch.K), 256, 0, e->stream>>>(attr_ptr(e, a), (float *)staging.p, e->n, (const unsigned *)e->dSlot.p);
-    CK(cudaGetLastError());
+    CKE(unpack_attr(e, a, (float *)staging.p));
     if (unpacked) { CK(cudaEventRecord(unpacked, e->stream)); CK(cudaStreamWaitEvent(copy, unpacked, 0)); }
     CK(cudaMemcpyAsync(host, staging.p, (size_t)e->batch.K * e->n * 3 * sizeof(float), cudaMemcpyDeviceToHost, copy));
     return 0;
@@ -282,8 +303,7 @@ static int download_attr(pbd_engine *e, int a, float *host, const DevBuf &stagin
 // masses of the first `replicas` replicas (n floats each), staged in stage[0]
 static int set_w(pbd_engine *e, const float *mass, unsigned replicas) {
     CK(cudaMemcpyAsync(e->stage[0].p, mass, (size_t)replicas * e->n * sizeof(float), cudaMemcpyHostToDevice, e->stream));
-    k_set_w<<<replica_grid(e, replicas), 256, 0, e->stream>>>(attr_ptr(e, PBD_ATTR_X), attr_ptr(e, PBD_ATTR_V), (const float *)e->stage[0].p, e->n, (const unsigned *)e->dSlot.p);
-    CK(cudaGetLastError());
+    CKE(pack_w(e, (const float *)e->stage[0].p, replicas, nullptr));
     CK(cudaStreamSynchronize(e->stream));  // staging buffers are reused by the next call
     return 0;
 }
@@ -459,6 +479,55 @@ extern "C" int pbd_get_attr(pbd_engine *e, int attr, float *dst) {
     CKE(download_attr(e, attr, dst, e->stage[0], e->stream));
     CK(cudaStreamSynchronize(e->stream));
     return 0;
+}
+
+// ---- particle state in device memory (pbd_set_attr_device, pbd_get_attr_device, pbd_set_masses_device) -----------------------------
+// `p` must be device or managed memory of the engine's device; host memory, pinned or not, is what the host calls take.
+static int device_memory_refusal(const pbd_engine *e, const char *what, const char *arg, const void *p) {
+    cudaPointerAttributes a{};
+    const cudaError_t err = cudaPointerGetAttributes(&a, p);
+    if (err != cudaSuccess) { cudaGetLastError(); return fail("%s: %s: cudaPointerGetAttributes -> %s", what, arg, cudaGetErrorString(err)); }
+    const bool onDevice = a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
+    if (onDevice && a.device == e->device) return 0;
+    if (onDevice) return fail("%s: %s is memory of device %d, the engine runs on device %d", what, arg, a.device, e->device);
+    return fail("%s: %s is %s host memory; the device calls take device memory (host arrays go through pbd_set_attr / pbd_get_attr / pbd_set_masses)",
+                what, arg, a.type == cudaMemoryTypeHost ? "pinned" : "pageable");
+}
+// A device-memory state call: every check before anything is enqueued, then `copy` on the engine stream, ordered after the work enqueued
+// so far on the caller's stream and before the work enqueued on it later.  The second wait is what lets a caching allocator hand `data`
+// out again on the caller's stream while the copy is still pending.  No staging and no host synchronisation.
+template <class F>
+static int device_call(pbd_engine *e, const char *what, const char *arg, const void *data, const unsigned char *mask, void *stream, F &&copy) {
+    if (!data) return fail("%s: %s == NULL", what, arg);
+    CKE(use(e));
+    const cudaStream_t s = stream ? (cudaStream_t)stream : e->stream;
+    cudaStreamCaptureStatus capturing = cudaStreamCaptureStatusNone;
+    CK(cudaStreamIsCapturing(s, &capturing));
+    if (capturing != cudaStreamCaptureStatusNone)
+        return fail("%s: the stream is being captured into a graph; the copy would run at every replay, outside the engine's order (call it outside the capture)", what);
+    CKE(device_memory_refusal(e, what, arg, data));
+    if (mask) CKE(device_memory_refusal(e, what, "replicas", mask));
+    if (e->n == 0) return 0;
+    const bool other = s != e->stream;
+    if (other) { CK(cudaEventRecord(e->evCaller, s)); CK(cudaStreamWaitEvent(e->stream, e->evCaller, 0)); }
+    CKE(copy());
+    if (other) { CK(cudaEventRecord(e->evEngine, e->stream)); CK(cudaStreamWaitEvent(s, e->evEngine, 0)); }
+    return 0;
+}
+
+extern "C" int pbd_set_attr_device(pbd_engine *e, int attr, const float *src, const unsigned char *replicas, void *stream) {
+    if (!e) return fail("pbd_set_attr_device: null engine");
+    if (attr < 0 || attr >= kNumAttrs) return fail("pbd_set_attr_device: bad attribute %d", attr);
+    return device_call(e, "pbd_set_attr_device", "src", src, replicas, stream, [&] { return pack_attr(e, attr, src, 1, e->batch.K, replicas); });
+}
+extern "C" int pbd_get_attr_device(pbd_engine *e, int attr, float *dst, void *stream) {
+    if (!e) return fail("pbd_get_attr_device: null engine");
+    if (attr < 0 || attr >= kNumAttrs) return fail("pbd_get_attr_device: bad attribute %d", attr);
+    return device_call(e, "pbd_get_attr_device", "dst", dst, nullptr, stream, [&] { return unpack_attr(e, attr, dst); });
+}
+extern "C" int pbd_set_masses_device(pbd_engine *e, const float *mass, const unsigned char *replicas, void *stream) {
+    if (!e) return fail("pbd_set_masses_device: null engine");
+    return device_call(e, "pbd_set_masses_device", "mass", mass, replicas, stream, [&] { return pack_w(e, mass, e->batch.K, replicas); });
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -958,11 +1027,13 @@ static int flatten(pbd_engine *e) {
     std::vector<unsigned char> key = image_key(e);
     if (key == e->imageKey) return 0;
     CKE(use(e));
+    // Work still pending on the engine stream -- a device get or set enqueued behind a caller's stream included -- reads the particle
+    // arrays and the slot map that relayout replaces, and upload_slot_map's copy is not ordered against the engine stream.
+    CK(cudaStreamSynchronize(e->stream));
     e->imageGen++;
     std::vector<float4> x0;  // resident: rest positions by host index
     if (pbd_b200::preferred_mode(e->mode, e->host, e->n, e->numConstraints, e->batch.K) == PBD_MODE_RESIDENT && e->n) {
         std::vector<float4> raw(e->n);
-        CK(cudaStreamSynchronize(e->stream));
         CK(cudaMemcpy(raw.data(), attr_ptr(e, PBD_ATTR_X0), (size_t)e->n * sizeof(float4), cudaMemcpyDeviceToHost));
         x0.resize(e->n);
         for (unsigned i = 0; i < e->n; i++) x0[i] = raw[e->slot[i]];

@@ -419,14 +419,18 @@ __global__ void __launch_bounds__(256) k_velocity(const float4 *__restrict__ pos
 
 // host AoS-3 <-> device float4 conversion (std::vector<Vector3r> layout on the host side); particle i of the host lives
 // in device slot slot[i] (de-interleaved formula of device_image.h, or the tile-major permutation of the tiled mode).  Replica
-// blockIdx.y of a batch: host arrays at y x n particles, device arrays at slot y x n + slot[i].
+// blockIdx.y of a batch: host arrays at y x n particles, device arrays at slot y x n + slot[i].  `mask` (k_pack3, k_set_w; nullptr: every
+// replica): replica y is written only where mask[y] != 0 -- one load per block, the same for all its threads -- and otherwise its row of
+// the source is not read.
 __global__ void k_relayout(const float4 *__restrict__ src, float4 *__restrict__ dst, unsigned n, const unsigned *__restrict__ oldSlot,
                            const unsigned *__restrict__ newSlot) {
     const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
     const size_t r = (size_t)blockIdx.y * n;
     if (i < n) dst[r + newSlot[i]] = src[r + oldSlot[i]];
 }
-__global__ void k_pack3(const float *__restrict__ src, float4 *__restrict__ dst, unsigned n, int keepW, const unsigned *__restrict__ slot) {
+__global__ void k_pack3(const float *__restrict__ src, float4 *__restrict__ dst, unsigned n, int keepW, const unsigned *__restrict__ slot,
+                        const unsigned char *__restrict__ mask) {
+    if (mask && !mask[blockIdx.y]) return;
     const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     src += (size_t)blockIdx.y * 3 * n; dst += (size_t)blockIdx.y * n;
@@ -503,7 +507,9 @@ __global__ void __launch_bounds__(128) k_derive_geometry(const __grid_constant__
         if (d.gs[k]) d.gs[k][o] = col(pc.gs[k]);
 }
 
-__global__ void k_set_w(float4 *__restrict__ pos, float4 *__restrict__ vel, const float *__restrict__ mass, unsigned n, const unsigned *__restrict__ slot) {
+__global__ void k_set_w(float4 *__restrict__ pos, float4 *__restrict__ vel, const float *__restrict__ mass, unsigned n, const unsigned *__restrict__ slot,
+                        const unsigned char *__restrict__ mask) {
+    if (mask && !mask[blockIdx.y]) return;
     const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     pos += (size_t)blockIdx.y * n; vel += (size_t)blockIdx.y * n; mass += (size_t)blockIdx.y * n;

@@ -253,6 +253,26 @@ int pbd_get_replicas(pbd_engine *e, unsigned *K);
  * pbd_set_replica_gravity: replica r integrates with gravity g[3r..3r+3) instead of pbd_set_params' vector.  g = NULL: back to it. */
 int pbd_set_replica_materials(pbd_engine *e, int type, const float *mat /* K * pbd_num_materials(type) */);
 int pbd_set_replica_gravity(pbd_engine *e, const float *g /* K*3 */);
+/* Per-constraint material parameters of every replica (K > 1).  mat: K*count*nMat floats, count = the number of constraints of `type`,
+ * nMat = pbd_num_materials(type); replica after replica, within a replica the constraints in the order they were added (the order of
+ * pbd_get_replica_geometry), each constraint's nMat values in the order of the material columns above.  Replica r then advances bit for bit
+ * as a single-scene engine whose constraints of `type` were added with replica r's values.  mat = NULL: back to the shared parameters.
+ * One material source per type: the shared parameters, pbd_set_replica_materials' rows, or these per-constraint values -- each set call
+ * selects its own, so pbd_set_replica_materials(type, rows or NULL) switches this override off.
+ * Lifetime: pbd_set_replicas and pbd_clear_constraints drop it; changing the mode keeps it; pbd_add_constraints keeps it -- the constraints
+ * there were keep every replica's values, the new ones carry the parameters they were added with in every replica.  A repeat call copies
+ * in stream order into device arrays that keep their address (the next step enqueued reads the new values, a captured step graph stays
+ * valid); a call that switches the override on plans the image again and may synchronise.
+ * Refused, with nothing changed: at K = 1, an unknown type, the joint types (no material parameters), a type without constraints.
+ * pbd_set_replica_constraint_materials_device: the same from device memory, with the stream contract and the refusals of
+ * pbd_set_attr_device (mat = NULL included).  replicas: NULL = every replica, else K bytes in device memory; a replica r with
+ * replicas[r] == 0 keeps exactly the parameters it was stepped with before the call (shared, rows or per-constraint) and its rows of mat
+ * are not read.  No host synchronisation once the override is on.
+ * pbd_get_replica_materials: K*count*nMat floats in that layout, the values every replica's constraints of `type` are stepped with,
+ * whichever source is in force.  Synchronises. */
+int pbd_set_replica_constraint_materials(pbd_engine *e, int type, const float *mat);
+int pbd_set_replica_constraint_materials_device(pbd_engine *e, int type, const float *mat, const unsigned char *replicas, void *stream);
+int pbd_get_replica_materials(pbd_engine *e, int type, float *dst);
 /* Per-replica rest shape of a batch (K > 1, refused at K = 1 like the two calls above).  x0: K*n*3 floats, replica after replica.  Sets
  * PBD_ATTR_X0 of every replica and gives every constraint of replica r the rest geometry that the constraint class's initConstraint derives
  * from replica r's rest positions (ShapeMatching: and from replica r's inverse masses at the time of the call), computed on the GPU with the

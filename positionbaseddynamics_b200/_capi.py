@@ -28,7 +28,8 @@ SYMBOLS = ["pbd_last_error", "pbd_device_count", "pbd_create", "pbd_destroy", "p
            "pbd_num_materials", "pbd_set_replica_materials", "pbd_set_replica_gravity",
            "pbd_set_replica_rest_positions", "pbd_get_replica_geometry",
            "pbd_set_colliders", "pbd_set_contact_params", "pbd_record_contacts", "pbd_get_contacts", "pbd_set_replica_colliders",
-           "pbd_set_attr_device", "pbd_get_attr_device", "pbd_set_masses_device"]
+           "pbd_set_attr_device", "pbd_get_attr_device", "pbd_set_masses_device",
+           "pbd_set_replica_constraint_materials", "pbd_set_replica_constraint_materials_device", "pbd_get_replica_materials"]
 
 
 SHAPE_BOX, SHAPE_SPHERE, SHAPE_TORUS, SHAPE_CYLINDER, SHAPE_HOLLOW_SPHERE, SHAPE_HOLLOW_BOX = range(6)
@@ -113,6 +114,9 @@ def lib():
         _lib.pbd_set_attr_device.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
         _lib.pbd_get_attr_device.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
         _lib.pbd_set_masses_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        _lib.pbd_set_replica_constraint_materials.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+        _lib.pbd_set_replica_constraint_materials_device.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+        _lib.pbd_get_replica_materials.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
     return _lib
 
 
@@ -160,6 +164,22 @@ def _stream(stream):
     if stream is None:
         return None
     return C.c_void_p(int(stream) or 1)
+
+
+def _host_materials(what, a, shape, writable=False):
+    """The checks in front of the host calls of per-constraint replica materials: a float32 numpy array of exactly `shape`, C-contiguous (and
+    writable where it is written).  Nothing is converted: a copy in another type or order would hide a caller's mistake in the layout."""
+    if not isinstance(a, np.ndarray):
+        raise TypeError("%s: wants a numpy array, got %s (device arrays go through set_replica_constraint_materials_device)" % (what, type(a).__name__))
+    if a.dtype != np.float32:
+        raise ValueError("%s: element type %s, wants float32" % (what, a.dtype))
+    if a.shape != tuple(shape):
+        raise ValueError("%s: shape %s, wants %s (replicas, constraints, material parameters)" % (what, a.shape, tuple(shape)))
+    if not a.flags.c_contiguous:
+        raise ValueError("%s: not C-contiguous" % what)
+    if writable and not a.flags.writeable:
+        raise ValueError("%s: read-only" % what)
+    return a
 
 
 def device_count():
@@ -286,6 +306,40 @@ class Engine:
             if mat.shape != (self.K, num_materials(ctype)):
                 raise ValueError("set_replica_materials: type %d wants a (%d, %d) array, got %s" % (ctype, self.K, num_materials(ctype), mat.shape))
         _ck(lib().pbd_set_replica_materials(self._h, int(ctype), _ptr(mat)))
+
+    def _constraint_materials_shape(self, ctype):
+        return (self.K, self.stats().constraints_per_type[ctype], num_materials(ctype))
+
+    def set_replica_constraint_materials(self, ctype, mat):
+        """Replica r's constraint i of `ctype` (in the order the constraints were added) carries the material parameters mat[r, i]
+        ((K, count, num_materials(ctype)) float32 numpy array, C-contiguous); None: the shared parameters again.  K > 1 only."""
+        if mat is not None:
+            _host_materials("set_replica_constraint_materials", mat, self._constraint_materials_shape(ctype))
+        _ck(lib().pbd_set_replica_constraint_materials(self._h, int(ctype), _ptr(mat)))
+
+    def set_replica_constraint_materials_device(self, ctype, mat, replicas=None, stream=None):
+        """pbd_set_replica_constraint_materials_device: the per-constraint materials of the replicas in `replicas` from mat, an object with
+        __cuda_array_interface__ holding K*count*num_materials(ctype) float32 in that layout (C-contiguous, any shape of that size); stream
+        and replicas as in set_attr_device.  Nothing blocks the host once the override is on."""
+        if mat is None:
+            raise TypeError("set_replica_constraint_materials_device: mat is None; the shared parameters come back with "
+                            "set_replica_constraint_materials(ctype, None)")
+        p = _device_ptr("set_replica_constraint_materials_device: mat", mat, ("<f4",), int(np.prod(self._constraint_materials_shape(ctype))))
+        mask = self._mask("set_replica_constraint_materials_device", replicas)
+        _ck(lib().pbd_set_replica_constraint_materials_device(self._h, int(ctype), C.c_void_p(p), mask, _stream(stream)))
+
+    def get_replica_materials(self, ctype, out=None):
+        """(K, count, num_materials(ctype)): the material parameters every replica's constraints of `ctype` are stepped with (shared, rows of
+        set_replica_materials or per constraint), constraints in the order they were added; into `out` if given (float32, C-contiguous,
+        writable, that shape)."""
+        shape = self._constraint_materials_shape(ctype)
+        if out is None:
+            out = np.zeros(shape, dtype=np.float32)
+        else:
+            _host_materials("get_replica_materials: out", out, shape, writable=True)
+        if out.size:
+            _ck(lib().pbd_get_replica_materials(self._h, int(ctype), _ptr(out)))
+        return out
 
     def set_replica_gravity(self, g):
         """Replica r integrates with gravity g[r] ((K, 3) array); None: the vector of set_params again.  K > 1 only."""

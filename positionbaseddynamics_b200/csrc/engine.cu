@@ -73,6 +73,10 @@ struct DevType {
     // replica batch: the geometry arrays every replica's projections read while per-replica rest shapes are on (K x count; they keep
     // their address while it stays on)
     DevBuf repGv[kMaxGeoV], repGs[kMaxGeoS];
+    // replica batch with per-constraint materials of every replica (pbd_set_replica_constraint_materials): the values in the order the
+    // constraints were added (K x count x nMat), and what the projections read, gathered from them into device order (one K x count array
+    // per material slot).  Both keep their address while K and count stay.
+    DevBuf cmat, repMat[kMaxMat];
     PodVector<unsigned> order;    // position in the device arrays -> insertion id
     unsigned count = 0;
     // pointers into the image (upload_image): the arrays the kernels read, and what a batch's per-replica geometry is derived from
@@ -98,8 +102,11 @@ struct pbd_engine {
     // with .w = the inverse mass at the time of the call; every image planned while restShapes is on derives its geometry from them.
     // restTables: images carry what a derivation reads (TypePlan::restBodies / restLocal), from the first pbd_set_replica_rest_positions
     // until the override is dropped, so that batches without it do not pay for them.
+    // cmatMask: the types whose materials are per constraint and per replica (pbd_set_replica_constraint_materials; DevType::cmat).  A type
+    // takes its materials from one source: the shared parameters, its rows of `mat` (matMask) or its per-constraint arrays (cmatMask).  The
+    // gather reads the image's restTables too, so images carry them while any type has the override on (rest_tables).
     struct Batch {
-        unsigned K = 1, matMask = 0;
+        unsigned K = 1, matMask = 0, cmatMask = 0;
         DevBuf mat, gravity, restX;
         bool gravitySet = false, restShapes = false, restTables = false;
     } batch;
@@ -162,6 +169,7 @@ struct pbd_engine {
 };
 
 static int use(pbd_engine *e) { CK(cudaSetDevice(e->device)); return 0; }
+static bool rest_tables(const pbd_engine *e) { return e->batch.restTables || e->batch.cmatMask; }
 
 static void model_changed(pbd_engine *e) { e->modelGen++; }  // what the device image is planned from (image_key) replaced
 static void drop_replica_geometry(pbd_engine *e) {
@@ -171,6 +179,20 @@ static void drop_replica_geometry(pbd_engine *e) {
         for (DevBuf &b : d.repGv) b.release();
         for (DevBuf &b : d.repGs) b.release();
     }
+}
+
+// per-constraint materials of the types in `types` back to their other source (what matMask says); the steps in flight are done first
+static int drop_constraint_materials(pbd_engine *e, unsigned types) {
+    if (!(e->batch.cmatMask & types)) return 0;
+    CKE(use(e));
+    CK(cudaStreamSynchronize(e->stream));
+    for (int t = 0; t < PBD_NUM_TYPES; t++)
+        if ((types >> t) & 1u) {
+            e->dev[t].cmat.release();
+            for (DevBuf &b : e->dev[t].repMat) b.release();
+        }
+    e->batch.cmatMask &= ~types;
+    return 0;
 }
 
 extern "C" int pbd_device_count(int *count) {
@@ -388,6 +410,7 @@ extern "C" int pbd_set_replicas(pbd_engine *e, unsigned K) {
     CK(cudaStreamSynchronize(e->stream));
     CKE(size_particles(e, K, true));  // replica 0 kept, the others copies of it
     e->batch.K = K;
+    CKE(drop_constraint_materials(e, ~0u));
     e->batch.mat.release(); e->batch.gravity.release(); e->batch.matMask = 0; e->batch.gravitySet = false;  // rows of the old K
     drop_replica_geometry(e);
     drop_replica_colliders(e);
@@ -424,6 +447,7 @@ extern "C" int pbd_set_replica_materials(pbd_engine *e, int type, const float *m
     CKE(replica_params_refusal(e, "pbd_set_replica_materials"));
     CKE(use(e));
     const unsigned bit = 1u << type;
+    CKE(drop_constraint_materials(e, bit));  // one source per type: this call's
     if (mat) CKE(write_replica_materials(e, type, mat, nMat * sizeof(float)));
     else if (e->batch.matMask & bit) CKE(write_replica_materials(e, type, e->dev[type].arrays.matU, 0));  // (an image planned again writes them too)
     if (mat) e->batch.matMask |= bit; else e->batch.matMask &= ~bit;
@@ -445,9 +469,12 @@ extern "C" int pbd_set_replica_gravity(pbd_engine *e, const float *g) {
 // With per-replica rest shapes the geometry arrays are the K x count ones, replica r's at r x replica_geo (0: the shared image's).
 static const float *replica_mat(const pbd_engine *e, int t) { return ((e->batch.matMask >> t) & 1u) ? (const float *)e->batch.mat.p + mat_offset(t) : nullptr; }
 static unsigned replica_geo(const pbd_engine *e, int t) { return e->batch.restShapes ? e->dev[t].count : 0u; }
+// with per-constraint materials of every replica the material arrays are the K x count ones, replica r's at r x replica_cmat (0: shared)
+static unsigned replica_cmat(const pbd_engine *e, int t) { return ((e->batch.cmatMask >> t) & 1u) ? e->dev[t].count : 0u; }
 static TypeArrays batch_arrays(const pbd_engine *e, int t) {
     TypeArrays a = e->dev[t].arrays;
     if ((e->batch.matMask >> t) & 1u) for (int k = 0; k < kMaxMat; k++) a.mat[k] = nullptr;
+    if ((e->batch.cmatMask >> t) & 1u) for (int k = 0; k < type_shape(t).nMat; k++) a.mat[k] = (const float *)e->dev[t].repMat[k].p;
     if (e->batch.restShapes) {
         for (int k = 0; k < kMaxGeoV; k++) if (a.gv[k]) a.gv[k] = (const float4 *)e->dev[t].repGv[k].p;
         for (int k = 0; k < kMaxGeoS; k++) if (a.gs[k]) a.gs[k] = (const float *)e->dev[t].repGs[k].p;
@@ -496,8 +523,9 @@ static int device_memory_refusal(const pbd_engine *e, const char *what, const ch
 // A device-memory state call: every check before anything is enqueued, then `copy` on the engine stream, ordered after the work enqueued
 // so far on the caller's stream and before the work enqueued on it later.  The second wait is what lets a caching allocator hand `data`
 // out again on the caller's stream while the copy is still pending.  No staging and no host synchronisation.
-template <class F>
-static int device_call(pbd_engine *e, const char *what, const char *arg, const void *data, const unsigned char *mask, void *stream, F &&copy) {
+// `prepare` runs after the checks and before the wait for the caller's stream (work that may synchronise the host goes there).
+template <class P, class F>
+static int device_call(pbd_engine *e, const char *what, const char *arg, const void *data, const unsigned char *mask, void *stream, P &&prepare, F &&copy) {
     if (!data) return fail("%s: %s == NULL", what, arg);
     CKE(use(e));
     const cudaStream_t s = stream ? (cudaStream_t)stream : e->stream;
@@ -508,11 +536,16 @@ static int device_call(pbd_engine *e, const char *what, const char *arg, const v
     CKE(device_memory_refusal(e, what, arg, data));
     if (mask) CKE(device_memory_refusal(e, what, "replicas", mask));
     if (e->n == 0) return 0;
+    CKE(prepare());
     const bool other = s != e->stream;
     if (other) { CK(cudaEventRecord(e->evCaller, s)); CK(cudaStreamWaitEvent(e->stream, e->evCaller, 0)); }
     CKE(copy());
     if (other) { CK(cudaEventRecord(e->evEngine, e->stream)); CK(cudaStreamWaitEvent(s, e->evEngine, 0)); }
     return 0;
+}
+template <class F>
+static int device_call(pbd_engine *e, const char *what, const char *arg, const void *data, const unsigned char *mask, void *stream, F &&copy) {
+    return device_call(e, what, arg, data, mask, stream, [] { return 0; }, copy);
 }
 
 extern "C" int pbd_set_attr_device(pbd_engine *e, int attr, const float *src, const unsigned char *replicas, void *stream) {
@@ -592,6 +625,7 @@ template <class V> static int upload_vec(DevBuf &buf, const V &v, cudaStream_t s
 // ------------------------------------------------------------------------------------------------------------
 extern "C" int pbd_clear_constraints(pbd_engine *e) {
     if (!e) return fail("null engine");
+    CKE(drop_constraint_materials(e, ~0u));
     for (auto &h : e->host) { h.ids.clear(); h.bodies.clear(); h.params.clear(); }
     e->numConstraints = 0;
     e->groupOff.clear(); e->groupIds.clear(); e->groupsSet = false;
@@ -623,6 +657,27 @@ static int check_added_geometry(pbd_engine *e, int type, unsigned count, const u
     return 0;
 }
 
+// With per-constraint materials of every replica on for `type`, `count` constraints added: every replica's values of the constraints there
+// are stay, the new ones carry the parameters they are added with in every replica (the image planned again gathers them)
+static int grow_constraint_materials(pbd_engine *e, int type, unsigned count, const float *params) {
+    if (!((e->batch.cmatMask >> type) & 1u) || !count) return 0;
+    CKE(use(e));
+    const TypeShape s = type_shape(type);
+    const PackColumns pc = pack_columns(type);
+    const size_t K = e->batch.K, c0 = e->host[type].ids.size(), c1 = c0 + count, w = (size_t)s.nMat * sizeof(float);
+    std::vector<float> added(K * count * s.nMat);
+    for (size_t r = 0; r < K; r++)
+        for (size_t i = 0; i < count; i++)
+            for (int k = 0; k < s.nMat; k++) added[(r * count + i) * s.nMat + k] = params[i * s.nParams + pc.mat[k]];
+    DevBuf grown;
+    CKE(grown.alloc(K * c1 * w));
+    CK(cudaMemcpy2DAsync(grown.p, c1 * w, e->dev[type].cmat.p, c0 * w, c0 * w, K, cudaMemcpyDeviceToDevice, e->stream));
+    CK(cudaMemcpy2DAsync((char *)grown.p + c0 * w, c1 * w, added.data(), count * w, count * w, K, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaStreamSynchronize(e->stream));  // before the old array is freed
+    std::swap(e->dev[type].cmat.p, grown.p); std::swap(e->dev[type].cmat.bytes, grown.bytes);
+    return 0;
+}
+
 extern "C" int pbd_add_constraints(pbd_engine *e, int type, unsigned count, const unsigned *bodies, const float *params, const unsigned *ids) {
     if (!e) return fail("null engine");
     if (type < 0 || type >= PBD_NUM_TYPES) return fail("pbd_add_constraints: unknown constraint type %d", type);
@@ -634,6 +689,7 @@ extern "C" int pbd_add_constraints(pbd_engine *e, int type, unsigned count, cons
         return fail("pbd_add_constraints: particle index %u out of range (n=%u)", bodies[badAt], e->n);
     }
     CKE(check_added_geometry(e, type, count, bodies, ids));
+    CKE(grow_constraint_materials(e, type, count, params));
     TypeStore &h = e->host[type];
     {
         const size_t b0 = h.ids.size();
@@ -1003,6 +1059,23 @@ static int apply_replica_geometry(pbd_engine *e, const float4 *rest, const char 
     return 0;
 }
 
+// ---- per-constraint materials of every replica of a batch (pbd_set_replica_constraint_materials) ---------------------------------
+// The device-ordered arrays of type t (sized here: they keep their address while K and count stay) <- `src`, K x count rows of nMat floats in
+// the order the constraints were added, through the image's device position -> insertion position map (restTables); with `keep` the rows
+// also go to DevType::cmat.  mask: the replicas written (nullptr: all).  Enqueued on the engine stream, no host synchronisation.
+static int gather_materials(pbd_engine *e, int t, const float *src, bool keep, const unsigned char *mask) {
+    DevType &d = e->dev[t];
+    if (!d.count) return 0;
+    if (!d.rest.local) return fail("per-constraint materials of type %d: the image lacks the device order tables", t);
+    const size_t cnt = (size_t)e->batch.K * d.count;
+    GatherMatArgs g{};
+    g.src = src; g.keep = keep ? (float *)d.cmat.p : nullptr; g.local = d.rest.local; g.mask = mask; g.count = d.count; g.nMat = type_shape(t).nMat;
+    for (int k = 0; k < g.nMat; k++) { CKE(d.repMat[k].alloc(pbd_b200::padded_bytes(cnt * sizeof(float)))); g.dst[k] = (float *)d.repMat[k].p; }
+    k_gather_materials<<<dim3(nblk(d.count, 128), e->batch.K), 128, 0, e->stream>>>(g);
+    CK(cudaGetLastError());
+    return 0;
+}
+
 template <class... V> static void append_bytes(std::vector<unsigned char> &key, const V &...v) {
     static_assert((std::is_scalar_v<std::remove_all_extents_t<V>> && ...), "padding bytes would make equal states compare unequal");
     size_t at = key.size();
@@ -1015,7 +1088,7 @@ template <class... V> static void append_bytes(std::vector<unsigned char> &key, 
 static std::vector<unsigned char> image_key(const pbd_engine *e) {
     std::vector<unsigned char> key;
     const bool tiled = pbd_b200::preferred_mode(e->mode, e->host, e->n, e->numConstraints, e->batch.K) == PBD_MODE_RESIDENT;
-    append_bytes(key, e->modelGen, e->n, e->nRb, e->rbX.p, e->rbQ.p, e->rbIinv.p, e->batch.K, tiled ? e->mode : -1, e->batch.restTables);
+    append_bytes(key, e->modelGen, e->n, e->nRb, e->rbX.p, e->rbQ.p, e->rbIinv.p, e->batch.K, tiled ? e->mode : -1, rest_tables(e));
     return key;
 }
 
@@ -1040,7 +1113,7 @@ static int flatten(pbd_engine *e) {
     }
     lap("colouring + rest positions");
     pbd_b200::PlanInput in{e->host, e->numConstraints, e->n, e->nRb, &e->groupOff, &e->groupIds, e->mode, x0.data(), 0u, 0u, e->smCount, nullptr,
-                           e->batch.restTables, e->batch.K};
+                           rest_tables(e), e->batch.K};
     if (const char *g = getenv("PBD_B200_CLUSTERS")) {  // development knob "GxC"
         unsigned gg = 0, cc = 0;
         if (sscanf(g, "%ux%u", &gg, &cc) == 2 && gg >= 1 && cc >= 1 && cc <= (unsigned)kMaxClusterCtas && (cc & (cc - 1)) == 0) { in.forcedG = gg; in.forcedC = cc; }
@@ -1060,6 +1133,8 @@ static int flatten(pbd_engine *e) {
     CK(cudaStreamSynchronize(e->stream));
     lap("relayout + upload");
     if (e->batch.restShapes) CKE(apply_replica_geometry(e, (const float4 *)e->batch.restX.p, "pbd_set_replica_rest_positions (image planned again)"));  // the new image's geometry, from the rest positions the override was given
+    for (int t = 0; t < PBD_NUM_TYPES; t++)  // the new image's device order of the per-constraint materials
+        if ((e->batch.cmatMask >> t) & 1u) CKE(gather_materials(e, t, (const float *)e->dev[t].cmat.p, false, nullptr));
 
     e->stats.num_constraints = e->numConstraints;  // per replica, like num_particles
     e->stats.num_groups = (unsigned)e->groupOff.size() - 1;
@@ -1101,6 +1176,97 @@ extern "C" int pbd_set_replica_rest_positions(pbd_engine *e, const float *x0) {
         CK(cudaStreamSynchronize(e->stream));
     }
     e->batch.restShapes = true;
+    return 0;
+}
+
+// The values replica r's constraints of `type` are stepped with while the type has no per-constraint override: its rows (matMask) or the
+// shared parameters, K x count x nMat in the order the constraints were added.  Reading the rows back synchronises.
+static int stepped_materials(pbd_engine *e, int type, std::vector<float> &out) {
+    const TypeStore &h = e->host[type];
+    const TypeShape s = type_shape(type);
+    const PackColumns pc = pack_columns(type);
+    const size_t K = e->batch.K, cnt = h.ids.size();
+    std::vector<float> rows;
+    if ((e->batch.matMask >> type) & 1u) {
+        rows.resize(K * s.nMat);
+        CK(cudaStreamSynchronize(e->stream));
+        CK(cudaMemcpy2D(rows.data(), s.nMat * sizeof(float), (const float *)e->batch.mat.p + mat_offset(type), kMatRowFloats * sizeof(float),
+                        s.nMat * sizeof(float), K, cudaMemcpyDeviceToHost));
+    }
+    out.resize(K * cnt * s.nMat);
+    for (size_t r = 0; r < K; r++)
+        for (size_t i = 0; i < cnt; i++)
+            for (int k = 0; k < s.nMat; k++) out[(r * cnt + i) * s.nMat + k] = rows.empty() ? h.params[i * s.nParams + pc.mat[k]] : rows[r * s.nMat + k];
+    return 0;
+}
+static int constraint_materials_refusal(const pbd_engine *e, const char *what, int type) {
+    CKE(replica_params_refusal(e, what));
+    if (type < 0 || type >= PBD_NUM_TYPES) return fail("%s: unknown constraint type %d", what, type);
+    if (type_shape(type).nMat == 0) return fail("%s: constraint type %d has no material parameters", what, type);
+    const size_t cnt = e->host[type].ids.size();
+    if (!cnt) return fail("%s: the model has no constraints of type %d", what, type);
+    if ((unsigned long long)e->batch.K * cnt >= (1ull << 32))  // the resident kernel addresses replica r's materials as i + r count in 32 bits
+        return fail("%s: %u replicas of %zu constraints of type %d exceed 2^32 material rows", what, e->batch.K, cnt, type);
+    return 0;
+}
+// Type `type` takes its materials from DevType::cmat from now on.  Switching the override on (may synchronise): `fill` -- the rows keep the
+// values the replicas were stepped with (a masked call leaves the other replicas as they were) -- and the image planned with the tables the
+// gather reads.  Every call: the image brought up to date, so that the gather runs in its device order.
+static int constraint_materials_on(pbd_engine *e, int type, bool fill) {
+    const unsigned bit = 1u << type;
+    if (!(e->batch.cmatMask & bit)) {
+        const size_t bytes = (size_t)e->batch.K * e->host[type].ids.size() * type_shape(type).nMat * sizeof(float);
+        CKE(e->dev[type].cmat.alloc(bytes));
+        if (fill) {
+            std::vector<float> now;
+            CKE(stepped_materials(e, type, now));
+            CK(cudaMemcpyAsync(e->dev[type].cmat.p, now.data(), bytes, cudaMemcpyHostToDevice, e->stream));
+            CK(cudaStreamSynchronize(e->stream));  // `now` dies here
+        }
+        if (e->batch.matMask & bit) {  // rows off: the table holds the shared parameters again (the resident batch kernels read it)
+            CKE(write_replica_materials(e, type, e->dev[type].arrays.matU, 0));
+            e->batch.matMask &= ~bit;
+        }
+        e->batch.cmatMask |= bit;  // image_key: planned again with the tables, if they were not there
+        CKE(flatten(e));
+        CKE(gather_materials(e, type, (const float *)e->dev[type].cmat.p, false, nullptr));  // (where flatten did not plan: the values now in force)
+    }
+    return flatten(e);
+}
+
+extern "C" int pbd_set_replica_constraint_materials(pbd_engine *e, int type, const float *mat) {
+    const char *what = "pbd_set_replica_constraint_materials";
+    CKE(constraint_materials_refusal(e, what, type));
+    CKE(use(e));
+    if (!mat) {  // the shared parameters
+        CKE(drop_constraint_materials(e, 1u << type));
+        return pbd_set_replica_materials(e, type, nullptr);
+    }
+    CKE(constraint_materials_on(e, type, false));
+    DevType &d = e->dev[type];
+    CK(cudaMemcpyAsync(d.cmat.p, mat, (size_t)e->batch.K * d.count * type_shape(type).nMat * sizeof(float), cudaMemcpyHostToDevice, e->stream));
+    return gather_materials(e, type, (const float *)d.cmat.p, false, nullptr);
+}
+extern "C" int pbd_set_replica_constraint_materials_device(pbd_engine *e, int type, const float *mat, const unsigned char *replicas, void *stream) {
+    const char *what = "pbd_set_replica_constraint_materials_device";
+    CKE(constraint_materials_refusal(e, what, type));
+    return device_call(e, what, "mat", mat, replicas, stream, [&] { return constraint_materials_on(e, type, replicas != nullptr); },
+                       [&] { return gather_materials(e, type, mat, true, replicas); });
+}
+extern "C" int pbd_get_replica_materials(pbd_engine *e, int type, float *dst) {
+    if (!e || !dst) return fail("pbd_get_replica_materials: null argument");
+    if (type < 0 || type >= PBD_NUM_TYPES) return fail("pbd_get_replica_materials: unknown constraint type %d", type);
+    if (type_shape(type).nMat == 0) return fail("pbd_get_replica_materials: constraint type %d has no material parameters", type);
+    CKE(use(e));
+    const DevType &d = e->dev[type];
+    if ((e->batch.cmatMask >> type) & 1u) {
+        CK(cudaStreamSynchronize(e->stream));
+        CK(cudaMemcpy(dst, d.cmat.p, (size_t)e->batch.K * e->host[type].ids.size() * type_shape(type).nMat * sizeof(float), cudaMemcpyDeviceToHost));
+        return 0;
+    }
+    std::vector<float> now;
+    CKE(stepped_materials(e, type, now));
+    if (!now.empty()) memcpy(dst, now.data(), now.size() * sizeof(float));
     return 0;
 }
 
@@ -1166,7 +1332,7 @@ template <class F> static int with_project_type(int type, int variant, F &&f) {
 static int launch_bucket(pbd_engine *e, const Bucket &b, float h, int iterZero, cudaStream_t s, bool pdl) {
     const TypeArrays a = batch_arrays(e, b.type);
     const unsigned block = project_block(e, b.count * e->batch.K);
-    const ReplicaStrides rs{e->n, {e->dev[b.type].count}, {replica_mat(e, b.type)}, {replica_geo(e, b.type)}};
+    const ReplicaStrides rs{e->n, {e->dev[b.type].count}, {replica_mat(e, b.type)}, {replica_geo(e, b.type)}, {replica_cmat(e, b.type)}};
     return with_project_type(b.type, a.variant, [&](auto T, auto V) -> int {
         constexpr int TT = decltype(T)::value, VAR = decltype(V)::value;
         if (e->batch.K > 1) CK(launch_step_kernel(k_project<TT, VAR, true>, dim3(nblk(b.count, block), e->batch.K), block, s, pdl, attr_ptr(e, PBD_ATTR_X), a, b.first, b.count, h, iterZero, rs));
@@ -1210,7 +1376,7 @@ static int launch_colour(pbd_engine *e, size_t b0, size_t b1, float h, int iterZ
     for (size_t c0 = b0; c0 < b1; c0 += kMultiSegments) {
         const size_t c1 = std::min(b1, c0 + (size_t)kMultiSegments);
         MultiArgs m{};
-        ReplicaStrides rs{e->n, {}, {}, {}};
+        ReplicaStrides rs{e->n, {}, {}, {}, {}};
         m.nSeg = (int)(c1 - c0);
         unsigned blocks = 0, total = 0;
         for (size_t i = c0; i < c1; i++) total += e->buckets[i].count;
@@ -1220,7 +1386,7 @@ static int launch_colour(pbd_engine *e, size_t b0, size_t b1, float h, int iterZ
             const int k = (int)(i - c0);
             m.type[k] = b.type; m.first[k] = b.first; m.count[k] = b.count; m.blockStart[k] = blocks;
             m.arrays[k] = batch_arrays(e, b.type);
-            rs.nLambda[k] = e->dev[b.type].count; rs.mat[k] = replica_mat(e, b.type); rs.nGeo[k] = replica_geo(e, b.type);
+            rs.nLambda[k] = e->dev[b.type].count; rs.mat[k] = replica_mat(e, b.type); rs.nGeo[k] = replica_geo(e, b.type); rs.nMat[k] = replica_cmat(e, b.type);
             blocks += nblk(b.count, block);
         }
         for (int k = m.nSeg; k <= kMultiSegments; k++) m.blockStart[k] = blocks;
@@ -1301,7 +1467,7 @@ static int enqueue_step_resident(pbd_engine *e, cudaStream_t s, unsigned long lo
     ra.secondOrder = e->velMethod;
     ra.xLaunch = (++e->xLaunch) << 32;  // above every flag value of the earlier launches, whatever subSteps / maxIter they ran with
     ra.rb = rb_state(e);
-    for (int t = 0; t < PBD_NUM_TYPES; t++) { ra.types[t] = batch_arrays(e, t); ra.lamCount[t] = e->dev[t].count; ra.geoCount[t] = replica_geo(e, t); }
+    for (int t = 0; t < PBD_NUM_TYPES; t++) { ra.types[t] = batch_arrays(e, t); ra.lamCount[t] = e->dev[t].count; ra.geoCount[t] = replica_geo(e, t); ra.matCount[t] = replica_cmat(e, t); }
     ra.replicas = e->res.replicas; ra.replicaStride = e->n;
     ra.repMat = (const float *)e->batch.mat.p; ra.repGravity = e->batch.gravitySet ? (const float *)e->batch.gravity.p : nullptr;
     *launches = 1;
@@ -1541,7 +1707,8 @@ static std::vector<unsigned char> graph_key(const pbd_engine *e) {
                  e->batch.gravitySet ? e->batch.gravity.p : nullptr, X, Q, V, W, oldX, lastX, oldQ, lastQ, I, Iinv, nRb);
     for (int t = 0; t < PBD_NUM_TYPES; t++) {
         const auto [idx2, idx4, idx3, gv, gs, mat, matU, lambda, rbX, rbQ, rbIinv, variant] = batch_arrays(e, t);
-        append_bytes(key, idx2, idx4, idx3, gv, gs, mat, matU, lambda, rbX, rbQ, rbIinv, variant, replica_mat(e, t), replica_geo(e, t), e->dev[t].count);
+        append_bytes(key, idx2, idx4, idx3, gv, gs, mat, matU, lambda, rbX, rbQ, rbIinv, variant, replica_mat(e, t), replica_geo(e, t), replica_cmat(e, t),
+                     e->dev[t].count);
     }
     return key;
 }

@@ -120,13 +120,15 @@ __device__ __forceinline__ void project_joint(const Acc &acc, const TypeArrays &
 }
 
 // VAR: compile-time layout variant of the type (IsometricBending: 0 = rank-1 Kp, 1 = full Q), -1 = read a.variant at run time
+// matOff: a batch's replica with per-constraint materials of its own reads them at i + matOff (resident.cuh, like geoOff)
 template <int T, class Acc, int VAR = -1>
 __device__ __forceinline__ void project_streamed_acc(const Acc &acc, const TypeArrays &a, unsigned i, const Streamed &s, float dt,
                                                      bool iterZero, bool lambdaGiven = false, float lambdaValue = 0.0f, const MatRow &matRow = MatRow{},
-                                                     unsigned geoOff = 0u) {
+                                                     unsigned geoOff = 0u, unsigned matOff = 0u) {
     if (T == PBD_BALLJOINT || T == PBD_RB_PARTICLE_BALLJOINT) { project_joint<T>(acc, a, s); return; }
     constexpr bool XPBD = type_shape(T).xpbd;
     constexpr int NB = type_shape(T).nBodies;
+    const unsigned mi = i + matOff;
     const typename Acc::Handle h0 = acc.handle(s.b.x), h1 = acc.handle(s.b.y), h2 = acc.handle(NB >= 3 ? s.b.z : s.b.x), h3 = acc.handle(NB >= 4 ? s.b.w : s.b.x);
     float4 p0 = acc.ld(h0), p1 = acc.ld(h1), p2, p3;
     if (NB >= 3) p2 = acc.ld(h2);
@@ -135,24 +137,24 @@ __device__ __forceinline__ void project_streamed_acc(const Acc &acc, const TypeA
     if (XPBD && !iterZero) lam = lambdaGiven ? lambdaValue : __ldcg(a.lambda + i);  // m_lambda; zero at the first sweep of a substep (Constraints.cpp:1241-1242)
 
     if (T == PBD_DISTANCE) {
-        project_distance(p0, p1, s.s0, matv(a, 0, i, matRow));
+        project_distance(p0, p1, s.s0, matv(a, 0, mi, matRow));
     } else if (T == PBD_DISTANCE_XPBD) {
-        project_distance_xpbd(p0, p1, s.s0, xpbd_alpha(matv(a, 0, i, matRow), dt), lam);
+        project_distance_xpbd(p0, p1, s.s0, xpbd_alpha(matv(a, 0, mi, matRow), dt), lam);
     } else if (T == PBD_FEMTRIANGLE) {
-        const FemTriMaterial m = femtri_material(matv(a, 0, i, matRow), matv(a, 1, i, matRow), matv(a, 2, i, matRow), matv(a, 3, i, matRow), matv(a, 4, i, matRow));
+        const FemTriMaterial m = femtri_material(matv(a, 0, mi, matRow), matv(a, 1, mi, matRow), matv(a, 2, mi, matRow), matv(a, 3, mi, matRow), matv(a, 4, mi, matRow));
         project_femtriangle(p0, p1, p2, s.s0, s.g0, m);
     } else if (T == PBD_STRAINTRIANGLE) {
-        project_straintriangle(p0, p1, p2, s.g0, matv(a, 0, i, matRow), matv(a, 1, i, matRow), matv(a, 2, i, matRow), matv(a, 3, i, matRow) != 0.0f, matv(a, 4, i, matRow) != 0.0f);
+        project_straintriangle(p0, p1, p2, s.g0, matv(a, 0, mi, matRow), matv(a, 1, mi, matRow), matv(a, 2, mi, matRow), matv(a, 3, mi, matRow) != 0.0f, matv(a, 4, mi, matRow) != 0.0f);
     } else if (T == PBD_DIHEDRAL) {
-        project_dihedral(p0, p1, p2, p3, s.s0, matv(a, 0, i, matRow));
+        project_dihedral(p0, p1, p2, p3, s.s0, matv(a, 0, mi, matRow));
     } else if (T == PBD_VOLUME) {
-        project_volume<false>(p0, p1, p2, p3, s.s0, matv(a, 0, i, matRow), 0.0f, lam);
+        project_volume<false>(p0, p1, p2, p3, s.s0, matv(a, 0, mi, matRow), 0.0f, lam);
     } else if (T == PBD_VOLUME_XPBD) {
-        const float k = matv(a, 0, i, matRow);
+        const float k = matv(a, 0, mi, matRow);
         project_volume<true>(p0, p1, p2, p3, s.s0, k, xpbd_alpha(k, dt), lam);
     } else if (T == PBD_ISOBENDING || T == PBD_ISOBENDING_XPBD) {
         constexpr bool X = (T == PBD_ISOBENDING_XPBD);
-        const float k = matv(a, 0, i, matRow);
+        const float k = matv(a, 0, mi, matRow);
         const float alpha = X ? xpbd_alpha(k, dt) : 0.0f;
         if (VAR == 0 || (VAR < 0 && a.variant == 0)) project_isobending_rank1<X>(p0, p1, p2, p3, s.g0, k, alpha, lam);
         else project_isobending_fullq<X>(p0, p1, p2, p3, s.g0, __ldg(a.gv[1] + (i + geoOff)), __ldg(a.gv[2] + (i + geoOff)), __ldg(a.gv[3] + (i + geoOff)), k, alpha, lam);
@@ -161,12 +163,12 @@ __device__ __forceinline__ void project_streamed_acc(const Acc &acc, const TypeA
         inv.m[0][0] = s.g0.x; inv.m[0][1] = s.g0.y; inv.m[0][2] = s.g0.z; inv.m[1][0] = s.g0.w;
         inv.m[1][1] = s.g1.x; inv.m[1][2] = s.g1.y; inv.m[2][0] = s.g1.z; inv.m[2][1] = s.g1.w;
         inv.m[2][2] = s.s0;
-        if (T == PBD_STRAINTET) project_straintet(p0, p1, p2, p3, inv, matv(a, 0, i, matRow), matv(a, 1, i, matRow), matv(a, 2, i, matRow) != 0.0f, matv(a, 3, i, matRow) != 0.0f);
-        else project_femtet<(T == PBD_FEMTET_XPBD)>(p0, p1, p2, p3, s.s1, inv, matv(a, 0, i, matRow), matv(a, 1, i, matRow), dt, lam);
+        if (T == PBD_STRAINTET) project_straintet(p0, p1, p2, p3, inv, matv(a, 0, mi, matRow), matv(a, 1, mi, matRow), matv(a, 2, mi, matRow) != 0.0f, matv(a, 3, mi, matRow) != 0.0f);
+        else project_femtet<(T == PBD_FEMTET_XPBD)>(p0, p1, p2, p3, s.s1, inv, matv(a, 0, mi, matRow), matv(a, 1, mi, matRow), dt, lam);
     } else if (T == PBD_SHAPEMATCHING) {
         const unsigned g = i + geoOff;
         project_shapematching(p0, p1, p2, p3, __ldg(a.gv[0] + g), __ldg(a.gv[1] + g), __ldg(a.gv[2] + g), __ldg(a.gv[3] + g), __ldg(a.gv[4] + g),
-                              __ldg(a.gv[5] + g), matv(a, 0, i, matRow));
+                              __ldg(a.gv[5] + g), matv(a, 0, mi, matRow));
     }
 
     if (XPBD) __stcg(a.lambda + i, lam);
@@ -203,13 +205,14 @@ constexpr int kMultiSegments = 4;
 // blockIdx.y, whose particles start at slot y x nPos and whose multipliers of segment k's type start at y x nLambda[k] (k_project: [0]).
 // mat[k]: segment k's type in replica 0's row of the batch's material table (rows of kMatRowFloats floats), or null: no replica has
 // material parameters of its own for that type.  nGeo[k]: with per-replica rest shapes (pbd_set_replica_rest_positions) the geometry
-// arrays hold every replica's, replica y's at y x nGeo[k]; 0: one geometry shared by all.
+// arrays hold every replica's, replica y's at y x nGeo[k]; 0: one geometry shared by all.  nMat[k]: with per-constraint materials of every
+// replica (pbd_set_replica_constraint_materials) the material arrays hold every replica's, replica y's at y x nMat[k]; 0: shared.
 struct ReplicaStrides {
-    unsigned nPos; unsigned nLambda[kMultiSegments]; const float *mat[kMultiSegments]; unsigned nGeo[kMultiSegments];
+    unsigned nPos; unsigned nLambda[kMultiSegments]; const float *mat[kMultiSegments]; unsigned nGeo[kMultiSegments]; unsigned nMat[kMultiSegments];
     __device__ __forceinline__ const float *mat_row(int k, unsigned rep) const { return mat[k] ? mat[k] + (size_t)rep * kMatRowFloats : nullptr; }
 };
-// the type's arrays with the multipliers and the geometry of replica `rep`
-__device__ __forceinline__ TypeArrays replica_arrays(const TypeArrays &a, unsigned rep, unsigned nLambda, unsigned nGeo) {
+// the type's arrays with the multipliers, the geometry and the per-constraint materials of replica `rep`
+__device__ __forceinline__ TypeArrays replica_arrays(const TypeArrays &a, unsigned rep, unsigned nLambda, unsigned nGeo, unsigned nMat = 0u) {
     TypeArrays r = a;
     if (r.lambda) r.lambda += (size_t)rep * nLambda;
     if (nGeo) {
@@ -218,6 +221,11 @@ __device__ __forceinline__ TypeArrays replica_arrays(const TypeArrays &a, unsign
         for (int k = 0; k < kMaxGeoV; k++) if (r.gv[k]) r.gv[k] += o;
 #pragma unroll
         for (int k = 0; k < kMaxGeoS; k++) if (r.gs[k]) r.gs[k] += o;
+    }
+    if (nMat) {
+        const size_t o = (size_t)rep * nMat;
+#pragma unroll
+        for (int k = 0; k < kMaxMat; k++) if (r.mat[k]) r.mat[k] += o;
     }
     return r;
 }
@@ -228,7 +236,7 @@ __global__ void __launch_bounds__(kProjectThreads) k_project(float4 *pos, TypeAr
     const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= count) return;  // an exited thread counts as having passed the dependency
     MatRow matRow;
-    if (BATCH) { pos += (size_t)blockIdx.y * rs.nPos; a = replica_arrays(a, blockIdx.y, rs.nLambda[0], rs.nGeo[0]); matRow = load_mat_row<T>(rs.mat_row(0, blockIdx.y)); }
+    if (BATCH) { pos += (size_t)blockIdx.y * rs.nPos; a = replica_arrays(a, blockIdx.y, rs.nLambda[0], rs.nGeo[0], rs.nMat[0]); matRow = load_mat_row<T>(rs.mat_row(0, blockIdx.y)); }
     const Streamed s = load_streamed<T>(a, first + i);
     pdl_wait_after(s.b.x ^ s.b.y, s.g0.x + s.g1.x + s.s0 + s.s1);
     project_streamed<T, VAR>(pos, a, first + i, s, dt, iterZero != 0, matRow);
@@ -291,7 +299,7 @@ __global__ void __launch_bounds__(kProjectThreads) k_project_multi(float4 *pos, 
     if (i >= m.count[s]) return;
     const unsigned ci = m.first[s] + i;
     TypeArrays batchArrays;
-    if (BATCH) { pos += (size_t)blockIdx.y * rs.nPos; batchArrays = replica_arrays(m.arrays[s], blockIdx.y, rs.nLambda[s], rs.nGeo[s]); }
+    if (BATCH) { pos += (size_t)blockIdx.y * rs.nPos; batchArrays = replica_arrays(m.arrays[s], blockIdx.y, rs.nLambda[s], rs.nGeo[s], rs.nMat[s]); }
     const TypeArrays &a = BATCH ? batchArrays : m.arrays[s];
     PBD_FOR_TYPE(kMaskAll, m.type[s],
         MatRow matRow;
@@ -505,6 +513,34 @@ __global__ void __launch_bounds__(128) k_derive_geometry(const __grid_constant__
 #pragma unroll
     for (int k = 0; k < kMaxGeoS; k++)
         if (d.gs[k]) d.gs[k][o] = col(pc.gs[k]);
+}
+
+// k_gather_materials: per-constraint material parameters of a batch (pbd_set_replica_constraint_materials), one thread per (constraint i of
+// one type in device order, replica blockIdx.y).  Replica r's row local[i] of `src` (K x count rows of nMat floats, in the order the
+// constraints were added) goes to dst[k][r count + i], the device-ordered arrays the projections read; with `keep` the row is also written
+// there (the engine's copy in the order they were added).  mask: as k_pack3 -- a replica left out keeps its values, and its rows of src are
+// not read.
+struct GatherMatArgs {
+    const float *src;
+    float *keep;
+    float *dst[kMaxMat];
+    const unsigned *local;       // [count] device position -> position among the type's constraints in the order they were added
+    const unsigned char *mask;
+    unsigned count;
+    int nMat;
+};
+__global__ void __launch_bounds__(128) k_gather_materials(const __grid_constant__ GatherMatArgs g) {
+    if (g.mask && !g.mask[blockIdx.y]) return;
+    const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= g.count) return;
+    const size_t row = ((size_t)blockIdx.y * g.count + __ldg(g.local + i)) * (unsigned)g.nMat, o = (size_t)blockIdx.y * g.count + i;
+#pragma unroll
+    for (int k = 0; k < kMaxMat; k++)
+        if (k < g.nMat) {
+            const float v = g.src[row + k];
+            g.dst[k][o] = v;
+            if (g.keep) g.keep[row + k] = v;
+        }
 }
 
 __global__ void k_set_w(float4 *__restrict__ pos, float4 *__restrict__ vel, const float *__restrict__ mass, unsigned n, const unsigned *__restrict__ slot,

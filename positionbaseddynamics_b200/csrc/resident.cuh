@@ -80,6 +80,8 @@ struct ResidentArgs {
     const float *repMat, *repGravity;
     // per-replica rest shapes (pbd_set_replica_rest_positions): replica r's geometry of type t at r x geoCount[t] (0: shared)
     unsigned geoCount[PBD_NUM_TYPES];
+    // per-constraint materials of every replica (pbd_set_replica_constraint_materials): replica r's of type t at r x matCount[t] (0: shared)
+    unsigned matCount[PBD_NUM_TYPES];
 };
 
 // ---- cluster primitives --------------------------------------------------------------------------------------------------
@@ -239,6 +241,7 @@ __device__ __forceinline__ void run_items(const ResidentArgs &A, const Acc &acc,
         TypeArrays batchArrays;  // a batch: the arrays with replica rep's multipliers
         if (BATCH) batchArrays = replica_arrays(A.types[T], rep, A.lamCount[T], 0u);
         const unsigned go = BATCH ? rep * A.geoCount[T] : 0u;  // replica rep's geometry (pbd_set_replica_rest_positions; 0: shared)
+        const unsigned mo = BATCH ? rep * A.matCount[T] : 0u;  // ... and materials (pbd_set_replica_constraint_materials; 0: shared)
         MatRow matRow;
         if (BATCH) { matRow = load_mat_row<T>(rows + mat_offset(T)); matRow.on = true; }
         const TypeArrays &ta = BATCH ? batchArrays : A.types[T];
@@ -255,7 +258,7 @@ __device__ __forceinline__ void run_items(const ResidentArgs &A, const Acc &acc,
                     const unsigned j2 = i + 2u * stride;
                     const bool h2 = j2 < n;
                     if (h2) fetch(j2, s2, l2);
-                    project_streamed_acc<T, Acc, 0>(acc, ta, first + i, s0, A.h, iterZero, true, l0, matRow, go);
+                    project_streamed_acc<T, Acc, 0>(acc, ta, first + i, s0, A.h, iterZero, true, l0, matRow, go, mo);
                     if (!h1) break;
                     s0 = s1; l0 = l1; s1 = s2; l1 = l2; h1 = h2; i += stride;
                 }
@@ -271,7 +274,7 @@ __device__ __forceinline__ void run_items(const ResidentArgs &A, const Acc &acc,
                 const bool more = j < n;
                 Streamed nxt; float lamN = 0.0f;
                 if (is_pipelined<T>() && more) { nxt = load_streamed<T>(ta, first + j, go); if (type_shape(T).xpbd && !iterZero) lamN = __ldcg(ta.lambda + first + j); }
-                project_streamed_acc<T, Acc, 0>(acc, ta, first + i, cur, A.h, iterZero, true, lam, matRow, go);  // variant 0 only: flatten refuses the full-Q bending layout in this mode
+                project_streamed_acc<T, Acc, 0>(acc, ta, first + i, cur, A.h, iterZero, true, lam, matRow, go, mo);  // variant 0 only: flatten refuses the full-Q bending layout in this mode
                 if (!more) break;
                 if (!is_pipelined<T>()) { nxt = load_streamed<T>(ta, first + j, go); if (type_shape(T).xpbd && !iterZero) lamN = __ldcg(ta.lambda + first + j); }
                 cur = nxt; lam = lamN; i = j;

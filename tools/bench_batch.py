@@ -4,7 +4,8 @@ stepped one after another by a K = 1 engine; the resident cluster size C swept o
 power limit read in the same run.  The four scenes run four different resident instantiations (cloth, FEM, cloth-XPBD and light type
 masks).
 
-    python tools/bench_batch.py [--out results.json] [--quick] [--replica-rows] [--sweep] [--rest-shapes] [--colliders] [--ks 8,132] [--no-baseline]
+    python tools/bench_batch.py [--out results.json] [--quick] [--replica-rows] [--sweep] [--rest-shapes] [--colliders] [--constraint-materials]
+                                [--ks 8,132] [--no-baseline]
 
 --replica-rows measures every batch twice in a row: with the shared parameters, and with per-replica material rows and gravity
 (pbd_set_replica_materials / pbd_set_replica_gravity) equal to the shared values, so that the work is identical and the difference is what
@@ -16,6 +17,11 @@ the geometry of K rest shapes against building K host models (the host mirror's 
 --colliders measures only the contact path of batches: cfg1 at K = 8, 132, 1056 and the 100x100 XPBD cloth at K = 33, 264, each in graph
 and resident mode, without and with three per-replica colliders (pbd_set_replica_colliders: a sphere, a rotated box and a torus cutting
 through the cloth's plane at random places, every replica its own), alternating.  The difference is the cost of the contact launch.
+--constraint-materials measures every batch four times in a row: with the shared parameters, with per-constraint materials of every replica
+(pbd_set_replica_constraint_materials) equal to the shared values, and both again, so that the work is identical and the difference is
+what reading the K x count material arrays costs; their size is printed beside each row.  It also times the device form of the call
+(pbd_set_replica_constraint_materials_device) for every replica and for a 10 % mask, 200 calls enqueued behind a spin so that the
+gathers run back to back, against the algorithmic bytes of the gather.
 --ks replaces the K sweep of every scene; --no-baseline skips the one-after-another baseline and the C sweep.  Without --rest-shapes or
 --replica-rows the script also runs against a build without those calls, so that shared-parameter batches can be compared across builds.
 
@@ -175,7 +181,50 @@ def replica_colliders(m, k):
     return rigid, body_x
 
 
-def engine(m, mode, k, clusters=None, rows=None, rest=False, colliders=False):
+def constraint_materials(m, k):
+    """{type: (k, count, nMat)}: every material-bearing type's per-constraint values, the shared ones in every replica."""
+    out = {}
+    for t in range(_capi.NUM_TYPES):
+        sel = np.nonzero(np.asarray(m["types"]) == t)[0]
+        if len(sel) and _capi.num_materials(t):
+            cols = MAT_FIRST_COLUMN[t] + np.arange(_capi.num_materials(t))
+            out[t] = np.ascontiguousarray(np.repeat(np.asarray(m["params"], np.float32)[sel][:, cols][None], k, 0))
+    return out
+
+
+def gather_timing(m, k, calls=200):
+    """µs per pbd_set_replica_constraint_materials_device call's gather, for every replica and for every tenth, against the algorithmic
+    bytes: per written (replica, constraint) nMat floats read, written to the device-ordered arrays and to the engine's copy, and one
+    4-byte map entry read."""
+    import torch
+    mats = constraint_materials(m, k)
+    eng = engine(m, _capi.MODE_GRAPH, k, cmat=mats)
+    out = []
+    try:
+        eng.step(1); eng.sync()
+        src = {t: torch.from_numpy(f.reshape(-1)).cuda() for t, f in mats.items()}
+        for label, mask in (("all", None), ("10 %", np.arange(k) % 10 == 0)):
+            dm = None if mask is None else torch.from_numpy(mask).cuda()
+            written = k if mask is None else int(mask.sum())
+            for t, f in mats.items():
+                nbytes = written * f.shape[1] * (3 * 4 * f.shape[2] + 4)
+                torch.cuda.synchronize()
+                s = torch.cuda.current_stream()
+                torch.cuda._sleep(50_000_000)  # the calls below are enqueued while this spins, then run back to back
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record(s)
+                for _ in range(calls):
+                    eng.set_replica_constraint_materials_device(t, src[t], replicas=dm, stream=s.cuda_stream)
+                e1.record(s)
+                e1.synchronize()
+                us = e0.elapsed_time(e1) * 1e3 / calls
+                out.append({"K": k, "type": t, "mask": label, "us": us, "bytes": nbytes, "tb_s": nbytes / (us * 1e-6) / 1e12})
+    finally:
+        eng.close()
+    return out
+
+
+def engine(m, mode, k, clusters=None, rows=None, rest=False, colliders=False, cmat=None):
     if clusters:
         os.environ["PBD_B200_CLUSTERS"] = "1x%d" % clusters  # the planner's cluster-size override (read when the image is planned)
     else:
@@ -194,6 +243,9 @@ def engine(m, mode, k, clusters=None, rows=None, rest=False, colliders=False):
         eng.set_replica_gravity(rows[1])
     if rest:  # every replica's rest shape = the model's: the same geometry, from the per-replica arrays
         eng.set_replica_rest_positions(np.repeat(np.asarray(m["x0"], np.float32)[None], k, 0))
+    if cmat is not None:
+        for t, f in cmat.items():
+            eng.set_replica_constraint_materials(t, f)
     if colliders:
         rigid, body_x = replica_colliders(m, k)
         eng.set_replica_colliders([_capi.ParticleCollider(0, len(m["x0"]), 0.5, 0.1)], rigid, body_x)
@@ -212,11 +264,11 @@ def timed(eng, warmup=3, min_s=0.4):
     return st.last_step_ms / steps, steps
 
 
-def measure(m, mode, k, clusters=None, rows=None, rest=False, colliders=False):
+def measure(m, mode, k, clusters=None, rows=None, rest=False, colliders=False, cmat=None):
     t0 = time.time()
     eng = None
     try:
-        eng = engine(m, mode, k, clusters, rows, rest, colliders)
+        eng = engine(m, mode, k, clusters, rows, rest, colliders, cmat)
         ms, steps = timed(eng)
         _, active = eng.get_mode()
     except _capi.PbdError as ex:
@@ -259,10 +311,12 @@ def main():
     ap.add_argument("--sweep", action="store_true", help="132 cfg1 replicas, each with its own stiffnesses")
     ap.add_argument("--rest-shapes", action="store_true", help="every batch also with per-replica rest shapes; device derivation against host builds")
     ap.add_argument("--colliders", action="store_true", help="only the contact path: batches without and with three per-replica colliders")
+    ap.add_argument("--constraint-materials", action="store_true", help="every batch also with per-constraint materials equal to the shared ones; gather timing")
     ap.add_argument("--ks", default=None, help="comma-separated K to measure instead of each scene's sweep")
     ap.add_argument("--no-baseline", action="store_true", help="skip the one-after-another baseline and the C sweep")
     a = ap.parse_args()
-    res = {"card": card(), "rows": [], "c_sweep": [], "replica_rows": [], "sweep": [], "rest_shapes": [], "derive": [], "colliders": []}
+    res = {"card": card(), "rows": [], "c_sweep": [], "replica_rows": [], "sweep": [], "rest_shapes": [], "derive": [], "colliders": [],
+           "constraint_materials": [], "gather": []}
     print("card: %s" % res["card"], flush=True)
     if a.colliders:
         for name, ks in COLLIDER_KS.items():
@@ -318,6 +372,22 @@ def main():
                 geo_mb = sum(k * int((np.asarray(m["types"]) == t).sum()) * GEO_BYTES.get(t, 0) for t in range(_capi.NUM_TYPES)) * 1e-6
                 res["rest_shapes"].append({"scene": name, "K": k, "mode": label, "shared_ms": ms[0::2], "rest_ms": ms[1::2], "geometry_mb": geo_mb})
                 print("  rest shapes K=%5d %-8s shared %.4f %.4f ms | per-replica %.4f %.4f ms (%.0f MB of geometry)" % (k, label, ms[0], ms[2], ms[1], ms[3], geo_mb), flush=True)
+        for k in (ks if a.constraint_materials else []):
+            if k == 1:
+                continue
+            cm = constraint_materials(m, k)
+            mb = sum(f.size for f in cm.values()) * 4 * 1e-6  # the device-ordered arrays the kernels read (the engine's copy is as large)
+            for label, md in (("graph", _capi.MODE_GRAPH), ("resident", _capi.MODE_RESIDENT)):
+                # shared, per-constraint, shared, per-constraint: the spread of each pair is next to the difference between them
+                ms = [measure(m, md, k, cmat=cm if i & 1 else None).get("ms", float("nan")) for i in range(4)]
+                res["constraint_materials"].append({"scene": name, "K": k, "mode": label, "shared_ms": ms[0::2], "constraint_ms": ms[1::2], "arrays_mb": mb})
+                print("  constraint materials K=%5d %-8s shared %.4f %.4f ms | per-constraint %.4f %.4f ms (%.0f MB of material arrays)"
+                      % (k, label, ms[0], ms[2], ms[1], ms[3], mb), flush=True)
+            for g in gather_timing(m, k):
+                g["scene"] = name
+                res["gather"].append(g)
+                print("  gather K=%5d type %2d %-4s %8.1f us  %.1f MB  %.2f TB/s (%.0f %% of 3.35 TB/s)"
+                      % (k, g["type"], g["mask"], g["us"], g["bytes"] * 1e-6, g["tb_s"], 100.0 * g["tb_s"] / 3.35), flush=True)
         if a.rest_shapes and name in DERIVE_K:
             d = derive_timing(name, m, DERIVE_K[name])
             res["derive"].append(d)

@@ -77,6 +77,8 @@ typedef struct pbd_stats {
     unsigned constraints_per_type[PBD_NUM_TYPES];
     double bytes_per_step;             /* algorithmic bytes of one step (DESIGN.md table) */
     float last_step_ms;                /* device time of the last pbd_step call (CUDA events on the engine stream), after pbd_sync */
+    unsigned long long images_planned; /* device images planned so far (a new model, mode, batch size or body arrays plan one) */
+    unsigned long long graph_captures; /* step graphs captured so far (PBD_MODE_GRAPH captures again when what the step reads changes) */
 } pbd_stats;
 
 const char *pbd_last_error(void);
@@ -236,8 +238,11 @@ int pbd_set_replica_colliders(pbd_engine *e, unsigned nParticleColliders, const 
  *  - Contacts: every replica against its own static colliders through pbd_set_replica_colliders (contact section above); the
  *    colliders of pbd_set_colliders belong to one scene.
  *  - pbd_get_stats: projections and bytes_per_step count every replica; num_particles and num_constraints are per replica.
- *  - K > 1 is refused with rigid bodies or joints, with pbd_set_colliders' colliders and in PBD_MODE_JACOBI.  PBD_MODE_RESIDENT runs one cluster of CTAs
- *    per replica and refuses a replica that does not fit one cluster; PBD_MODE_AUTO then runs the graph mode.
+ *  - Rigid bodies and joints: every replica with its own bodies through pbd_set_replica_rigid_bodies (below); the bodies of
+ *    pbd_set_rigid_bodies belong to one scene.
+ *  - K > 1 is refused with pbd_set_rigid_bodies' bodies (and joints without per-replica bodies), with pbd_set_colliders' colliders and in
+ *    PBD_MODE_JACOBI.  PBD_MODE_RESIDENT runs one cluster of CTAs per replica and refuses a replica that does not fit one cluster;
+ *    PBD_MODE_AUTO then runs the graph mode.
  * pbd_set_replicas: 1 <= K <= 65535 and K*n < 2^31.  Every replica starts as a copy of replica 0's current state (x, v, x0, oldX,
  * lastX, masses), the XPBD multipliers at zero, and the image is planned again.  At K = 1 every call behaves as for one scene. */
 int pbd_set_replicas(pbd_engine *e, unsigned K);
@@ -292,6 +297,28 @@ int pbd_set_replica_rest_positions(pbd_engine *e, const float *x0);
  * pbd_num_materials(type) (the non-material columns of the type's parameter layout, in layout order), constraints in the order they were
  * added.  Without an override: the shared geometry, repeated for every replica.  Refused for the joint types. */
 int pbd_get_replica_geometry(pbd_engine *e, int type, float *dst);
+/* Rigid bodies of every replica (K > 1).  mass, x, q, inertia, v, omega: K*n rows each, replica after replica, in the layouts of
+ * pbd_set_rigid_bodies (q as (w,x,y,z), principal inertia; v and omega may be NULL = 0).  Defines n bodies per replica: joints added
+ * afterwards index 0 .. n-1 and mean "this replica's body i".  Each replica's old and last state equal its current state; each may have its
+ * own masses and inertia, and a body may be static in one replica and dynamic in another.  Replica r then advances bit for bit as a
+ * single-scene engine given replica r's rows through pbd_set_rigid_bodies and the same constraints and groups; per-replica gravity
+ * (pbd_set_replica_gravity) moves replica r's bodies too.  pbd_get_rigid_bodies returns K*n rows.
+ * A repeat call with the same n copies in stream order into device arrays that keep their address: no host synchronisation, no new plan
+ * or graph capture.  A different n may synchronise and recolours (as pbd_set_rigid_bodies).  pbd_set_replicas(K') starts every replica
+ * from replica 0's bodies (state, history, masses, inertia) and keeps them per-replica bodies; pbd_set_rigid_bodies makes them one
+ * scene's again.  Contacts stay with static colliders (pbd_set_replica_colliders, whose bodies are its own).
+ * Refused, with nothing changed: at K = 1, a null mass / x / q / inertia with n > 0, K*n >= 2^31, PBD_MODE_JACOBI. */
+int pbd_set_replica_rigid_bodies(pbd_engine *e, unsigned n, const float *mass, const float *x, const float *q, const float *inertia,
+                                 const float *v, const float *omega);
+/* Rigid-body state in device memory, at any K where the engine holds bodies: the layouts above (K*n rows), the stream contract, mask
+ * semantics and refusals of pbd_set_attr_device.  The set writes x and q (required), v and omega (NULL = 0), and mass / inertia (NULL = each
+ * body keeps its own), converted on the device with the host call's IEEE divisions, so a device set and a host set of the same rows give
+ * identical bits; every written replica's old and last state equal its new current state.  A replica outside `replicas` stays bit for bit
+ * as it was and its rows are not read.  The contact path reads written masses back before it next checks that colliders of
+ * pbd_set_colliders sit on static bodies.  The get writes any of x, q, v, omega that is not NULL. */
+int pbd_set_rigid_bodies_device(pbd_engine *e, const float *mass, const float *x, const float *q, const float *inertia, const float *v,
+                                const float *omega, const unsigned char *replicas, void *stream);
+int pbd_get_rigid_bodies_device(pbd_engine *e, float *x, float *q, float *v, float *omega, void *stream);
 
 int pbd_get_lambdas(pbd_engine *e, int type, float *dst, unsigned *ids); /* debug: per-type XPBD multipliers + insertion ids */
 int pbd_get_stats(pbd_engine *e, pbd_stats *out);

@@ -29,7 +29,8 @@ SYMBOLS = ["pbd_last_error", "pbd_device_count", "pbd_create", "pbd_destroy", "p
            "pbd_set_replica_rest_positions", "pbd_get_replica_geometry",
            "pbd_set_colliders", "pbd_set_contact_params", "pbd_record_contacts", "pbd_get_contacts", "pbd_set_replica_colliders",
            "pbd_set_attr_device", "pbd_get_attr_device", "pbd_set_masses_device",
-           "pbd_set_replica_constraint_materials", "pbd_set_replica_constraint_materials_device", "pbd_get_replica_materials"]
+           "pbd_set_replica_constraint_materials", "pbd_set_replica_constraint_materials_device", "pbd_get_replica_materials",
+           "pbd_set_replica_rigid_bodies", "pbd_set_rigid_bodies_device", "pbd_get_rigid_bodies_device"]
 
 
 SHAPE_BOX, SHAPE_SPHERE, SHAPE_TORUS, SHAPE_CYLINDER, SHAPE_HOLLOW_SPHERE, SHAPE_HOLLOW_BOX = range(6)
@@ -53,7 +54,7 @@ class Stats(C.Structure):
     _fields_ = [("projections", C.c_ulonglong), ("kernel_launches", C.c_ulonglong), ("steps", C.c_ulonglong),
                 ("num_particles", C.c_uint), ("num_constraints", C.c_uint), ("num_groups", C.c_uint),
                 ("num_buckets", C.c_uint), ("constraints_per_type", C.c_uint * NUM_TYPES),
-                ("bytes_per_step", C.c_double), ("last_step_ms", C.c_float)]
+                ("bytes_per_step", C.c_double), ("last_step_ms", C.c_float), ("images_planned", C.c_ulonglong), ("graph_captures", C.c_ulonglong)]
 
 
 class PbdError(RuntimeError):
@@ -117,6 +118,9 @@ def lib():
         _lib.pbd_set_replica_constraint_materials.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         _lib.pbd_set_replica_constraint_materials_device.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
         _lib.pbd_get_replica_materials.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+        _lib.pbd_set_replica_rigid_bodies.argtypes = [C.c_void_p, C.c_uint] + [C.c_void_p] * 6
+        _lib.pbd_set_rigid_bodies_device.argtypes = [C.c_void_p] * 9
+        _lib.pbd_get_rigid_bodies_device.argtypes = [C.c_void_p] * 6
     return _lib
 
 
@@ -212,7 +216,8 @@ class Engine:
     A replica batch (set_replicas(K), K > 1) steps K independent copies of the model's state at once: the particle state calls then
     take and return (K, n, 3) / (K, n) arrays and lambdas() (K, count); at K = 1 the shapes are those of one scene.  The replicas share
     the model's parameters, gravity and rest geometry unless set_replica_materials / set_replica_gravity / set_replica_rest_positions
-    give each its own; set_replica_colliders gives each replica its own static colliders."""
+    give each its own; set_replica_colliders gives each replica its own static colliders, set_replica_rigid_bodies its own rigid bodies
+    (get_rigid_bodies then returns (K, n, 13))."""
 
     def __init__(self, device=0, stream=None):
         self._h = C.c_void_p()
@@ -377,13 +382,54 @@ class Engine:
         omega = _f32(omega).reshape(-1, 3) if omega is not None else None
         _ck(lib().pbd_set_rigid_bodies(self._h, self.n_rb, _ptr(mass), _ptr(x), _ptr(q), _ptr(inertia), _ptr(v), _ptr(omega)))
 
+    def set_replica_rigid_bodies(self, mass, x, q, inertia, v=None, omega=None):
+        """pbd_set_replica_rigid_bodies: n bodies per replica, replica r's from row r of mass (K, n), x (K, n, 3), q (K, n, 4) as (w, x, y, z),
+        inertia (K, n, 3) principal moments, v / omega (K, n, 3) or None (= 0).  Joints index a replica's bodies 0 .. n-1.  K > 1 only."""
+        mass = _f32(mass)
+        if mass.ndim != 2 or mass.shape[0] != self.K:
+            raise ValueError("set_replica_rigid_bodies: mass wants a (%d, n) array, got %s" % (self.K, mass.shape))
+        n = mass.shape[1]
+        arrays = []
+        for name, a, width in (("x", x, 3), ("q", q, 4), ("inertia", inertia, 3), ("v", v, 3), ("omega", omega, 3)):
+            if a is not None:
+                a = _f32(a)
+                if a.shape != (self.K, n, width):
+                    raise ValueError("set_replica_rigid_bodies: %s wants a (%d, %d, %d) array, got %s" % (name, self.K, n, width, a.shape))
+            arrays.append(a)
+        _ck(lib().pbd_set_replica_rigid_bodies(self._h, n, _ptr(mass), *[_ptr(a) for a in arrays]))
+        self.n_rb = n
+
     def get_rigid_bodies(self):
-        """[n, 13]: x(3) q(w,x,y,z) v(3) omega(3)."""
+        """[n, 13], or (K, n, 13) for a batch: x(3) q(w,x,y,z) v(3) omega(3)."""
         n = getattr(self, "n_rb", 0)
-        x = np.zeros((max(n, 1), 3), np.float32); q = np.zeros((max(n, 1), 4), np.float32)
-        v = np.zeros((max(n, 1), 3), np.float32); w = np.zeros((max(n, 1), 3), np.float32)
+        rows = self.K * n
+        x = np.zeros((max(rows, 1), 3), np.float32); q = np.zeros((max(rows, 1), 4), np.float32)
+        v = np.zeros((max(rows, 1), 3), np.float32); w = np.zeros((max(rows, 1), 3), np.float32)
         _ck(lib().pbd_get_rigid_bodies(self._h, _ptr(x), _ptr(q), _ptr(v), _ptr(w)))
-        return np.concatenate([x, q, v, w], axis=1)[:n]
+        out = np.concatenate([x, q, v, w], axis=1)[:rows]
+        return out.reshape(self.K, n, 13) if self.K > 1 else out
+
+    # rigid-body state in device memory: the layouts of the host calls (K*n rows, replica after replica; q as (w, x, y, z)), as objects
+    # with __cuda_array_interface__; stream and replicas as in set_attr_device.
+    def set_rigid_bodies_device(self, x, q, v=None, omega=None, mass=None, inertia=None, replicas=None, stream=None):
+        """pbd_set_rigid_bodies_device: the bodies of the replicas in `replicas` from x (K*n*3 floats) and q (K*n*4); v / omega None = 0;
+        mass (K*n) / inertia (K*n*3) None = each body keeps its own.  Old and last state become the new current state."""
+        rows = self.K * getattr(self, "n_rb", 0)
+        ptrs = [C.c_void_p(_device_ptr("set_rigid_bodies_device: " + name, a, ("<f4",), rows * width)) if a is not None else None
+                for name, a, width in (("mass", mass, 1), ("x", x, 3), ("q", q, 4), ("inertia", inertia, 3), ("v", v, 3), ("omega", omega, 3))]
+        if ptrs[1] is None or ptrs[2] is None:
+            raise TypeError("set_rigid_bodies_device: x and q are required")
+        mask = self._mask("set_rigid_bodies_device", replicas)
+        _ck(lib().pbd_set_rigid_bodies_device(self._h, *ptrs, mask, _stream(stream)))
+
+    def get_rigid_bodies_device(self, x=None, q=None, v=None, omega=None, stream=None):
+        """pbd_get_rigid_bodies_device: every replica's bodies into x (K*n*3 floats), q (K*n*4, (w, x, y, z)), v, omega (K*n*3); any may be
+        None.  Returns (x, q, v, omega)."""
+        rows = self.K * getattr(self, "n_rb", 0)
+        ptrs = [C.c_void_p(_device_ptr("get_rigid_bodies_device: " + name, a, ("<f4",), rows * width, writable=True)) if a is not None else None
+                for name, a, width in (("x", x, 3), ("q", q, 4), ("v", v, 3), ("omega", omega, 3))]
+        _ck(lib().pbd_get_rigid_bodies_device(self._h, *ptrs, _stream(stream)))
+        return x, q, v, omega
 
     # constraints -----------------------------------------------------------------------------------
     def clear_constraints(self):

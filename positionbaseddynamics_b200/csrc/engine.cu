@@ -12,6 +12,7 @@
 #include <cstdio>
 #include <cstring>
 #include <cstdlib>
+#include <array>
 #include <string>
 #include <vector>
 #include "kernels.cuh"
@@ -110,8 +111,12 @@ struct pbd_engine {
         DevBuf mat, gravity, restX;
         bool gravitySet = false, restShapes = false, restTables = false;
     } batch;
-    // rigid bodies coupled through joints (SURVEY.md 8f-1): float4 arrays X(xyz,invMass) Q(x,y,z,w) V(xyz,mass) W(omega) + history + inertia
+    // rigid bodies coupled through joints (SURVEY.md 8f-1): float4 arrays X(xyz,invMass) Q(x,y,z,w) V(xyz,mass) W(omega) + history + inertia.
+    // nRb bodies per replica, K x nRb rows, replica r's at [r nRb, (r + 1) nRb).  rbReplica: the bodies came from
+    // pbd_set_replica_rigid_bodies (every replica has its own; a batch admits them), not from pbd_set_rigid_bodies (one scene's).
     unsigned nRb = 0;
+    bool rbReplica = false;
+    bool rbMassStale = false;  // rbMass (contact path, below) predates a device write of the masses: read back before it is used
     DevBuf rbX, rbQ, rbV, rbW, rbOldX, rbLastX, rbOldQ, rbLastQ, rbI, rbIinv;
     // constraints (host copy, insertion order) and groups
     TypeStore host[PBD_NUM_TYPES];
@@ -337,12 +342,15 @@ extern "C" int pbd_set_masses(pbd_engine *e, const float *mass) {
     return set_w(e, mass, e->batch.K);
 }
 
-// replica 0 of every particle array copied to replicas 1 .. K-1 (doubling copies)
+// the first `one` bytes of `p` copied to the K - 1 places after them (doubling copies)
+static int broadcast_rows(pbd_engine *e, void *p, size_t one, unsigned K) {
+    for (size_t have = 1; have < K; have *= 2)
+        CK(cudaMemcpyAsync((char *)p + have * one, p, std::min(have, (size_t)K - have) * one, cudaMemcpyDeviceToDevice, e->stream));
+    return 0;
+}
+// replica 0 of every particle array copied to replicas 1 .. K-1
 static int broadcast_replica0(pbd_engine *e, unsigned K) {
-    const size_t one = (size_t)e->n * sizeof(float4);
-    for (DevBuf &b : e->attr)
-        for (size_t have = 1; have < K; have *= 2)
-            CK(cudaMemcpyAsync((char *)b.p + have * one, b.p, std::min(have, (size_t)K - have) * one, cudaMemcpyDeviceToDevice, e->stream));
+    for (DevBuf &b : e->attr) CKE(broadcast_rows(e, b.p, (size_t)e->n * sizeof(float4), K));
     return 0;
 }
 // The particle arrays sized for K replicas of n, and stage[0] for their host copies.  keepReplica0: replica 0 moves into fresh arrays
@@ -362,9 +370,31 @@ static int size_particles(pbd_engine *e, unsigned K, bool keepReplica0) {
     return keep ? broadcast_replica0(e, K) : 0;
 }
 
+// the rigid-body arrays, in the order of rb_state's members
+static std::array<DevBuf *, 10> rb_bufs(pbd_engine *e) {
+    return {&e->rbX, &e->rbQ, &e->rbV, &e->rbW, &e->rbOldX, &e->rbLastX, &e->rbOldQ, &e->rbLastQ, &e->rbI, &e->rbIinv};
+}
+// A batch's per-replica bodies resized for K replicas: replica 0 moves into fresh arrays, replicas 1 .. K-1 become copies of it.
+static int size_bodies(pbd_engine *e, unsigned K) {
+    const size_t one = (size_t)e->nRb * sizeof(float4);
+    if (!e->rbReplica || !one) return 0;
+    for (DevBuf *b : rb_bufs(e)) {
+        DevBuf grown;
+        CKE(grown.alloc(one * K));
+        CK(cudaMemcpyAsync(grown.p, b->p, one, cudaMemcpyDeviceToDevice, e->stream));
+        CKE(broadcast_rows(e, grown.p, one, K));
+        CK(cudaStreamSynchronize(e->stream));  // before `grown` frees the old array
+        std::swap(b->p, grown.p); std::swap(b->bytes, grown.bytes);
+    }
+    std::vector<float> mass((size_t)K * e->nRb);
+    for (size_t i = 0; i < mass.size(); i++) mass[i] = e->rbMass[i % e->nRb];
+    e->rbMass.swap(mass);
+    return 0;
+}
+
 extern "C" int pbd_set_particles(pbd_engine *e, unsigned n, const float *x, const float *x0, const float *v, const float *mass) {
     if (!e || (n && (!x || !mass))) return fail("pbd_set_particles: null argument");
-    const std::string why = pbd_b200::batch_refusal(e->batch.K, n, e->mode, e->nRb, e->host);
+    const std::string why = pbd_b200::batch_refusal(e->batch.K, n, e->mode, e->nRb, e->host, e->rbReplica);
     if (!why.empty()) return fail("pbd_set_particles: %s", why.c_str());
     CKE(use(e));
     CK(cudaStreamSynchronize(e->stream));
@@ -403,12 +433,13 @@ static void drop_replica_colliders(pbd_engine *e) {
 
 extern "C" int pbd_set_replicas(pbd_engine *e, unsigned K) {
     if (!e) return fail("null engine");
-    const std::string why = pbd_b200::batch_refusal(K, e->n, e->mode, e->nRb, e->host);
+    const std::string why = pbd_b200::batch_refusal(K, e->n, e->mode, e->nRb, e->host, e->rbReplica);
     if (!why.empty()) return fail("pbd_set_replicas: %s", why.c_str());
     CKE(collider_refusal(e, K, e->pColliders.size() + e->rColliders.size()));
     CKE(use(e));
     CK(cudaStreamSynchronize(e->stream));
     CKE(size_particles(e, K, true));  // replica 0 kept, the others copies of it
+    CKE(size_bodies(e, K));           // likewise
     e->batch.K = K;
     CKE(drop_constraint_materials(e, ~0u));
     e->batch.mat.release(); e->batch.gravity.release(); e->batch.matMask = 0; e->batch.gravitySet = false;  // rows of the old K
@@ -468,14 +499,14 @@ extern "C" int pbd_set_replica_gravity(pbd_engine *e, const float *g) {
 // batches of DESIGN.md section 6 7-17 % in graph mode); and its arrays -- without the per-constraint material arrays in that case.
 // With per-replica rest shapes the geometry arrays are the K x count ones, replica r's at r x replica_geo (0: the shared image's).
 static const float *replica_mat(const pbd_engine *e, int t) { return ((e->batch.matMask >> t) & 1u) ? (const float *)e->batch.mat.p + mat_offset(t) : nullptr; }
-static unsigned replica_geo(const pbd_engine *e, int t) { return e->batch.restShapes ? e->dev[t].count : 0u; }
+static unsigned replica_geo(const pbd_engine *e, int t) { return e->batch.restShapes && t < PBD_BALLJOINT ? e->dev[t].count : 0u; }  // (joints: no rest shape)
 // with per-constraint materials of every replica the material arrays are the K x count ones, replica r's at r x replica_cmat (0: shared)
 static unsigned replica_cmat(const pbd_engine *e, int t) { return ((e->batch.cmatMask >> t) & 1u) ? e->dev[t].count : 0u; }
 static TypeArrays batch_arrays(const pbd_engine *e, int t) {
     TypeArrays a = e->dev[t].arrays;
     if ((e->batch.matMask >> t) & 1u) for (int k = 0; k < kMaxMat; k++) a.mat[k] = nullptr;
     if ((e->batch.cmatMask >> t) & 1u) for (int k = 0; k < type_shape(t).nMat; k++) a.mat[k] = (const float *)e->dev[t].repMat[k].p;
-    if (e->batch.restShapes) {
+    if (replica_geo(e, t)) {
         for (int k = 0; k < kMaxGeoV; k++) if (a.gv[k]) a.gv[k] = (const float4 *)e->dev[t].repGv[k].p;
         for (int k = 0; k < kMaxGeoS; k++) if (a.gs[k]) a.gs[k] = (const float *)e->dev[t].repGs[k].p;
     }
@@ -524,8 +555,10 @@ static int device_memory_refusal(const pbd_engine *e, const char *what, const ch
 // so far on the caller's stream and before the work enqueued on it later.  The second wait is what lets a caching allocator hand `data`
 // out again on the caller's stream while the copy is still pending.  No staging and no host synchronisation.
 // `prepare` runs after the checks and before the wait for the caller's stream (work that may synchronise the host goes there).
+// `rows`: what the call moves; none is a no-op.
 template <class P, class F>
-static int device_call(pbd_engine *e, const char *what, const char *arg, const void *data, const unsigned char *mask, void *stream, P &&prepare, F &&copy) {
+static int device_call(pbd_engine *e, const char *what, const char *arg, const void *data, const unsigned char *mask, void *stream, size_t rows,
+                       P &&prepare, F &&copy) {
     if (!data) return fail("%s: %s == NULL", what, arg);
     CKE(use(e));
     const cudaStream_t s = stream ? (cudaStream_t)stream : e->stream;
@@ -535,7 +568,7 @@ static int device_call(pbd_engine *e, const char *what, const char *arg, const v
         return fail("%s: the stream is being captured into a graph; the copy would run at every replay, outside the engine's order (call it outside the capture)", what);
     CKE(device_memory_refusal(e, what, arg, data));
     if (mask) CKE(device_memory_refusal(e, what, "replicas", mask));
-    if (e->n == 0) return 0;
+    if (!rows) return 0;
     CKE(prepare());
     const bool other = s != e->stream;
     if (other) { CK(cudaEventRecord(e->evCaller, s)); CK(cudaStreamWaitEvent(e->stream, e->evCaller, 0)); }
@@ -545,7 +578,7 @@ static int device_call(pbd_engine *e, const char *what, const char *arg, const v
 }
 template <class F>
 static int device_call(pbd_engine *e, const char *what, const char *arg, const void *data, const unsigned char *mask, void *stream, F &&copy) {
-    return device_call(e, what, arg, data, mask, stream, [] { return 0; }, copy);
+    return device_call(e, what, arg, data, mask, stream, e->n, [] { return 0; }, copy);
 }
 
 extern "C" int pbd_set_attr_device(pbd_engine *e, int attr, const float *src, const unsigned char *replicas, void *stream) {
@@ -566,6 +599,34 @@ extern "C" int pbd_set_masses_device(pbd_engine *e, const float *mass, const uns
 // ------------------------------------------------------------------------------------------------------------
 // rigid bodies (host arrays are tiny: plain synchronous copies)
 // ------------------------------------------------------------------------------------------------------------
+// `rows` bodies in the layouts of pbd_set_rigid_bodies -> the device arrays' float4 rows (v / omega may be null: 0)
+struct BodyUpload { std::vector<float4> X, Q, V, W, I, Ii; };
+static void convert_bodies(size_t rows, const float *mass, const float *x, const float *q, const float *inertia, const float *v, const float *omega, BodyUpload &u) {
+    u.X.resize(rows); u.Q.resize(rows); u.V.resize(rows); u.W.resize(rows); u.I.resize(rows); u.Ii.resize(rows);
+    for (size_t i = 0; i < rows; i++) {
+        const float m = mass[i];
+        u.X[i] = make_float4(x[3 * i], x[3 * i + 1], x[3 * i + 2], (m != 0.0f) ? 1.0f / m : 0.0f);
+        u.Q[i] = make_float4(q[4 * i + 1], q[4 * i + 2], q[4 * i + 3], q[4 * i]);  // (w,x,y,z) -> (x,y,z,w)
+        u.V[i] = v ? make_float4(v[3 * i], v[3 * i + 1], v[3 * i + 2], m) : make_float4(0.f, 0.f, 0.f, m);
+        u.W[i] = omega ? make_float4(omega[3 * i], omega[3 * i + 1], omega[3 * i + 2], 0.f) : make_float4(0.f, 0.f, 0.f, 0.f);
+        u.I[i] = make_float4(inertia[3 * i], inertia[3 * i + 1], inertia[3 * i + 2], 0.f);
+        u.Ii[i] = make_float4(1.0f / inertia[3 * i], 1.0f / inertia[3 * i + 1], 1.0f / inertia[3 * i + 2], 0.f);  // RigidBody::setInertiaTensor (RigidBody.h:416-420)
+    }
+}
+// the converted rows into the body arrays (sized first when `size`), old and last state = the current state (RigidBody::initBody)
+static int upload_bodies(pbd_engine *e, const BodyUpload &u, bool size) {
+    const size_t b = u.X.size() * sizeof(float4);
+    const std::vector<float4> *src[10] = {&u.X, &u.Q, &u.V, &u.W, &u.X, &u.X, &u.Q, &u.Q, &u.I, &u.Ii};
+    const std::array<DevBuf *, 10> dst = rb_bufs(e);
+    for (int k = 0; k < 10; k++) {
+        if (size) CKE(dst[k]->alloc(b));
+        // Stream-ordered: the next step enqueued reads the new rows.  The sources are pageable, so the driver has staged them when the
+        // call returns and the vectors may go.
+        CK(cudaMemcpyAsync(dst[k]->p, src[k]->data(), b, cudaMemcpyHostToDevice, e->stream));
+    }
+    return 0;
+}
+
 extern "C" int pbd_set_rigid_bodies(pbd_engine *e, unsigned n, const float *mass, const float *x, const float *q, const float *inertia,
                                     const float *v, const float *omega) {
     if (!e || (n && (!mass || !x || !q || !inertia))) return fail("pbd_set_rigid_bodies: null argument");
@@ -574,39 +635,89 @@ extern "C" int pbd_set_rigid_bodies(pbd_engine *e, unsigned n, const float *mass
     CKE(use(e));
     CK(cudaStreamSynchronize(e->stream));
     if (n != e->nRb) e->groupsSet = false;  // the colouring covers the bodies
-    e->nRb = n;
-    e->rbMass.assign(mass, mass + n);
+    e->nRb = n; e->rbReplica = false;
+    e->rbMass.assign(mass, mass + n); e->rbMassStale = false;
     if (n == 0) return 0;
-    std::vector<float4> X(n), Q(n), V(n), W(n), I(n), Ii(n);
-    for (unsigned i = 0; i < n; i++) {
-        const float m = mass[i];
-        X[i] = make_float4(x[3 * i], x[3 * i + 1], x[3 * i + 2], (m != 0.0f) ? 1.0f / m : 0.0f);
-        Q[i] = make_float4(q[4 * i + 1], q[4 * i + 2], q[4 * i + 3], q[4 * i]);  // (w,x,y,z) -> (x,y,z,w)
-        V[i] = v ? make_float4(v[3 * i], v[3 * i + 1], v[3 * i + 2], m) : make_float4(0.f, 0.f, 0.f, m);
-        W[i] = omega ? make_float4(omega[3 * i], omega[3 * i + 1], omega[3 * i + 2], 0.f) : make_float4(0.f, 0.f, 0.f, 0.f);
-        I[i] = make_float4(inertia[3 * i], inertia[3 * i + 1], inertia[3 * i + 2], 0.f);
-        Ii[i] = make_float4(1.0f / inertia[3 * i], 1.0f / inertia[3 * i + 1], 1.0f / inertia[3 * i + 2], 0.f);  // RigidBody::setInertiaTensor (RigidBody.h:416-420)
-    }
-    const size_t b = (size_t)n * sizeof(float4);
-    struct { DevBuf *d; const std::vector<float4> *h; } up[] = {{&e->rbX, &X}, {&e->rbQ, &Q}, {&e->rbV, &V}, {&e->rbW, &W}, {&e->rbOldX, &X}, {&e->rbLastX, &X},
-                                                              {&e->rbOldQ, &Q}, {&e->rbLastQ, &Q}, {&e->rbI, &I}, {&e->rbIinv, &Ii}};
-    for (auto &u : up) { CKE(u.d->alloc(b)); CK(cudaMemcpy(u.d->p, u.h->data(), b, cudaMemcpyHostToDevice)); }
+    BodyUpload u;
+    convert_bodies(n, mass, x, q, inertia, v, omega, u);
+    CKE(upload_bodies(e, u, true));
+    CK(cudaStreamSynchronize(e->stream));
     return 0;
+}
+
+extern "C" int pbd_set_replica_rigid_bodies(pbd_engine *e, unsigned n, const float *mass, const float *x, const float *q, const float *inertia,
+                                            const float *v, const float *omega) {
+    const char *what = "pbd_set_replica_rigid_bodies";
+    if (!e) return fail("%s: null engine", what);
+    if (e->batch.K == 1) return fail("%s: a single-scene engine takes its bodies from pbd_set_rigid_bodies (pbd_set_replicas first)", what);
+    if (n && (!mass || !x || !q || !inertia)) return fail("%s: null argument", what);
+    const size_t rows = (size_t)e->batch.K * n;
+    if (rows >= (1ull << 31)) return fail("%s: %u replicas of %u bodies exceed 2^31 bodies", what, e->batch.K, n);
+    const std::string why = pbd_b200::batch_refusal(e->batch.K, e->n, e->mode, n, e->host, true);
+    if (!why.empty()) return fail("%s: %s", what, why.c_str());
+    CKE(use(e));
+    BodyUpload u;
+    convert_bodies(rows, mass, x, q, inertia, v, omega, u);
+    // the same n: copies in stream order into arrays that keep their address (no re-plan, no new graph capture); else what
+    // pbd_set_rigid_bodies does
+    const bool keep = e->rbReplica && n == e->nRb;
+    if (!keep) {
+        CK(cudaStreamSynchronize(e->stream));
+        if (n != e->nRb) e->groupsSet = false;
+        e->nRb = n; e->rbReplica = true;
+    }
+    e->rbMass.assign(mass, mass + rows); e->rbMassStale = false;
+    return rows ? upload_bodies(e, u, !keep) : 0;
 }
 
 extern "C" int pbd_get_rigid_bodies(pbd_engine *e, float *x, float *q, float *v, float *omega) {
     if (!e) return fail("null engine");
     CKE(use(e));
     CK(cudaStreamSynchronize(e->stream));
-    const unsigned n = e->nRb;
+    const size_t n = (size_t)e->batch.K * e->nRb;  // every replica's
     if (n == 0) return 0;
     std::vector<float4> t(n);
-    const size_t b = (size_t)n * sizeof(float4);
-    if (x) { CK(cudaMemcpy(t.data(), e->rbX.p, b, cudaMemcpyDeviceToHost)); for (unsigned i = 0; i < n; i++) { x[3 * i] = t[i].x; x[3 * i + 1] = t[i].y; x[3 * i + 2] = t[i].z; } }
-    if (q) { CK(cudaMemcpy(t.data(), e->rbQ.p, b, cudaMemcpyDeviceToHost)); for (unsigned i = 0; i < n; i++) { q[4 * i] = t[i].w; q[4 * i + 1] = t[i].x; q[4 * i + 2] = t[i].y; q[4 * i + 3] = t[i].z; } }
-    if (v) { CK(cudaMemcpy(t.data(), e->rbV.p, b, cudaMemcpyDeviceToHost)); for (unsigned i = 0; i < n; i++) { v[3 * i] = t[i].x; v[3 * i + 1] = t[i].y; v[3 * i + 2] = t[i].z; } }
-    if (omega) { CK(cudaMemcpy(t.data(), e->rbW.p, b, cudaMemcpyDeviceToHost)); for (unsigned i = 0; i < n; i++) { omega[3 * i] = t[i].x; omega[3 * i + 1] = t[i].y; omega[3 * i + 2] = t[i].z; } }
+    const size_t b = n * sizeof(float4);
+    if (x) { CK(cudaMemcpy(t.data(), e->rbX.p, b, cudaMemcpyDeviceToHost)); for (size_t i = 0; i < n; i++) { x[3 * i] = t[i].x; x[3 * i + 1] = t[i].y; x[3 * i + 2] = t[i].z; } }
+    if (q) { CK(cudaMemcpy(t.data(), e->rbQ.p, b, cudaMemcpyDeviceToHost)); for (size_t i = 0; i < n; i++) { q[4 * i] = t[i].w; q[4 * i + 1] = t[i].x; q[4 * i + 2] = t[i].y; q[4 * i + 3] = t[i].z; } }
+    if (v) { CK(cudaMemcpy(t.data(), e->rbV.p, b, cudaMemcpyDeviceToHost)); for (size_t i = 0; i < n; i++) { v[3 * i] = t[i].x; v[3 * i + 1] = t[i].y; v[3 * i + 2] = t[i].z; } }
+    if (omega) { CK(cudaMemcpy(t.data(), e->rbW.p, b, cudaMemcpyDeviceToHost)); for (size_t i = 0; i < n; i++) { omega[3 * i] = t[i].x; omega[3 * i + 1] = t[i].y; omega[3 * i + 2] = t[i].z; } }
     return 0;
+}
+
+// ---- rigid-body state in device memory (pbd_set_rigid_bodies_device, pbd_get_rigid_bodies_device): device_call's stream contract -------
+static RbState rb_state(const pbd_engine *e);
+// the optional arrays of a device body call: device memory of the engine's device, checked before anything is enqueued
+static int body_arrays_refusal(const pbd_engine *e, const char *what, std::initializer_list<std::pair<const char *, const void *>> arrays) {
+    for (const auto &a : arrays) if (a.second) CKE(device_memory_refusal(e, what, a.first, a.second));
+    return 0;
+}
+extern "C" int pbd_set_rigid_bodies_device(pbd_engine *e, const float *mass, const float *x, const float *q, const float *inertia, const float *v,
+                                           const float *omega, const unsigned char *replicas, void *stream) {
+    const char *what = "pbd_set_rigid_bodies_device";
+    if (!e) return fail("%s: null engine", what);
+    if (!e->nRb) return fail("%s: the engine holds no rigid bodies (pbd_set_rigid_bodies / pbd_set_replica_rigid_bodies first)", what);
+    if (!q) return fail("%s: q == NULL", what);
+    CKE(body_arrays_refusal(e, what, {{"q", q}, {"mass", mass}, {"inertia", inertia}, {"v", v}, {"omega", omega}}));
+    return device_call(e, what, "x", x, replicas, stream, (size_t)e->batch.K * e->nRb, [] { return 0; }, [&]() -> int {
+        k_set_bodies<<<dim3(nblk(e->nRb, 128), e->batch.K), 128, 0, e->stream>>>(rb_state(e), BodyRows{(float *)x, (float *)q, (float *)v, (float *)omega, mass, inertia, replicas});
+        CK(cudaGetLastError());
+        if (mass) e->rbMassStale = true;
+        return 0;
+    });
+}
+extern "C" int pbd_get_rigid_bodies_device(pbd_engine *e, float *x, float *q, float *v, float *omega, void *stream) {
+    const char *what = "pbd_get_rigid_bodies_device";
+    if (!e) return fail("%s: null engine", what);
+    const float *first = x ? x : q ? q : v ? v : omega;
+    if (!first) return 0;  // nothing asked for
+    CKE(body_arrays_refusal(e, what, {{"x", x}, {"q", q}, {"v", v}, {"omega", omega}}));
+    const unsigned rows = e->batch.K * e->nRb;
+    return device_call(e, what, x ? "x" : q ? "q" : v ? "v" : "omega", first, nullptr, stream, rows, [] { return 0; }, [&]() -> int {
+        k_get_bodies<<<nblk(rows, 128), 128, 0, e->stream>>>(rb_state(e), rows, BodyRows{x, q, v, omega, nullptr, nullptr, nullptr});
+        CK(cudaGetLastError());
+        return 0;
+    });
 }
 
 template <class V> static int upload_vec(DevBuf &buf, const V &v, cudaStream_t s) {  // V: std::vector / PodVector of PODs
@@ -904,7 +1015,7 @@ extern "C" int pbd_set_params(pbd_engine *e, float dt, unsigned subSteps, unsign
 extern "C" int pbd_set_mode(pbd_engine *e, int mode) {
     if (!e) return fail("null engine");
     if (mode != PBD_MODE_GRAPH && mode != PBD_MODE_RESIDENT && mode != PBD_MODE_LAUNCH && mode != PBD_MODE_JACOBI && mode != PBD_MODE_AUTO) return fail("unknown solver mode %d", mode);
-    const std::string why = pbd_b200::batch_refusal(e->batch.K, e->n, mode, e->nRb, e->host);
+    const std::string why = pbd_b200::batch_refusal(e->batch.K, e->n, mode, e->nRb, e->host, e->rbReplica);
     if (!why.empty()) return fail("pbd_set_mode: %s", why.c_str());
     e->mode = mode;
     return 0;
@@ -1088,7 +1199,7 @@ template <class... V> static void append_bytes(std::vector<unsigned char> &key, 
 static std::vector<unsigned char> image_key(const pbd_engine *e) {
     std::vector<unsigned char> key;
     const bool tiled = pbd_b200::preferred_mode(e->mode, e->host, e->n, e->numConstraints, e->batch.K) == PBD_MODE_RESIDENT;
-    append_bytes(key, e->modelGen, e->n, e->nRb, e->rbX.p, e->rbQ.p, e->rbIinv.p, e->batch.K, tiled ? e->mode : -1, rest_tables(e));
+    append_bytes(key, e->modelGen, e->n, e->nRb, e->rbReplica, e->rbX.p, e->rbQ.p, e->rbIinv.p, e->batch.K, tiled ? e->mode : -1, rest_tables(e));
     return key;
 }
 
@@ -1104,6 +1215,7 @@ static int flatten(pbd_engine *e) {
     // arrays and the slot map that relayout replaces, and upload_slot_map's copy is not ordered against the engine stream.
     CK(cudaStreamSynchronize(e->stream));
     e->imageGen++;
+    e->stats.images_planned++;
     std::vector<float4> x0;  // resident: rest positions by host index
     if (pbd_b200::preferred_mode(e->mode, e->host, e->n, e->numConstraints, e->batch.K) == PBD_MODE_RESIDENT && e->n) {
         std::vector<float4> raw(e->n);
@@ -1113,7 +1225,7 @@ static int flatten(pbd_engine *e) {
     }
     lap("colouring + rest positions");
     pbd_b200::PlanInput in{e->host, e->numConstraints, e->n, e->nRb, &e->groupOff, &e->groupIds, e->mode, x0.data(), 0u, 0u, e->smCount, nullptr,
-                           rest_tables(e), e->batch.K};
+                           rest_tables(e), e->batch.K, e->rbReplica};
     if (const char *g = getenv("PBD_B200_CLUSTERS")) {  // development knob "GxC"
         unsigned gg = 0, cc = 0;
         if (sscanf(g, "%ux%u", &gg, &cc) == 2 && gg >= 1 && cc >= 1 && cc <= (unsigned)kMaxClusterCtas && (cc & (cc - 1)) == 0) { in.forcedG = gg; in.forcedC = cc; }
@@ -1250,7 +1362,7 @@ extern "C" int pbd_set_replica_constraint_materials(pbd_engine *e, int type, con
 extern "C" int pbd_set_replica_constraint_materials_device(pbd_engine *e, int type, const float *mat, const unsigned char *replicas, void *stream) {
     const char *what = "pbd_set_replica_constraint_materials_device";
     CKE(constraint_materials_refusal(e, what, type));
-    return device_call(e, what, "mat", mat, replicas, stream, [&] { return constraint_materials_on(e, type, replicas != nullptr); },
+    return device_call(e, what, "mat", mat, replicas, stream, e->n, [&] { return constraint_materials_on(e, type, replicas != nullptr); },
                        [&] { return gather_materials(e, type, mat, true, replicas); });
 }
 extern "C" int pbd_get_replica_materials(pbd_engine *e, int type, float *dst) {
@@ -1332,7 +1444,7 @@ template <class F> static int with_project_type(int type, int variant, F &&f) {
 static int launch_bucket(pbd_engine *e, const Bucket &b, float h, int iterZero, cudaStream_t s, bool pdl) {
     const TypeArrays a = batch_arrays(e, b.type);
     const unsigned block = project_block(e, b.count * e->batch.K);
-    const ReplicaStrides rs{e->n, {e->dev[b.type].count}, {replica_mat(e, b.type)}, {replica_geo(e, b.type)}, {replica_cmat(e, b.type)}};
+    const ReplicaStrides rs{e->n, {e->dev[b.type].count}, {replica_mat(e, b.type)}, {replica_geo(e, b.type)}, {replica_cmat(e, b.type)}, e->nRb};
     return with_project_type(b.type, a.variant, [&](auto T, auto V) -> int {
         constexpr int TT = decltype(T)::value, VAR = decltype(V)::value;
         if (e->batch.K > 1) CK(launch_step_kernel(k_project<TT, VAR, true>, dim3(nblk(b.count, block), e->batch.K), block, s, pdl, attr_ptr(e, PBD_ATTR_X), a, b.first, b.count, h, iterZero, rs));
@@ -1376,7 +1488,7 @@ static int launch_colour(pbd_engine *e, size_t b0, size_t b1, float h, int iterZ
     for (size_t c0 = b0; c0 < b1; c0 += kMultiSegments) {
         const size_t c1 = std::min(b1, c0 + (size_t)kMultiSegments);
         MultiArgs m{};
-        ReplicaStrides rs{e->n, {}, {}, {}, {}};
+        ReplicaStrides rs{e->n, {}, {}, {}, {}, e->nRb};
         m.nSeg = (int)(c1 - c0);
         unsigned blocks = 0, total = 0;
         for (size_t i = c0; i < c1; i++) total += e->buckets[i].count;
@@ -1414,7 +1526,13 @@ static int enqueue_step_launches(pbd_engine *e, cudaStream_t s, unsigned long lo
     unsigned long long L = 0;
     auto launched = [&](int kind) { L++; return log ? log->mark(s, kind) : 0; };
     for (unsigned sub = 0; sub < e->subSteps; sub++) {
-        if (e->nRb) { CK(launch_step_kernel(k_rb_integrate, nblk(e->nRb, 256), 256, s, pdl, rb, h, e->g[0], e->g[1], e->g[2])); CKE(launched(kLaunchIntegrate)); }
+        if (e->nRb) {
+            if (e->batch.K > 1)  // replica blockIdx.y's bodies, under its own gravity row where it has one
+                CK(launch_step_kernel(k_rb_integrate_batch, dim3(nblk(e->nRb, 256), e->batch.K), 256, s, pdl, rb, h, e->g[0], e->g[1], e->g[2],
+                                      e->batch.gravitySet ? (const float *)e->batch.gravity.p : (const float *)nullptr));
+            else CK(launch_step_kernel(k_rb_integrate, nblk(e->nRb, 256), 256, s, pdl, rb, h, e->g[0], e->g[1], e->g[2]));
+            CKE(launched(kLaunchIntegrate));
+        }
         if (n) {
             if (e->batch.gravitySet)  // replica blockIdx.y under its own row
                 CK(launch_step_kernel(k_integrate<true>, replica_grid(e, e->batch.K), 256, s, pdl, x, v, oldX, lastX, e->n, h, 0.0f, 0.0f, 0.0f,
@@ -1435,7 +1553,11 @@ static int enqueue_step_launches(pbd_engine *e, cudaStream_t s, unsigned long lo
             CK(launch_step_kernel(k_velocity, nblk(n, 256), 256, s, pdl, x, v, oldX, lastX, n, invH, e->velMethod));
             CKE(launched(kLaunchVelocity));
         }
-        if (e->nRb) { CK(launch_step_kernel(k_rb_velocity, nblk(e->nRb, 256), 256, s, pdl, rb, invH, (float)(2.0 / (double)h), e->velMethod)); CKE(launched(kLaunchVelocity)); }
+        if (e->nRb) {
+            if (e->batch.K > 1) CK(launch_step_kernel(k_rb_velocity_batch, dim3(nblk(e->nRb, 256), e->batch.K), 256, s, pdl, rb, invH, (float)(2.0 / (double)h), e->velMethod));
+            else CK(launch_step_kernel(k_rb_velocity, nblk(e->nRb, 256), 256, s, pdl, rb, invH, (float)(2.0 / (double)h), e->velMethod));
+            CKE(launched(kLaunchVelocity));
+        }
     }
     *launches = L;
     return 0;
@@ -1490,14 +1612,20 @@ static int enqueue_step_resident(pbd_engine *e, cudaStream_t s, unsigned long lo
         }
     } dump{e, s, batch ? nullptr : tracePath, (size_t)kTracePhases * ra.nTiles * kTraceSlots};
     const pbd_b200::ResidentShape &r = e->res;
-    return with_resident_kernel(r.mask, r.C, batch, [&](auto kernel) -> int {
+    CKE(with_resident_kernel(r.mask, r.C, batch, [&](auto kernel) -> int {
         CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynamicSmem));
         if (r.C > 8) CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
         cudaLaunchConfig_t cfg; cudaLaunchAttribute attr[1];
         resident_launch_config(r.mask, r.C, batch, r.G * r.C, r.smem, s, cfg, attr);
         CK(cudaLaunchKernelEx(&cfg, kernel, ra));
         return 0;
-    });
+    }));
+    if (batch && e->nRb) {  // a batch's body velocities of the last substep (resident.cuh: the others at the head of the next substep)
+        k_rb_velocity_batch<<<dim3(nblk(e->nRb, 256), e->batch.K), 256, 0, s>>>(ra.rb, ra.invH, ra.twoInvH, ra.secondOrder);
+        CK(cudaGetLastError());
+        *launches = 2;
+    }
+    return 0;
 }
 
 // Jacobi comparison path (kernels.cuh): per sweep one launch per type over all its constraints + the averaging pass
@@ -1562,6 +1690,18 @@ static int convert_ranges(const pbd_engine *e, const char *what, unsigned nP, co
     return 0;
 }
 
+// the host copy of the body masses the contact path checks: read back (V.w, in stream order) after a device write of the masses
+static int body_masses(pbd_engine *e) {
+    if (!e->rbMassStale) return 0;
+    const size_t rows = (size_t)e->batch.K * e->nRb;
+    std::vector<float4> V(rows);
+    CK(cudaStreamSynchronize(e->stream));
+    if (rows) CK(cudaMemcpy(V.data(), e->rbV.p, rows * sizeof(float4), cudaMemcpyDeviceToHost));
+    for (size_t i = 0; i < rows; i++) e->rbMass[i] = V[i].w;
+    e->rbMassStale = false;
+    return 0;
+}
+
 extern "C" int pbd_set_colliders(pbd_engine *e, unsigned nP, const pbd_particle_collider *pc, unsigned nR, const pbd_rigid_collider *rc) {
     if (!e || (nP && !pc) || (nR && !rc)) return fail("pbd_set_colliders: null argument");
     CKE(collider_refusal(e, e->batch.K, (size_t)nP + nR));
@@ -1571,6 +1711,7 @@ extern "C" int pbd_set_colliders(pbd_engine *e, unsigned nP, const pbd_particle_
     std::vector<RigidCollider> R(nR);
     std::vector<unsigned> start;
     CKE(convert_ranges(e, "pbd_set_colliders", nP, pc, P, start));
+    CKE(body_masses(e));
     for (unsigned i = 0; i < nR; i++) {
         const pbd_rigid_collider &c = rc[i];
         CKE(convert_collider("pbd_set_colliders", i, c, R[i]));
@@ -1668,6 +1809,7 @@ static int enqueue_contacts(pbd_engine *e, cudaStream_t s, unsigned long long *l
     const pbd_engine::ReplicaColliders &rep = e->repColliders;
     const bool batch = rep.nRigid != 0;
     if (batch ? rep.total == 0 : (e->rColliders.empty() || e->contactTotal == 0)) return 0;
+    if (!batch) CKE(body_masses(e));
     if (!batch)
         for (const RigidCollider &c : e->rColliders)  // the bodies may have been replaced since pbd_set_colliders
             if (c.body >= e->nRb || e->rbMass[c.body] != 0.0f) return fail("contact path: collider on rigid body %u, which is missing or not static any more (pbd_set_colliders again)", c.body);
@@ -1729,6 +1871,7 @@ static int ensure_graph(pbd_engine *e) {
     if (err != cudaSuccess) { e->graphExec = nullptr; return fail("cudaGraphInstantiate -> %s", cudaGetErrorString(err)); }
     e->graphKey.swap(key);
     e->graphLaunches = L;
+    e->stats.graph_captures++;
     return 0;
 }
 

@@ -135,9 +135,12 @@ static inline unsigned exec_tile(int t, const unsigned *b, int nb, const std::ve
 static std::string choose_resident_shape(const PlanInput &in, ResidentShape &r) {
     unsigned present = 0, nTypes = 0;
     for (int t = 0; t < PBD_NUM_TYPES; t++) if (!in.store[t].ids.empty()) { present |= 1u << t; nTypes++; }
+    // the leanest instantiation that covers the model; a batch with rigid bodies one with the joint types, whose batched form steps them
+    constexpr unsigned joints = type_bit(PBD_BALLJOINT) | type_bit(PBD_RB_PARTICLE_BALLJOINT);
+    const bool batchBodies = in.replicas > 1 && (in.nRb || (present & joints));
     r.mask = kMaskAll;
-    for (unsigned m : {kMaskClothXPBD, kMaskCloth, kMaskFem, kMaskLight, kMaskSolid})  // the leanest instantiation that covers the model
-        if ((present & ~m) == 0) { r.mask = m; break; }
+    for (unsigned m : {kMaskClothXPBD, kMaskCloth, kMaskFem, kMaskLight, kMaskSolid})
+        if ((present & ~m) == 0 && (!batchBodies || (m & joints) == joints)) { r.mask = m; break; }
     r.threads = resident_threads(r.mask, in.replicas > 1);
     const unsigned nGroups = (unsigned)std::max<size_t>(in.groupOff->size(), 2) - 1;
     const unsigned perPhase = in.numConstraints / std::max(1u, nGroups);
@@ -710,20 +713,20 @@ static std::string plan_mode(const PlanInput &in, bool tiled, ImagePlan &out) {
     return (unsigned)mc < r.G ? fmt("resident mode: the device runs %d clusters of %u CTAs at a time, the scene needs %u co-resident", mc, r.C, r.G) : "";
 }
 
-std::string batch_refusal(unsigned replicas, unsigned n, int mode, unsigned nRb, const TypeStore *store) {
+std::string batch_refusal(unsigned replicas, unsigned n, int mode, unsigned nRb, const TypeStore *store, bool replicaBodies) {
     if (replicas == 0) return "replica batch: at least one replica";
     if ((unsigned long long)replicas * n >= (1ull << 31))
         return fmt("replica batch: %u replicas of %u particles exceed 2^31 particles", replicas, n);
     if (replicas == 1) return "";
     if (replicas > 65535u) return fmt("replica batch: %u replicas, at most 65535 (the projection kernels run one replica per grid row)", replicas);
-    if (nRb || !store[PBD_BALLJOINT].ids.empty() || !store[PBD_RB_PARTICLE_BALLJOINT].ids.empty())
-        return "replica batch: rigid bodies and joints are stepped one scene per engine (pbd_set_replicas 1)";
+    if (!replicaBodies && (nRb || !store[PBD_BALLJOINT].ids.empty() || !store[PBD_RB_PARTICLE_BALLJOINT].ids.empty()))
+        return "replica batch: rigid bodies and joints are stepped one scene per engine (pbd_set_replicas 1); a batch takes per-replica bodies from pbd_set_replica_rigid_bodies";
     if (mode == PBD_MODE_JACOBI) return "replica batch: PBD_MODE_JACOBI steps one scene per engine (pbd_set_replicas 1)";
     return "";
 }
 
 std::string plan_image(const PlanInput &in, ImagePlan &out) {
-    const std::string refusal = batch_refusal(in.replicas, in.n, in.mode, in.nRb, in.store);
+    const std::string refusal = batch_refusal(in.replicas, in.n, in.mode, in.nRb, in.store, in.replicaBodies);
     if (!refusal.empty()) return refusal;
     out.mode = preferred_mode(in.mode, in.store, in.n, in.numConstraints, in.replicas);
     const std::string err = plan_mode(in, out.mode == PBD_MODE_RESIDENT, out);

@@ -53,6 +53,7 @@ struct PlanInput {
     ClusterQuery maxClusters;                      // resident: what the device keeps co-resident
     bool restTables = false;                       // replica batch with per-replica rest shapes: also TypePlan::restBodies / restLocal
     unsigned replicas = 1;                         // replica batch: every replica runs this one image (n, the constraints: one replica)
+    bool replicaBodies = false;                    // replica batch: every replica has nRb rigid bodies of its own (pbd_set_replica_rigid_bodies)
 };
 
 // One constraint type's arrays in device order (the host side of pbdk::TypeArrays).
@@ -85,7 +86,8 @@ struct ImagePlan {
 
 // Why a batch of `replicas` replicas of n particles cannot run `mode` with these rigid bodies and constraints, or "" (also for one replica
 // within the size limits).  plan_image checks it first; the engine also before it changes the batch size, the mode or the rigid bodies.
-std::string batch_refusal(unsigned replicas, unsigned n, int mode, unsigned nRb, const TypeStore *store);
+// Bodies and joints are admitted in a batch only where every replica has bodies of its own (replicaBodies).
+std::string batch_refusal(unsigned replicas, unsigned n, int mode, unsigned nRb, const TypeStore *store, bool replicaBodies = false);
 
 // Plans the image of `in` into `out`; returns "" or why the model cannot be flattened (for this mode and, resident, this device).
 std::string plan_image(const PlanInput &in, ImagePlan &out);

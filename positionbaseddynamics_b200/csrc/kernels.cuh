@@ -100,32 +100,36 @@ struct GlobalAcc {
 };
 
 // Gather -> project -> scatter for constraint i (index into the type's arrays) whose streamed part is already here.
-// Joints couple rigid bodies (their own small state arrays, L2 only) with each other or with a particle.
+// Joints couple rigid bodies (their own small state arrays, L2 only) with each other or with a particle.  rbOff: a batch's replica
+// reads its bodies at index + rbOff (resident.cuh, like geoOff)
 template <int T, class Acc>
-__device__ __forceinline__ void project_joint(const Acc &acc, const TypeArrays &a, const Streamed &s) {
-    float4 X0 = __ldcg(a.rbX + s.b.x), Q0 = __ldcg(a.rbQ + s.b.x);
-    const float4 I0 = __ldg(a.rbIinv + s.b.x);
+__device__ __forceinline__ void project_joint(const Acc &acc, const TypeArrays &a, const Streamed &s, unsigned rbOff = 0u) {
+    const unsigned b0 = s.b.x + rbOff;
+    float4 X0 = __ldcg(a.rbX + b0), Q0 = __ldcg(a.rbQ + b0);
+    const float4 I0 = __ldg(a.rbIinv + b0);
     if (T == PBD_BALLJOINT) {
-        float4 X1 = __ldcg(a.rbX + s.b.y), Q1 = __ldcg(a.rbQ + s.b.y);
-        const float4 I1 = __ldg(a.rbIinv + s.b.y);
+        const unsigned b1 = s.b.y + rbOff;
+        float4 X1 = __ldcg(a.rbX + b1), Q1 = __ldcg(a.rbQ + b1);
+        const float4 I1 = __ldg(a.rbIinv + b1);
         project_balljoint(X0, Q0, mk(I0.x, I0.y, I0.z), X1, Q1, mk(I1.x, I1.y, I1.z), mk(s.g0.x, s.g0.y, s.g0.z), mk(s.g1.x, s.g1.y, s.g1.z));
-        if (X1.w != 0.0f) { __stcg(a.rbX + s.b.y, X1); __stcg(a.rbQ + s.b.y, Q1); }
+        if (X1.w != 0.0f) { __stcg(a.rbX + b1, X1); __stcg(a.rbQ + b1, Q1); }
     } else {
         const typename Acc::Handle hp = acc.handle(s.b.y);
         float4 p = acc.ld(hp);
         project_rb_particle_balljoint(X0, Q0, mk(I0.x, I0.y, I0.z), p, mk(s.g0.x, s.g0.y, s.g0.z));
         acc.st(hp, p);
     }
-    if (X0.w != 0.0f) { __stcg(a.rbX + s.b.x, X0); __stcg(a.rbQ + s.b.x, Q0); }
+    if (X0.w != 0.0f) { __stcg(a.rbX + b0, X0); __stcg(a.rbQ + b0, Q0); }
 }
 
 // VAR: compile-time layout variant of the type (IsometricBending: 0 = rank-1 Kp, 1 = full Q), -1 = read a.variant at run time
-// matOff: a batch's replica with per-constraint materials of its own reads them at i + matOff (resident.cuh, like geoOff)
+// matOff: a batch's replica with per-constraint materials of its own reads them at i + matOff (resident.cuh, like geoOff); rbOff: its
+// rigid bodies (project_joint)
 template <int T, class Acc, int VAR = -1>
 __device__ __forceinline__ void project_streamed_acc(const Acc &acc, const TypeArrays &a, unsigned i, const Streamed &s, float dt,
                                                      bool iterZero, bool lambdaGiven = false, float lambdaValue = 0.0f, const MatRow &matRow = MatRow{},
-                                                     unsigned geoOff = 0u, unsigned matOff = 0u) {
-    if (T == PBD_BALLJOINT || T == PBD_RB_PARTICLE_BALLJOINT) { project_joint<T>(acc, a, s); return; }
+                                                     unsigned geoOff = 0u, unsigned matOff = 0u, unsigned rbOff = 0u) {
+    if (T == PBD_BALLJOINT || T == PBD_RB_PARTICLE_BALLJOINT) { project_joint<T>(acc, a, s, rbOff); return; }
     constexpr bool XPBD = type_shape(T).xpbd;
     constexpr int NB = type_shape(T).nBodies;
     const unsigned mi = i + matOff;
@@ -207,14 +211,21 @@ constexpr int kMultiSegments = 4;
 // material parameters of its own for that type.  nGeo[k]: with per-replica rest shapes (pbd_set_replica_rest_positions) the geometry
 // arrays hold every replica's, replica y's at y x nGeo[k]; 0: one geometry shared by all.  nMat[k]: with per-constraint materials of every
 // replica (pbd_set_replica_constraint_materials) the material arrays hold every replica's, replica y's at y x nMat[k]; 0: shared.
+// nRb: the rigid bodies of a replica (pbd_set_replica_rigid_bodies), replica y's at y x nRb of the joints' body arrays.
 struct ReplicaStrides {
     unsigned nPos; unsigned nLambda[kMultiSegments]; const float *mat[kMultiSegments]; unsigned nGeo[kMultiSegments]; unsigned nMat[kMultiSegments];
+    unsigned nRb;
     __device__ __forceinline__ const float *mat_row(int k, unsigned rep) const { return mat[k] ? mat[k] + (size_t)rep * kMatRowFloats : nullptr; }
 };
-// the type's arrays with the multipliers, the geometry and the per-constraint materials of replica `rep`
-__device__ __forceinline__ TypeArrays replica_arrays(const TypeArrays &a, unsigned rep, unsigned nLambda, unsigned nGeo, unsigned nMat = 0u) {
+// the type's arrays with the multipliers, the geometry, the per-constraint materials and the rigid bodies of replica `rep` (the body arrays
+// are set for the joint types only)
+__device__ __forceinline__ TypeArrays replica_arrays(const TypeArrays &a, unsigned rep, unsigned nLambda, unsigned nGeo, unsigned nMat = 0u, unsigned nRb = 0u) {
     TypeArrays r = a;
     if (r.lambda) r.lambda += (size_t)rep * nLambda;
+    if (nRb && r.rbX) {
+        const size_t o = (size_t)rep * nRb;
+        r.rbX += o; r.rbQ += o; r.rbIinv += o;
+    }
     if (nGeo) {
         const size_t o = (size_t)rep * nGeo;
 #pragma unroll
@@ -236,7 +247,7 @@ __global__ void __launch_bounds__(kProjectThreads) k_project(float4 *pos, TypeAr
     const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= count) return;  // an exited thread counts as having passed the dependency
     MatRow matRow;
-    if (BATCH) { pos += (size_t)blockIdx.y * rs.nPos; a = replica_arrays(a, blockIdx.y, rs.nLambda[0], rs.nGeo[0], rs.nMat[0]); matRow = load_mat_row<T>(rs.mat_row(0, blockIdx.y)); }
+    if (BATCH) { pos += (size_t)blockIdx.y * rs.nPos; a = replica_arrays(a, blockIdx.y, rs.nLambda[0], rs.nGeo[0], rs.nMat[0], rs.nRb); matRow = load_mat_row<T>(rs.mat_row(0, blockIdx.y)); }
     const Streamed s = load_streamed<T>(a, first + i);
     pdl_wait_after(s.b.x ^ s.b.y, s.g0.x + s.g1.x + s.s0 + s.s1);
     project_streamed<T, VAR>(pos, a, first + i, s, dt, iterZero != 0, matRow);
@@ -299,7 +310,7 @@ __global__ void __launch_bounds__(kProjectThreads) k_project_multi(float4 *pos, 
     if (i >= m.count[s]) return;
     const unsigned ci = m.first[s] + i;
     TypeArrays batchArrays;
-    if (BATCH) { pos += (size_t)blockIdx.y * rs.nPos; batchArrays = replica_arrays(m.arrays[s], blockIdx.y, rs.nLambda[s], rs.nGeo[s], rs.nMat[s]); }
+    if (BATCH) { pos += (size_t)blockIdx.y * rs.nPos; batchArrays = replica_arrays(m.arrays[s], blockIdx.y, rs.nLambda[s], rs.nGeo[s], rs.nMat[s], rs.nRb); }
     const TypeArrays &a = BATCH ? batchArrays : m.arrays[s];
     PBD_FOR_TYPE(kMaskAll, m.type[s],
         MatRow matRow;
@@ -405,6 +416,59 @@ __global__ void k_rb_velocity(RbState r, float invH, float twoInvH, int secondOr
     if (i >= r.n) return;
     pdl_wait();
     rb_velocity_body(r, i, invH, twoInvH, secondOrder);
+}
+
+// A replica batch's bodies (pbd_set_replica_rigid_bodies): r.n bodies per replica, replica blockIdx.y's at rows y n .. y n + n - 1; the
+// integration under that replica's row of `replicaG` (pbd_set_replica_gravity; null: gx, gy, gz)
+__global__ void k_rb_integrate_batch(RbState r, float h, float gx, float gy, float gz, const float *__restrict__ replicaG) {
+    pdl_launch_dependents();
+    const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= r.n) return;
+    if (replicaG) { gx = __ldg(replicaG + 3u * blockIdx.y); gy = __ldg(replicaG + 3u * blockIdx.y + 1u); gz = __ldg(replicaG + 3u * blockIdx.y + 2u); }
+    pdl_wait();
+    rb_integrate_body(r, blockIdx.y * r.n + i, h, gx, gy, gz);
+}
+__global__ void k_rb_velocity_batch(RbState r, float invH, float twoInvH, int secondOrder) {
+    pdl_launch_dependents();
+    const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= r.n) return;
+    pdl_wait();
+    rb_velocity_body(r, blockIdx.y * r.n + i, invH, twoInvH, secondOrder);
+}
+
+// Rigid-body state <-> the host calls' layouts in device memory (pbd_set_rigid_bodies_device / pbd_get_rigid_bodies_device): rows of
+// x(3), q(4, as w x y z), v(3), omega(3), mass(1), inertia(3), replica after replica (r.n bodies per replica; a single scene is replica 0).
+// The set writes what pbd_set_rigid_bodies uploads, with the same IEEE divisions: X.w = 1/mass (0 for a static body), V.w = mass, the
+// inverse of the principal inertia, oldX = lastX = X, oldQ = lastQ = Q.  mass / inertia null: each body keeps its own; v / omega null: 0.
+// mask: as k_pack3 -- replica y is written only where mask[y] != 0, and otherwise its rows are not read.
+struct BodyRows { float *x, *q, *v, *omega; const float *mass, *inertia; const unsigned char *mask; };
+__global__ void k_set_bodies(RbState r, BodyRows s) {
+    if (s.mask && !s.mask[blockIdx.y]) return;
+    const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= r.n) return;
+    const size_t b = (size_t)blockIdx.y * r.n + i;
+    float4 X = make_float4(s.x[3 * b], s.x[3 * b + 1], s.x[3 * b + 2], 0.0f), V = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (s.mass) { const float m = s.mass[b]; X.w = (m != 0.0f) ? __fdiv_rn(1.0f, m) : 0.0f; V.w = m; }
+    else { X.w = r.X[b].w; V.w = r.V[b].w; }
+    if (s.v) { V.x = s.v[3 * b]; V.y = s.v[3 * b + 1]; V.z = s.v[3 * b + 2]; }
+    const float4 Q = make_float4(s.q[4 * b + 1], s.q[4 * b + 2], s.q[4 * b + 3], s.q[4 * b]);
+    const float4 W = s.omega ? make_float4(s.omega[3 * b], s.omega[3 * b + 1], s.omega[3 * b + 2], 0.f) : make_float4(0.f, 0.f, 0.f, 0.f);
+    r.X[b] = X; r.oldX[b] = X; r.lastX[b] = X;
+    r.Q[b] = Q; r.oldQ[b] = Q; r.lastQ[b] = Q;
+    r.V[b] = V; r.W[b] = W;
+    if (s.inertia) {
+        const float ix = s.inertia[3 * b], iy = s.inertia[3 * b + 1], iz = s.inertia[3 * b + 2];
+        const_cast<float4 *>(r.I)[b] = make_float4(ix, iy, iz, 0.f);
+        const_cast<float4 *>(r.Iinv)[b] = make_float4(__fdiv_rn(1.0f, ix), __fdiv_rn(1.0f, iy), __fdiv_rn(1.0f, iz), 0.f);
+    }
+}
+__global__ void k_get_bodies(RbState r, unsigned rows, BodyRows d) {
+    const unsigned b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= rows) return;
+    if (d.x) { const float4 X = r.X[b]; d.x[3 * b] = X.x; d.x[3 * b + 1] = X.y; d.x[3 * b + 2] = X.z; }
+    if (d.q) { const float4 Q = r.Q[b]; d.q[4 * b] = Q.w; d.q[4 * b + 1] = Q.x; d.q[4 * b + 2] = Q.y; d.q[4 * b + 3] = Q.z; }
+    if (d.v) { const float4 V = r.V[b]; d.v[3 * b] = V.x; d.v[3 * b + 1] = V.y; d.v[3 * b + 2] = V.z; }
+    if (d.omega) { const float4 W = r.W[b]; d.omega[3 * b] = W.x; d.omega[3 * b + 1] = W.y; d.omega[3 * b + 2] = W.z; }
 }
 
 // v = (1/h)(x - oldX)   or   (1/h)(1.5 x - 2 oldX + 0.5 lastX)

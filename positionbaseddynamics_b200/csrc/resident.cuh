@@ -67,7 +67,8 @@ struct ResidentArgs {
     int secondOrder;
     unsigned long long *xFlags;   // [nTiles][kXFlagStride] arrival flag of every CTA: (launch ordinal << 32) | arrivals in this launch
     unsigned long long xLaunch;   // this launch's ordinal << 32 (the host counts resident launches: flags stay monotone across launches)
-    RbState rb;                   // rigid bodies coupled through joints (global memory; single-cluster scenes only)
+    RbState rb;                   // rigid bodies coupled through joints (global memory; single-cluster scenes only); a batch's replica r
+                                  // at rows r x rb.n (pbd_set_replica_rigid_bodies)
     unsigned long long *trace;    // development aid (PBD_B200_TRACE): globaltimer per (phase, CTA, kTraceSlots)
     unsigned tracePhases;
     TypeArrays types[PBD_NUM_TYPES];
@@ -242,6 +243,7 @@ __device__ __forceinline__ void run_items(const ResidentArgs &A, const Acc &acc,
         if (BATCH) batchArrays = replica_arrays(A.types[T], rep, A.lamCount[T], 0u);
         const unsigned go = BATCH ? rep * A.geoCount[T] : 0u;  // replica rep's geometry (pbd_set_replica_rest_positions; 0: shared)
         const unsigned mo = BATCH ? rep * A.matCount[T] : 0u;  // ... and materials (pbd_set_replica_constraint_materials; 0: shared)
+        const unsigned ro = BATCH ? rep * A.rb.n : 0u;         // ... and rigid bodies (pbd_set_replica_rigid_bodies)
         MatRow matRow;
         if (BATCH) { matRow = load_mat_row<T>(rows + mat_offset(T)); matRow.on = true; }
         const TypeArrays &ta = BATCH ? batchArrays : A.types[T];
@@ -258,7 +260,7 @@ __device__ __forceinline__ void run_items(const ResidentArgs &A, const Acc &acc,
                     const unsigned j2 = i + 2u * stride;
                     const bool h2 = j2 < n;
                     if (h2) fetch(j2, s2, l2);
-                    project_streamed_acc<T, Acc, 0>(acc, ta, first + i, s0, A.h, iterZero, true, l0, matRow, go, mo);
+                    project_streamed_acc<T, Acc, 0>(acc, ta, first + i, s0, A.h, iterZero, true, l0, matRow, go, mo, ro);
                     if (!h1) break;
                     s0 = s1; l0 = l1; s1 = s2; l1 = l2; h1 = h2; i += stride;
                 }
@@ -274,7 +276,7 @@ __device__ __forceinline__ void run_items(const ResidentArgs &A, const Acc &acc,
                 const bool more = j < n;
                 Streamed nxt; float lamN = 0.0f;
                 if (is_pipelined<T>() && more) { nxt = load_streamed<T>(ta, first + j, go); if (type_shape(T).xpbd && !iterZero) lamN = __ldcg(ta.lambda + first + j); }
-                project_streamed_acc<T, Acc, 0>(acc, ta, first + i, cur, A.h, iterZero, true, lam, matRow, go, mo);  // variant 0 only: flatten refuses the full-Q bending layout in this mode
+                project_streamed_acc<T, Acc, 0>(acc, ta, first + i, cur, A.h, iterZero, true, lam, matRow, go, mo, ro);  // variant 0 only: flatten refuses the full-Q bending layout in this mode
                 if (!more) break;
                 if (!is_pipelined<T>()) { nxt = load_streamed<T>(ta, first + j, go); if (type_shape(T).xpbd && !iterZero) lamN = __ldcg(ta.lambda + first + j); }
                 cur = nxt; lam = lamN; i = j;
@@ -344,6 +346,12 @@ __global__ void __launch_bounds__(THREADS, 1) k_step_resident(const __grid_const
     const unsigned XT = BATCH ? 0u : A.xThreads, RT = THREADS - XT;
     const bool isX = !BATCH && threadIdx.x >= RT;
     const unsigned xtid = threadIdx.x - RT;
+    // rigid bodies: stepped by CTA 0 of the cluster, replica rep's at rows rep x rb.n.  A batch's instantiations without the joint types
+    // have no body path (the planner gives a batch with bodies the solid or the all-types instantiation).  A batch updates a substep's body
+    // velocities at the head of the next substep, in the thread that integrates the body next, and the last substep's after the launch
+    // (k_rb_velocity_batch, engine.cu): the same arithmetic, but no body code after the colour phases, where the batched solid kernel
+    // would spill more.
+    constexpr bool bodies = !BATCH || (MASK & (type_bit(PBD_BALLJOINT) | type_bit(PBD_RB_PARTICLE_BALLJOINT))) != 0u;
     constexpr bool single = SINGLE;  // one CTA per cluster: plain shared-memory accesses, __syncthreads between colours
     typedef typename std::conditional<SINGLE, LocalXAcc, ClusterAcc>::type XAcc;
     typedef typename std::conditional<SINGLE, LocalAcc, SmemAcc>::type RAcc;
@@ -411,8 +419,13 @@ __global__ void __launch_bounds__(THREADS, 1) k_step_resident(const __grid_const
                     float4 x = tile[tile_swizzle(i)];
                     if (integrate_particle(A, t0 + i, x, gx, gy, gz)) tile[tile_swizzle(i)] = x;
                 }
-                if (!BATCH && cta == 0)  // every body, in CTA 0: with G > 1 no joint reads them, in one cluster the cluster barrier orders them
-                    for (unsigned i = threadIdx.x; i < A.rb.n; i += RT) rb_integrate_body(A.rb, i, A.h, A.gx, A.gy, A.gz);
+                if (bodies && cta == 0) {  // every body, in CTA 0: with G > 1 no joint reads them, in one cluster the cluster barrier orders them
+                    const unsigned r0 = BATCH ? rep * A.rb.n : 0u;
+                    for (unsigned i = threadIdx.x; i < A.rb.n; i += RT) {
+                        if (BATCH && sub) rb_velocity_body(A.rb, r0 + i, A.invH, A.twoInvH, A.secondOrder);  // the previous substep's
+                        rb_integrate_body(A.rb, r0 + i, A.h, gx, gy, gz);
+                    }
+                }
             }
             x_count(0);
             colour_arrive(single);
@@ -479,7 +492,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_step_resident(const __grid_const
                 for (unsigned i = xtid; i < nGl; i += XT) velocity_particle(A, t0 + nSm + i, __ldcg(A.pos + t0 + nSm + i));
             } else {
                 for (unsigned i = threadIdx.x; i < nSm; i += RT) velocity_particle(A, t0 + i, tile[tile_swizzle(i)]);
-                if (!BATCH && cta == 0)  // (replica batches hold no rigid bodies)
+                if (!BATCH && cta == 0)  // (a batch: at the head of the next substep)
                     for (unsigned i = threadIdx.x; i < A.rb.n; i += RT) rb_velocity_body(A.rb, i, A.invH, A.twoInvH, A.secondOrder);
             }
         }

@@ -5,7 +5,7 @@ power limit read in the same run.  The four scenes run four different resident i
 masks).
 
     python tools/bench_batch.py [--out results.json] [--quick] [--replica-rows] [--sweep] [--rest-shapes] [--colliders] [--constraint-materials]
-                                [--ks 8,132] [--no-baseline]
+                                [--rigid] [--ks 8,132] [--no-baseline]
 
 --replica-rows measures every batch twice in a row: with the shared parameters, and with per-replica material rows and gravity
 (pbd_set_replica_materials / pbd_set_replica_gravity) equal to the shared values, so that the work is identical and the difference is what
@@ -22,6 +22,11 @@ through the cloth's plane at random places, every replica its own), alternating.
 what reading the K x count material arrays costs; their size is printed beside each row.  It also times the device form of the call
 (pbd_set_replica_constraint_materials_device) for every replica and for a 10 % mask, 200 calls enqueued behind a spin so that the
 gathers run back to back, against the algorithmic bytes of the gather.
+--rigid measures only batches of the rigid-body cloth coupling rig (a 20 x 20 cloth, 12 bodies, 8 BallJoints, 4 RigidBodyParticleBallJoints,
+tests/rigid_batch_util.py), every replica with its own bodies (pbd_set_replica_rigid_bodies): ms per batched step at K = 1, 33, 132, 528 in
+graph and in forced resident mode, against the K replicas stepped one after another by a K = 1 engine (per replica its particles and bodies
+uploaded, one step, both read back), and the cost of one masked device write of the bodies per step (pbd_set_rigid_bodies_device, half the
+replicas): the write alone, 200 enqueued back to back, and steps with a write before each against steps without, wall clock after a sync.
 --ks replaces the K sweep of every scene; --no-baseline skips the one-after-another baseline and the C sweep.  Without --rest-shapes or
 --replica-rows the script also runs against a build without those calls, so that shared-parameter batches can be compared across builds.
 
@@ -54,6 +59,95 @@ SCENES = {  # name: (builder, sub_steps, max_iter, K sweep)
     "cloth100_femtri": (lambda m: scenes.cloth(m, 100, 100, cloth_method=2, bending_method=1, sub_steps=1, max_iter=5), 1, 5, [1, 8, 33, 66, 132, 264]),
 }
 C_SWEEP = {"cfg1": [8, 132, 528], "cfg3": [8, 33, 66]}  # K at which every cluster size C is measured
+RIGID_KS = [1, 33, 132, 528]
+
+
+def rigid_engine(m, mode, k):
+    import rigid_batch_util as rb
+    if k == 1:
+        return rb.engine(m, mode, bodies=rb.replica_bodies(m, 0))
+    return rb.engine(m, mode, replicas=k, bodies=[rb.replica_bodies(m, r) for r in range(k)])
+
+
+def rigid_one_after_another(m, k):
+    """ms for K rig replicas stepped one after another by one K = 1 engine in graph mode: per replica its x, v and bodies uploaded, one
+    step, x, v and bodies read back; wall clock around the sequence, after one warm-up pass."""
+    import rigid_batch_util as rb
+    eng = rigid_engine(m, _capi.MODE_GRAPH, 1)
+    try:
+        xs = np.repeat(np.asarray(m["x"], np.float32)[None], k, 0)
+        vs = np.zeros_like(xs)
+        mass, _, _, inertia, _, _ = rb.replica_bodies(m, 0)
+        bodies = np.repeat(eng.get_rigid_bodies()[None], k, 0)
+        for passes in range(2):  # the first pass warms up
+            eng.sync()
+            t0 = time.perf_counter()
+            for r in range(k):
+                eng.set_attr(_capi.ATTR_X, xs[r]); eng.set_attr(_capi.ATTR_V, vs[r])
+                b = bodies[r]
+                eng.set_rigid_bodies(mass, b[:, :3], b[:, 3:7], inertia, v=b[:, 7:10], omega=b[:, 10:13])
+                eng.step(1)
+                eng.get_attr(_capi.ATTR_X, xs[r]); eng.get_attr(_capi.ATTR_V, vs[r]); bodies[r] = eng.get_rigid_bodies()
+            eng.sync()
+            ms = (time.perf_counter() - t0) * 1e3
+        return ms
+    finally:
+        eng.close()
+
+
+def rigid_write_timing(m, k, calls=200):
+    """A masked device write of every body of half the replicas (pbd_set_rigid_bodies_device, x and q from torch): ms per write alone
+    (`calls` enqueued back to back), and ms per step with and without a write before each step (graph mode), wall clock after a sync."""
+    import torch
+    eng = rigid_engine(m, _capi.MODE_GRAPH, k)
+    try:
+        st = eng.get_rigid_bodies()
+        x = torch.from_numpy(np.ascontiguousarray(st[..., :3]).reshape(-1)).cuda()
+        q = torch.from_numpy(np.ascontiguousarray(st[..., 3:7]).reshape(-1)).cuda()
+        mask = (torch.arange(k, device="cuda") % 2 == 0).to(torch.uint8)
+        s = torch.cuda.current_stream().cuda_stream
+
+        def wall(f, n):
+            f(); torch.cuda.synchronize(); eng.sync()
+            t0 = time.perf_counter()
+            for _ in range(n):
+                f()
+            torch.cuda.synchronize(); eng.sync()
+            return (time.perf_counter() - t0) * 1e3 / n
+        write = lambda: eng.set_rigid_bodies_device(x, q, replicas=mask, stream=s)
+        alone = wall(write, calls)
+        steps = [wall(lambda: eng.step(1), 100), wall(lambda: (write(), eng.step(1)), 100), wall(lambda: eng.step(1), 100), wall(lambda: (write(), eng.step(1)), 100)]
+        return {"K": k, "write_ms": alone, "step_ms": steps[0::2], "step_with_write_ms": steps[1::2]}
+    finally:
+        eng.close()
+
+
+def rigid_main(a, res):
+    import rigid_batch_util as rb
+    m = rb.model("rig")
+    print("rig: %d particles, %d bodies, %d constraints, %d x %d" % (len(m["x"]), len(m["bm"]), len(m["types"]), m["sub"], m["it"]), flush=True)
+    for k in ([int(v) for v in a.ks.split(",")] if a.ks else RIGID_KS):
+        row = {"K": k, "baseline_ms": float("nan") if a.no_baseline else rigid_one_after_another(m, k)}
+        for label, md in (("graph", _capi.MODE_GRAPH), ("resident", _capi.MODE_RESIDENT)):
+            eng = None
+            try:
+                eng = rigid_engine(m, md, k)
+                ms, steps = timed(eng)
+                row[label] = {"ms": ms, "steps": steps, "active": eng.get_mode()[1]}
+            except _capi.PbdError as ex:
+                row[label] = {"error": str(ex)}
+            finally:
+                if eng is not None:
+                    eng.close()
+        if k > 1:
+            row["write"] = rigid_write_timing(m, k)
+        res["rigid"].append(row)
+        fmt = lambda r: ("%8.4f ms" % r["ms"]) if "ms" in r else ("refused: " + r["error"][:60])
+        w = row.get("write")
+        print("  rig K=%4d  graph %s | resident %s | one after another %9.3f ms%s" % (
+            k, fmt(row["graph"]), fmt(row["resident"]), row["baseline_ms"],
+            (" | masked body write %.4f ms alone, step %.4f %.4f ms, with a write %.4f %.4f ms" % (w["write_ms"], *w["step_ms"], *w["step_with_write_ms"])) if w else ""),
+            flush=True)
 
 
 def card():
@@ -312,12 +406,20 @@ def main():
     ap.add_argument("--rest-shapes", action="store_true", help="every batch also with per-replica rest shapes; device derivation against host builds")
     ap.add_argument("--colliders", action="store_true", help="only the contact path: batches without and with three per-replica colliders")
     ap.add_argument("--constraint-materials", action="store_true", help="every batch also with per-constraint materials equal to the shared ones; gather timing")
+    ap.add_argument("--rigid", action="store_true", help="only batches of the rigid-body coupling rig and the masked device body write")
     ap.add_argument("--ks", default=None, help="comma-separated K to measure instead of each scene's sweep")
     ap.add_argument("--no-baseline", action="store_true", help="skip the one-after-another baseline and the C sweep")
     a = ap.parse_args()
     res = {"card": card(), "rows": [], "c_sweep": [], "replica_rows": [], "sweep": [], "rest_shapes": [], "derive": [], "colliders": [],
-           "constraint_materials": [], "gather": []}
+           "constraint_materials": [], "gather": [], "rigid": []}
     print("card: %s" % res["card"], flush=True)
+    if a.rigid:
+        rigid_main(a, res)
+        if a.out:
+            os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
+            with open(a.out, "w") as f:
+                json.dump(res, f, indent=1)
+        return
     if a.colliders:
         for name, ks in COLLIDER_KS.items():
             m = model(name)

@@ -222,6 +222,40 @@ int pbd_get_contacts(pbd_engine *e, pbd_contact *out, unsigned capacity, unsigne
 int pbd_set_replica_colliders(pbd_engine *e, unsigned nParticleColliders, const pbd_particle_collider *pc,
                               unsigned nRigidColliders, const pbd_rigid_collider *rc,
                               const float *body_x, const float *body_v, const float *body_omega);
+/* Move the rigid colliders of a replica batch from device memory (K > 1, after pbd_set_replica_colliders switched them on with nR per
+ * replica).  pose: K*nR*21 floats; each row is the float fields R[9], v1[3], v2[3], aabb_min[3], aabb_max[3] of a pbd_rigid_collider, in
+ * that order (the struct from &rc.R[0] to its end).  body_x: K*nR*3 floats, required; body_v and body_omega: K*nR*3 floats or NULL (= 0).
+ * All are the arrays of pbd_set_replica_colliders, replica after replica, colliders in list order.  Only where the obstacles are changes:
+ * shape, dims, thickness, invert_sdf, coefficients, body ids, particle ranges and counts stay those of the host call.  The engine then
+ * steps bit for bit as if pbd_set_replica_colliders had been called with the same ranges and counts and these placement floats and body
+ * rows, so a device set and a host set of the same rows give identical bits.  The rows are written in place (the tables keep their
+ * address): no host synchronisation, no new plan, no new graph capture.
+ * Stream contract, mask and memory refusals of pbd_set_attr_device: a replica r with replicas[r] == 0 keeps its colliders and bodies bit
+ * for bit and its rows are not read.  Refused, with the colliders in force left as they were: at K = 1, without replica colliders in force,
+ * a null pose or body_x, host memory (pinned or pageable), memory of another device, a host-memory mask, a stream being captured. */
+int pbd_set_replica_collider_poses_device(pbd_engine *e, const float *pose, const float *body_x, const float *body_v,
+                                          const float *body_omega, const unsigned char *replicas, void *stream);
+/* Contact sensors: per rigid collider of the colliders in force, the contacts found and the impulse received, kept on the device.
+ * While sensing is on (pbd_sense_contacts(e, 1); off by default), the contact launch of every step also produces, for each replica r
+ * (r = 0 for pbd_set_colliders' single scene) and each rigid collider k:
+ *   count[r*nR + k]:         the contacts the collision test of that step found between collider k and replica r's particles -- the
+ *                            entries pbd_get_contacts lists for that collider, static particles included;
+ *   impulse[3*(r*nR + k)..]: the impulse the particles exerted on collider k during the step's velocity solve, in mass x velocity units
+ *                            (divide by dt for the mean force): -sum p over the collider's contacts and the maxIterationsV sweeps, p being
+ *                            every impulse (normal, penalty, friction) the solve adds to a particle's velocity (particles of mass 0 get
+ *                            none); the -p the reference's velocitySolve_ParticleRigidBodyContactConstraint would apply to a dynamic body.
+ * The values are those of the last step enqueued before the get; they are zero when sensing is switched on and when the collider or particle
+ * range counts change.  Sums are taken in an order fixed by K, the particle ranges and the collider list (no floating-point atomics), so
+ * they are the same bits in every mode and run, and replica r of a batch reports what a single-scene engine given replica r's rows reports.
+ * Sensing changes no state; it costs one more launch per step (counted in pbd_stats.kernel_launches) and K*ceil(total/128)*nR*16 bytes of
+ * device memory, allocated by this call and by the collider calls, never inside a step.  Switching it plans and captures nothing again;
+ * pbd_set_replicas keeps the switch.
+ * pbd_get_contact_sensors: host arrays, count K*nR unsigned, impulse K*nR*3 floats, either may be NULL; synchronises.
+ * pbd_get_contact_sensors_device: the same into device memory, with the stream contract and memory refusals of pbd_get_attr_device.
+ * Both are refused while sensing is off or no rigid colliders are in force. */
+int pbd_sense_contacts(pbd_engine *e, int on);
+int pbd_get_contact_sensors(pbd_engine *e, unsigned *count, float *impulse);
+int pbd_get_contact_sensors_device(pbd_engine *e, unsigned *count, float *impulse, void *stream);
 
 /* ---- Replica batch: K independent copies of one model's state stepped together on one device ---------------------------------
  * One engine holds one model (particles, constraints, groups, parameters) and K copies of its state; one pbd_step advances all K,

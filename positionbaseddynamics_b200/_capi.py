@@ -30,7 +30,8 @@ SYMBOLS = ["pbd_last_error", "pbd_device_count", "pbd_create", "pbd_destroy", "p
            "pbd_set_colliders", "pbd_set_contact_params", "pbd_record_contacts", "pbd_get_contacts", "pbd_set_replica_colliders",
            "pbd_set_attr_device", "pbd_get_attr_device", "pbd_set_masses_device",
            "pbd_set_replica_constraint_materials", "pbd_set_replica_constraint_materials_device", "pbd_get_replica_materials",
-           "pbd_set_replica_rigid_bodies", "pbd_set_rigid_bodies_device", "pbd_get_rigid_bodies_device"]
+           "pbd_set_replica_rigid_bodies", "pbd_set_rigid_bodies_device", "pbd_get_rigid_bodies_device",
+           "pbd_set_replica_collider_poses_device", "pbd_sense_contacts", "pbd_get_contact_sensors", "pbd_get_contact_sensors_device"]
 
 
 SHAPE_BOX, SHAPE_SPHERE, SHAPE_TORUS, SHAPE_CYLINDER, SHAPE_HOLLOW_SPHERE, SHAPE_HOLLOW_BOX = range(6)
@@ -121,6 +122,10 @@ def lib():
         _lib.pbd_set_replica_rigid_bodies.argtypes = [C.c_void_p, C.c_uint] + [C.c_void_p] * 6
         _lib.pbd_set_rigid_bodies_device.argtypes = [C.c_void_p] * 9
         _lib.pbd_get_rigid_bodies_device.argtypes = [C.c_void_p] * 6
+        _lib.pbd_set_replica_collider_poses_device.argtypes = [C.c_void_p] * 7
+        _lib.pbd_sense_contacts.argtypes = [C.c_void_p, C.c_int]
+        _lib.pbd_get_contact_sensors.argtypes = [C.c_void_p] * 3
+        _lib.pbd_get_contact_sensors_device.argtypes = [C.c_void_p] * 4
     return _lib
 
 
@@ -225,6 +230,8 @@ class Engine:
         self.n = 0
         self.K = 1
         self._nc = 0  # constraints added so far (sizes the buffer of groups())
+        self.n_rigid_colliders = 0  # rigid colliders per replica in force (sizes the contact sensors)
+        self._replica_colliders = False
 
     def _batch_shape(self, *tail):
         return ((self.K,) if self.K > 1 else ()) + (self.n,) + tail
@@ -297,6 +304,8 @@ class Engine:
         """K copies of replica 0's current state (x, v, x0, oldX, lastX, masses), multipliers zero; the image is re-planned."""
         _ck(lib().pbd_set_replicas(self._h, int(k)))
         self.K = int(k)
+        if self._replica_colliders:  # dropped with the old K
+            self.n_rigid_colliders, self._replica_colliders = 0, False
 
     def replicas(self):
         k = C.c_uint(0)
@@ -511,6 +520,7 @@ class Engine:
         pa = (ParticleCollider * max(len(particle_colliders), 1))(*particle_colliders)
         ra = (RigidCollider * max(len(rigid_colliders), 1))(*rigid_colliders)
         _ck(lib().pbd_set_colliders(self._h, len(particle_colliders), C.cast(pa, C.c_void_p), len(rigid_colliders), C.cast(ra, C.c_void_p)))
+        self.n_rigid_colliders, self._replica_colliders = len(rigid_colliders), False
 
     def set_replica_colliders(self, particle_colliders, rigid_colliders, body_x=None, body_v=None, body_omega=None):
         """pbd_set_replica_colliders: every replica against its own static colliders.  particle_colliders: ParticleCollider ranges of
@@ -519,6 +529,7 @@ class Engine:
         rigid_colliders None: no contacts.  K > 1 only."""
         if rigid_colliders is None:
             _ck(lib().pbd_set_replica_colliders(self._h, 0, None, 0, None, None, None, None))
+            self.n_rigid_colliders, self._replica_colliders = 0, False
             return
         if len(rigid_colliders) != self.K or len(set(len(r) for r in rigid_colliders)) > 1:
             raise ValueError("set_replica_colliders: wants %d lists of the same number of rigid colliders, got %s" % (self.K, [len(r) for r in rigid_colliders]))
@@ -534,6 +545,42 @@ class Engine:
         pa = (ParticleCollider * max(len(particle_colliders), 1))(*particle_colliders)
         ra = (RigidCollider * max(len(flat), 1))(*flat)
         _ck(lib().pbd_set_replica_colliders(self._h, len(particle_colliders), C.cast(pa, C.c_void_p), nr, C.cast(ra, C.c_void_p), *[_ptr(a) for a in arrays]))
+        self.n_rigid_colliders, self._replica_colliders = nr, nr > 0
+
+    def set_replica_collider_poses_device(self, pose, body_x, body_v=None, body_omega=None, replicas=None, stream=None):
+        """pbd_set_replica_collider_poses_device: move the replica colliders of set_replica_colliders from device memory.  pose: K*nR*21
+        float32, each row R[9], v1[3], v2[3], aabb_min[3], aabb_max[3] of a RigidCollider; body_x (required), body_v, body_omega: K*nR*3
+        float32 (v, omega None = 0).  Objects with __cuda_array_interface__; stream and replicas as in set_attr_device.  Everything else
+        about the colliders stays as set_replica_colliders left it."""
+        rows = self.K * self.n_rigid_colliders
+        p = _device_ptr("set_replica_collider_poses_device: pose", pose, ("<f4",), rows * 21)
+        ptrs = [C.c_void_p(_device_ptr("set_replica_collider_poses_device: " + name, a, ("<f4",), rows * 3)) if a is not None else None
+                for name, a in (("body_x", body_x), ("body_v", body_v), ("body_omega", body_omega))]
+        if ptrs[0] is None:
+            raise TypeError("set_replica_collider_poses_device: body_x is required")
+        mask = self._mask("set_replica_collider_poses_device", replicas)
+        _ck(lib().pbd_set_replica_collider_poses_device(self._h, C.c_void_p(p), *ptrs, mask, _stream(stream)))
+
+    # contact sensors: per replica and rigid collider, the contacts found and the impulse received (mass x velocity) in the last step
+    def sense_contacts(self, on=True):
+        """pbd_sense_contacts: switch the contact sensors on or off (off by default)."""
+        _ck(lib().pbd_sense_contacts(self._h, int(bool(on))))
+
+    def contact_sensors(self):
+        """pbd_get_contact_sensors: (counts (K, nR) uint32, impulses (K, nR, 3) float32) of the last step; synchronises."""
+        count = np.zeros((self.K, self.n_rigid_colliders), np.uint32)
+        impulse = np.zeros((self.K, self.n_rigid_colliders, 3), np.float32)
+        _ck(lib().pbd_get_contact_sensors(self._h, _ptr(count), _ptr(impulse)))
+        return count, impulse
+
+    def get_contact_sensors_device(self, count=None, impulse=None, stream=None):
+        """pbd_get_contact_sensors_device: the sensors into count (K*nR uint32) and impulse (K*nR*3 float32), objects with
+        __cuda_array_interface__, writable; either may be None.  Stream as in get_attr_device.  Returns (count, impulse)."""
+        rows = self.K * self.n_rigid_colliders
+        pc = C.c_void_p(_device_ptr("get_contact_sensors_device: count", count, ("<u4",), rows, writable=True)) if count is not None else None
+        pi = C.c_void_p(_device_ptr("get_contact_sensors_device: impulse", impulse, ("<f4",), rows * 3, writable=True)) if impulse is not None else None
+        _ck(lib().pbd_get_contact_sensors_device(self._h, pc, pi, _stream(stream)))
+        return count, impulse
 
     def set_contact_params(self, tolerance=0.01, stiffness=100.0, max_iter_v=5):
         _ck(lib().pbd_set_contact_params(self._h, float(tolerance), float(stiffness), int(max_iter_v)))

@@ -127,12 +127,20 @@ struct LiveContact {  // ParticleRigidBodyContactConstraint: m_constraintInfo (3
     unsigned body;  // where the carrying body's state sits in rbX / rbV / rbW
 };
 
+// Contact sensors of one particle (contacts_particle<*, true>): per rigid collider k of its replica, whether the collision test found a
+// contact, and the sum of the impulses p the solve added to the particle's velocity through that contact, sweep after sweep.
+struct ContactSense {
+    unsigned count[kMaxRigidColliders];
+    float p[kMaxRigidColliders][3];
+};
+
 // One thread per particle of the registered triangle / tet models: collision test against every rigid collider in list order (the
 // order of the reference's contact list for this particle), contact initialisation with the velocities before any contact impulse,
 // then maxIterV sweeps over the particle's contacts.  BATCH: the particle, colliders and bodies of replica `replica` (ContactArgs::n);
 // one scene: the body of a collider is its `body`, which indexes rbX / rbV / rbW.
-template <bool BATCH>
-__device__ __forceinline__ void contacts_particle(const ContactArgs &A, const unsigned gid, const unsigned replica) {
+// SENSE: also fills *sense (zeroed by the caller); the arithmetic that moves the particle is the same.
+template <bool BATCH, bool SENSE = false>
+__device__ __forceinline__ void contacts_particle(const ContactArgs &A, const unsigned gid, const unsigned replica, ContactSense *sense = nullptr) {
     if (gid >= A.total) return;
     unsigned r = 0;
     while (r + 1 < A.nRanges && gid >= A.rangeStart[r + 1]) r++;
@@ -146,6 +154,7 @@ __device__ __forceinline__ void contacts_particle(const ContactArgs &A, const un
     const float invMass0 = X.w;
 
     LiveContact live[kMaxRigidColliders];
+    unsigned char liveCollider[SENSE ? kMaxRigidColliders : 1];  // SENSE: the collider of each live contact
     unsigned nLive = 0;
     for (unsigned k = 0; k < A.nRigid; k++) {
         const RigidCollider &c = A.rigid[first + k];
@@ -187,6 +196,7 @@ __device__ __forceinline__ void contacts_particle(const ContactArgs &A, const un
                 A.record[at] = rec;
             }
         }
+        if constexpr (SENSE) { liveCollider[nLive] = (unsigned char)k; sense->count[k] = 1u; }
         nLive++;
     }
     if (nLive == 0 || invMass0 == 0.0f) return;  // velocitySolve returns false when both sides are static
@@ -212,7 +222,10 @@ __device__ __forceinline__ void contacts_particle(const ContactArgs &A, const un
             else if (L.friction * pn < -L.pMax) ft = L.pMax;
             else ft = -L.friction * pn;
             for (int i = 0; i < 3; i++) p[i] += ft * L.t[i];
-            if (mass0 != 0.0f) { V.x += invMass0 * p[0]; V.y += invMass0 * p[1]; V.z += invMass0 * p[2]; }
+            if (mass0 != 0.0f) {
+                V.x += invMass0 * p[0]; V.y += invMass0 * p[1]; V.z += invMass0 * p[2];
+                if constexpr (SENSE) { float *s = sense->p[liveCollider[k]]; s[0] += p[0]; s[1] += p[1]; s[2] += p[2]; }
+            }
         }
     }
     A.vel[slot] = V;
@@ -221,5 +234,82 @@ __device__ __forceinline__ void contacts_particle(const ContactArgs &A, const un
 __global__ void __launch_bounds__(128) k_contacts(const ContactArgs A) { contacts_particle<false>(A, blockIdx.x * blockDim.x + threadIdx.x, 0u); }
 // grid (ceil(total / 128), K): replica = blockIdx.y, so that every collider and body load of a block is uniform
 __global__ void __launch_bounds__(128) k_contacts_batch(const ContactArgs A) { contacts_particle<true>(A, blockIdx.x * blockDim.x + threadIdx.x, blockIdx.y); }
+
+#ifdef __CUDACC__
+// ---- contact sensors (pbd_sense_contacts) ------------------------------------------------------------------------------------------
+// The contact launch with sensing on: the same grid as k_contacts / k_contacts_batch, each thread running contacts_particle<*, true>.  Each
+// block then sums its 128 particles' sensors per collider in a fixed order -- within a warp by a shuffle tree (lane i takes lane i + 16,
+// + 8, ..., + 1), then the four warp sums in warp order -- into partial[(replica * gridDim.x + block) * nRigid + k]: the impulse sum in
+// xyz, the contact count in w (as bits).  k_contact_sensors_sum adds a collider's partials in block order.  The order depends only on
+// the particle ranges, so replica r of a batch sums exactly as a single scene given its rows, in every mode.
+constexpr unsigned kSenseThreads = 128;
+template <bool BATCH>
+__device__ __forceinline__ void contacts_sense(const ContactArgs &A, const unsigned replica, float4 *__restrict__ partial) {
+    ContactSense s;
+    for (int k = 0; k < kMaxRigidColliders; k++) { s.count[k] = 0u; s.p[k][0] = s.p[k][1] = s.p[k][2] = 0.0f; }
+    contacts_particle<BATCH, true>(A, blockIdx.x * blockDim.x + threadIdx.x, replica, &s);
+    __shared__ float4 warpSum[kSenseThreads / 32][kMaxRigidColliders];
+    const unsigned lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+    for (unsigned k = 0; k < A.nRigid; k++) {
+        float x = s.p[k][0], y = s.p[k][1], z = s.p[k][2];
+        unsigned c = s.count[k];
+        for (int off = 16; off > 0; off >>= 1) {
+            x += __shfl_down_sync(0xffffffffu, x, off); y += __shfl_down_sync(0xffffffffu, y, off); z += __shfl_down_sync(0xffffffffu, z, off);
+            c += __shfl_down_sync(0xffffffffu, c, off);
+        }
+        if (lane == 0) warpSum[warp][k] = make_float4(x, y, z, __uint_as_float(c));
+    }
+    __syncthreads();
+    if (threadIdx.x < A.nRigid) {
+        const unsigned k = threadIdx.x;
+        float4 t = warpSum[0][k];
+        unsigned c = __float_as_uint(t.w);
+        for (unsigned w = 1; w < kSenseThreads / 32; w++) {
+            const float4 u = warpSum[w][k];
+            t.x += u.x; t.y += u.y; t.z += u.z; c += __float_as_uint(u.w);
+        }
+        t.w = __uint_as_float(c);
+        partial[((size_t)replica * gridDim.x + blockIdx.x) * A.nRigid + k] = t;
+    }
+}
+__global__ void __launch_bounds__(kSenseThreads) k_contacts_sense(const ContactArgs A, float4 *partial) { contacts_sense<false>(A, 0u, partial); }
+__global__ void __launch_bounds__(kSenseThreads) k_contacts_sense_batch(const ContactArgs A, float4 *partial) { contacts_sense<true>(A, blockIdx.y, partial); }
+
+// one thread per (replica, collider) row of K * nRigid: its `blocks` partials summed in block order; the impulse on the collider is the
+// negated sum of what its contacts added to the particles
+__global__ void __launch_bounds__(128) k_contact_sensors_sum(const float4 *__restrict__ partial, unsigned rows, unsigned nRigid, unsigned blocks,
+                                                             unsigned *__restrict__ count, float *__restrict__ impulse) {
+    const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= rows) return;
+    const unsigned r = i / nRigid, k = i - r * nRigid;
+    const float4 *p = partial + (size_t)r * blocks * nRigid + k;
+    float x = 0.0f, y = 0.0f, z = 0.0f;
+    unsigned c = 0u;
+    for (unsigned b = 0; b < blocks; b++) {
+        const float4 u = p[(size_t)b * nRigid];
+        x += u.x; y += u.y; z += u.z; c += __float_as_uint(u.w);
+    }
+    count[i] = c;
+    impulse[3 * i] = 0.0f - x; impulse[3 * i + 1] = 0.0f - y; impulse[3 * i + 2] = 0.0f - z;  // (+0 where nothing touched, not -0)
+}
+
+// pbd_set_replica_collider_poses_device: one grid row per replica (blockIdx.y), thread k < nRigid writes the placement of collider k and
+// the body carrying it.  pose rows: R[9], v1[3], v2[3], aabbMin[3], aabbMax[3]; bodies: w = 0, as the host call writes them.
+struct ColliderPoses { const float *pose, *x, *v, *omega; const unsigned char *mask; };
+__global__ void k_set_collider_poses(RigidCollider *__restrict__ rigid, float4 *__restrict__ bX, float4 *__restrict__ bV, float4 *__restrict__ bW,
+                                     unsigned nRigid, const ColliderPoses s) {
+    if (s.mask && !s.mask[blockIdx.y]) return;
+    const unsigned k = threadIdx.x;
+    if (k >= nRigid) return;
+    const size_t i = (size_t)blockIdx.y * nRigid + k;
+    const float *p = s.pose + 21 * i;
+    RigidCollider &c = rigid[i];
+    for (int j = 0; j < 9; j++) c.R[j] = p[j];
+    for (int j = 0; j < 3; j++) { c.v1[j] = p[9 + j]; c.v2[j] = p[12 + j]; c.aabbMin[j] = p[15 + j]; c.aabbMax[j] = p[18 + j]; }
+    bX[i] = make_float4(s.x[3 * i], s.x[3 * i + 1], s.x[3 * i + 2], 0.f);
+    bV[i] = s.v ? make_float4(s.v[3 * i], s.v[3 * i + 1], s.v[3 * i + 2], 0.f) : make_float4(0.f, 0.f, 0.f, 0.f);
+    bW[i] = s.omega ? make_float4(s.omega[3 * i], s.omega[3 * i + 1], s.omega[3 * i + 2], 0.f) : make_float4(0.f, 0.f, 0.f, 0.f);
+}
+#endif
 
 }  // namespace pbdk

@@ -165,6 +165,14 @@ struct pbd_engine {
         unsigned nRigid = 0, total = 0;
         DevBuf dRanges, dStart, dRigid, dX, dV, dW;
     } repColliders;
+    // contact sensors (pbd_sense_contacts): per replica and rigid collider, the contacts found and the impulse received in the last step.
+    // partial: the contact launch's per-block sums (K x blocks x nRigid float4), summed into count / impulse by k_contact_sensors_sum.
+    // Sized for the colliders in force (K, nRigid, blocks) by size_sensors, outside the steps; all zero when nRigid == 0.
+    struct Sensors {
+        bool on = false;
+        unsigned K = 0, nRigid = 0, blocks = 0;
+        DevBuf partial, count, impulse;
+    } sensors;
     bool timingPending = false;
     std::vector<unsigned> slot;          // host particle index -> device slot (formula layouts or the tile-major permutation)
     DevBuf dSlot, dSlotOld, relayoutTmp;
@@ -430,6 +438,33 @@ static void drop_replica_colliders(pbd_engine *e) {
     c.ranges.clear(); c.nRigid = c.total = 0;
     for (DevBuf *b : {&c.dRanges, &c.dStart, &c.dRigid, &c.dX, &c.dV, &c.dW}) b->release();
 }
+// The contact sensors sized for the colliders in force: a batch's replica colliders, else pbd_set_colliders' one scene.  New sizes (sensing
+// switched on, other collider or particle counts, another K) zero the outputs once the steps in flight are done; the same sizes keep them.
+static int size_sensors(pbd_engine *e) {
+    pbd_engine::Sensors &s = e->sensors;
+    const pbd_engine::ReplicaColliders &rep = e->repColliders;
+    const bool batch = rep.nRigid != 0;
+    unsigned K = 0, nR = 0, blocks = 0;
+    if (s.on && (batch || !e->rColliders.empty())) {
+        K = batch ? e->batch.K : 1u;
+        nR = batch ? rep.nRigid : (unsigned)e->rColliders.size();
+        blocks = nblk(batch ? rep.total : e->contactTotal, kSenseThreads);
+    }
+    if (K == s.K && nR == s.nRigid && blocks == s.blocks) return 0;
+    CKE(use(e));
+    CK(cudaStreamSynchronize(e->stream));
+    s.K = K; s.nRigid = nR; s.blocks = blocks;
+    for (DevBuf *b : {&s.partial, &s.count, &s.impulse}) b->release();
+    if (!nR) return 0;
+    const size_t rows = (size_t)K * nR;
+    CKE(s.partial.alloc(std::max<size_t>(rows * blocks, 1) * sizeof(float4)));
+    CKE(s.count.alloc(rows * sizeof(unsigned)));
+    CKE(s.impulse.alloc(rows * 3 * sizeof(float)));
+    CK(cudaMemsetAsync(s.count.p, 0, rows * sizeof(unsigned), e->stream));
+    CK(cudaMemsetAsync(s.impulse.p, 0, rows * 3 * sizeof(float), e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+    return 0;
+}
 
 extern "C" int pbd_set_replicas(pbd_engine *e, unsigned K) {
     if (!e) return fail("null engine");
@@ -445,6 +480,7 @@ extern "C" int pbd_set_replicas(pbd_engine *e, unsigned K) {
     e->batch.mat.release(); e->batch.gravity.release(); e->batch.matMask = 0; e->batch.gravitySet = false;  // rows of the old K
     drop_replica_geometry(e);
     drop_replica_colliders(e);
+    CKE(size_sensors(e));  // sensing stays on; the one scene's colliders, if any, keep their sensors
     CK(cudaStreamSynchronize(e->stream));
     model_changed(e);  // every replica is redefined: planned again, with the shared material rows and zero multipliers
     return 0;
@@ -1725,7 +1761,7 @@ extern "C" int pbd_set_colliders(pbd_engine *e, unsigned nP, const pbd_particle_
     if (nP) { CKE(upload_vec(e->dPColliders, e->pColliders, e->stream)); CKE(upload_vec(e->dRangeStart, start, e->stream)); }
     if (nR) CKE(upload_vec(e->dRColliders, e->rColliders, e->stream));
     CK(cudaStreamSynchronize(e->stream));
-    return 0;
+    return size_sensors(e);
 }
 extern "C" int pbd_set_replica_colliders(pbd_engine *e, unsigned nP, const pbd_particle_collider *pc, unsigned nR, const pbd_rigid_collider *rc,
                                          const float *body_x, const float *body_v, const float *body_omega) {
@@ -1752,7 +1788,7 @@ extern "C" int pbd_set_replica_colliders(pbd_engine *e, unsigned nP, const pbd_p
     if (nR == 0) {  // off
         CK(cudaStreamSynchronize(e->stream));
         drop_replica_colliders(e);
-        return 0;
+        return size_sensors(e);
     }
     const struct { DevBuf *d; const void *h; size_t bytes; } up[] = {
         {&c.dRanges, P.data(), nP * sizeof(ParticleCollider)}, {&c.dStart, start.data(), (nP + 1) * sizeof(unsigned)},
@@ -1767,7 +1803,63 @@ extern "C" int pbd_set_replica_colliders(pbd_engine *e, unsigned nP, const pbd_p
     // ones.  The sources are pageable, so the driver has staged them when the call returns and the vectors may go.
     for (const auto &u : up) if (u.bytes) CK(cudaMemcpyAsync(u.d->p, u.h, u.bytes, cudaMemcpyHostToDevice, e->stream));
     c.ranges.swap(P); c.nRigid = nR; c.total = start[nP];
+    return size_sensors(e);  // the same counts: nothing to do, no synchronisation
+}
+
+// pbd_set_replica_collider_poses_device: the placement rows of a batch's colliders and their bodies, written in place by
+// k_set_collider_poses under device_call's stream contract
+extern "C" int pbd_set_replica_collider_poses_device(pbd_engine *e, const float *pose, const float *body_x, const float *body_v,
+                                                     const float *body_omega, const unsigned char *replicas, void *stream) {
+    const char *what = "pbd_set_replica_collider_poses_device";
+    if (!e) return fail("%s: null engine", what);
+    if (e->batch.K == 1) return fail("%s: a single-scene engine places its colliders through pbd_set_colliders (pbd_set_replicas first)", what);
+    pbd_engine::ReplicaColliders &c = e->repColliders;
+    if (!c.nRigid) return fail("%s: no replica colliders in force (pbd_set_replica_colliders first)", what);
+    if (!body_x) return fail("%s: body_x == NULL", what);
+    CKE(body_arrays_refusal(e, what, {{"body_x", body_x}, {"body_v", body_v}, {"body_omega", body_omega}}));
+    return device_call(e, what, "pose", pose, replicas, stream, (size_t)e->batch.K * c.nRigid, [] { return 0; }, [&]() -> int {
+        k_set_collider_poses<<<dim3(1, e->batch.K), kMaxRigidColliders, 0, e->stream>>>((RigidCollider *)c.dRigid.p, (float4 *)c.dX.p, (float4 *)c.dV.p,
+                                                                                   (float4 *)c.dW.p, c.nRigid, ColliderPoses{pose, body_x, body_v, body_omega, replicas});
+        CK(cudaGetLastError());
+        return 0;
+    });
+}
+
+// ---- contact sensors -----------------------------------------------------------------------------------------------------------------
+extern "C" int pbd_sense_contacts(pbd_engine *e, int on) {
+    if (!e) return fail("pbd_sense_contacts: null engine");
+    e->sensors.on = on != 0;
+    return size_sensors(e);
+}
+static int sensors_refusal(const pbd_engine *e, const char *what) {
+    if (!e->sensors.on) return fail("%s: contact sensing is off (pbd_sense_contacts)", what);
+    if (!e->sensors.nRigid) return fail("%s: no rigid colliders in force (pbd_set_colliders / pbd_set_replica_colliders)", what);
     return 0;
+}
+extern "C" int pbd_get_contact_sensors(pbd_engine *e, unsigned *count, float *impulse) {
+    const char *what = "pbd_get_contact_sensors";
+    if (!e) return fail("%s: null engine", what);
+    CKE(sensors_refusal(e, what));
+    CKE(use(e));
+    CK(cudaStreamSynchronize(e->stream));
+    const size_t rows = (size_t)e->sensors.K * e->sensors.nRigid;
+    if (count) CK(cudaMemcpy(count, e->sensors.count.p, rows * sizeof(unsigned), cudaMemcpyDeviceToHost));
+    if (impulse) CK(cudaMemcpy(impulse, e->sensors.impulse.p, rows * 3 * sizeof(float), cudaMemcpyDeviceToHost));
+    return 0;
+}
+extern "C" int pbd_get_contact_sensors_device(pbd_engine *e, unsigned *count, float *impulse, void *stream) {
+    const char *what = "pbd_get_contact_sensors_device";
+    if (!e) return fail("%s: null engine", what);
+    CKE(sensors_refusal(e, what));
+    if (!count && !impulse) return 0;  // nothing asked for
+    CKE(body_arrays_refusal(e, what, {{"count", count}, {"impulse", impulse}}));
+    const size_t rows = (size_t)e->sensors.K * e->sensors.nRigid;
+    return device_call(e, what, count ? "count" : "impulse", count ? (const void *)count : (const void *)impulse, nullptr, stream, rows, [] { return 0; },
+                       [&]() -> int {
+        if (count) CK(cudaMemcpyAsync(count, e->sensors.count.p, rows * sizeof(unsigned), cudaMemcpyDeviceToDevice, e->stream));
+        if (impulse) CK(cudaMemcpyAsync(impulse, e->sensors.impulse.p, rows * 3 * sizeof(float), cudaMemcpyDeviceToDevice, e->stream));
+        return 0;
+    });
 }
 extern "C" int pbd_set_contact_params(pbd_engine *e, float tolerance, float stiffness, unsigned maxIterationsV) {
     if (!e) return fail("null engine");
@@ -1831,10 +1923,24 @@ static int enqueue_contacts(pbd_engine *e, cudaStream_t s, unsigned long long *l
     a.tolerance = e->contactTolerance; a.stiffness = e->contactStiffness; a.maxIterV = e->maxIterV;
     a.record = e->contactCap ? (ContactRecord *)e->dContacts.p : nullptr; a.recordCount = (unsigned *)e->dContactCount.p; a.recordCap = e->contactCap;
     if (e->contactCap) CK(cudaMemsetAsync(e->dContactCount.p, 0, sizeof(unsigned), s));
-    if (batch) k_contacts_batch<<<dim3((a.total + 127u) / 128u, e->batch.K), 128, 0, s>>>(a);
-    else k_contacts<<<(a.total + 127u) / 128u, 128, 0, s>>>(a);
+    const dim3 grid((a.total + 127u) / 128u, batch ? e->batch.K : 1u);
+    const pbd_engine::Sensors &S = e->sensors;
+    if (!S.on) {
+        if (batch) k_contacts_batch<<<grid, 128, 0, s>>>(a);
+        else k_contacts<<<grid, 128, 0, s>>>(a);
+        CK(cudaGetLastError());
+        *launches += 1;
+        return 0;
+    }
+    // sensing: the same contacts with per-block sensor sums, then their sum per collider in block order (size_sensors sized the buffers)
+    if (S.K != grid.y || S.nRigid != a.nRigid || S.blocks != grid.x) return fail("contact sensors sized for %u x %u colliders and %u blocks, the launch has %u x %u and %u", S.K, S.nRigid, S.blocks, grid.y, a.nRigid, grid.x);
+    float4 *partial = (float4 *)S.partial.p;
+    if (batch) k_contacts_sense_batch<<<grid, kSenseThreads, 0, s>>>(a, partial);
+    else k_contacts_sense<<<grid, kSenseThreads, 0, s>>>(a, partial);
+    const unsigned rows = S.K * S.nRigid;
+    k_contact_sensors_sum<<<nblk(rows, 128), 128, 0, s>>>(partial, rows, S.nRigid, S.blocks, (unsigned *)S.count.p, (float *)S.impulse.p);
     CK(cudaGetLastError());
-    *launches += 1;
+    *launches += 2;
     return 0;
 }
 

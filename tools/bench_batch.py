@@ -5,7 +5,7 @@ power limit read in the same run.  The four scenes run four different resident i
 masks).
 
     python tools/bench_batch.py [--out results.json] [--quick] [--replica-rows] [--sweep] [--rest-shapes] [--colliders] [--constraint-materials]
-                                [--rigid] [--ks 8,132] [--no-baseline]
+                                [--rigid] [--contact-sensors] [--ks 8,132] [--no-baseline]
 
 --replica-rows measures every batch twice in a row: with the shared parameters, and with per-replica material rows and gravity
 (pbd_set_replica_materials / pbd_set_replica_gravity) equal to the shared values, so that the work is identical and the difference is what
@@ -27,6 +27,10 @@ tests/rigid_batch_util.py), every replica with its own bodies (pbd_set_replica_r
 graph and in forced resident mode, against the K replicas stepped one after another by a K = 1 engine (per replica its particles and bodies
 uploaded, one step, both read back), and the cost of one masked device write of the bodies per step (pbd_set_rigid_bodies_device, half the
 replicas): the write alone, 200 enqueued back to back, and steps with a write before each against steps without, wall clock after a sync.
+--contact-sensors measures the contact path's device interface on the --colliders workloads, in graph and resident mode: steps with the
+three per-replica colliders and the contact sensors off, on, off, on (pbd_sense_contacts; device time), and 200 steps each preceded by a move
+of every replica's colliders (wall clock after a sync), the rows drawn by a torch op on the GPU: no move, the host call
+pbd_set_replica_colliders after copying the rows to the host, and the device call pbd_set_replica_collider_poses_device.
 --ks replaces the K sweep of every scene; --no-baseline skips the one-after-another baseline and the C sweep.  Without --rest-shapes or
 --replica-rows the script also runs against a build without those calls, so that shared-parameter batches can be compared across builds.
 
@@ -318,7 +322,7 @@ def gather_timing(m, k, calls=200):
     return out
 
 
-def engine(m, mode, k, clusters=None, rows=None, rest=False, colliders=False, cmat=None):
+def engine(m, mode, k, clusters=None, rows=None, rest=False, colliders=False, cmat=None, sense=False):
     if clusters:
         os.environ["PBD_B200_CLUSTERS"] = "1x%d" % clusters  # the planner's cluster-size override (read when the image is planned)
     else:
@@ -344,6 +348,7 @@ def engine(m, mode, k, clusters=None, rows=None, rest=False, colliders=False, cm
         rigid, body_x = replica_colliders(m, k)
         eng.set_replica_colliders([_capi.ParticleCollider(0, len(m["x0"]), 0.5, 0.1)], rigid, body_x)
         eng.set_contact_params(0.05, 100.0, 5)
+        eng.sense_contacts(sense)
     return eng
 
 
@@ -358,11 +363,11 @@ def timed(eng, warmup=3, min_s=0.4):
     return st.last_step_ms / steps, steps
 
 
-def measure(m, mode, k, clusters=None, rows=None, rest=False, colliders=False, cmat=None):
+def measure(m, mode, k, clusters=None, rows=None, rest=False, colliders=False, cmat=None, sense=False):
     t0 = time.time()
     eng = None
     try:
-        eng = engine(m, mode, k, clusters, rows, rest, colliders, cmat)
+        eng = engine(m, mode, k, clusters, rows, rest, colliders, cmat, sense)
         ms, steps = timed(eng)
         _, active = eng.get_mode()
     except _capi.PbdError as ex:
@@ -371,6 +376,47 @@ def measure(m, mode, k, clusters=None, rows=None, rest=False, colliders=False, c
         if eng is not None:
             eng.close()
     return {"ms": ms, "steps": steps, "active": active, "wall_s": time.time() - t0}
+
+
+def pose_write_timing(m, mode, k, steps=200):
+    """ms per step (wall clock, after a sync) of `steps` steps, each preceded by a move of every replica's colliders drawn by a torch op on the
+    GPU: {"none": rows drawn but not written, "host": rows copied to the host and written by pbd_set_replica_colliders, "device": written by
+    pbd_set_replica_collider_poses_device}."""
+    import ctypes as C
+    import torch
+    eng = engine(m, mode, k, colliders=True)
+    try:
+        rigid, body_x = replica_colliders(m, k)
+        nr = len(rigid[0])
+        ra = (_capi.RigidCollider * (k * nr))(*[c for r in rigid for c in r])
+        fields = np.frombuffer(ra, np.float32).reshape(k * nr, 30)  # the 21 placement floats are columns 9 .. 29
+        pc = (_capi.ParticleCollider * 1)(_capi.ParticleCollider(0, len(m["x0"]), 0.5, 0.1))
+        base, bx0 = torch.from_numpy(fields[:, 9:].copy()).cuda(), torch.from_numpy(body_x.reshape(-1, 3).copy()).cuda()
+        shift = torch.zeros(k * nr, 21, device="cuda")
+        s = torch.cuda.current_stream().cuda_stream
+        out = {}
+        for how in ("none", "host", "device", "none", "host", "device"):
+            for passes in range(2):  # the first pass warms up
+                torch.cuda.synchronize(); eng.sync()
+                t0 = time.perf_counter()
+                for t in range(steps):
+                    d = 1e-4 * (t % 50)
+                    pose = base + shift.fill_(d)   # stands for a policy's action: the rows are born on the GPU
+                    bx = bx0 + d
+                    if how == "host":
+                        fields[:, 9:] = pose.cpu().numpy()
+                        host_x = bx.cpu().numpy()
+                        _capi._ck(_capi.lib().pbd_set_replica_colliders(eng._h, 1, C.cast(pc, C.c_void_p), nr, C.cast(ra, C.c_void_p),
+                                                                        C.c_void_p(host_x.ctypes.data), None, None))
+                    elif how == "device":
+                        eng.set_replica_collider_poses_device(pose, bx, stream=s)
+                    eng.step(1)
+                torch.cuda.synchronize(); eng.sync()
+                ms = (time.perf_counter() - t0) * 1e3 / steps
+            out.setdefault(how, []).append(ms)
+        return out
+    finally:
+        eng.close()
 
 
 def one_after_another(m, mode, k):
@@ -406,6 +452,7 @@ def main():
     ap.add_argument("--rest-shapes", action="store_true", help="every batch also with per-replica rest shapes; device derivation against host builds")
     ap.add_argument("--colliders", action="store_true", help="only the contact path: batches without and with three per-replica colliders")
     ap.add_argument("--constraint-materials", action="store_true", help="every batch also with per-constraint materials equal to the shared ones; gather timing")
+    ap.add_argument("--contact-sensors", action="store_true", help="only the contact path: sensing off / on, and per-step collider moves by host and device calls")
     ap.add_argument("--rigid", action="store_true", help="only batches of the rigid-body coupling rig and the masked device body write")
     ap.add_argument("--ks", default=None, help="comma-separated K to measure instead of each scene's sweep")
     ap.add_argument("--no-baseline", action="store_true", help="skip the one-after-another baseline and the C sweep")
@@ -415,6 +462,27 @@ def main():
     print("card: %s" % res["card"], flush=True)
     if a.rigid:
         rigid_main(a, res)
+        if a.out:
+            os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
+            with open(a.out, "w") as f:
+                json.dump(res, f, indent=1)
+        return
+    if a.contact_sensors:
+        res["contact_sensors"], res["pose_writes"] = [], []
+        for name, ks in COLLIDER_KS.items():
+            m = model(name)
+            for k in ([int(v) for v in a.ks.split(",")] if a.ks else ks):
+                for label, md in (("graph", _capi.MODE_GRAPH), ("resident", _capi.MODE_RESIDENT)):
+                    # off, on, off, on: the spread of each pair is next to the difference between them
+                    ms = [measure(m, md, k, colliders=True, sense=bool(i & 1)).get("ms", float("nan")) for i in range(4)]
+                    extra = min(ms[1::2]) - min(ms[0::2])
+                    res["contact_sensors"].append({"scene": name, "K": k, "mode": label, "off_ms": ms[0::2], "on_ms": ms[1::2], "sensing_ms": extra})
+                    print("  sensors %-13s K=%5d %-8s off %.4f %.4f ms | on %.4f %.4f ms | sensing %+.4f ms (%+.1f %%)"
+                          % (name, k, label, ms[0], ms[2], ms[1], ms[3], extra, 100.0 * extra / min(ms[0::2])), flush=True)
+                    w = pose_write_timing(m, md, k)
+                    res["pose_writes"].append({"scene": name, "K": k, "mode": label, **{h + "_ms": v for h, v in w.items()}})
+                    print("  pose writes %-13s K=%5d %-8s per step: no move %.4f %.4f ms | host call %.4f %.4f ms | device call %.4f %.4f ms"
+                          % (name, k, label, *w["none"], *w["host"], *w["device"]), flush=True)
         if a.out:
             os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
             with open(a.out, "w") as f:

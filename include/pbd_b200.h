@@ -180,7 +180,9 @@ int pbd_set_masses_device(pbd_engine *e, const float *mass, const unsigned char 
  * A collider on a rigid body with mass != 0 is refused (its contacts couple through the body and are inherently sequential);
  * rigid-rigid and particle-tet contacts are not covered -- such models stay on the reference's CPU time step.
  *   pbd_particle_collider: one DistanceFieldCollisionObjectWithoutGeometry (particles [offset, offset+count) of a model, the
- *                          model's restitution / friction coefficients);
+ *                          model's restitution / friction coefficients).  The ranges of one call must not overlap: a particle
+ *                          belongs to at most one range (empty ranges overlap nothing), and both collider calls refuse
+ *                          overlapping ranges, with the colliders of the previous call left in force;
  *   pbd_rigid_collider:    one DistanceFieldCollision{Box,Sphere,Torus,Cylinder,HollowSphere,HollowBox} in the order of
  *                          CollisionDetection::getCollisionObjects(): `dim` = m_box (half extents) | m_radius | m_radii | m_dim
  *                          (radius, half height), m_thickness, m_invertSDF, the body's coefficients, RigidBody::getTransformationR

@@ -1714,14 +1714,25 @@ static int convert_collider(const char *what, unsigned i, const pbd_rigid_collid
     for (int k = 0; k < 9; k++) d.R[k] = c.R[k];
     return 0;
 }
-// one replica's particle ranges and the prefix sums of their counts; refused: a range beyond the engine's n particles
+// one replica's particle ranges and the prefix sums of their counts; refused: a range beyond the engine's n particles, and two ranges
+// that share a particle (the contact kernel runs one thread per range entry: two threads would solve the same particle and one store
+// would be lost)
 static int convert_ranges(const pbd_engine *e, const char *what, unsigned nP, const pbd_particle_collider *pc, std::vector<ParticleCollider> &P,
                           std::vector<unsigned> &start) {
     P.resize(nP); start.assign(nP + 1, 0u);
+    std::vector<unsigned> byOffset;
     for (unsigned i = 0; i < nP; i++) {
         if ((unsigned long long)pc[i].offset + pc[i].count > e->n) return fail("%s: particle collider %u covers [%u, %u), the engine holds %u particles", what, i, pc[i].offset, pc[i].offset + pc[i].count, e->n);
         P[i].offset = pc[i].offset; P[i].count = pc[i].count; P[i].restitution = pc[i].restitution; P[i].friction = pc[i].friction;
         start[i + 1] = start[i] + pc[i].count;
+        if (pc[i].count) byOffset.push_back(i);
+    }
+    std::sort(byOffset.begin(), byOffset.end(), [&](unsigned a, unsigned b) { return pc[a].offset < pc[b].offset; });
+    for (size_t j = 1; j < byOffset.size(); j++) {
+        const pbd_particle_collider &a = pc[byOffset[j - 1]], &b = pc[byOffset[j]];
+        if (b.offset < a.offset + a.count)
+            return fail("%s: particle colliders %u [%u, %u) and %u [%u, %u) overlap (each particle may belong to one range only)", what, byOffset[j - 1],
+                        a.offset, a.offset + a.count, byOffset[j], b.offset, b.offset + b.count);
     }
     return 0;
 }

@@ -672,6 +672,21 @@ int preferred_mode(int requested, const TypeStore *store, unsigned n, unsigned n
     return replicas >= (clothFem ? 1u : 2u) * kAutoResidentMinReplicas ? PBD_MODE_RESIDENT : PBD_MODE_GRAPH;
 }
 
+// The resident batch kernels address replica r's per-replica rest geometry and per-constraint materials of type t as the element
+// offset r x count + i in 32 bits (resident.cuh: run_items / prefetch_first, load_streamed's geoOff, project_streamed_acc's matOff; kept
+// narrow for the registers, DESIGN.md section 3), where the per-bucket kernels move a pointer by a size_t offset.  A batch whose tables
+// carry either override (PlanInput::restTables) therefore needs K x count < 2^32 for every particle type, else the resident mode would
+// read another replica's rows.  The calls that switch the overrides on refuse such a batch, but constraints added afterwards grow the
+// counts of a batch that is planned again; this keeps that batch out of the resident mode (AUTO: graph).
+static std::string replica_offset_refusal(const PlanInput &in) {
+    if (in.replicas < 2 || !in.restTables) return "";
+    for (int t = 0; t < PBD_BALLJOINT; t++)
+        if ((unsigned long long)in.replicas * in.store[t].ids.size() >= (1ull << 32))
+            return fmt("resident mode: %u replicas of %zu constraints of type %d with per-replica rest shapes or materials exceed the "
+                       "2^32 rows the resident kernel addresses (use PBD_MODE_GRAPH)", in.replicas, in.store[t].ids.size(), t);
+    return "";
+}
+
 // the image of the resident mode (tiled) or of the others
 static std::string plan_mode(const PlanInput &in, bool tiled, ImagePlan &out) {
     Lap lap;
@@ -681,6 +696,7 @@ static std::string plan_mode(const PlanInput &in, bool tiled, ImagePlan &out) {
     if (!err.empty()) return err;
     Ctx c{in, out, tiled, {}, {}};
     if (tiled) {
+        if (!(err = replica_offset_refusal(in)).empty()) return err;
         if (!(err = place_in_tiles(c)).empty()) return err;
     } else {
         out.slot.resize(in.n);

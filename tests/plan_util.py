@@ -266,10 +266,15 @@ def check_plan(sc, p, tiled):
 def item_kinds(sc, p):
     """(X items, shared-memory items whose particles live in another CTA of the cluster (DSMEM), shared-memory items of the executing
     CTA's own tile) of a resident plan."""
+    return tuple(int(v) for v in np.sum(list(item_kinds_by_type(sc, p).values()) or [(0, 0, 0)], axis=0))
+
+
+def item_kinds_by_type(sc, p):
+    """item_kinds of every type the scene has: {type: (X items, DSMEM items, own-tile items)}."""
     G, C = (int(v) for v in u32(p, "res")[:2])
     buckets = np.frombuffer(p["buckets"], np.int32).reshape(-1, 4)
     tile_off = u32(p, "tileOff").astype(np.int64).reshape(len(buckets), 2 * G * C + 1)
-    nx = ndsmem = nlocal = 0
+    kinds = {}
     for t in range(NUM_TYPES):
         cnt = len(sc.store[t][0])
         if not cnt:
@@ -285,5 +290,5 @@ def item_kinds(sc, p):
         for k in pk:
             v = idx[:, k]
             remote |= ((v & SMEM_FLAG) != 0) & (((v >> RANK_SHIFT) & 15) != ex % C)
-        nx += int(isx.sum()); ndsmem += int((~isx & remote).sum()); nlocal += int((~isx & ~remote).sum())
-    return nx, ndsmem, nlocal
+        kinds[t] = (int(isx.sum()), int((~isx & remote).sum()), int((~isx & ~remote).sum()))
+    return kinds

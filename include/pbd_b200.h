@@ -170,6 +170,21 @@ int pbd_set_attr_device(pbd_engine *e, int attr, const float *src, const unsigne
 int pbd_get_attr_device(pbd_engine *e, int attr, float *dst, void *stream);
 int pbd_set_masses_device(pbd_engine *e, const float *mass, const unsigned char *replicas, void *stream);
 
+/* External forces on the particles (wind, drag, a pointer pulling a vertex, an action given as a force).  f: K*n*3 floats (N, world frame)
+ * in the layout of pbd_set_attr, replica after replica.  In every substep of every step a particle with mass integrates with the
+ * acceleration a = g + f * w, g its replica's gravity (pbd_set_params or pbd_set_replica_gravity), w its inverse mass when it is integrated:
+ * a later pbd_set_masses[_device] changes the acceleration, not the force.  A particle with mass 0 ignores its force.  A force stays until
+ * it is replaced or cleared, the same in every substep.  Zero forces step to the same bits as no forces.
+ * pbd_set_external_forces: from host memory; synchronises.  f = NULL clears every force, and the steps run without the force read again.
+ * pbd_set_external_forces_device: from device memory, with the stream contract, mask and refusals of pbd_set_attr_device.  The first set
+ * after the forces were cleared zeroes the replicas the mask leaves out.
+ * Both write a device table that keeps its address while n and K stand, so a new force between two steps neither plans the image again
+ * nor captures the step graph again; setting or clearing forces captures it once.  Adding constraints keeps the forces (they move with
+ * the particles); pbd_set_particles and pbd_set_replicas clear them.  bytes_per_step counts 16 more bytes per particle and substep while
+ * forces are set. */
+int pbd_set_external_forces(pbd_engine *e, const float *f);
+int pbd_set_external_forces_device(pbd_engine *e, const float *f, const unsigned char *replicas, void *stream);
+
 /* ---- Contact path (SURVEY.md section 8 row f-4, its data-parallel part) ----------------------------------------------------
  * Particles of triangle / tet models against analytic distance fields carried by STATIC rigid bodies, and the velocity-level
  * contact solve: DistanceFieldCollisionDetection::collisionDetection + collisionDetectionRBSolid

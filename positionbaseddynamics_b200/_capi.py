@@ -28,7 +28,7 @@ SYMBOLS = ["pbd_last_error", "pbd_device_count", "pbd_create", "pbd_destroy", "p
            "pbd_num_materials", "pbd_set_replica_materials", "pbd_set_replica_gravity",
            "pbd_set_replica_rest_positions", "pbd_get_replica_geometry",
            "pbd_set_colliders", "pbd_set_contact_params", "pbd_record_contacts", "pbd_get_contacts", "pbd_set_replica_colliders",
-           "pbd_set_attr_device", "pbd_get_attr_device", "pbd_set_masses_device",
+           "pbd_set_attr_device", "pbd_get_attr_device", "pbd_set_masses_device", "pbd_set_external_forces", "pbd_set_external_forces_device",
            "pbd_set_replica_constraint_materials", "pbd_set_replica_constraint_materials_device", "pbd_get_replica_materials",
            "pbd_set_replica_rigid_bodies", "pbd_set_rigid_bodies_device", "pbd_get_rigid_bodies_device",
            "pbd_set_replica_collider_poses_device", "pbd_sense_contacts", "pbd_get_contact_sensors", "pbd_get_contact_sensors_device"]
@@ -116,6 +116,8 @@ def lib():
         _lib.pbd_set_attr_device.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
         _lib.pbd_get_attr_device.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
         _lib.pbd_set_masses_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        _lib.pbd_set_external_forces.argtypes = [C.c_void_p, C.c_void_p]
+        _lib.pbd_set_external_forces_device.argtypes = [C.c_void_p] * 4
         _lib.pbd_set_replica_constraint_materials.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         _lib.pbd_set_replica_constraint_materials_device.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
         _lib.pbd_get_replica_materials.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
@@ -298,6 +300,36 @@ class Engine:
         mask = self._mask("set_masses_device", replicas)
         if self.K * self.n:
             _ck(lib().pbd_set_masses_device(self._h, C.c_void_p(p), mask, _stream(stream)))
+
+    # external forces -------------------------------------------------------------------------------
+    # Particle i of replica r integrates with a = g_r + f[r, i] * w (w its inverse mass at that time) in every substep until the forces are
+    # replaced or cleared; a particle with mass 0 ignores its force.  set_particles and set_replicas clear them.
+    def set_external_forces(self, f):
+        """pbd_set_external_forces: f, a float32 numpy array (K, n, 3) -- (n, 3) at K = 1 -- C-contiguous, in newtons; None clears every
+        force.  Nothing is converted: a copy in another type or order would hide a caller's mistake in the layout."""
+        if f is not None:
+            if not isinstance(f, np.ndarray):
+                raise TypeError("set_external_forces: wants a numpy array, got %s (device arrays go through set_external_forces_device)"
+                                % type(f).__name__)
+            if f.dtype != np.float32:
+                raise ValueError("set_external_forces: element type %s, wants float32" % f.dtype)
+            if f.shape != self._batch_shape(3):
+                raise ValueError("set_external_forces: shape %s, wants %s" % (f.shape, self._batch_shape(3)))
+            if not f.flags.c_contiguous:
+                raise ValueError("set_external_forces: not C-contiguous")
+            if not f.size:
+                return
+        _ck(lib().pbd_set_external_forces(self._h, _ptr(f)))
+
+    def set_external_forces_device(self, f, replicas=None, stream=None):
+        """pbd_set_external_forces_device: the forces of the replicas in `replicas` from f (K*n*3 floats, the layout of
+        set_external_forces); stream and replicas as in set_attr_device.  Replicas left out keep their forces (zero after a clear)."""
+        if f is None:
+            raise TypeError("set_external_forces_device: f is None; forces are cleared with set_external_forces(None)")
+        p = _device_ptr("set_external_forces_device: f", f, ("<f4",), self.K * self.n * 3)
+        mask = self._mask("set_external_forces_device", replicas)
+        if self.K * self.n:
+            _ck(lib().pbd_set_external_forces_device(self._h, C.c_void_p(p), mask, _stream(stream)))
 
     # replica batch ---------------------------------------------------------------------------------
     def set_replicas(self, k):

@@ -96,6 +96,10 @@ struct pbd_engine {
     // masses in stage[0]); stage[1] only for pbd_step_host, so that its x and v uploads do not wait on each other.
     unsigned n = 0;
     DevBuf attr[kNumAttrs], stage[2], jacobiDelta;
+    // external forces (pbd_set_external_forces): K x n float4 in slot order like the particle arrays (.w unused), null while none is set.
+    // Not an attribute: it keeps its address while n and K stand, is moved by relayout with them, and is released by pbd_set_particles and
+    // pbd_set_replicas.
+    DevBuf force;
     // A replica batch and what its replicas have of their own (batch_arrays, replica_mat and replica_geo turn it into what the kernels see).
     // mat [K][kMatRowFloats]: the uniform material parameters of every type, replica by replica -- the shared ones of the image, or a
     // replica's own (pbd_set_replica_materials, the types of matMask); gravity [K][3] (pbd_set_replica_gravity).
@@ -278,7 +282,7 @@ static int upload_slot_map(pbd_engine *e) {
     CK(cudaMemcpy(e->dSlot.p, e->slot.data(), (size_t)e->n * sizeof(unsigned), cudaMemcpyHostToDevice));
     return 0;
 }
-// move every particle array from the current slot map to `newSlot`
+// move every particle array, and the external forces if any are set, from the current slot map to `newSlot`
 static int relayout(pbd_engine *e, const std::vector<unsigned> &newSlot) {
     if (e->n == 0 || newSlot == e->slot) { e->slot = newSlot; return 0; }
     const size_t nb = (size_t)e->n * sizeof(unsigned);
@@ -287,11 +291,14 @@ static int relayout(pbd_engine *e, const std::vector<unsigned> &newSlot) {
     e->slot = newSlot;
     CKE(upload_slot_map(e));
     CKE(e->relayoutTmp.alloc((size_t)e->batch.K * e->n * sizeof(float4)));
-    for (DevBuf &b : e->attr) {
-        k_relayout<<<dim3((e->n + 255) / 256, e->batch.K), 256, 0, e->stream>>>((const float4 *)b.p, (float4 *)e->relayoutTmp.p, e->n, (const unsigned *)e->dSlotOld.p, (const unsigned *)e->dSlot.p);
+    std::vector<DevBuf *> moved;
+    for (DevBuf &b : e->attr) moved.push_back(&b);
+    if (e->force.p) moved.push_back(&e->force);
+    for (DevBuf *b : moved) {
+        k_relayout<<<dim3((e->n + 255) / 256, e->batch.K), 256, 0, e->stream>>>((const float4 *)b->p, (float4 *)e->relayoutTmp.p, e->n, (const unsigned *)e->dSlotOld.p, (const unsigned *)e->dSlot.p);
         CK(cudaGetLastError());
         CK(cudaStreamSynchronize(e->stream));
-        std::swap(b.p, e->relayoutTmp.p); std::swap(b.bytes, e->relayoutTmp.bytes);
+        std::swap(b->p, e->relayoutTmp.p); std::swap(b->bytes, e->relayoutTmp.bytes);
     }
     return 0;
 }
@@ -409,6 +416,7 @@ extern "C" int pbd_set_particles(pbd_engine *e, unsigned n, const float *x, cons
     e->n = n; model_changed(e);  // and the formula slot map below
     CKE(size_particles(e, e->batch.K, false));
     drop_replica_geometry(e);  // every replica's state is redefined
+    e->force.release();        // forces of the old particles
     e->slot.resize(n);
     for (unsigned i = 0; i < n; i++) e->slot[i] = particle_slot(i, n);
     if (n == 0) return 0;
@@ -478,6 +486,7 @@ extern "C" int pbd_set_replicas(pbd_engine *e, unsigned K) {
     e->batch.K = K;
     CKE(drop_constraint_materials(e, ~0u));
     e->batch.mat.release(); e->batch.gravity.release(); e->batch.matMask = 0; e->batch.gravitySet = false;  // rows of the old K
+    e->force.release();  // likewise
     drop_replica_geometry(e);
     drop_replica_colliders(e);
     CKE(size_sensors(e));  // sensing stays on; the one scene's colliders, if any, keep their sensors
@@ -630,6 +639,40 @@ extern "C" int pbd_get_attr_device(pbd_engine *e, int attr, float *dst, void *st
 extern "C" int pbd_set_masses_device(pbd_engine *e, const float *mass, const unsigned char *replicas, void *stream) {
     if (!e) return fail("pbd_set_masses_device: null engine");
     return device_call(e, "pbd_set_masses_device", "mass", mass, replicas, stream, [&] { return pack_w(e, mass, e->batch.K, replicas); });
+}
+
+// ---- external forces (pbd_set_external_forces, pbd_set_external_forces_device) ----------------------------------------------------------
+// The table is allocated and zeroed by the first set of the current n and K, so replicas a masked set leaves out have zero force; later
+// sets write it in place (k_pack3 through the slot map, .w = 0), so its address -- what a captured step reads -- stays.
+static int ensure_forces(pbd_engine *e) {
+    if (e->force.p) return 0;
+    CKE(e->force.alloc((size_t)e->batch.K * e->n * sizeof(float4)));
+    CK(cudaMemsetAsync(e->force.p, 0, e->force.bytes, e->stream));
+    return 0;
+}
+static int pack_forces(pbd_engine *e, const float *f, const unsigned char *mask) {
+    k_pack3<<<replica_grid(e, e->batch.K), 256, 0, e->stream>>>(f, (float4 *)e->force.p, e->n, 0, (const unsigned *)e->dSlot.p, mask);
+    CK(cudaGetLastError());
+    return 0;
+}
+extern "C" int pbd_set_external_forces(pbd_engine *e, const float *f) {
+    if (!e) return fail("pbd_set_external_forces: null engine");
+    CKE(use(e));
+    if (!f) {  // cleared: the steps go back to the integration without forces
+        if (e->force.p) { CK(cudaStreamSynchronize(e->stream)); e->force.release(); }
+        return 0;
+    }
+    if (e->n == 0) return 0;
+    CKE(ensure_forces(e));
+    CK(cudaMemcpyAsync(e->stage[0].p, f, (size_t)e->batch.K * e->n * 3 * sizeof(float), cudaMemcpyHostToDevice, e->stream));
+    CKE(pack_forces(e, (const float *)e->stage[0].p, nullptr));
+    CK(cudaStreamSynchronize(e->stream));  // staging buffers are reused by the next call
+    return 0;
+}
+extern "C" int pbd_set_external_forces_device(pbd_engine *e, const float *f, const unsigned char *replicas, void *stream) {
+    if (!e) return fail("pbd_set_external_forces_device: null engine");
+    return device_call(e, "pbd_set_external_forces_device", "f", f, replicas, stream, e->n, [&] { return ensure_forces(e); },
+                       [&] { return pack_forces(e, f, replicas); });
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -1559,6 +1602,7 @@ static int enqueue_step_launches(pbd_engine *e, cudaStream_t s, unsigned long lo
     const bool pdl = !log;
     const RbState rb = rb_state(e);
     float4 *x = attr_ptr(e, PBD_ATTR_X), *v = attr_ptr(e, PBD_ATTR_V), *oldX = attr_ptr(e, PBD_ATTR_OLDX), *lastX = attr_ptr(e, PBD_ATTR_LASTX);
+    const float4 *force = (const float4 *)e->force.p;  // the integration's force form only while forces are set
     unsigned long long L = 0;
     auto launched = [&](int kind) { L++; return log ? log->mark(s, kind) : 0; };
     for (unsigned sub = 0; sub < e->subSteps; sub++) {
@@ -1570,9 +1614,15 @@ static int enqueue_step_launches(pbd_engine *e, cudaStream_t s, unsigned long lo
             CKE(launched(kLaunchIntegrate));
         }
         if (n) {
-            if (e->batch.gravitySet)  // replica blockIdx.y under its own row
+            if (e->batch.gravitySet && force)  // replica blockIdx.y under its own row
+                CK(launch_step_kernel(k_integrate_force<true>, replica_grid(e, e->batch.K), 256, s, pdl, x, v, oldX, lastX, e->n, h, 0.0f, 0.0f, 0.0f,
+                                      (const float *)e->batch.gravity.p, force));
+            else if (e->batch.gravitySet)
                 CK(launch_step_kernel(k_integrate<true>, replica_grid(e, e->batch.K), 256, s, pdl, x, v, oldX, lastX, e->n, h, 0.0f, 0.0f, 0.0f,
                                       (const float *)e->batch.gravity.p));
+            else if (force)
+                CK(launch_step_kernel(k_integrate_force<false>, nblk(n, 256), 256, s, pdl, x, v, oldX, lastX, n, h, e->g[0], e->g[1], e->g[2],
+                                      (const float *)nullptr, force));
             else
                 CK(launch_step_kernel(k_integrate<false>, nblk(n, 256), 256, s, pdl, x, v, oldX, lastX, n, h, e->g[0], e->g[1], e->g[2],
                                       (const float *)nullptr));
@@ -1628,6 +1678,7 @@ static int enqueue_step_resident(pbd_engine *e, cudaStream_t s, unsigned long lo
     for (int t = 0; t < PBD_NUM_TYPES; t++) { ra.types[t] = batch_arrays(e, t); ra.lamCount[t] = e->dev[t].count; ra.geoCount[t] = replica_geo(e, t); ra.matCount[t] = replica_cmat(e, t); }
     ra.replicas = e->res.replicas; ra.replicaStride = e->n;
     ra.repMat = (const float *)e->batch.mat.p; ra.repGravity = e->batch.gravitySet ? (const float *)e->batch.gravity.p : nullptr;
+    ra.force = (const float4 *)e->force.p;
     *launches = 1;
     ra.trace = nullptr; ra.tracePhases = 0;
     static const char *tracePath = getenv("PBD_B200_TRACE");  // development aid: dump per-phase timelines of one step (tools/trace_resident.py)
@@ -1680,7 +1731,9 @@ static int enqueue_step_jacobi(pbd_engine *e, cudaStream_t s, unsigned long long
     float4 *delta = (float4 *)e->jacobiDelta.p;
     unsigned long long L = 0;
     for (unsigned sub = 0; sub < e->subSteps; sub++) {
-        k_integrate<false><<<nblk(n, 256), 256, 0, s>>>(x, v, oldX, lastX, n, h, e->g[0], e->g[1], e->g[2], nullptr); L++;
+        if (e->force.p) k_integrate_force<false><<<nblk(n, 256), 256, 0, s>>>(x, v, oldX, lastX, n, h, e->g[0], e->g[1], e->g[2], nullptr, (const float4 *)e->force.p);
+        else k_integrate<false><<<nblk(n, 256), 256, 0, s>>>(x, v, oldX, lastX, n, h, e->g[0], e->g[1], e->g[2], nullptr);
+        L++;
         for (unsigned it = 0; it < e->maxIter; it++) {
             for (int t = 0; t < PBD_BALLJOINT; t++) {
                 const unsigned cnt = e->dev[t].count;
@@ -1963,7 +2016,7 @@ static std::vector<unsigned char> graph_key(const pbd_engine *e) {
     const auto [X, Q, V, W, oldX, lastX, oldQ, lastQ, I, Iinv, nRb] = rb_state(e);
     append_bytes(key, e->imageGen, e->n, e->batch.K, e->dt, e->subSteps, e->maxIter, e->velMethod, e->g,
                  attr_ptr(e, PBD_ATTR_X), attr_ptr(e, PBD_ATTR_V), attr_ptr(e, PBD_ATTR_OLDX), attr_ptr(e, PBD_ATTR_LASTX),
-                 e->batch.gravitySet ? e->batch.gravity.p : nullptr, X, Q, V, W, oldX, lastX, oldQ, lastQ, I, Iinv, nRb);
+                 e->batch.gravitySet ? e->batch.gravity.p : nullptr, e->force.p, X, Q, V, W, oldX, lastX, oldQ, lastQ, I, Iinv, nRb);
     for (int t = 0; t < PBD_NUM_TYPES; t++) {
         const auto [idx2, idx4, idx3, gv, gs, mat, matU, lambda, rbX, rbQ, rbIinv, variant] = batch_arrays(e, t);
         append_bytes(key, idx2, idx4, idx3, gv, gs, mat, matU, lambda, rbX, rbQ, rbIinv, variant, replica_mat(e, t), replica_geo(e, t), replica_cmat(e, t),
@@ -2117,8 +2170,9 @@ extern "C" int pbd_get_stats(pbd_engine *e, pbd_stats *out) {
     CKE(use(e)); CKE(flatten(e));
     double sweep = 0.0;
     for (int t = 0; t < PBD_NUM_TYPES; t++) sweep += (double)e->dev[t].count * algorithmic_bytes(t, e->dev[t].arrays.variant);
-    // per particle per substep: integrate 48 read + 64 write = 112, velocity update 32 read + 16 write = 48 (SURVEY.md 8d)
-    const double perParticle = 112.0 + 48.0 + (e->velMethod ? 16.0 : 0.0);
+    // per particle per substep: integrate 48 read + 64 write = 112, velocity update 32 read + 16 write = 48 (SURVEY.md 8d); the force
+    // read while external forces are set, 16
+    const double perParticle = 112.0 + 48.0 + (e->velMethod ? 16.0 : 0.0) + (e->force.p ? 16.0 : 0.0);
     e->stats.bytes_per_step = (sweep * e->maxIter + (double)e->n * perParticle) * e->subSteps * e->batch.K;
     *out = e->stats;
     return 0;

@@ -341,12 +341,18 @@ __device__ __forceinline__ void velocity_update(float4 &v, const float4 &x, cons
     }
 }
 
-// lastX = oldX; oldX = x; if (mass != 0) { v += g h; x += v h }
+// The acceleration of a particle with an external force (pbd_set_external_forces): a = g + f w per component, w = the particle's inverse
+// mass (x.w) at integration time.  Every mode integrates through this one function, so they agree bit for bit; f = 0 gives exactly g.
+__device__ __forceinline__ void external_acceleration(float &gx, float &gy, float &gz, const float4 &f, float w) {
+    gx = fmaf(f.x, w, gx); gy = fmaf(f.y, w, gy); gz = fmaf(f.z, w, gz);
+}
+
+// lastX = oldX; oldX = x; if (mass != 0) { v += a h; x += v h }, a = g (+ f w with FORCE: `force` at the particle's slot)
 // BATCH: the n particles of replica blockIdx.y under that replica's row of `replicaG` (pbd_set_replica_gravity)
-template <bool BATCH>
-__global__ void __launch_bounds__(256) k_integrate(float4 *__restrict__ pos, float4 *__restrict__ vel,
-                                                   float4 *__restrict__ oldp, float4 *__restrict__ lastp, unsigned n,
-                                                   float h, float gx, float gy, float gz, const float *__restrict__ replicaG) {
+template <bool BATCH, bool FORCE>
+__device__ __forceinline__ void integrate_slot(float4 *__restrict__ pos, float4 *__restrict__ vel, float4 *__restrict__ oldp,
+                                               float4 *__restrict__ lastp, unsigned n, float h, float gx, float gy, float gz,
+                                               const float *__restrict__ replicaG, const float4 *__restrict__ force) {
     pdl_launch_dependents();
     unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -360,10 +366,25 @@ __global__ void __launch_bounds__(256) k_integrate(float4 *__restrict__ pos, flo
     __stcg(oldp + i, x);
     float4 v = __ldcs(vel + i);
     if (v.w != 0.0f) {  // v.w carries the mass (TimeIntegration.cpp:14 tests mass != 0)
+        if (FORCE) external_acceleration(gx, gy, gz, __ldcs(force + i), x.w);
         semi_implicit_euler(x, v, h, gx, gy, gz);
         __stcs(vel + i, v);
         __stcg(pos + i, x);
     }
+}
+template <bool BATCH>
+__global__ void __launch_bounds__(256) k_integrate(float4 *__restrict__ pos, float4 *__restrict__ vel,
+                                                   float4 *__restrict__ oldp, float4 *__restrict__ lastp, unsigned n,
+                                                   float h, float gx, float gy, float gz, const float *__restrict__ replicaG) {
+    integrate_slot<BATCH, false>(pos, vel, oldp, lastp, n, h, gx, gy, gz, replicaG, nullptr);
+}
+// k_integrate with every particle's external force (K x n float4 in slot order, .w unused); launched only while forces are set
+template <bool BATCH>
+__global__ void __launch_bounds__(256) k_integrate_force(float4 *__restrict__ pos, float4 *__restrict__ vel,
+                                                         float4 *__restrict__ oldp, float4 *__restrict__ lastp, unsigned n,
+                                                         float h, float gx, float gy, float gz, const float *__restrict__ replicaG,
+                                                         const float4 *__restrict__ force) {
+    integrate_slot<BATCH, true>(pos, vel, oldp, lastp, n, h, gx, gy, gz, replicaG, force);
 }
 
 // Rigid-body prologue / epilogue (a handful of bodies: one thread each).

@@ -83,6 +83,8 @@ struct ResidentArgs {
     unsigned geoCount[PBD_NUM_TYPES];
     // per-constraint materials of every replica (pbd_set_replica_constraint_materials): replica r's of type t at r x matCount[t] (0: shared)
     unsigned matCount[PBD_NUM_TYPES];
+    // external forces (pbd_set_external_forces): K x n float4 in slot order, read at integration only; null while none is set
+    const float4 *force;
 };
 
 // ---- cluster primitives --------------------------------------------------------------------------------------------------
@@ -284,12 +286,14 @@ __device__ __forceinline__ void run_items(const ResidentArgs &A, const Acc &acc,
         })
 }
 
-// semi-implicit Euler of one particle whose position is `x` (TimeStepController.cpp:112-118, TimeIntegration.cpp:7-19)
+// semi-implicit Euler of one particle whose position is `x` (TimeStepController.cpp:112-118, TimeIntegration.cpp:7-19), with its external
+// force at `slot` while forces are set (the substep prologue is the only place that tests A.force)
 __device__ __forceinline__ bool integrate_particle(const ResidentArgs &A, unsigned slot, float4 &x, float gx, float gy, float gz) {
     __stcs(A.lastp + slot, __ldcs(A.oldp + slot));
     __stcs(A.oldp + slot, x);
     float4 v = __ldcs(A.vel + slot);
     if (v.w == 0.0f) return false;  // v.w carries the mass
+    if (A.force) external_acceleration(gx, gy, gz, __ldcs(A.force + slot), x.w);
     semi_implicit_euler(x, v, A.h, gx, gy, gz);
     __stcs(A.vel + slot, v);
     return true;

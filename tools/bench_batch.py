@@ -5,7 +5,7 @@ power limit read in the same run.  The four scenes run four different resident i
 masks).
 
     python tools/bench_batch.py [--out results.json] [--quick] [--replica-rows] [--sweep] [--rest-shapes] [--colliders] [--constraint-materials]
-                                [--rigid] [--contact-sensors] [--ks 8,132] [--no-baseline]
+                                [--rigid] [--contact-sensors] [--forces] [--ks 8,132] [--no-baseline]
 
 --replica-rows measures every batch twice in a row: with the shared parameters, and with per-replica material rows and gravity
 (pbd_set_replica_materials / pbd_set_replica_gravity) equal to the shared values, so that the work is identical and the difference is what
@@ -31,6 +31,10 @@ replicas): the write alone, 200 enqueued back to back, and steps with a write be
 three per-replica colliders and the contact sensors off, on, off, on (pbd_sense_contacts; device time), and 200 steps each preceded by a move
 of every replica's colliders (wall clock after a sync), the rows drawn by a torch op on the GPU: no move, the host call
 pbd_set_replica_colliders after copying the rows to the host, and the device call pbd_set_replica_collider_poses_device.
+--forces measures external forces (pbd_set_external_forces) on the cfg2 single scene, cfg1 at K = 132 and 1056 and the 100x100 XPBD cloth
+at K = 264, in graph and resident mode: steps with forces off, on, off, on, the forces all zero so that the work is identical but the force
+read (device time), and, on the batches, 200 steps each preceded by a write of every particle's force drawn by a torch op on the GPU (wall
+clock after a sync): no write, the host call after copying the forces to the host, and the device call pbd_set_external_forces_device.
 --ks replaces the K sweep of every scene; --no-baseline skips the one-after-another baseline and the C sweep.  Without --rest-shapes or
 --replica-rows the script also runs against a build without those calls, so that shared-parameter batches can be compared across builds.
 
@@ -162,8 +166,8 @@ def card():
         return "unknown (%s)" % ex
 
 
-def model(name):
-    build, sub, it, _ = SCENES[name]
+def model(name, table=SCENES):
+    build, sub, it, _ = table[name]
     hm = HostModel()
     build(hm)
     hm.init_groups()
@@ -322,7 +326,7 @@ def gather_timing(m, k, calls=200):
     return out
 
 
-def engine(m, mode, k, clusters=None, rows=None, rest=False, colliders=False, cmat=None, sense=False):
+def engine(m, mode, k, clusters=None, rows=None, rest=False, colliders=False, cmat=None, sense=False, forces=False):
     if clusters:
         os.environ["PBD_B200_CLUSTERS"] = "1x%d" % clusters  # the planner's cluster-size override (read when the image is planned)
     else:
@@ -349,6 +353,8 @@ def engine(m, mode, k, clusters=None, rows=None, rest=False, colliders=False, cm
         eng.set_replica_colliders([_capi.ParticleCollider(0, len(m["x0"]), 0.5, 0.1)], rigid, body_x)
         eng.set_contact_params(0.05, 100.0, 5)
         eng.sense_contacts(sense)
+    if forces:  # zero forces: the same answer as none, through the integration's force form
+        eng.set_external_forces(np.zeros(((k,) if k > 1 else ()) + (len(m["x0"]), 3), np.float32))
     return eng
 
 
@@ -363,11 +369,11 @@ def timed(eng, warmup=3, min_s=0.4):
     return st.last_step_ms / steps, steps
 
 
-def measure(m, mode, k, clusters=None, rows=None, rest=False, colliders=False, cmat=None, sense=False):
+def measure(m, mode, k, clusters=None, rows=None, rest=False, colliders=False, cmat=None, sense=False, forces=False):
     t0 = time.time()
     eng = None
     try:
-        eng = engine(m, mode, k, clusters, rows, rest, colliders, cmat, sense)
+        eng = engine(m, mode, k, clusters, rows, rest, colliders, cmat, sense, forces)
         ms, steps = timed(eng)
         _, active = eng.get_mode()
     except _capi.PbdError as ex:
@@ -419,6 +425,59 @@ def pose_write_timing(m, mode, k, steps=200):
         eng.close()
 
 
+# --forces: (scene, K) rows; cfg2 is the single-scene flagship (bench.py)
+FORCE_SCENES = dict(SCENES, cfg2=(lambda m: scenes.cfg2(m), 1, 20, [1]))
+FORCE_ROWS = [("cfg2", 1), ("cfg1", 132), ("cfg1", 1056), ("cloth100_xpbd", 264)]
+
+
+def force_write_timing(m, mode, k, steps=200):
+    """ms per step (wall clock, after a sync) of `steps` steps, each preceded by a write of every particle's force drawn by a torch op on the
+    GPU: {"none": forces drawn but not written, "host": copied to the host and written by pbd_set_external_forces, "device": written by
+    pbd_set_external_forces_device}."""
+    import torch
+    eng = engine(m, mode, k, forces=True)
+    try:
+        shape = ((k,) if k > 1 else ()) + (len(m["x0"]), 3)
+        base = torch.zeros(shape, device="cuda")
+        s = torch.cuda.current_stream().cuda_stream
+        out = {}
+        for how in ("none", "host", "device", "none", "host", "device"):
+            for passes in range(2):  # the first pass warms up
+                torch.cuda.synchronize(); eng.sync()
+                t0 = time.perf_counter()
+                for t in range(steps):
+                    f = base + 1e-3 * (t % 50)  # stands for a policy's action: the forces are born on the GPU
+                    if how == "host":
+                        eng.set_external_forces(f.cpu().numpy())
+                    elif how == "device":
+                        eng.set_external_forces_device(f, stream=s)
+                    eng.step(1)
+                torch.cuda.synchronize(); eng.sync()
+                ms = (time.perf_counter() - t0) * 1e3 / steps
+            out.setdefault(how, []).append(ms)
+        return out
+    finally:
+        eng.close()
+
+
+def forces_main(a, res):
+    res["forces"], res["force_writes"] = [], []
+    for name, k in FORCE_ROWS:
+        m = model(name, FORCE_SCENES)
+        for label, md in (("graph", _capi.MODE_GRAPH), ("resident", _capi.MODE_RESIDENT)):
+            # off, on, off, on with zero forces: the same work but the force read; the spread of each pair is next to the difference
+            ms = [measure(m, md, k, forces=bool(i & 1)).get("ms", float("nan")) for i in range(4)]
+            extra = min(ms[1::2]) - min(ms[0::2])
+            res["forces"].append({"scene": name, "K": k, "mode": label, "off_ms": ms[0::2], "on_ms": ms[1::2], "forces_ms": extra})
+            print("  forces %-13s K=%5d %-8s off %.4f %.4f ms | on %.4f %.4f ms | forces %+.4f ms (%+.1f %%)"
+                  % (name, k, label, ms[0], ms[2], ms[1], ms[3], extra, 100.0 * extra / min(ms[0::2])), flush=True)
+            if name != "cfg2":
+                w = force_write_timing(m, md, k)
+                res["force_writes"].append({"scene": name, "K": k, "mode": label, **{h + "_ms": v for h, v in w.items()}})
+                print("  force writes %-13s K=%5d %-8s per step: no write %.4f %.4f ms | host call %.4f %.4f ms | device call %.4f %.4f ms"
+                      % (name, k, label, *w["none"], *w["host"], *w["device"]), flush=True)
+
+
 def one_after_another(m, mode, k):
     """ms for K replicas stepped one after another by one K = 1 engine: per replica, its x and v uploaded, one step, x and v read
     back (the replicas' states are kept on the host between their steps); wall clock around the sequence, after one warm-up pass."""
@@ -453,6 +512,7 @@ def main():
     ap.add_argument("--colliders", action="store_true", help="only the contact path: batches without and with three per-replica colliders")
     ap.add_argument("--constraint-materials", action="store_true", help="every batch also with per-constraint materials equal to the shared ones; gather timing")
     ap.add_argument("--contact-sensors", action="store_true", help="only the contact path: sensing off / on, and per-step collider moves by host and device calls")
+    ap.add_argument("--forces", action="store_true", help="only external forces: zero forces off / on, and per-step force writes by host and device calls")
     ap.add_argument("--rigid", action="store_true", help="only batches of the rigid-body coupling rig and the masked device body write")
     ap.add_argument("--ks", default=None, help="comma-separated K to measure instead of each scene's sweep")
     ap.add_argument("--no-baseline", action="store_true", help="skip the one-after-another baseline and the C sweep")
@@ -460,8 +520,8 @@ def main():
     res = {"card": card(), "rows": [], "c_sweep": [], "replica_rows": [], "sweep": [], "rest_shapes": [], "derive": [], "colliders": [],
            "constraint_materials": [], "gather": [], "rigid": []}
     print("card: %s" % res["card"], flush=True)
-    if a.rigid:
-        rigid_main(a, res)
+    if a.rigid or a.forces:
+        (rigid_main if a.rigid else forces_main)(a, res)
         if a.out:
             os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
             with open(a.out, "w") as f:

@@ -87,7 +87,8 @@ struct Ctx {
     ImagePlan &out;
     bool tiled;                               // the resident mode's image
     std::vector<unsigned> tileOf;             // host particle -> tile (cluster = tile / C, rank = tile % C)
-    std::vector<unsigned char> homedGlobal;   // host particle lives in global memory (touched by a constraint that spans clusters)
+    std::vector<unsigned char> homedGlobal;   // host particle lives in global memory (touched by a constraint run in another tile)
+    std::vector<unsigned> owner[PBD_NUM_TYPES];  // independent CTAs: local index of a constraint -> its owner tile (else empty)
     unsigned nTiles() const { return out.res.G * out.res.C; }
 };
 
@@ -114,9 +115,14 @@ static void bisect(std::vector<unsigned> &idx, size_t lo, size_t hi, unsigned t0
     #pragma omp taskwait
 }
 
-// Executing tile of a constraint: the tile that holds most of its shared-memory particles (ties: the lowest tile); none -> the tile of
-// its first particle (0 for a joint between rigid bodies).  *touchesGlobal: one of its particles is global-homed.
-static inline unsigned exec_tile(int t, const unsigned *b, int nb, const std::vector<unsigned> &tileOf, const std::vector<unsigned char> &homedGlobal, bool *touchesGlobal) {
+// Executing tile of constraint `local` of type t: its owner with independent CTAs (every shared-memory particle of it is homed there);
+// else the tile that holds most of its shared-memory particles (ties: the lowest tile); none -> the tile of its first particle (0 for a
+// joint between rigid bodies).  *touchesGlobal: one of its particles is global-homed.
+static inline unsigned exec_tile(const Ctx &c, int t, unsigned local, bool *touchesGlobal) {
+    const int nb = type_shape(t).nBodies;
+    const unsigned *b = &c.in.store[t].bodies[(size_t)local * nb];
+    const std::vector<unsigned> &tileOf = c.tileOf;
+    const std::vector<unsigned char> &homedGlobal = c.homedGlobal;
     bool x = false;
     unsigned best = 0xffffffffu, bestCnt = 0, first = 0xffffffffu;
     for (int k = 0; k < nb; k++) {
@@ -128,7 +134,42 @@ static inline unsigned exec_tile(int t, const unsigned *b, int nb, const std::ve
         if (cnt > bestCnt || (cnt == bestCnt && tileOf[b[k]] < best)) { best = tileOf[b[k]]; bestCnt = cnt; }
     }
     *touchesGlobal = x;
+    if (!c.owner[t].empty()) return c.owner[t][local];
     return (best != 0xffffffffu) ? best : (first != 0xffffffffu ? first : 0u);
+}
+
+// Independent CTAs (G > 1, C = 1): homing by constraint owner.  A constraint's owner is the tile that holds most of its particles
+// (ties: the lowest tile; rigid bodies do not count), and the owner runs it.  A particle stays in the shared memory of its tile when
+// every constraint through it is owned there, else it is global-homed (its tile still integrates it and updates its velocity).  So an
+// item's shared-memory particles are always its owner's, and a constraint across a cut makes global only its particles outside its
+// owner.  Making global every particle of a constraint whose particles lie in two tiles (the cluster regimes' rule) puts a band as wide
+// as the widest stencil (a bending constraint: two cells) on both sides of every cut: at cfg2 10.4 % X items and 6.5 % global-homed
+// particles, against 6.4 % and 3.3 % here (DESIGN.md section 6).  The tiles stay the particles' bisection, so each holds its share of
+// the particles whatever the constraints are.
+static void home_by_owner(Ctx &c) {
+    const unsigned *tileOf = c.tileOf.data();
+    unsigned char *hg = c.homedGlobal.data();
+    for (int t = 0; t < PBD_NUM_TYPES; t++) {
+        const TypeStore &h = c.in.store[t];
+        const int nb = type_shape(t).nBodies;
+        std::vector<unsigned> &owner = c.owner[t];
+        owner.assign(h.ids.size(), 0u);
+        #pragma omp parallel for schedule(static) num_threads(host_threads())
+        for (long long k0 = 0; k0 < (long long)h.ids.size(); k0++) {
+            const unsigned *b = &h.bodies[(size_t)k0 * nb];
+            unsigned best = 0xffffffffu, bestCnt = 0;
+            for (int k = 0; k < nb; k++) {
+                if (is_rb_body(t, k)) continue;
+                unsigned cnt = 0;
+                for (int j = 0; j < nb; j++) cnt += (!is_rb_body(t, j) && tileOf[b[j]] == tileOf[b[k]]);
+                if (cnt > bestCnt || (cnt == bestCnt && tileOf[b[k]] < best)) { best = tileOf[b[k]]; bestCnt = cnt; }
+            }
+            if (best == 0xffffffffu) continue;  // no particle (a joint between rigid bodies): tile 0
+            owner[k0] = best;
+            for (int k = 0; k < nb; k++)
+                if (!is_rb_body(t, k) && tileOf[b[k]] != best) hg[b[k]] = 1;  // every writer stores the same byte
+        }
+    }
 }
 
 // shape of the launch: type mask / block size of the instantiation, clusters x CTAs per cluster
@@ -219,8 +260,10 @@ static std::string place_in_tiles(Ctx &c) {
             }
             lo = hi;
         }
-        // global-homed = touched by a constraint whose particles lie in more than one cluster
-        if (G > 1)
+        // global-homed: independent CTAs, touched by a constraint owned by another tile; clusters of several CTAs, touched by a
+        // constraint whose particles lie in more than one cluster
+        if (G > 1 && C == 1) home_by_owner(c);
+        else if (G > 1)
             for (int t = 0; t < PBD_NUM_TYPES; t++) {
                 const TypeStore &h = in.store[t];
                 const int nb = type_shape(t).nBodies;
@@ -234,8 +277,10 @@ static std::string place_in_tiles(Ctx &c) {
                 }
             }
         // threads of a CTA dedicated to the X items: in proportion to their share, times 3.1 because an X item waits for L2 where
-        // the others read shared memory.  The factor is carried over from an earlier GPU; on an H100 80GB HBM3 (400 W) cfg2 is flat in
-        // it: 160 / 192 / 224 / 256 X threads -> 2.07 / 2.05 / 2.09 / 2.11 ms, within the run-to-run spread.
+        // the others read shared memory.  The factor is carried over from an earlier GPU.  H100 80GB HBM3 (700 W), ms per step at 128 /
+        // 160 / 192 / 224 X threads, two alternating runs each, with a first homing by owner of nearly the same X share (DESIGN.md
+        // section 6): cfg2 1.694 / 1.675 / 1.699 / 1.739 (this rule: 128), cfg5 1.142-1.145 / 1.136-1.145 / 1.124-1.140 / 1.128-1.140
+        // (this rule: 256).
         if (G > 1) {
             unsigned long long xItems = 0;
             for (int t = 0; t < PBD_NUM_TYPES; t++) {
@@ -355,7 +400,7 @@ static void sort_bucket(const Ctx &c, unsigned g, int t, std::vector<unsigned> &
         unsigned long long run = 0;
         if (tiled) {
             bool x = false;
-            const unsigned exec = exec_tile(t, b, nb, c.tileOf, c.homedGlobal, &x);
+            const unsigned exec = exec_tile(c, t, items[i], &x);
             run = 2ull * exec + (x ? 0u : 1u);
         }
         keyed[i] = std::make_pair((run << 51) | mn, items[i]);
@@ -610,18 +655,20 @@ static std::string build_phase_tables(Ctx &c, const std::vector<unsigned> (&orde
         unsigned long long xItems = 0, mxRun = 0;
         std::vector<unsigned long long> perTile(T, 0);  // items a tile executes over one sweep
         unsigned long long lockstep = 0;                // ... and the sum over the colours of the largest tile's items of the colour
+        unsigned long long rLargest = 0, xLargest = 0;  // sum over the colours of the largest tile's R / X items of the colour
         for (unsigned cl = 0; cl < nC; cl++) {
-            unsigned long long mx = 0;
+            unsigned long long mx = 0, mxR = 0, mxX = 0;
             for (unsigned t = 0; t < T; t++) {
-                unsigned long long items = 0;
+                unsigned long long items = 0, rItems = 0;
                 for (unsigned bi = colourStart[cl]; bi < colourStart[cl + 1]; bi++) {
                     xItems += run(bi, t)[1] - run(bi, t)[0];
                     items += run(bi, t)[2] - run(bi, t)[0];
+                    rItems += run(bi, t)[2] - run(bi, t)[1];
                     mxRun = std::max<unsigned long long>(mxRun, run(bi, t)[2] - run(bi, t)[0]);
                 }
-                perTile[t] += items; mx = std::max(mx, items);
+                perTile[t] += items; mx = std::max(mx, items); mxR = std::max(mxR, rItems); mxX = std::max(mxX, items - rItems);
             }
-            lockstep += mx;
+            lockstep += mx; rLargest += mxR; xLargest += mxX;
         }
         std::vector<unsigned> hist(kMaxXNeighbours + 1, 0u);
         for (unsigned t = 0; t < T; t++) hist[nNbr[t]]++;
@@ -632,6 +679,10 @@ static std::string build_phase_tables(Ctx &c, const std::vector<unsigned> (&orde
         const unsigned long long mxTile = T ? *std::max_element(perTile.begin(), perTile.end()) : 0;
         fprintf(stderr, "\n[pbd_b200] resident: items per sweep, sum over colours of the largest tile %llu, largest tile over all colours %llu (lockstep penalty %.2f %%)\n",
                 lockstep, mxTile, mxTile ? 100.0 * ((double)lockstep / mxTile - 1.0) : 0.0);
+        // what a colour phase waits for: the CTA with the most shared-memory (R) items, and the one with the most X items, of the colour
+        fprintf(stderr, "[pbd_b200] resident: largest tile's items per colour (mean over colours): R %.1f (%.1f per R thread), X %.1f (%.2f per X thread)\n",
+                (double)rLargest / std::max(1u, nC), (double)rLargest / std::max(1u, nC) / std::max(1u, pl.res.threads - pl.res.xThreads),
+                (double)xLargest / std::max(1u, nC), (double)xLargest / std::max(1u, nC) / std::max(1u, pl.res.xThreads));
         // the constraint stream of one sweep as this image streams it from DRAM: the 32-bit indices, the per-constraint geometry and
         // material arrays, the multipliers (read and written)
         double idxBytes = 0, constBytes = 0;
